@@ -7,10 +7,13 @@ Contract: python bench.py --gpus N --steps K --warmup W   (torchrun for N>1) pri
   e2e     : the same metric through the reference-facing call g4r_train_steps (host schedule arrays -> H2D -> column plans ->
             steps -> D2H costs), wall clock between barriers
   roofline: the kernel that ran in the timed region: whole-step algorithmic bytes (SURVEY 8d) / measured step time vs the
-            measured HBM peak; the per-phase `k_lossgrad` figure is kept as a sub-field
+            H100 SXM data-sheet HBM3 bandwidth; the per-phase `k_lossgrad` figure is kept as a sub-field
   cpu_baseline: the NumPy oracle (port of the reference; Theano is not installable) on the host cores, bounded sample
 --impl reference : times that CPU port alone (rank 0 only), same metric / config.
 --workload cfg1|cfg2|cfg2x|cfg3|cfg4 : the other BASELINE.json configurations (default cfg2 = the headline)
+--dump-outputs DIR : after the timed steps, write what they computed as DIR/<name>.npy (float32): the cost of every timed
+            mini-batch and the model parameters after the last one (a fixed, seeded sample of the rows of a table larger than
+            8 MB).  Inputs depend only on the arguments, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -131,37 +134,28 @@ class ClockSampler(threading.Thread):
                 'samples_timed': int(sum(1 for r in self.rows if r[3])), 'source': self.source}
 
 
+# NVIDIA's H100 SXM data sheet (700 W card): dense BF16 tensor rate and HBM3 bandwidth.  Data-sheet figures, not measurements.
 def peak_tensor():
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))['bf16_tflops_sustained']), 'measured sustained bf16 (MEASURED_PEAKS.json)'
-        except Exception:
-            pass
-    return 2250.0, 'nominal dense bf16 (B200_PROFILING.md)'
+    return 989.0, 'H100 SXM data sheet, dense bf16'
 
 
 def peak_hbm():
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-        except Exception:
-            pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet, HBM3'
 
 
-def ncu_traffic(wl):
-    """DRAM bytes per mini-batch of the dominant kernel from the committed ncu --set full capture (profiles/ncu_traffic.json)."""
-    p = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    try:
-        d = json.load(open(p))
-        e = d.get(wl)
-        if e:
-            return e['dram_bytes_per_step'], e['source'], e.get('kernel')
-    except Exception:
-        pass
-    return None, None, None
+DUMP_TABLE_BYTES = 8 << 20
+
+
+def dump_outputs(eng, out_dir, costs, names):
+    """costs of the timed mini-batches + every parameter tensor after the last one (float32, < 64 MB for every workload)"""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'costs.npy'), np.asarray(costs, dtype=np.float32))
+    for name in names:
+        a = eng.get(name)
+        if a.nbytes > DUMP_TABLE_BYTES:
+            keep = max(1, DUMP_TABLE_BYTES // (a.shape[1] * 4))
+            a = a[np.sort(np.random.RandomState(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def build_workload(wl, n_steps_needed, seed=0):
@@ -247,6 +241,7 @@ def main():
     ap.add_argument('--steps', type=int, default=4000)
     ap.add_argument('--warmup', type=int, default=200)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write what the timed steps computed as DIR/<name>.npy (single GPU)')
     ap.add_argument('--workload', default='cfg2', choices=sorted(WORKLOADS))
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--replicated', action='store_true', help='N>1: replicated tables + NCCL exchange (round-1 path) instead of row sharding')
@@ -258,6 +253,8 @@ def main():
     if args.impl == 'reference':
         run_reference(args, rank, world)
         return
+    if args.dump_outputs and world > 1:
+        raise SystemExit('--dump-outputs needs --gpus 1')
     import torch
     from gru4rec_b200 import _lib
     if not torch.cuda.is_available():
@@ -357,6 +354,8 @@ def main():
         wall = time.time() - t0
         costs = np.concatenate(cost_parts)
         launches = eng.kernel_launches() - launches0
+        if args.dump_outputs:
+            dump_outputs(eng, args.dump_outputs, costs, sorted(host))
         if dist is not None:
             t = torch.tensor([dev_ms], device='cuda'); dist.all_reduce(t, op=dist.ReduceOp.MAX); dev_ms = float(t.item())
         value = world * K / (dev_ms / 1000.0)
@@ -442,7 +441,7 @@ def main():
     achieved = step_bytes / step_s / 1e9
     tensor = None
     if world == 1 and eng.uses_tensor_cores():
-        # the step ran on the tcgen05 path (g4r_tcstep.cuh): the contractions bound it, not the row traffic.  fp32-equivalent
+        # the step ran on the tensor-core path (g4r_tcstep.cuh): the contractions bound it, not the row traffic.  fp32-equivalent
         # FLOPs of the eight products: gates, candidate, scores, dSy, dL/dh, d(H*r), dL/d(input), dense gradients
         L = mk['layers'][-1]
         macs = 16.0 * B * L * L + 3.0 * B * N * L
@@ -450,9 +449,8 @@ def main():
         tensor = {'flops_per_step': 2.0 * macs, 'achieved': 2.0 * macs / step_s / 1e12, 'peak': tf_peak / 6.0, 'unit': 'TFLOP/s',
                   'peak_source': tf_src + '; bf16 dense / 2 (TF32 rate) / 3 (3xTF32: three tensor-core products per fp32 product)'}
         tensor['frac'] = tensor['achieved'] / tensor['peak']
-        kernel = ('k_ts_gemm (tcgen05 kind::tf32, 3xTF32, 128x256 tiles, K split over thread-block clusters; 8 products per mini-batch on 3 streams '
+        kernel = ('k_ts_gemm (wgmma tf32, 3xTF32, 128x256 tiles, K split over thread-block clusters; 8 products per mini-batch on 3 streams '
                   '+ operand-preparation / loss / sparse-update kernels; one CUDA graph per 16 mini-batches)')
-    traffic, traffic_src, traffic_kernel = ncu_traffic(args.workload) if world == 1 else (None, None, None)
     if world == 1:
         par = 'dp1'
     elif sharded:
@@ -467,8 +465,8 @@ def main():
         'dtype': 'f32', 'data': 'synthetic',
         'config': bench_config(wl, world, {
             'parallelism': par,
-            'l2': 'inputs larger than L2 at the headline shape: item tables + Adagrad/momentum state = 180 MB, rows touched change every step (no flush '
-                  'between steps; ncu shows the sampled rows staying L2-resident in steady state, see roofline.traffic)',
+            'l2': 'inputs larger than the 50 MB L2 at the headline shape: item tables + Adagrad/momentum state = 180 MB, rows touched change every '
+                  'step (no flush between steps)',
             'step_mode': int(cfg.step_mode), 'fast_windows': fastw, 'upload_and_plan_ms_per_window': (plan_s / max(n_win, 1) * 1000.0) if device_timed else None, 'events_per_sec': value * B, 'timing': 'cuda events, max over ranks' if device_timed else 'wall clock between barriers, max over ranks',
             'vs_baseline_source': 'BASELINE.md: ~%g mb/s published by the reference: %s' % (wl['published'], wl['published_src'])}),
         'e2e': {'value': e2e_value, 'unit': 'mb/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': 4},
@@ -478,14 +476,10 @@ def main():
                      'achieved': tensor['achieved'] if tensor else achieved, 'peak': tensor['peak'] if tensor else peak,
                      'unit': 'TFLOP/s' if tensor else 'GB/s', 'frac': tensor['frac'] if tensor else achieved / peak,
                      'tensor': tensor, 'hbm': {'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak},
-                     # DRAM bytes (ncu dram__bytes_read.sum + dram__bytes_write.sum) on the same footing as algorithmic_bytes_per_launch:
-                     # the committed capture's bytes per mini-batch x the K mini-batches of the timed region
-                     'traffic': (traffic * K) if traffic is not None else None, 'traffic_per_step': traffic,
-                     'traffic_source': traffic_src, 'traffic_kernel': traffic_kernel,
                      'peak_source': peak_src, 'algorithmic_bytes_per_launch': step_bytes * K, 'algorithmic_bytes_per_step': step_bytes,
                      'us_per_step': step_s * 1e6,
-                     'note': ('tensor-core path: a chain of 7 dependent split-K products per mini-batch (each ~4 us of tcgen05 issue + ~12 us of launch, '
-                              'operand fetch, L2 exchange and epilogue latency); the fraction is against the 3xTF32-equivalent tensor peak') if tensor else
+                     'note': ('tensor-core path: a chain of 7 dependent split-K products per mini-batch (launch, operand fetch, L2 exchange and '
+                              'epilogue latency between them); the fraction is against the 3xTF32-equivalent tensor peak') if tensor else
                              ('latency-bound: ~15 dependent phases per mini-batch over an L2-resident working set (SURVEY fact 5); the HBM roofline is the '
                               'contract\'s denominator, not the binding limit'),
                      'k_fast_update_phase': fast_phase, 'per_phase_mode': per_phase},

@@ -180,7 +180,7 @@ def make_config(n_items, mk, sample_store=0, eval_lanes=0, max_resident_steps=0,
     cfg.eval_batch_size = eval_lanes
     cfg.step_mode = step_mode
     cfg.mg_replicated = 1 if replicated else 0     # multi-GPU: replicated tables + NCCL exchange instead of row sharding
-    cfg.eval_tc = 0 if eval_tc is None else (2 if eval_tc else 1)   # scoring path: auto / force tcgen05 tiles / force fp32 FFMA tiles
+    cfg.eval_tc = 0 if eval_tc is None else (2 if eval_tc else 1)   # scoring path: auto / force tensor-core tiles / force fp32 FFMA tiles
     set_adapt_params(cfg, mk.get('adapt', 'adagrad'), mk.get('adapt_params', []), mk.get('grad_cap', 0.0))
     return cfg
 
@@ -249,7 +249,7 @@ class Engine(object):
         if use_torch_allocator:
             import torch
             if not torch.cuda.is_available():
-                raise RuntimeError('gru4rec_b200 needs a CUDA device (B200 / sm_100a); there is no CPU fallback')
+                raise RuntimeError('gru4rec_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback')
             self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device='cuda:%d' % device)
             ws_ptr = C.c_void_p(self._ws.data_ptr())
         h = C.c_void_p()

@@ -38,7 +38,7 @@ __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, i
   float sc = a + md.By[item];
   const float pre = sc;
   if (md.fact.kind <= G4R_ACT_SELU) sc = act_fwd(md.fact, sc);
-  if (lohi_stride > 0) {      // tcgen05 ranking: the two pre-activation thresholds of this lane (g4r_eval_tc.cuh)
+  if (lohi_stride > 0) {      // tensor-core ranking: the two pre-activation thresholds of this lane (g4r_eval_tc.cuh)
     float lo, hi;
     tc_thresholds(md.fact, md.fact.kind <= G4R_ACT_SELU, sc, pre, lo, hi);
     tgt[lohi_stride + b] = lo; tgt[2 * lohi_stride + b] = hi;
@@ -204,7 +204,7 @@ struct EvalCtx {
   int cap = 0;
   int slot = -1;
   int* dCand = nullptr; int n_cand = 0; size_t cand_cap = 0;     // candidate subset of evaluate_gpu(items=...), item indices
-  unsigned char *dAsplit = nullptr, *dBsplit = nullptr;           // tcgen05 path: hi / lo TF32 operand blocks (g4r_eval_tc.cuh)
+  unsigned char *dAsplit = nullptr, *dBsplit = nullptr;           // tensor-core path: hi / lo TF32 operand blocks (g4r_eval_tc.cuh)
 };
 
 static void eval_release(g4r_handle* h) {
@@ -273,7 +273,7 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
   CK(cudaMemcpyAsync(e->dCut, cut_off, n_cut * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(e->dSums, 0, 128 * sizeof(double), st));
   // tensor-core scoring (full-catalogue ranking of a wide batch): the item table is split once per evaluation into hi / lo
-  // TF32 operand blocks; cfg.eval_tc: 1 forces the fp32 FFMA tiles, 2 forces tcgen05
+  // TF32 operand blocks; cfg.eval_tc: 1 forces the fp32 FFMA tiles, 2 forces the wgmma 3xTF32 tiles
   const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC,      // + the bias column
              tc_tiles = (I + TC_N - 1) / TC_N, tc_lblocks = (Be + TC_M - 1) / TC_M;
   const bool tc_possible = e->n_cand == 0 && mode != 3 && h->cfg.eval_tc != 1 && (h->cfg.eval_tc == 2 || (Bs >= 64 && I >= 2048));

@@ -1,36 +1,32 @@
-// g4r_eval_tc.cuh -- full-catalogue scoring of evaluate_gpu on the 5th-generation tensor cores (tcgen05 + TMEM).
+// g4r_eval_tc.cuh -- full-catalogue scoring of evaluate_gpu on the Hopper tensor cores (wgmma, sm_90a).
 //
 // What is computed (reference: yhat = h Wy^T + By, gru4rec.py:502; ranks = (others > targets).sum + 1, evaluation.py:57-64):
 // for every lane b of the evaluation batch the number of catalogue items whose score beats / ties the score of the lane's
 // target.  The [items x lanes] score matrix (37,483 x 512 at the RSC15 shape: 3.8 GFLOP per mini-batch, the largest dense
-// contraction of the whole path) is never written: each 128-lane x 256-item tile is accumulated in TMEM by UMMA
-// (tcgen05.mma kind::tf32, M = 128, N = 256, K = 8), read back with tcgen05.ld, and reduced to the two counters in registers.
+// contraction of the whole path) is never written: each 128-lane x 256-item tile is accumulated in registers by
+// wgmma.mma_async (kind tf32, m64n128k8 per warpgroup) and reduced to the two counters right there.
 //
 // fp32 fidelity on TF32 tensor cores: 3xTF32 -- every fp32 operand x is split as hi = tf32(x), lo = tf32(x - hi) and the
 // product is accumulated as lo*hi + hi*lo + hi*hi (the dropped lo*lo term and the roundings are ~2^-21 relative), i.e. ~1e-6
 // relative on the scores, far inside the 1e-4 bar on Recall / MRR.  The target's own column is excluded explicitly (it is
 // the one comparison that must be exact), so a rank can only move where two DIFFERENT items' scores differ by < 1e-6 relative.
 //
-// Structure (one CTA per SM, 320 threads, persistent over its item tiles):
-//   pre-pass   k_tc_split writes the operands as hi / lo TF32 blocks in the K-major 128-byte-swizzle UMMA layout: the item table
+// Structure (one CTA per SM, 512 threads = four warpgroups, persistent over its item tiles):
+//   pre-pass   k_tc_split writes the operands as hi / lo TF32 blocks in the K-major 128-byte-swizzle layout: the item table
 //              once per evaluation, the hidden states once per mini-batch; one extra K column carries the item bias (1.0 on the
 //              hidden-state side), so the accumulator is the complete pre-activation score
-//   warp 8     TMA producer (one thread): two bulk copies (cp.async.bulk -> mbarrier complete_tx) per 32-wide K chunk fill a
-//              96 KB stage [A hi | A lo | B hi | B lo]; two stages
-//   warp 9     MMA issuer (one thread): 12 tcgen05.mma per chunk, tcgen05.commit hands the stage back / publishes the accumulator
-//   warps 0-7  epilogue: wait for the accumulator (2 x 256 TMEM columns, double buffered), tcgen05.ld 32 columns at a time, two
-//              compares per item against the lane's pre-activation thresholds (k_eval_tgt computes them once per lane) -- a
-//              thread owns one evaluation lane (TMEM lane), so the two counters are thread-local; two warps per lane quarter
-//              split the tile's columns
-// All waits are mbarrier try_wait loops with a time-out that sets an error flag (a wrong phase must not hang the box).
+//   loads      thread 0: two bulk copies (cp.async.bulk -> mbarrier complete_tx) per 32-wide K chunk fill a 96 KB stage
+//              [A hi | A lo | B hi | B lo]; two stages, a stage is refilled once all four warpgroups have released it
+//   MMA        each warpgroup: 12 wgmma per chunk on its 64 x 128 quarter of the tile
+//   epilogue   two compares per item against the lane's pre-activation thresholds (k_eval_tgt computes them once per lane),
+//              counters thread-local, summed over the four threads of a quad at the end of a lane block
+// All waits are mbarrier try_wait loops with a time-out that traps (a wrong phase must not hang the device).
 #pragma once
 
-constexpr int TC_M = 128;            // evaluation lanes per tile (UMMA M, TMEM lanes: one per epilogue thread)
-constexpr int TC_N = 256;            // items per tile (UMMA N, TMEM columns per accumulator)
+constexpr int TC_M = 128;            // evaluation lanes per tile (two warpgroups of 64 rows)
+constexpr int TC_N = 256;            // items per tile (two warpgroups of 128 columns)
 constexpr int TC_KC = 32;            // K chunk per pipeline stage (floats)
-constexpr int TC_EPI_WARPS = 8;      // two warps per TMEM lane quarter (each takes half of the tile's columns)
-constexpr int TC_EPI_THREADS = TC_EPI_WARPS * 32;
-constexpr int TC_THREADS = TC_EPI_THREADS + 64;     // + TMA producer warp + MMA issuer warp
+constexpr int TC_THREADS = 512;      // four consumer warpgroups: rows (wg & 1) * 64, columns (wg >> 1) * 128 of the tile
 constexpr int TC_STAGES = 2;
 constexpr uint32_t TC_A_BYTES = TC_M * TC_KC * 4;       // 16 KB per hi / lo array
 constexpr uint32_t TC_B_BYTES = TC_N * TC_KC * 4;       // 32 KB
@@ -40,10 +36,7 @@ constexpr unsigned long long TC_TIMEOUT_NS = 2000000000ull;
 struct TcSmem {
   alignas(1024) unsigned char stage[TC_STAGES][TC_STAGE_BYTES];   // [A hi | A lo | B hi | B lo]
   alignas(8) unsigned long long stage_full[TC_STAGES];    // operand blocks of the stage have landed (TMA complete_tx)
-  unsigned long long stage_free[TC_STAGES];    // MMAs that read the stage have completed (tcgen05.commit)
-  unsigned long long acc_full[2];              // all MMAs of the tile have completed (tcgen05.commit)
-  unsigned long long acc_free[2];              // epilogue has drained the accumulator (256 arrivals)
-  uint32_t tmem_base;
+  unsigned long long stage_free[TC_STAGES];    // the four warpgroups' MMAs that read the stage have completed
   int err;
 };
 
@@ -71,20 +64,63 @@ __device__ __forceinline__ bool tc_mbar_wait(unsigned long long* bar, unsigned i
 }
 __device__ __forceinline__ uint32_t tc_tf32(float x) { uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x)); return r; }
 // K-major operand blocks in the 128-byte-swizzle layout: a row is 32 tf32 values = 128 bytes, eight rows form a 1024-byte atom in
-// which the 16-byte piece c of row r sits at position c ^ (r % 8) (the tensor core reads a whole 128-byte row per access; the
-// unswizzled 8 x 16-byte core-matrix layout measured ~8x slower operand fetch).  SBO (next 8 rows) = 1024 B, LBO unused (1);
-// blocks are 1024-byte aligned, a K step of 8 values advances the start address by 32 bytes inside the atom.
+// which the 16-byte piece c of row r sits at position c ^ (r % 8) (the tensor core reads a whole 128-byte row per access without
+// bank conflicts).  wgmma shared-memory descriptor: SBO (next 8 rows) = 1024 B, LBO unused for swizzled K-major operands (1),
+// layout type 1 = 128-byte swizzle; blocks are 1024-byte aligned, a K step of 8 values advances the start address by 32 bytes
+// inside the atom, 64 rows further is +8 KB.
 __device__ __forceinline__ uint64_t tc_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
 }
 // byte offset of the 16-byte piece (row r, k = 4 * kq .. 4 * kq + 3) inside a block of rows x 32 k-values
 __device__ __forceinline__ uint32_t tc_block_off(int r, int kq) { return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((kq ^ (r & 7)) << 4)); }
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-               :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
+
+// ---- warpgroup MMA (wgmma, sm_90a): D[64 x NW] += A[64 x 8] B[NW x 8]^T in TF32, both operands K-major in shared memory, D in
+// registers.  Accumulator fragment of thread t of the warpgroup: d[i] = D[16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2)]
+// [8 * (i / 4) + 2 * (t % 4) + i % 2] ----
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from touching the accumulator registers across the asynchronous MMAs
+template <int NR>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; i++) asm volatile("" : "+f"(d[i]) :: "memory");
 }
-__device__ __forceinline__ void tc_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(tc_smem_u32(bar)) : "memory");
+#define WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wg_mma_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+               "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+               "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24), WG_D8(32), WG_D8(40), WG_D8(48), WG_D8(56)
+               : "l"(a_desc), "l"(b_desc) : "memory");
+}
+__device__ __forceinline__ void wg_mma_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+               "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24)
+               : "l"(a_desc), "l"(b_desc) : "memory");
+}
+#undef WG_D8
+// one 32-wide K chunk of a 3xTF32 product for one warpgroup: lo*hi + hi*lo + hi*hi over four steps of 8, then wait for it (the
+// operand blocks are zero beyond the live K, so a partial last chunk needs no special case)
+template <int NR>
+__device__ __forceinline__ void wg_chunk_3xtf32(float (&d)[NR], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+  wg_fence_acc(d);
+  wg_fence();
+#pragma unroll
+  for (int j = 0; j < TC_KC / 8; j++) {
+    const uint32_t o = (uint32_t)j * 32u;      // 8 values along K = 32 bytes inside the swizzle atom
+    wg_mma_tf32(d, tc_desc(a_lo + o), tc_desc(b_hi + o));
+    wg_mma_tf32(d, tc_desc(a_hi + o), tc_desc(b_lo + o));
+    wg_mma_tf32(d, tc_desc(a_hi + o), tc_desc(b_hi + o));
+  }
+  wg_commit();
+  wg_wait0();
+  wg_fence_acc(d);
 }
 
 // Pre-split operand blocks in global memory (written once per evaluation for the item table, once per mini-batch for the hidden
@@ -160,131 +196,91 @@ __device__ __forceinline__ void tc_thresholds(const ActSpec a, bool elem_act, fl
 
 // cnt[b*2 + 0] += #items with score > target score of lane b; cnt[b*2 + 1] += #items with score == target (the target itself
 // counts as one tie, exactly as in the fp32 kernel where its score equals the target score bit for bit).
-// Tile = 128 evaluation lanes (UMMA M, TMEM lanes: one lane per epilogue thread, so the counting is thread-local) x 256 items
-// (UMMA N, TMEM columns).  Asplit: hidden-state blocks of 128 lanes, Bsplit: item-table blocks of 256 items (k_tc_split).
+// Tile = 128 evaluation lanes x 256 items; warpgroup wg accumulates rows (wg & 1) * 64 .. + 63 x columns (wg >> 1) * 128 .. + 127 in
+// registers, so a thread holds two lanes x 32 items and counts them thread-locally.  Asplit: hidden-state blocks of 128 lanes,
+// Bsplit: item-table blocks of 256 items (k_tc_split).  Thread 0 also feeds the stages: it issues the bulk copies of a stage as
+// soon as all four warpgroups have finished the MMAs that read it.
 __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, const float* __restrict__ tgt, int tgt_stride, int* cnt,
                                                            const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit) {
   extern __shared__ __align__(1024) unsigned char tc_raw[];
   TcSmem& sm = *reinterpret_cast<TcSmem*>(tc_raw);
   const ModelDev& md = MD;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int M = md.wM[s], I = md.n_items, K = md.L + 1;        // + the bias column
   const int n_tiles = (I + TC_N - 1) / TC_N;         // item tiles
   const int n_lb = (M + TC_M - 1) / TC_M;            // lane blocks
   const int n_chunk = (K + TC_KC - 1) / TC_KC;
+  const int my_tiles = blockIdx.x < n_tiles ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const unsigned int total = (unsigned int)(n_lb * my_tiles * n_chunk);     // (lane block, tile, chunk) sequence of this CTA
   if (tid == 0) {
-    for (int i = 0; i < TC_STAGES; i++) { tc_mbar_init(&sm.stage_free[i], 1); tc_mbar_init(&sm.stage_full[i], 1); }
-    for (int i = 0; i < 2; i++) { tc_mbar_init(&sm.acc_full[i], 1); tc_mbar_init(&sm.acc_free[i], TC_EPI_THREADS); }
+    for (int i = 0; i < TC_STAGES; i++) { tc_mbar_init(&sm.stage_free[i], 4); tc_mbar_init(&sm.stage_full[i], 1); }
     sm.err = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (warp == TC_EPI_WARPS) {   // TMEM: 512 columns = two 128 x 256 fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(tc_smem_u32(&sm.tmem_base)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = sm.tmem_base;
-  // instruction descriptor: D = F32, A = B = TF32, both K-major, N = 256, M = 128
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TC_N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-  if (warp == TC_EPI_WARPS) {
-    // ================= TMA producer (one thread): operand blocks -> shared memory stages =================
-    if (lane == 0) {
-      unsigned int it = 0;
-      for (int lb = 0; lb < n_lb; lb++)
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x)
-          for (int c = 0; c < n_chunk; c++, it++) {
-            const uint32_t st = it & 1u, use = it >> 1;
-            if (use > 0) tc_mbar_wait(&sm.stage_free[st], (use - 1) & 1u, &sm.err);     // the MMAs of the previous use are done
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(tc_smem_u32(&sm.stage_full[st])), "r"(TC_STAGE_BYTES) : "memory");
-            tc_bulk_copy(sm.stage[st], Asplit + ((size_t)lb * n_chunk + c) * 2 * TC_A_BYTES, 2 * TC_A_BYTES, &sm.stage_full[st]);
-            tc_bulk_copy(sm.stage[st] + 2 * TC_A_BYTES, Bsplit + ((size_t)t * n_chunk + c) * 2 * TC_B_BYTES, 2 * TC_B_BYTES, &sm.stage_full[st]);
-          }
-    }
-  } else if (warp == TC_EPI_WARPS + 1) {
-    // ================= MMA issuer (one thread) =================
-    if (lane == 0) {
-      unsigned int it = 0, wi = 0;
-      for (int lb = 0; lb < n_lb; lb++)
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, wi++) {
-          const uint32_t acc = wi & 1u;
-          if (wi >= 2) tc_mbar_wait(&sm.acc_free[acc], ((wi >> 1) - 1) & 1u, &sm.err);   // epilogue drained this accumulator
-          for (int c = 0; c < n_chunk; c++, it++) {
-            const uint32_t st = it & 1u, use = it >> 1;
-            tc_mbar_wait(&sm.stage_full[st], use & 1u, &sm.err);                         // operand blocks have landed
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_hi = tc_smem_u32(sm.stage[st]), a_lo = a_hi + TC_A_BYTES, b_hi = a_hi + 2 * TC_A_BYTES, b_lo = b_hi + TC_B_BYTES;
-            const uint32_t d = tmem + acc * TC_N;
-            const int ksteps = (min(TC_KC, K - c * TC_KC) + 7) / 8;
-            for (int j = 0; j < ksteps; j++) {
-              const uint32_t o = (uint32_t)j * 32u;      // 8 values along K = 32 bytes inside the swizzle atom
-              tc_mma_tf32(d, tc_desc(a_lo + o), tc_desc(b_hi + o), idesc, (c == 0 && j == 0) ? 0u : 1u);
-              tc_mma_tf32(d, tc_desc(a_hi + o), tc_desc(b_lo + o), idesc, 1u);
-              tc_mma_tf32(d, tc_desc(a_hi + o), tc_desc(b_hi + o), idesc, 1u);
-            }
-            tc_commit(&sm.stage_free[st]);
-            if (c == n_chunk - 1) tc_commit(&sm.acc_full[acc]);
-          }
-        }
-    }
-  } else if (warp < TC_EPI_WARPS) {
-    // ================= epilogue: TMEM -> registers -> thread-local counters =================
-    // warp w reads TMEM lanes 32 * (w % 4) .. + 31 (its evaluation lanes) and the column half w / 4 of the tile
-    unsigned int wi = 0;
-    const bool elem_act = md.fact.kind <= G4R_ACT_SELU;
-    const int q4 = warp & 3, half = warp >> 2;
-    for (int lb = 0; lb < n_lb; lb++) {
-      const int b = lb * TC_M + q4 * 32 + lane;
-      const bool vrow = b < M;
-      const int yit = vrow ? md.wY[(size_t)s * md.B + b] : -1;
-      const float lo = vrow ? tgt[tgt_stride + b] : INFINITY, hi = vrow ? tgt[2 * tgt_stride + b] : INFINITY;   // k_eval_tgt
-      int cgt = 0, cge = 0;
-      for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, wi++) {
-        const uint32_t acc = wi & 1u;
-        const int i0 = t * TC_N;
-        tc_mbar_wait(&sm.acc_full[acc], (wi >> 1) & 1u, &sm.err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int self_col = yit - i0;                       // the target's own column (if it falls into this tile)
-#pragma unroll 1
-        for (int q = 0; q < 4; q++) {
-          const int c0 = half * 128 + q * 32;
-          uint32_t r[32];
-          const uint32_t taddr = tmem + ((uint32_t)(q4 * 32) << 16) + acc * TC_N + c0;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                       : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                         "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-                         "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-                         "=r"(r[30]), "=r"(r[31]) : "r"(taddr) : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  auto issue = [&](unsigned int it) {
+    const int c = (int)(it % n_chunk), q = (int)(it / n_chunk), t = blockIdx.x + (q % my_tiles) * gridDim.x, lb = q / my_tiles;
+    const uint32_t st = it % TC_STAGES;
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(tc_smem_u32(&sm.stage_full[st])), "r"(TC_STAGE_BYTES) : "memory");
+    tc_bulk_copy(sm.stage[st], Asplit + ((size_t)lb * n_chunk + c) * 2 * TC_A_BYTES, 2 * TC_A_BYTES, &sm.stage_full[st]);
+    tc_bulk_copy(sm.stage[st] + 2 * TC_A_BYTES, Bsplit + ((size_t)t * n_chunk + c) * 2 * TC_B_BYTES, 2 * TC_B_BYTES, &sm.stage_full[st]);
+  };
+  if (tid == 0) for (unsigned int it = 0; it < total && it < (unsigned)TC_STAGES; it++) issue(it);
+  __syncwarp();
+  const int wr = (wg & 1) * 64, wc = (wg >> 1) * 128;          // this warpgroup's rows / columns of the tile
+  const int rq = (warp & 3) * 16 + (lane >> 2);                 // first of the thread's two rows inside the warpgroup's 64
+  unsigned int it = 0;
+  for (int lb = 0; lb < n_lb; lb++) {
+    int bb[2], yit[2]; bool vrow[2]; float lo[2], hi[2];
+    int cgt[2] = {0, 0}, cge[2] = {0, 0};
 #pragma unroll
-          for (int j = 0; j < 32; j++) {
-            const float x = __uint_as_float(r[j]);
-            cgt += (x > hi) ? 1 : 0;
-            cge += (x >= lo) ? 1 : 0;
-          }
-          if ((unsigned)(self_col - c0) < 32u) {             // rare: take the target's own column back out, it counts as exactly one tie
-            float xs = 0.f;
+    for (int h = 0; h < 2; h++) {
+      bb[h] = lb * TC_M + wr + rq + 8 * h;
+      vrow[h] = bb[h] < M;
+      yit[h] = vrow[h] ? md.wY[(size_t)s * md.B + bb[h]] : -1;
+      lo[h] = vrow[h] ? tgt[tgt_stride + bb[h]] : INFINITY; hi[h] = vrow[h] ? tgt[2 * tgt_stride + bb[h]] : INFINITY;   // k_eval_tgt
+    }
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      float d[64];
 #pragma unroll
-            for (int j = 0; j < 32; j++) if (j == self_col - c0) xs = __uint_as_float(r[j]);
-            cgt -= (xs > hi) ? 1 : 0;
-            cge -= (xs >= lo) ? 1 : 0;
-            cge += 1;                                        // == (self: not above) + one tie
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        tc_mbar_arrive(&sm.acc_free[acc]);
+      for (int i = 0; i < 64; i++) d[i] = 0.f;
+      for (int c = 0; c < n_chunk; c++, it++) {
+        const uint32_t st = it % TC_STAGES, use = it / TC_STAGES;
+        tc_mbar_wait(&sm.stage_full[st], use & 1u, &sm.err);                         // operand blocks have landed
+        const uint32_t a_hi = tc_smem_u32(sm.stage[st]) + wr * 128, a_lo = a_hi + TC_A_BYTES;
+        const uint32_t b_hi = tc_smem_u32(sm.stage[st]) + 2 * TC_A_BYTES + wc * 128, b_lo = b_hi + TC_B_BYTES;
+        wg_chunk_3xtf32(d, a_hi, a_lo, b_hi, b_lo);
+        if ((tid & 127) == 0) tc_mbar_arrive(&sm.stage_free[st]);
+        if (tid == 0 && it + TC_STAGES < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + TC_STAGES); }
+        __syncwarp();
       }
-      const int ceq = cge - cgt;                            // lo <= x <= hi
-      if (vrow) { if (cgt) atomicAdd(&cnt[b * 2], cgt); if (ceq) atomicAdd(&cnt[b * 2 + 1], ceq); }
+      // two compares per item against the lane's pre-activation thresholds
+      const int c0 = t * TC_N + wc + 2 * (lane & 3);                // item of d[0]
+#pragma unroll
+      for (int i = 0; i < 64; i++) {
+        const int h = (i >> 1) & 1;
+        cgt[h] += (d[i] > hi[h]) ? 1 : 0;
+        cge[h] += (d[i] >= lo[h]) ? 1 : 0;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int rel = yit[h] - c0;                                 // the target's own column, if this thread holds it
+        if (rel >= 0 && rel < 128 && (rel & 7) < 2) {               // rare: take it back out, it counts as exactly one tie
+          float xs = 0.f;
+#pragma unroll
+          for (int i = 0; i < 64; i++) if (((i >> 1) & 1) == h && (i >> 2) * 8 + (i & 1) == rel) xs = d[i];
+          cgt[h] -= (xs > hi[h]) ? 1 : 0;
+          cge[h] -= (xs >= lo[h]) ? 1 : 0;
+          cge[h] += 1;                                               // == (self: not above) + one tie
+        }
+      }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == TC_EPI_WARPS) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(512u) : "memory");
+#pragma unroll
+    for (int h = 0; h < 2; h++) {                                    // the four threads of a quad share the two rows
+      int g = cgt[h], e = cge[h] - cgt[h];                           // lo <= x <= hi
+      g += __shfl_xor_sync(0xffffffffu, g, 1); g += __shfl_xor_sync(0xffffffffu, g, 2);
+      e += __shfl_xor_sync(0xffffffffu, e, 1); e += __shfl_xor_sync(0xffffffffu, e, 2);
+      if ((lane & 3) == 0 && vrow[h]) { if (g) atomicAdd(&cnt[bb[h] * 2], g); if (e) atomicAdd(&cnt[bb[h] * 2 + 1], e); }
+    }
   }
 }

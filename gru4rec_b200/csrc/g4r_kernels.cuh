@@ -1,4 +1,4 @@
-// g4r_kernels.cuh -- device code of the GRU4Rec session-parallel training step for sm_100a.
+// g4r_kernels.cuh -- device code of the GRU4Rec session-parallel training step for sm_90a (H100).
 //
 // One mini-batch (reference: one call of the compiled Theano `train_function`, gru4rec.py:584,623) is a
 // fixed sequence of phases.  Each phase is a __device__ function parameterised on (cta, n_cta) so the same

@@ -48,7 +48,7 @@ struct g4r_handle {
   char* ws = nullptr; size_t ws_bytes = 0; bool own_ws = false;
   size_t ws_off = 0;
   std::map<std::string, TensorInfo> tensors;
-  int Bmax = 0, n_sm = 148;
+  int Bmax = 0, n_sm = 132;
   int CAP = 0;
   // window staging (pinned host) and device arrays (non-const views of md.w*)
   int *hX = nullptr, *hY = nullptr, *hSlot = nullptr, *hM = nullptr, *hSti = nullptr; uint8_t* hF = nullptr; uint32_t* hG = nullptr;
@@ -312,7 +312,7 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     tsb.O = cv.take<float>((size_t)tsb.Mpad * tsb.ldO); tsb.bias = cv.take<float>(tsb.Nk);
   }
   // evaluation
-  int* dRank = cv.take<int>((size_t)Be * 4); float* dTgt = cv.take<float>((size_t)Be * 3);   // target scores | lower | upper pre-activation thresholds (tcgen05 ranking)
+  int* dRank = cv.take<int>((size_t)Be * 4); float* dTgt = cv.take<float>((size_t)Be * 3);   // target scores | lower | upper pre-activation thresholds (tensor-core ranking)
   if (!cv.dry) {
     md.wX = dX; md.wY = dY; md.wSlot = dSlot; md.wM = dM; md.wSti = dSti; md.wXnext = dXnext; md.wF = dF; md.wXflag = dXflag; md.wG = dG;
     md.ST = dST; md.logP0t = dL0t; md.logP0s = dL0s;
@@ -528,6 +528,18 @@ static int ts_opt_in(g4r_handle* h) {
     if (raise_smem_limit(f, sizeof(TsSmem)) != cudaSuccess) return G4R_ERR_CUDA;
     if (cudaFuncSetAttribute(f, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) return G4R_ERR_CUDA;
   }
+  // a cluster larger than the portable 8 (one CTA per SM) must fit into one GPC: halve it until the device can schedule one
+  while (g_ts_cluster_big > 8) {
+    cudaLaunchConfig_t lc = {};
+    cudaLaunchAttribute at[1];
+    lc.gridDim = dim3(g_ts_cluster_big); lc.blockDim = dim3(TS_THREADS); lc.dynamicSmemBytes = sizeof(TsSmem);
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = g_ts_cluster_big; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    lc.attrs = at; lc.numAttrs = 1;
+    int ncl = 0;
+    if (cudaOccupancyMaxActiveClusters(&ncl, k_ts_gemm<TS_EPI_DH>, &lc) == cudaSuccess && ncl >= 1) break;
+    cudaGetLastError();
+    g_ts_cluster_big /= 2;
+  }
   return G4R_OK;
 }
 static int enqueue_tc_step(g4r_handle* h, const int* base, int off) {
@@ -652,7 +664,7 @@ extern "C" int g4r_workspace_bytes(const g4r_config* cfg, size_t* bytes) {
   std::string err;
   int rc = validate_config(*cfg, err);
   if (rc) { g_create_error = err; return rc; }
-  int n_sm = 148;
+  int n_sm = 132;
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) == cudaSuccess && dev_count > cfg->device) {
     cudaDeviceProp p; if (cudaGetDeviceProperties(&p, cfg->device) == cudaSuccess) n_sm = p.multiProcessorCount;
@@ -1009,7 +1021,7 @@ extern "C" int g4r_gather_rows(g4r_handle* h, const float* table, int64_t rows, 
   CK(cudaMemcpyAsync(dt, table, rows * cols * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(di, idx, n_idx * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemsetAsync(derr, 0, sizeof(int), h->stream));
-  k_gather_rows<<<(unsigned)std::min<int64_t>(n_idx, 148 * 8), 128, 0, h->stream>>>(dt, rows, cols, di, n_idx, dout, derr);
+  k_gather_rows<<<(unsigned)std::min<int64_t>(n_idx, (int64_t)h->n_sm * 8), 128, 0, h->stream>>>(dt, rows, cols, di, n_idx, dout, derr);
   h->launches++;
   int herr = 0;
   CK(cudaMemcpyAsync(out, dout, n_idx * cols * sizeof(float), cudaMemcpyDeviceToHost, h->stream));

@@ -2,30 +2,30 @@
 // (constrained_embedding, one GRU layer, hidden size >= 160, batch <= 256: paramfiles/{rees46,coveo,diginetica,yoochoose,
 // retailrocket}_*_best.py of the reference -- B = 48..240, L = 224..512, 2048 negative samples).  At these shapes a mini-batch is
 // ~4 GFLOP of dense contractions (gru4rec.py:460-461 gates, :493 sampled scores, and their gradients from T.grad, :383-384);
-// the generic kernels run them on FP32 FFMA tiles at ~4 TFLOP/s.  Here every contraction is a tcgen05 GEMM:
+// the generic kernels run them on FP32 FFMA tiles.  Here every contraction is a wgmma GEMM (Hopper tensor cores):
 //
-//   operands  fp32 values are split into hi = tf32(x), lo = tf32(x - hi) ("3xTF32": lo*hi + hi*lo + hi*hi accumulated in fp32 in
-//             TMEM reproduces the fp32 product to ~2^-21 relative) and stored as [hi | lo] blocks of 128 rows x 32 k-values in the
-//             K-major 128-byte-swizzle UMMA layout by small "prep" kernels that also do the gathers
+//   operands  fp32 values are split into hi = tf32(x), lo = tf32(x - hi) ("3xTF32": lo*hi + hi*lo + hi*hi accumulated in fp32
+//             reproduces the fp32 product to ~2^-21 relative) and stored as [hi | lo] blocks of 128 rows x 32 k-values in the
+//             K-major 128-byte-swizzle layout by small "prep" kernels that also do the gathers
 //             (Wy[item] rows of the score columns, H through the lane slots), transposes and elementwise products (H * r);
-//   GEMM      128 x 256 output tiles (a tcgen05.mma costs ~150 cycles to issue whatever its N, so N is as wide as the
-//             instruction allows); K is split over the CTAs of a thread-block cluster.  Per CTA: a TMA thread streams the operand
-//             blocks with bulk copies into a 2-stage shared-memory ring (mbarrier complete_tx), an MMA thread issues tcgen05.mma
-//             kind::tf32 (M = 128, N = 256, K = 8) and hands stages back with tcgen05.commit, four warps read the accumulator with
-//             tcgen05.ld; the partial tile goes through L2, and after a cluster barrier each CTA adds the K splits of its band of
-//             rows in K order and applies the fused epilogue (gates + sigmoid + the H*r operand, candidate + GRU update + dropout +
-//             reset + the score operand, score + bias, dSy rows, b1 = elementwise GRU backward + operands, da_r, dL/d(input));
+//   GEMM      128 x 256 output tiles (128 x 128 where the product has at most 128 columns); K is split over the CTAs of a
+//             thread-block cluster.  Per CTA: thread 0 streams the operand blocks with bulk copies into a shared-memory ring
+//             (mbarrier complete_tx), four warpgroups issue wgmma.mma_async kind tf32 (m64, N = NT / 2, k8) on their quarter of the
+//             tile with the accumulator in registers; the partial tile goes through L2, and after a cluster barrier each CTA adds
+//             the K splits of its band of rows in K order and applies the fused epilogue (gates + sigmoid + the H*r operand,
+//             candidate + GRU update + dropout + reset + the score operand, score + bias, dSy rows, b1 = elementwise GRU backward +
+//             operands, da_r, dL/d(input));
 //             the two dense-gradient products leave their partial tiles to an elementwise kernel that does the optimizer step;
 //   schedule  three streams joined by events (captured into the step graph), programmatic dependent launch along the main chain;
 //   the rest  row statistics + dL/do (one kernel per step), and the deterministic sparse updates reuse the generic phases
 //             (g4r_kernels.cuh) -- same numerics, same duplicate rules.
-// Included from g4r_lib.cu after g4r_eval.cuh (uses its mbarrier / UMMA helpers).
+// Included from g4r_lib.cu after g4r_eval.cuh (uses its mbarrier / wgmma helpers).
 #pragma once
 #include <cooperative_groups.h>
 
 constexpr int TS_RB = 128;                               // rows per operand block
 constexpr uint32_t TS_BLK = TS_RB * TC_KC * 4;           // bytes of one hi (or lo) block: 16 KB
-constexpr int TS_THREADS = 512;                          // 4 TMEM-reading warps + TMA warp + MMA warp; all 16 warps run the reduce / epilogue
+constexpr int TS_THREADS = 512;                          // four MMA warpgroups (64 rows x NT / 2 columns each); all 16 warps run the reduce / epilogue
 
 
 
@@ -320,13 +320,11 @@ __global__ void __launch_bounds__(256) k_ts_bh(int slot, const int* base, int of
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// the GEMM: D[128 x NT tile] = A[128 x K] B[NT x K]^T, 3xTF32.  A tcgen05.mma costs ~150 cycles to issue whatever its N
-// (scripts/micro/mma_rate.cu), so the tiles are as wide as the instruction allows (N = 256 wherever the product has more than
-// 128 columns) and the parallelism comes from splitting K over the CTAs of a thread-block CLUSTER: each CTA accumulates its K
-// slice in TMEM, parks the partial tile in its own shared memory, and after a cluster barrier every CTA sums one band of rows over
-// all peers through distributed shared memory (fixed order) and applies the fused epilogue with coalesced accesses.
-// (TsGemm.P != nullptr: partial tiles go to global memory instead and k_ts_epi reduces them -- the dense-update products, whose
-// epilogue is a full optimizer step per element and wants the whole GPU.)
+// the GEMM: D[128 x NT tile] = A[128 x K] B[NT x K]^T, 3xTF32.  The parallelism comes from splitting K over the CTAs of a
+// thread-block CLUSTER: each CTA accumulates its K slice in registers, writes the partial tile to L2, and after a cluster barrier
+// every CTA sums one band of rows over all peers (fixed order) and applies the fused epilogue with coalesced accesses.
+// (TsGemm.fused == 0: k_ts_epi reduces the partial tiles instead -- the dense-update products, whose epilogue is a full optimizer
+// step per element and wants the whole GPU.)
 // ---------------------------------------------------------------------------------------------------------------------
 enum { TS_EPI_F1 = 0, TS_EPI_F2, TS_EPI_SCORE, TS_EPI_DSY, TS_EPI_DH, TS_EPI_B2, TS_EPI_B3, TS_EPI_DENSE_A, TS_EPI_DENSE_B };
 // live extent of a product at this step (dynamic mini-batch size / column count)
@@ -458,8 +456,6 @@ struct TsSmem {
   alignas(1024) unsigned char stage[TS_SMEM_OPER];
   alignas(8) unsigned long long stage_full[4];
   unsigned long long stage_free[4];
-  unsigned long long acc_full;
-  uint32_t tmem_base;
   int err;
 };
 __device__ __forceinline__ void ts_cluster_sync() {
@@ -468,12 +464,61 @@ __device__ __forceinline__ void ts_cluster_sync() {
 }
 
 #define TS_STAMP(i) do { if (g.dbg) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); g.dbg[(size_t)blockIdx.x * 16 + (i)] = t_; } } while (0)
+// main loop of one CTA: its K slice of the 128 x NT tile, warpgroup wg accumulating rows (wg & 1) * 64 .. + 63 x columns
+// (wg >> 1) * NT / 2 .. in registers (NR = NT / 4 floats per thread); thread 0 also issues the bulk copies of the stage ring.
+// On return the stages are free and the partial tile is in sT [128 x (NT + 4)] (row-major, in the stage memory).
+template <int NR>
+__device__ __forceinline__ void ts_mainloop(TsSmem& sm, const TsGemm& g, int mt, int nt, int c_beg, int c_end, float* sT) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int NT = 4 * NR;
+  const int nb = NT / TS_RB;                                  // 128-row operand blocks per N tile
+  const uint32_t b_bytes = (uint32_t)NT * TC_KC * 4;          // one hi (or lo) slab of the N tile
+  const uint32_t stage_bytes = 2 * TS_BLK + 2 * b_bytes;      // 64 KB (NT = 128, 3 stages) or 96 KB (NT = 256, 2 stages)
+  const uint32_t n_stage = TS_SMEM_OPER / stage_bytes;
+  const unsigned int total = c_end > c_beg ? (unsigned int)(c_end - c_beg) : 0u;
+  auto issue = [&](unsigned int it) {
+    const int c = c_beg + (int)it;
+    unsigned char* dst = sm.stage + (it % n_stage) * stage_bytes;
+    unsigned long long* bar = &sm.stage_full[it % n_stage];
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(tc_smem_u32(bar)), "r"(stage_bytes) : "memory");
+    tc_bulk_copy(dst, g.A + ((size_t)mt * g.chunks + c) * 2 * TS_BLK, 2 * TS_BLK, bar);
+    for (int q = 0; q < nb; q++) {                  // smem: [hi of all blocks | lo of all blocks]
+      const unsigned char* bsrc = g.Bm + ((size_t)(nt * nb + q) * g.chunks + c) * 2 * TS_BLK;
+      tc_bulk_copy(dst + 2 * TS_BLK + q * TS_BLK, bsrc, TS_BLK, bar);
+      tc_bulk_copy(dst + 2 * TS_BLK + b_bytes + q * TS_BLK, bsrc + TS_BLK, TS_BLK, bar);
+    }
+  };
+  if (tid == 0) { for (unsigned int it = 0; it < total && it < n_stage; it++) issue(it); TS_STAMP(2); }
+  __syncwarp();
+  const int wr = (wg & 1) * 64, wc = (wg >> 1) * (NT / 2);
+  float d[NR];
+#pragma unroll
+  for (int i = 0; i < NR; i++) d[i] = 0.f;                    // a K split without chunks contributes zeros
+  for (unsigned int it = 0; it < total; it++) {
+    const uint32_t st = it % n_stage, use = it / n_stage;
+    tc_mbar_wait(&sm.stage_full[st], use & 1u, &sm.err);
+    if (it == 0 && tid == 0) TS_STAMP(3);
+    const uint32_t a_hi = tc_smem_u32(sm.stage + st * stage_bytes) + wr * 128, a_lo = a_hi + TS_BLK;
+    const uint32_t b_hi = tc_smem_u32(sm.stage + st * stage_bytes) + 2 * TS_BLK + wc * 128, b_lo = b_hi + b_bytes;
+    wg_chunk_3xtf32(d, a_hi, a_lo, b_hi, b_lo);
+    if ((tid & 127) == 0) tc_mbar_arrive(&sm.stage_free[st]);
+    if (tid == 0 && it + n_stage < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + n_stage); }
+    __syncwarp();
+  }
+  if (tid == 0) TS_STAMP(4);
+  __syncthreads();                                            // every warpgroup is done with the stages: they become sT
+  const int ldt = NT + 4;
+  const int r0 = wr + (warp & 3) * 16 + (lane >> 2), cq = wc + 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < NR; i += 2)
+    *reinterpret_cast<float2*>(sT + (size_t)(r0 + 8 * ((i >> 1) & 1)) * ldt + cq + (i >> 2) * 8) = make_float2(d[i], d[i + 1]);
+}
 template <int EPI>
 __global__ void __launch_bounds__(TS_THREADS, 1) k_ts_gemm(int slot, const int* base, int off, TsGemm g, TsBuf tb) {
   extern __shared__ __align__(1024) unsigned char ts_raw[];
   TsSmem& sm = *reinterpret_cast<TsSmem*>(ts_raw);
   const ModelDev& md = MD; const int s = STEP_IDX;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int M = md.wM[s];
   const int N = M + (md.wSti[s] >= 0 ? md.S : 0);
   // the cluster = the K splits of one tile (consecutive blocks): all of them take the same early exit
@@ -483,26 +528,12 @@ __global__ void __launch_bounds__(TS_THREADS, 1) k_ts_gemm(int slot, const int* 
   if (!ts_tile_live<EPI>(md, tb, M, N, m0, n0)) { pdl_wait(); return; }     // dynamic batch size / column count; unused blocks of the dense-gradient products
   const int cps = (g.chunks + g.ksplit - 1) / g.ksplit;
   const int c_beg = ks * cps, c_end = min(g.chunks, c_beg + cps);
-  const bool empty = c_beg >= c_end;                          // a K split without chunks contributes zeros
-  const uint32_t b_bytes = (uint32_t)g.NT * TC_KC * 4;        // one hi (or lo) slab of the N tile
-  const uint32_t stage_bytes = 2 * TS_BLK + 2 * b_bytes;      // 64 KB (NT = 128, 3 stages) or 96 KB (NT = 256, 2 stages)
-  const uint32_t n_stage = TS_SMEM_OPER / stage_bytes;
   if (tid == 0) {
-    for (int i = 0; i < 4; i++) { tc_mbar_init(&sm.stage_free[i], 1); tc_mbar_init(&sm.stage_full[i], 1); }
-    tc_mbar_init(&sm.acc_full, 1);
+    for (int i = 0; i < 4; i++) { tc_mbar_init(&sm.stage_free[i], 4); tc_mbar_init(&sm.stage_full[i], 1); }
     sm.err = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(tc_smem_u32(&sm.tmem_base)), "r"((uint32_t)g.NT) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = sm.tmem_base;
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(g.NT >> 3) << 17) | ((uint32_t)(TS_RB >> 4) << 24);
   if (tid == 0) TS_STAMP(1);
   pdl_wait();               // everything above overlapped the previous kernel of the stream; its results are visible from here on
   pdl_trigger();
@@ -513,84 +544,14 @@ __global__ void __launch_bounds__(TS_THREADS, 1) k_ts_gemm(int slot, const int* 
     md.cost[s] = c;
     if (c != c) atomicExch(md.nanflag, 1);
   }
-  if (warp == 4) {
-    if (lane == 0) {
-      unsigned int it = 0;
-      const int nb = g.NT / TS_RB;                      // 128-row operand blocks per N tile
-      for (int c = c_beg; c < c_end; c++, it++) {
-        const uint32_t st = it % n_stage, use = it / n_stage;
-        unsigned char* dst = sm.stage + st * stage_bytes;
-        if (use > 0) tc_mbar_wait(&sm.stage_free[st], (use - 1) & 1u, &sm.err);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(tc_smem_u32(&sm.stage_full[st])), "r"(stage_bytes) : "memory");
-        tc_bulk_copy(dst, g.A + ((size_t)mt * g.chunks + c) * 2 * TS_BLK, 2 * TS_BLK, &sm.stage_full[st]);
-        for (int q = 0; q < nb; q++) {                  // smem: [hi of all blocks | lo of all blocks]
-          const unsigned char* bsrc = g.Bm + ((size_t)(nt * nb + q) * g.chunks + c) * 2 * TS_BLK;
-          tc_bulk_copy(dst + 2 * TS_BLK + q * TS_BLK, bsrc, TS_BLK, &sm.stage_full[st]);
-          tc_bulk_copy(dst + 2 * TS_BLK + b_bytes + q * TS_BLK, bsrc + TS_BLK, TS_BLK, &sm.stage_full[st]);
-        }
-        if (c == c_beg) TS_STAMP(2);
-      }
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      unsigned int it = 0;
-      for (int c = c_beg; c < c_end; c++, it++) {
-        const uint32_t st = it % n_stage, use = it / n_stage;
-        tc_mbar_wait(&sm.stage_full[st], use & 1u, &sm.err);
-        if (c == c_beg) TS_STAMP(3);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_hi = tc_smem_u32(sm.stage + st * stage_bytes), a_lo = a_hi + TS_BLK, b_hi = a_hi + 2 * TS_BLK, b_lo = b_hi + b_bytes;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const uint32_t o = (uint32_t)j * 32u;        // 8 values along K = 32 bytes inside the swizzle atom
-          tc_mma_tf32(tmem, tc_desc(a_lo + o), tc_desc(b_hi + o), idesc, (c == c_beg && j == 0) ? 0u : 1u);
-          tc_mma_tf32(tmem, tc_desc(a_hi + o), tc_desc(b_lo + o), idesc, 1u);
-          tc_mma_tf32(tmem, tc_desc(a_hi + o), tc_desc(b_hi + o), idesc, 1u);
-        }
-        tc_commit(&sm.stage_free[st]);
-      }
-      if (empty) tc_mbar_arrive(&sm.acc_full); else tc_commit(&sm.acc_full);
-      TS_STAMP(4);
-    }
-  } else if (warp < 4) {
-    tc_mbar_wait(&sm.acc_full, 0u, &sm.err);
-    if (tid == 0) TS_STAMP(5);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  }
-  // TMEM lane = tile row: an epilogue thread holds its row in 32-column groups
-  auto load_group = [&](int q, uint32_t (&r)[32]) {
-    if (empty) {
-#pragma unroll
-      for (int j = 0; j < 32; j++) r[j] = 0u;
-      return;
-    }
-    const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + q * 32;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-                   "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-                   "=r"(r[30]), "=r"(r[31]) : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  };
-  // split K through global memory (L2).  TMEM lane = tile row, so a thread holds one row: the tile is transposed through shared
-  // memory (the operand stages are free once the accumulator is complete) and all warps store it as whole 512-byte row pieces
+  // split K through global memory (L2): the register tiles are transposed through shared memory (the operand stages are free once
+  // the accumulation is complete) and all warps store the tile as whole 512-byte row pieces
   {
     float* sT = reinterpret_cast<float*>(sm.stage);
-    const int ldt = g.NT + 4, q4 = g.NT / 4;
-    if (warp < 4) {
-      float* srow = sT + (size_t)(warp * 32 + lane) * ldt;
-      for (int q = 0; q < g.NT / 32; q++) {
-        uint32_t r[32];
-        load_group(q, r);
-#pragma unroll
-        for (int j = 0; j < 8; j++)
-          *reinterpret_cast<uint4*>(srow + q * 32 + j * 4) = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (g.NT == 256) ts_mainloop<64>(sm, g, mt, nt, c_beg, c_end, sT); else ts_mainloop<32>(sm, g, mt, nt, c_beg, c_end, sT);
     __syncthreads();
     if (tid == 0) TS_STAMP(6);
+    const int ldt = g.NT + 4, q4 = g.NT / 4;
     float* ptile = g.P + ((size_t)ks * g.m_tiles * TS_RB + m0) * g.ldP + n0;
     for (int idx = tid; idx < TS_RB * q4; idx += TS_THREADS) {
       const int row = idx / q4, c = (idx % q4) * 4;
@@ -600,8 +561,7 @@ __global__ void __launch_bounds__(TS_THREADS, 1) k_ts_gemm(int slot, const int* 
   if (g.fused) {
     // the K splits of a tile are the CTAs of one cluster (co-resident): after the cluster barrier (release / acquire) CTA `ks` adds
     // the splits of its band of rows in K order -- the same sum whatever the schedule -- and applies the epilogue, consecutive
-    // threads on consecutive column quads.  (Measured: exchanging the tiles through distributed shared memory instead costs
-    // 6.7 us per 128 KB tile at ~20 B/clk per SM; L2 moves the same bytes in ~1.3 us.)
+    // threads on consecutive column quads
     __threadfence();
     ts_cluster_sync();
     if (tid == 0) TS_STAMP(7);
@@ -629,11 +589,5 @@ __global__ void __launch_bounds__(TS_THREADS, 1) k_ts_gemm(int slot, const int* 
       for (int u = 0; u < 4; u++) if (ok[u]) ts_epilogue4<EPI>(md, tb, s, mm[u], nn[u], acc[u]);
     }
     if (tid == 0) TS_STAMP(8);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 4) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"((uint32_t)g.NT) : "memory");
   }
 }

@@ -1,9 +1,9 @@
-"""GRU4Rec with the reference's class surface (hidasib/GRU4Rec gru4rec.py:27-781) on the B200 engine.
+"""GRU4Rec with the reference's class surface (hidasib/GRU4Rec gru4rec.py:27-781) on the H100 engine.
 
 `run.py -g gru4rec_b200.gru4rec` (or the root-level shim module `gru4rec`) selects this class through the
 reference's own plugin seam (run.py:21,39).  Constructor arguments, set_params() coercions and prints,
 fit() / predict_next_batch() / savemodel() / loadmodel() signatures and printed lines follow the reference;
-the per-mini-batch work runs in libg4r.so (hand-written sm_100a CUDA) through ctypes.  PyTorch is used
+the per-mini-batch work runs in libg4r.so (hand-written sm_90a CUDA) through ctypes.  PyTorch is used
 only to allocate the device workspace.  There is no CPU fallback.
 
 Interface restatement, stated plainly: `__init__` (argument list, defaults, attribute assignments), `set_params` (the
@@ -107,7 +107,7 @@ class GRU4Rec:
     # have no counterpart here (the device kernels are selected from the `loss` / `final_act` / `hidden_act` strings).
     def _make_stub(name):
         def stub(self, *a, **k):
-            raise NotImplementedError('Theano graph builders are not part of the B200 implementation')
+            raise NotImplementedError('Theano graph builders are not part of the CUDA implementation')
         stub.__name__ = name            # bound methods are pickled by name: it must be the reference's method name
         stub.__qualname__ = 'GRU4Rec.' + name
         return stub
@@ -121,19 +121,19 @@ class GRU4Rec:
         def __init__(self, lmbd=1.0, alpha=1.0):
             self.lmbd = lmbd; self.alpha = alpha
         def execute(self, X):
-            raise NotImplementedError('Theano graph builders are not part of the B200 implementation')
+            raise NotImplementedError('Theano graph builders are not part of the CUDA implementation')
 
     class Elu:
         def __init__(self, alpha=1.0):
             self.alpha = alpha
         def execute(self, X):
-            raise NotImplementedError('Theano graph builders are not part of the B200 implementation')
+            raise NotImplementedError('Theano graph builders are not part of the CUDA implementation')
 
     class LeakyReLU:
         def __init__(self, leak=0.0):
             self.leak = leak
         def execute(self, X):
-            raise NotImplementedError('Theano graph builders are not part of the B200 implementation')
+            raise NotImplementedError('Theano graph builders are not part of the CUDA implementation')
 
     # ---- same validation behaviour as the reference setters (gru4rec.py:136-161) ----
     def set_loss_function(self, loss):

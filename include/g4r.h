@@ -1,5 +1,5 @@
 /*
- * g4r.h -- C ABI of libg4r.so: the B200 (sm_100a) GRU4Rec session-parallel training step.
+ * g4r.h -- C ABI of libg4r.so: the H100 (sm_90a) GRU4Rec session-parallel training step.
  *
  * This is the drop-in boundary for the hot path of hidasib/GRU4Rec.  In the reference the boundary is
  * the set of compiled Theano functions that gru4rec.py / evaluation.py call once per mini-batch; each
@@ -67,10 +67,10 @@ typedef struct g4r_config {
                                      2: role-specialised persistent kernel where the shape allows, else 1;
                                      3: as 2, launched as thread-block clusters: the GRU phases run on one cluster with the
                                         dense weights and optimizer state resident in shared memory (else 1);
-                                     4: tensor-core step (tcgen05 GEMMs) whenever the model allows it -- modes 1-3 pick it
+                                     4: tensor-core step (wgmma GEMMs) whenever the model allows it -- modes 1-3 pick it
                                         automatically for constrained-embedding models with a layer of >= 160 units */
   int32_t mg_replicated;          /* 1: multi-GPU with replicated tables + NCCL exchange instead of row sharding */
-  int32_t eval_tc;                /* scoring path: 0 auto, 1 fp32 FFMA tiles only, 2 tcgen05 (3xTF32) tiles whenever the ranking is full-catalogue */
+  int32_t eval_tc;                /* scoring path: 0 auto, 1 fp32 FFMA tiles only, 2 wgmma (3xTF32) tiles whenever the ranking is full-catalogue */
   float adapt_p1, adapt_p1c;      /* adapt_params[0] and 1 - adapt_params[0] (rmsprop / adadelta decay; adam beta1), gru4rec.py:301-304,342-343,368-369 */
   float adapt_p2, adapt_p2c;      /* adapt_params[1] and 1 - adapt_params[1] (adam beta2) */
   float grad_cap;                 /* > 0: gradients are scaled to this global L2 norm when they exceed it (gru4rec.py:386-389) */
@@ -151,7 +151,7 @@ const char* g4r_phase_name(int32_t i);
 /* step_mode 2: number of windows run by the role-specialised kernel, and (out) windows that fell back to the
  * generic persistent kernel because a chunk of score columns was wider than 16. */
 int64_t g4r_fast_windows(const g4r_handle* h, int64_t* fallback_windows);
-/* 1 if the handle trains with the tensor-core step (tcgen05 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh): constrained
+/* 1 if the handle trains with the tensor-core step (wgmma 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh): constrained
  * embedding, one layer, batch <= 256, SGD / Adagrad (+momentum); automatic for layers >= 160 units, forced with step_mode 4. */
 int g4r_uses_tensor_cores(const g4r_handle* h);
 /* Persistent mode (step_mode 1): enable %globaltimer stamps at the phase boundaries of every step and/or read

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Command-line driver with the interface of the reference's run.py (hidasib/GRU4Rec run.py:10-133): same flags, same
 parameter-file / parameter-string formats, same printed lines (paropt.py parses `PRIMARY METRIC:`).  The model class comes
-in through the reference's plugin seam `-g GRFILE` (default: the root-level `gru4rec` module = the B200 implementation)."""
+in through the reference's plugin seam `-g GRFILE` (default: the root-level `gru4rec` module = the CUDA implementation)."""
 import argparse
 import importlib
 import importlib.util

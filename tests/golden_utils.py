@@ -73,3 +73,32 @@ def fit_data(orc, g, tr):
 def epoch_order(g, d, e):
     """session order of epoch e: recorded np.random.permutation for train_random_order (gru4rec.py:593), else base_order"""
     return g['epoch_orders'][e] if 'epoch_orders' in g else d['base_order']
+
+
+def datatools_cases():
+    """(frame, key columns, any_order) of the sort_if_needed / compute_offset comparison (tests/golden/datatools/cases.npz): random
+    frames of 1..300 events, unsorted, sorted by (session, time), by (session, time, item), and grouped by session in random order."""
+    rs = np.random.RandomState(0)
+    for n in (1, 2, 50, 300):
+        for trial in range(8):
+            df = pd.DataFrame({'SessionId': rs.randint(0, max(2, n // 4), n), 'Time': rs.randint(0, 40, n), 'ItemId': rs.randint(0, 9, n)})
+            if trial % 4 == 1: df = df.sort_values(['SessionId', 'Time']).reset_index(drop=True)
+            if trial % 4 == 2: df = df.sort_values(['SessionId', 'Time', 'ItemId']).reset_index(drop=True)
+            if trial % 4 == 3:      # sessions grouped but in arbitrary order
+                df = df.sort_values(['SessionId', 'Time']).reset_index(drop=True)
+                df = pd.concat([df[df.SessionId == s] for s in rs.permutation(df['SessionId'].unique())]).reset_index(drop=True)
+            for cols in (['SessionId', 'Time'], ['SessionId', 'Time', 'ItemId'], ['SessionId']):
+                for any_order in (False, True):
+                    yield df, cols, any_order
+
+
+def datatools_outcome(mod, df, cols, any_order):
+    """what sort_if_needed of module `mod` printed (minus the timing line), the frame it left (index and columns) and the offsets"""
+    import contextlib
+    import io
+    a, out = df.copy(), io.StringIO()
+    with contextlib.redirect_stdout(out):
+        mod.sort_if_needed(a, cols, any_order)
+    lines = [l for l in out.getvalue().splitlines() if not l.startswith('Data is sorted in')]
+    frame = np.stack([a.index.values] + [a[c].values for c in ('SessionId', 'Time', 'ItemId')], axis=1)
+    return lines, frame, mod.compute_offset(a, 'SessionId')

@@ -1,4 +1,4 @@
-"""-m gpu: full-catalogue evaluation on the tensor cores (tcgen05 3xTF32 tiles, csrc/g4r_eval_tc.cuh) against the fp32 FFMA
+"""-m gpu: full-catalogue evaluation on the tensor cores (wgmma 3xTF32 tiles, csrc/g4r_eval_tc.cuh) against the fp32 FFMA
 tiles and the oracle's evaluate_gpu restatement (evaluation.py:57-75)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""-m gpu: the tensor-core training step (tcgen05 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh) against the oracle:
+"""-m gpu: the tensor-core training step (wgmma 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh) against the oracle:
 constrained embedding, one layer -- the family of the reference's shipped parameter files (paramfiles/*_best.py)."""
 import numpy as np
 import pytest

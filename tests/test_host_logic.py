@@ -126,81 +126,25 @@ def test_loadmodel_reads_reference_written_pickle():
     assert m._engine is None          # no device work until predict / evaluate is called
 
 
-def test_pickle_written_here_loads_into_the_reference_class(tmp_path):
-    """savemodel() of this class -> the REFERENCE's GRU4Rec.loadmodel + evaluate_gpu (run on the Theano shim) reproduce the
-    oracle's Recall/MRR.  Needs /root/reference (not present on the GPU box)."""
-    import subprocess, sys, json
-    if not os.path.exists('/root/reference/gru4rec.py'):
-        pytest.skip('reference tree not available')
-    import gru4rec
-    import pandas as pd
-    from golden_utils import load_golden, frames, init_weights
-    g = load_golden('bprmax_none')
-    mk = g['model_kwargs']
-    _, te = frames(g)
-    m = gru4rec.GRU4Rec(**mk)
-    m.n_items = int(g['n_items'])
-    m.itemidmap = pd.Series(data=np.arange(m.n_items), index=g['itemidmap_index'], name='ItemIdx')
-    fw = init_weights(g, 'final_')
-    m._host = {'Wx0': fw['Wx'][0], 'Wh0': fw['Wh'][0], 'Wrz0': fw['Wrz'][0], 'Bh0': fw['Bh'][0], 'Wy': fw['Wy'], 'By': fw['By']}
-    m.error_during_train = False
-    fn = str(tmp_path / 'b200_model.pickle')
-    m.savemodel(fn)
-    te_fn = str(tmp_path / 'test.pickle'); te.to_pickle(te_fn)
-    code = (
-        "import sys, os, io, json, contextlib\n"
-        "sys.path.insert(0, %r); import theano_shim; theano_shim.install()\n"
-        "sys.path.insert(0, '/root/reference'); cwd = os.getcwd()\n"
-        "import gru4rec as ref, evaluation as ev, pandas as pd; os.chdir(cwd)\n"
-        "g = ref.GRU4Rec.loadmodel(%r)\n"
-        "assert type(g).__module__ == 'gru4rec' and hasattr(g.Wy, 'get_value')\n"
-        "te = pd.read_pickle(%r)\n"
-        "buf = io.StringIO()\n"
-        "with contextlib.redirect_stdout(buf): rec, mrr = ev.evaluate_gpu(g, te, cut_off=[1, 5, 20], batch_size=7)\n"
-        "print(json.dumps([[float(x) for x in rec], [float(x) for x in mrr]]))\n"
-    ) % (os.path.join(ROOT, 'oracle'), fn, te_fn)
-    out = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
-    assert out.returncode == 0, out.stderr[-2000:]
-    rec, mrr = json.loads(out.stdout.strip().splitlines()[-1])
-    np.testing.assert_allclose(rec, g['eval_standard_recall'], rtol=1e-6)
-    np.testing.assert_allclose(mrr, g['eval_standard_mrr'], rtol=1e-6)
-
-
 def test_datatools_behaves_like_the_reference_module():
-    """gru4rec_b200/datatools.py is an independent implementation; wherever the reference checkout is available (this container,
-    not the GPU box) its datatools.py -- plain pandas/NumPy, importable without Theano -- is run side by side on random frames:
-    same printed decision, same in-place result, same int32 offsets."""
-    import io, contextlib, importlib.util
-    import pandas as pd
-    ref_path = '/root/reference/datatools.py'
-    if not os.path.exists(ref_path):
-        pytest.skip('reference checkout not available')
-    spec = importlib.util.spec_from_file_location('ref_datatools', ref_path)
-    ref = importlib.util.module_from_spec(spec); spec.loader.exec_module(ref)
+    """gru4rec_b200/datatools.py is an independent implementation; the reference's datatools.py was run on the same random frames
+    (oracle/make_datatools_golden.py -> tests/golden/datatools/cases.npz): same printed decision, same in-place result, same
+    int32 offsets."""
+    import json
+    from golden_utils import GOLDEN_DIR, datatools_cases, datatools_outcome
     from gru4rec_b200 import datatools as mine
-    rs = np.random.RandomState(0)
+    g = np.load(os.path.join(GOLDEN_DIR, 'datatools', 'cases.npz'))
+    lines = json.loads(str(g['lines']))
+    frames = np.split(g['frames'], np.cumsum(g['frame_rows'])[:-1])
+    offsets = np.split(g['offsets'], np.cumsum(g['offset_len'])[:-1])
     n_cases = 0
-    for n in (1, 2, 50, 300):
-        for trial in range(8):
-            df = pd.DataFrame({'SessionId': rs.randint(0, max(2, n // 4), n), 'Time': rs.randint(0, 40, n), 'ItemId': rs.randint(0, 9, n)})
-            if trial % 4 == 1: df = df.sort_values(['SessionId', 'Time']).reset_index(drop=True)
-            if trial % 4 == 2: df = df.sort_values(['SessionId', 'Time', 'ItemId']).reset_index(drop=True)
-            if trial % 4 == 3:      # sessions grouped but in arbitrary order
-                df = df.sort_values(['SessionId', 'Time']).reset_index(drop=True)
-                df = pd.concat([df[df.SessionId == s] for s in rs.permutation(df['SessionId'].unique())]).reset_index(drop=True)
-            for cols in (['SessionId', 'Time'], ['SessionId', 'Time', 'ItemId'], ['SessionId']):
-                for any_order in (False, True):
-                    a, b = df.copy(), df.copy()
-                    out_a, out_b = io.StringIO(), io.StringIO()
-                    with contextlib.redirect_stdout(out_a): ref.sort_if_needed(a, cols, any_order)
-                    with contextlib.redirect_stdout(out_b): mine.sort_if_needed(b, cols, any_order)
-                    keep = lambda t: [l for l in t.getvalue().splitlines() if not l.startswith('Data is sorted in')]
-                    assert keep(out_a) == keep(out_b)
-                    assert a.equals(b)
-                    oa, ob = ref.compute_offset(a, 'SessionId'), mine.compute_offset(b, 'SessionId')
-                    assert oa.dtype == ob.dtype and np.array_equal(oa, ob)
-                    n_cases += 1
-    assert n_cases == 192
+    for k, (df, cols, any_order) in enumerate(datatools_cases()):
+        l, f, o = datatools_outcome(mine, df, cols, any_order)
+        assert l == lines[k], k
+        np.testing.assert_array_equal(f, frames[k].astype(f.dtype), err_msg=str(k))
+        assert o.dtype == np.dtype(str(g['offset_dtype'])) and np.array_equal(o, offsets[k]), k
+        n_cases += 1
+    assert n_cases == 192 == len(lines)
 
 
 def test_set_params_matches_the_reference_class():
