@@ -41,7 +41,7 @@ EXPORTS = [
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
-    'g4r_eval_schedule', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
+    'g4r_eval_schedule', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
 ]
 
 _lib = None
@@ -105,6 +105,7 @@ def load():
     lib.g4r_mg_shard_rows.argtypes = [i64, i32, i32]; lib.g4r_mg_shard_rows.restype = i64
     lib.g4r_mg_segment_bytes.argtypes = [C.POINTER(G4RConfig), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.g4r_eval_schedule.argtypes = [vp, vp, vp, i32, i32, vp, vp, C.POINTER(i64)]
+    lib.g4r_eval_counts.argtypes = [vp, vp, i64]
     lib.g4r_set_eval_items.argtypes = [vp, vp, i64]
     lib.g4r_predict.argtypes = [vp, vp, i32, vp, vp]
     lib.g4r_reset_eval_hidden.argtypes = [vp]
@@ -467,6 +468,13 @@ class Engine(object):
         n = C.c_int64()
         self._check(self.lib.g4r_eval_schedule(self.h, sched.h, _ptr(cut), len(cut), mode, _ptr(rec), _ptr(mrr), C.byref(n)))
         return rec, mrr, n.value
+
+    def eval_counts(self, n_lanes):
+        """[n_lanes x 2] int32: (#items scoring above the target, #items tied with it incl. the target) of every lane of the last
+        mini-batch ranked by eval_schedule (a diagnostic of the ranking kernels)."""
+        out = np.zeros((n_lanes, 2), dtype=np.int32)
+        self._check(self.lib.g4r_eval_counts(self.h, _ptr(out), n_lanes))
+        return out
 
     def set_eval_items(self, items=None):
         """Candidate item indices for eval_schedule (evaluate_gpu(items=...)); None / empty restores the whole catalogue."""

@@ -346,6 +346,16 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
   return G4R_OK;
 }
 
+extern "C" int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes) {
+  if (!h || !out || n_lanes < 0) return G4R_ERR_INVALID;
+  const int Be = h->cfg.eval_batch_size > 0 ? h->cfg.eval_batch_size : h->cfg.batch_size;
+  if (n_lanes > Be) FAIL(G4R_ERR_INVALID, "n_lanes exceeds eval_batch_size");
+  cudaSetDevice(h->cfg.device);
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(out, h->dRankCnt, (size_t)n_lanes * 2 * sizeof(int), cudaMemcpyDeviceToHost));
+  return G4R_OK;
+}
+
 // evaluate_gpu(items=...) (evaluation.py:52-56,84-100): the targets are ranked against this candidate list (item indices,
 // duplicates allowed as in the reference) instead of the whole catalogue; n = 0 restores the full-catalogue ranking.
 extern "C" int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n) {

@@ -128,9 +128,9 @@ __device__ __forceinline__ void wg_chunk_3xtf32(float (&d)[NR], uint32_t a_hi, u
 // (tc_block_off).  The scoring kernel then feeds the tensor cores with plain bulk copies (TMA) -- no register staging on the
 // critical path.
 // The contraction runs over K + 1 values: column K holds `one` on the hidden-state side and the item bias on the table side
-// (bias != nullptr), so the accumulator is the complete pre-activation score; table rows past the catalogue get a bias of -3e38,
-// which no threshold ever reaches (the epilogue needs no per-column validity test).
-constexpr float TC_PAD_BIAS = -3.0e38f;
+// (bias != nullptr), so the accumulator is the complete pre-activation score.  Table rows past the catalogue are all zero: no pad
+// score can be kept out of the counts by its value (a flat activation gives a lower threshold of -inf), so the epilogue bounds the
+// columns of the last item tile instead.
 template <int RB>
 __global__ void __launch_bounds__(256) k_tc_split(const float* __restrict__ src, int nrows, int ld, int K, unsigned char* __restrict__ dst, int n_chunk,
                                                   const float* __restrict__ bias, float one) {
@@ -144,7 +144,7 @@ __global__ void __launch_bounds__(256) k_tc_split(const float* __restrict__ src,
     const int row = rb * RB + r;
     if (row < nrows && k0 + cc * 4 < K) v = ld4(src + (size_t)row * ld + k0 + cc * 4);
     if (K - (k0 + cc * 4) >= 0 && K - (k0 + cc * 4) < 4) {       // the extra column (K % 4 == 0 is not required)
-      const float x = bias ? (row < nrows ? bias[row] : TC_PAD_BIAS) : one;
+      const float x = bias ? (row < nrows ? bias[row] : 0.f) : one;
       const int u = K - (k0 + cc * 4);
       if (u == 0) v = make_float4(x, 0.f, 0.f, 0.f); else if (u == 1) v.y = x, v.z = 0.f, v.w = 0.f; else if (u == 2) v.z = x, v.w = 0.f; else v.w = x;
     }
@@ -254,13 +254,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, cons
         if (tid == 0 && it + TC_STAGES < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + TC_STAGES); }
         __syncwarp();
       }
-      // two compares per item against the lane's pre-activation thresholds
+      // two compares per item against the lane's pre-activation thresholds; columns past the catalogue (last tile) do not count
       const int c0 = t * TC_N + wc + 2 * (lane & 3);                // item of d[0]
+      const int n_live = I - c0;                                    // d[i] holds item c0 + 8 * (i / 4) + i % 2
 #pragma unroll
       for (int i = 0; i < 64; i++) {
         const int h = (i >> 1) & 1;
-        cgt[h] += (d[i] > hi[h]) ? 1 : 0;
-        cge[h] += (d[i] >= lo[h]) ? 1 : 0;
+        const bool live = (i >> 2) * 8 + (i & 1) < n_live;
+        cgt[h] += (live && d[i] > hi[h]) ? 1 : 0;
+        cge[h] += (live && d[i] >= lo[h]) ? 1 : 0;
       }
 #pragma unroll
       for (int h = 0; h < 2; h++) {

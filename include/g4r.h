@@ -195,6 +195,10 @@ int g4r_mg_segment_bytes(const g4r_config* cfg, size_t* total, size_t* inbox_byt
  * recall_sum/mrr_sum: n_cut doubles each (sums, not yet divided by the number of events). */
 int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
                       double* recall_sum, double* mrr_sum, int64_t* n_events);
+/* Diagnostic: the per-lane counts of the last mini-batch ranked by g4r_eval_schedule.  out[2 b] = number of items whose score
+ * beats the target score of lane b, out[2 b + 1] = number of items whose score equals it (the target itself included).
+ * n_lanes <= the scoring batch size; lanes past that mini-batch's size hold stale values. */
+int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes);
 /* evaluate_gpu(items=...) (evaluation.py:15,52-56,84-100): rank the targets against the `n` candidate item indices instead of
  * the whole catalogue for subsequent g4r_eval_schedule calls (the target's own score competes only if the target is listed,
  * as in the reference); n = 0 restores the full-catalogue ranking.  G4R_ERR_INDEX on an out-of-range index. */

@@ -709,6 +709,7 @@ class OracleGRU4Rec:
         G['dWh'] = [None] * nl
         G['dWrz'] = [None] * nl
         G['dBh'] = [None] * nl
+        G['dvec'] = [None] * nl           # [da_h | da_r | da_z] per layer: lets tests compare the device's gate gradients directly
         first = nl - len(C['layers'])
         for li in range(len(C['layers']) - 1, -1, -1):
             lc = C['layers'][li]
@@ -727,6 +728,7 @@ class OracleGRU4Rec:
             da_rz = np.hstack([da_r, da_z])
             G['dWrz'][i] = H.T @ da_rz
             dvec = np.hstack([da_h, da_rz])
+            G['dvec'][i] = dvec
             G['dBh'][i] = dvec.sum(axis=0)
             if lc['inp'] is not None:
                 G['dWx'][i] = lc['inp'].T @ dvec

@@ -103,6 +103,161 @@ def oracle_multi_step(m, Hs, inputs):
     return costs
 
 
+# ---------------- product-level comparison with a float64 oracle ----------------
+# The tensor-core kernels compute every fp32 product as 3xTF32 (~2^-21 relative per product); a product that lost one of its
+# cross terms is 2xTF32 / 1xTF32 (~2^-11).  The bar sits between the two: per tensor max |dev - ref| <= F64_REL * max |ref|, and
+# |dev - ref| <= F64_RTOL * |ref| on every element above 1 % of max |ref|.  The gradient chain (dL/dh sums 2048 score columns whose
+# loss gradients cancel) needs more room than one product: a float32 run of the oracle itself is up to 9.1e-6 / 2.3e-4 away from
+# float64 on the cases of TC_CASES, so the bar is 4x that.  The device and a 2xTF32 product, measured against it: see
+# tests/test_gpu_tcstep.py::test_tc_step_products_match_float64.
+F64_REL = 4e-5
+F64_RTOL = 1e-3
+
+
+def f64_errors(dev, ref, extra_atol=0.0):
+    """(max |dev - ref| / max |ref|, max relative error over the elements above 1 % of max |ref|); `extra_atol` (scalar or per
+    element) is an allowance subtracted from |dev - ref| first."""
+    dev = np.asarray(dev, np.float64)
+    ref = np.asarray(ref, np.float64).reshape(dev.shape)
+    scale = max(float(np.abs(ref).max()) if ref.size else 0.0, 1e-30)
+    err = np.maximum(np.abs(dev - ref) - extra_atol, 0.0)
+    big = np.abs(ref) > 0.01 * scale
+    rel = float((err[big] / np.abs(ref[big])).max()) if big.any() else 0.0
+    return float(err.max()) / scale if err.size else 0.0, rel
+
+
+def assert_f64_close(dev, ref, what, extra_atol=0.0):
+    a, r = f64_errors(dev, ref, extra_atol)
+    assert a <= F64_REL and r <= F64_RTOL, '%s: max err / max |ref| = %.3g (bar %g), max relative err above 1%% of max = %.3g (bar %g)' % (
+        what, a, F64_REL, r, F64_RTOL)
+
+
+def oracle_f64(eng, mk, n_items, step_count, P0=None):
+    """A float64 oracle holding the device's current float32 weights, hidden state and optimizer state, at dropout step
+    `step_count`: the reference for one step of the device, free of the float32 rounding of a second implementation."""
+    m = orc.OracleGRU4Rec(dtype=np.float64, **mk)
+    m.init(n_items)
+    for name in param_names(m):
+        p = oracle_param(m, name)
+        p[...] = eng.get(name).reshape(p.shape)
+        if m.adapt:
+            m.opt[(name, 'acc')] = eng.get(name + '.acc').reshape(p.shape).astype(np.float64)
+        if m.momentum > 0:
+            m.opt[(name, 'vel')] = eng.get(name + '.vel').reshape(p.shape).astype(np.float64)
+    for i in range(len(m.layers)):
+        m.H[i][...] = eng.get('H%d' % i)
+    m.step_count = step_count
+    m.P0 = None if P0 is None else np.asarray(P0, np.float64)
+    return m
+
+
+def _tc_mk(L, B, S, loss, fact, **kw):
+    mk = dict(layers=[L], batch_size=B, n_sample=S, loss=loss, final_act=fact, constrained_embedding=True, adapt=None, learning_rate=0.5,
+              momentum=0.0, sample_alpha=0.5)
+    mk.update(kw)
+    return mk
+
+
+# shapes of the tensor-core training step and the edge each one covers: name -> (model keywords, n_items, step_mode)
+TC_CASES = {
+    # K padding of every operand
+    'L16_B8_xe_logq': (_tc_mk(16, 8, 32, 'cross-entropy', 'softmax', logq=1.0), 300, 4),
+    # Lk2 = 96 for 72 live values, Bk = 64, N = 93 (not a multiple of 4)
+    'L36_B33_bpr': (_tc_mk(36, 33, 60, 'bpr', 'linear'), 500, 4),
+    # the automatic switch (L >= 160); 2L = 320: the second N tile of the gates is 1/4 live
+    'L160_B64_bprmax': (_tc_mk(160, 64, 2048, 'bpr-max', 'elu-0.5', bpreg=1.95), 4000, 2),
+    # Lp = L, 3L = 768 = six full row tiles; both dropouts
+    'L256_B128_top1max_drop': (_tc_mk(256, 128, 1024, 'top1-max', 'tanh', dropout_p_hidden=0.2, dropout_p_embed=0.3), 4000, 2),
+    # Lp = 512: G8a column tiles with 4 live columns; two lane tiles; relu hidden activation
+    'L260_B129_top1_relu': (_tc_mk(260, 129, 2048, 'top1', 'tanh', hidden_act='relu'), 4000, 2),
+    # G7 K = 33 chunks on the 16-CTA cluster: five empty K splits
+    'L344_B48_xe_logq': (_tc_mk(344, 48, 2048, 'cross-entropy', 'softmax', logq=1.0), 4000, 2),
+    # the largest batch and the largest shipped L
+    'L512_B256_xelogit': (_tc_mk(512, 256, 2048, 'xe_logit', 'softmax_logit'), 4000, 2),
+    # the optimizer epilogues: Adagrad + momentum + L2
+    'L224_B80_bprmax_adagrad': (_tc_mk(224, 80, 2048, 'bpr-max', 'elu-0.5', adapt='adagrad', momentum=0.4, lmbd=1e-3, learning_rate=0.05,
+                                       bpreg=1.95), 4000, 2),
+}
+
+
+def tc_step_inputs(n_items, B, S, seed):
+    """Sample store and (X, Y, R) of two steps: step 1 with M = B lanes; step 2 with M < B, a reset lane, a duplicated input item,
+    a target that is also one of the samples, and half of the sample row drawn from 8 items (heavy duplicates)."""
+    rs = np.random.RandomState(seed)
+    store = rs.randint(0, n_items, size=(4, S)).astype(np.int64)
+    store[1, :S // 2] = rs.randint(0, 8, size=S // 2)
+    X1, Y1 = rs.randint(0, n_items, B), rs.randint(0, n_items, B)
+    M2 = B - max(1, B // 5)
+    X2, Y2 = rs.randint(0, n_items, M2), rs.randint(0, n_items, M2)
+    X2[-1] = X2[0]
+    Y2[1] = store[1, 3]
+    R2 = np.zeros(M2, bool)
+    R2[M2 // 2] = True
+    return store, [(X1, Y1, np.zeros(B, bool)), (X2, Y2, R2)]
+
+
+def tc_setup(mk, n_items, step_mode, seed=0, torch_alloc=True):
+    """Engine with random weights, a random hidden state, biases, logQ support and the sample store of tc_step_inputs."""
+    rs = np.random.RandomState(seed)
+    m = orc.OracleGRU4Rec(**mk)
+    m.init(n_items)
+    m.H[0][:] = rs.randn(*m.H[0].shape).astype(np.float32) * 0.5
+    m.By[:] = rs.randn(*m.By.shape).astype(np.float32) * 0.1
+    m.Bh[0][:] = rs.randn(*m.Bh[0].shape).astype(np.float32) * 0.1
+    store, steps = tc_step_inputs(n_items, mk['batch_size'], mk['n_sample'], seed + 1)
+    eng = _lib.Engine(make_cfg(n_items, mk, sample_store=store.size, step_mode=step_mode), use_torch_allocator=torch_alloc)
+    push_weights(eng, m)
+    eng.set_sample_store(store)
+    P0 = None
+    if mk.get('logq', 0):
+        P0 = rs.randint(1, 50, size=n_items).astype(np.float32)
+        eng.set_logq_support(P0)
+    return eng, store, steps, P0
+
+
+def tc_run_steps(eng, mk, n_items, store, steps, P0):
+    """Runs `steps` through Engine.train_step; before each step a float64 oracle is re-seeded from the device state (errors do not
+    compound), after it every product output the device keeps is paired with the oracle's.  With plain SGD the gradients are
+    recovered from the updates, W0 - W1 = lr * g; otherwise the updated weights and optimizer state are compared.
+    Returns ([(what, dev, ref, extra_atol)], {output name: device array}) -- the second for bitwise comparisons."""
+    lr = mk['learning_rate']
+    sgd = mk.get('adapt', 'adagrad') is None and not mk.get('momentum', 0) and not mk.get('lmbd', 0)
+    checks, outs = [], {}
+    for k, (X, Y, R) in enumerate(steps):
+        m = oracle_f64(eng, mk, n_items, k, P0)
+        names = param_names(m)
+        W0 = {n: eng.get(n).astype(np.float64) for n in names}
+        cost = eng.train_step(X, Y, R)
+        ref_cost = m.train_step(X, Y, R, samples=store[k])
+        C, G = m.last_cache, m.last_grads
+        M, N = len(X), len(C['Y'])
+        order = np.lexsort((np.arange(N), C['Y']))          # DSY rows: score columns sorted by (item, position) (k_plan)
+        dev = dict(cost=np.float64(cost), y0=eng.get('y0')[:M], H0=eng.get('H0')[:M], dvec0=eng.get('dvec0')[:M], dSx=eng.get('dSx')[:M],
+                   DSY=eng.get('DSY')[:N])
+        ref = dict(cost=ref_cost, y0=C['y_last'], H0=C['H_new'][0], dvec0=G['dvec'][0], dSx=G['dSx'], DSY=G['dSy'][order])
+        W1 = {n: eng.get(n).astype(np.float64) for n in names}
+        tag = 'step %d (M=%d) ' % (k + 1, M)
+        checks += [(tag + n, dev[n], ref[n], 0.0) for n in dev]
+        outs.update({'%d_%s' % (k, n): v for n, v in dev.items()})
+        outs.update({'%d_%s' % (k, n): v for n, v in W1.items()})
+        if sgd:
+            ulp = lambda n: 2.0 ** -23 * (np.abs(W0[n]) + np.abs(W1[n])) / lr      # rounding of one fp32 update
+            for n, g in (('Wx0', G['dWx'][0]), ('Wh0', G['dWh'][0]), ('Wrz0', G['dWrz'][0]), ('Bh0', G['dBh'][0])):
+                checks.append((tag + 'd' + n + ' recovered', (W0[n] - W1[n]) / lr, g, ulp(n)))
+            # sparse rows: one fp32 update per duplicate; rows nobody scored or fed in stay bit-identical
+            for n, idx, g in (('Wy', C['Xc'], np.vstack([G['dSx'], G['dSy']])), ('By', C['Y'], G['dSBy'])):
+                cnt = np.bincount(idx, minlength=n_items)
+                gref = np.zeros(W0[n].shape)
+                np.add.at(gref, idx, g)
+                assert np.array_equal(W0[n][cnt == 0], W1[n][cnt == 0]), tag + n + ': an untouched row changed'
+                rows = cnt > 0
+                checks.append((tag + 'd' + n + ' rows recovered', ((W0[n] - W1[n]) / lr)[rows], gref[rows], cnt[rows, None] * ulp(n)[rows]))
+        else:
+            checks += [(tag + n + ' updated', W1[n], oracle_param(m, n), 0.0) for n in names]
+            checks += [(tag + '%s.%s' % key, eng.get('%s.%s' % key), val, 0.0) for key, val in m.opt.items()]
+    return checks, outs
+
+
 def assert_step_costs(costs, ref, err_msg=''):
     """Per-mini-batch costs of a whole trajectory at the north-star tolerance (1e-4 relative, every step).  fp32 rounding alone
     stays two orders of magnitude below it (tests/test_oracle_grads.py::test_fp32_trajectory_noise_level)."""

@@ -89,7 +89,7 @@ CASES = {
 }
 
 
-@pytest.mark.parametrize('step_mode', [0, 1, 2, 3])
+@pytest.mark.parametrize('step_mode', [0, 1, 2, 3, 4])
 @pytest.mark.parametrize('name', sorted(CASES))
 def test_train_steps_match_oracle(name, step_mode):
     mk = CASES[name]
@@ -97,6 +97,8 @@ def test_train_steps_match_oracle(name, step_mode):
     B = mk['batch_size']
     rows = 12
     eng, m, store, rs = make_pair(n_items, mk, n_store_rows=rows if mk['n_sample'] else 0, seed=11, step_mode=step_mode)
+    if step_mode == 4 and not eng.uses_tensor_cores():
+        pytest.skip('the tensor-core step takes constrained embedding, one layer, L % 4 == 0, SGD / Adagrad')
     costs_d, costs_o = [], []
     for t in range(rows - 1 if mk['n_sample'] else 10):
         X = rs.randint(0, n_items, B); Y = rs.randint(0, n_items, B)

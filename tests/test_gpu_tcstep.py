@@ -1,13 +1,18 @@
 """-m gpu: the tensor-core training step (wgmma 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh) against the oracle:
 constrained embedding, one layer -- the family of the reference's shipped parameter files (paramfiles/*_best.py)."""
+import os
+import subprocess
+import sys
 import numpy as np
 import pytest
 import gru4rec_oracle as orc
 from gru4rec_b200 import _lib
 from gru4rec_b200.synth import make_sessions, make_session_arrays
-from gpu_utils import make_cfg, push_weights, compare_weights, assert_step_costs
+from gpu_utils import (make_cfg, push_weights, compare_weights, assert_step_costs, TC_CASES, tc_setup, tc_run_steps, f64_errors, F64_REL,
+                       F64_RTOL)
 
 pytestmark = pytest.mark.gpu
+HERE = os.path.dirname(os.path.abspath(__file__))
 
 SMALL = [
     dict(layers=[16], batch_size=8, n_sample=32, loss='cross-entropy', final_act='softmax', constrained_embedding=True, learning_rate=0.1, momentum=0.2, logq=1.0, sample_alpha=0.5),
@@ -84,3 +89,69 @@ def test_tensor_core_step_shipped_shapes(L, B, loss, fact, extra):
     np.testing.assert_allclose(costs, ref, rtol=1e-4, atol=1e-6)
     compare_weights(eng, m, rtol=2e-3, atol=2e-5, what='tensor-core step, shipped shape')
     eng.close()
+
+
+def _f64_failures(checks):
+    out = []
+    for what, dev, ref, extra in checks:
+        a, r = f64_errors(dev, ref, extra)
+        if a > F64_REL or r > F64_RTOL:
+            out.append('%s: %.3g / %.3g' % (what, a, r))
+    return out
+
+
+@pytest.mark.parametrize('name', sorted(TC_CASES))
+def test_tc_step_products_match_float64(name):
+    """Every product of the tensor-core step against a float64 oracle run on the same float32 inputs, two steps (M = B, then M < B
+    with a reset lane and duplicates; the oracle is re-seeded from the device in between): y, H, dvec = [da_h | da_r | da_z], dSx,
+    the dSy rows, the cost, and -- plain SGD -- dWx, dWh, dWrz, dBh and the Wy / By row gradients recovered from the updates; the
+    Adagrad case compares the updated weights and optimizer state.  Failures are listed as
+    'max err / max |ref|  /  max relative err above 1 % of max' against the bar of gpu_utils.F64_REL / F64_RTOL (4e-5 / 1e-3).
+    Measured on an H100 80GB HBM3 (400 W power limit), worst tensor over all cases: the device 4.8e-6 / 7.6e-5; a float32 run of
+    the oracle 9.1e-6 / 2.3e-4; the device with the a_lo * b_hi term of every product dropped (2xTF32) at least 2.9e-4 / 1.5e-2 in
+    every case, up to 0.23 / 2.5."""
+    mk, n_items, step_mode = TC_CASES[name]
+    eng, store, steps, P0 = tc_setup(mk, n_items, step_mode)
+    assert eng.uses_tensor_cores()
+    checks, _ = tc_run_steps(eng, mk, n_items, store, steps, P0)
+    failed = _f64_failures(checks)
+    assert not failed, '\n'.join(failed)
+    eng.close()
+
+
+def test_tc_step_bitwise_repeatable():
+    """Two engines alive in one process, same inputs: the K splits are summed in a fixed order, so every output is bit for bit
+    the same."""
+    mk, n_items, step_mode = TC_CASES['L344_B48_xe_logq']
+    runs = [tc_setup(mk, n_items, step_mode) for _ in range(2)]
+    outs = [tc_run_steps(eng, mk, n_items, store, steps, P0)[1] for eng, store, steps, P0 in runs]
+    for k in outs[0]:
+        assert np.array_equal(outs[0][k], outs[1][k]), k
+    for r in runs:
+        r[0].close()
+
+
+# (G4R_TS_CLUSTER, G4R_TS_CLUSTER_BIG, G4R_TS_PDL); the first is the default
+LAUNCH_CONFIGS = [(8, 16, 1), (8, 16, 0), (8, 8, 1), (1, 16, 1), (2, 8, 1), (4, 16, 1)]
+
+
+def test_tc_step_launch_configurations(tmp_path):
+    """The cluster cap of the K splits, the cluster size of the long-K products and programmatic dependent launch change how the
+    products are split and overlapped, not what they compute.  They are read once per process, so every configuration runs the
+    L = 344 and L = 512 cases in a worker process (tests/tc_config_worker.py): each passes the float64 comparison, and PDL on / off
+    are bitwise identical."""
+    res = {}
+    for cfg in LAUNCH_CONFIGS:
+        out = str(tmp_path / ('cfg_%d_%d_%d.npz' % cfg))
+        env = dict(os.environ, G4R_TS_CLUSTER=str(cfg[0]), G4R_TS_CLUSTER_BIG=str(cfg[1]), G4R_TS_PDL=str(cfg[2]))
+        p = subprocess.run([sys.executable, os.path.join(HERE, 'tc_config_worker.py'), out, 'L344_B48_xe_logq', 'L512_B256_xelogit'],
+                           env=env, capture_output=True, text=True, timeout=900)
+        assert p.returncode == 0, '%s: worker failed\n%s' % (cfg, p.stderr[-4000:])
+        with np.load(out) as z:
+            res[cfg] = {k: z[k] for k in z.files}
+        failed = [str(v) for k, v in res[cfg].items() if k.endswith(':failures') and str(v)]
+        assert not failed, '%s:\n%s' % (cfg, '\n'.join(failed))
+    a, b = res[(8, 16, 1)], res[(8, 16, 0)]
+    assert a.keys() == b.keys()
+    for k in a:
+        assert np.array_equal(a[k], b[k]), 'PDL on / off differ: ' + k
