@@ -7,6 +7,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libg4r.so')
 G4R_MAX_LAYERS = 8
+G4R_TOPK_MAX = 1024
 
 G4R_OK, G4R_ERR_INVALID, G4R_ERR_INDEX, G4R_ERR_CUDA, G4R_ERR_NAN, G4R_ERR_STATE = 0, -1, -2, -3, -4, -5
 LOSS = {'cross-entropy': 0, 'bpr-max': 1, 'top1-max': 2, 'bpr': 3, 'top1': 4, 'xe_logit': 5}
@@ -42,6 +43,7 @@ EXPORTS = [
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
     'g4r_eval_schedule', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
+    'g4r_predict_topk',
 ]
 
 _lib = None
@@ -109,6 +111,7 @@ def load():
     lib.g4r_set_eval_items.argtypes = [vp, vp, i64]
     lib.g4r_predict.argtypes = [vp, vp, i32, vp, vp]
     lib.g4r_reset_eval_hidden.argtypes = [vp]
+    lib.g4r_predict_topk.argtypes = [vp, vp, i32, vp, i32, vp, vp]
     _lib = lib
     return lib
 
@@ -135,6 +138,13 @@ def parse_act(name):
         p = [float(x) for x in name.split('-')[1:]]
         return ACT['selu'], p[0], p[1]
     raise NotImplementedError
+
+
+def check_topk(k, n_items):
+    """k of a top-k request: 1 <= k <= min(n_items, G4R_TOPK_MAX), else ValueError"""
+    if not isinstance(k, (int, np.integer)) or isinstance(k, bool) or not 1 <= k <= min(n_items, G4R_TOPK_MAX):
+        raise ValueError('k must be an integer in 1 .. min(n_items, %d) = %d, got %r' % (G4R_TOPK_MAX, min(n_items, G4R_TOPK_MAX), k))
+    return int(k)
 
 
 def set_adapt_params(cfg, adapt, adapt_params, grad_cap):
@@ -490,6 +500,18 @@ class Engine(object):
         out = np.empty((len(X), self.cfg.n_items), dtype=np.float32)
         self._check(self.lib.g4r_predict(self.h, _ptr(X), len(X), _ptr(rm), _ptr(out)))
         return out
+
+    def predict_topk(self, X, k, reset_mask=None):
+        """predict() reduced on the device to the k best items of every lane: (items int32 [batch, k], scores float32 [batch, k]),
+        best first.  Order: the activated score (the pre-activation score for softmax), then the smaller item index; the scores
+        are predict()'s values.  Advances the hidden state exactly as predict() does."""
+        k = check_topk(k, self.cfg.n_items)
+        X = np.ascontiguousarray(X, dtype=np.int32)
+        rm = None if reset_mask is None else np.ascontiguousarray(reset_mask, dtype=np.uint8)
+        items = np.empty((len(X), k), dtype=np.int32)
+        scores = np.empty((len(X), k), dtype=np.float32)
+        self._check(self.lib.g4r_predict_topk(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(items), _ptr(scores)))
+        return items, scores
 
     def reset_eval_hidden(self):
         self._check(self.lib.g4r_reset_eval_hidden(self.h))

@@ -205,11 +205,14 @@ struct EvalCtx {
   int slot = -1;
   int* dCand = nullptr; int n_cand = 0; size_t cand_cap = 0;     // candidate subset of evaluate_gpu(items=...), item indices
   unsigned char *dAsplit = nullptr, *dBsplit = nullptr;           // tensor-core path: hi / lo TF32 operand blocks (g4r_eval_tc.cuh)
+  void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
 };
+static void topk_release(EvalCtx& e);
 
 static void eval_release(g4r_handle* h) {
   if (!h->eval_ctx) return;
   EvalCtx& e = *static_cast<EvalCtx*>(h->eval_ctx);
+  topk_release(e);
   cudaFreeHost(e.hX); cudaFreeHost(e.hY); cudaFreeHost(e.hSlot); cudaFreeHost(e.hF); cudaFreeHost(e.hM); cudaFreeHost(e.hSti); cudaFreeHost(e.hG);
   cudaFree(e.dX); cudaFree(e.dY); cudaFree(e.dSlot); cudaFree(e.dF); cudaFree(e.dM); cudaFree(e.dSti); cudaFree(e.dG);
   cudaFree(e.dCut); cudaFree(e.dSums); if (e.dOut) cudaFree(e.dOut); if (e.dCand) cudaFree(e.dCand);
@@ -378,12 +381,9 @@ extern "C" int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n
   return G4R_OK;
 }
 
-extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, float* out) {
-  if (!h || !X || !out) return G4R_ERR_INVALID;
-  cudaSetDevice(h->cfg.device);
-  EvalCtx* e = nullptr;
-  int rc = eval_ctx(h, &e);
-  if (rc) return rc;
+// the single mini-batch of a predict call (lanes 0 .. batch-1, reset_mask zeroes lanes first) staged on the scoring path; nothing
+// reaches the device unless every input index is valid
+static int predict_stage(g4r_handle* h, EvalCtx* e, const int32_t* X, int32_t batch, const uint8_t* reset_mask) {
   const int Be = e->Be, I = h->md.n_items;
   if (batch <= 0 || batch > Be) FAIL(G4R_ERR_INVALID, "predict batch exceeds eval_batch_size");
   cudaStream_t st = h->stream;
@@ -400,6 +400,19 @@ extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const
   CK(cudaMemcpyAsync(e->dM, e->hM, sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(e->dSti, e->hSti, sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(e->dG, e->hG, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  return G4R_OK;
+}
+
+extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, float* out) {
+  if (!h || !X || !out) return G4R_ERR_INVALID;
+  cudaSetDevice(h->cfg.device);
+  EvalCtx* e = nullptr;
+  int rc = eval_ctx(h, &e);
+  if (rc) return rc;
+  rc = predict_stage(h, e, X, batch, reset_mask);
+  if (rc) return rc;
+  const int I = h->md.n_items;
+  cudaStream_t st = h->stream;
   const size_t need = (size_t)batch * I;
   if (e->out_cap < need) { if (e->dOut) cudaFree(e->dOut); CK(cudaMalloc(&e->dOut, need * sizeof(float))); e->out_cap = need; }
   eval_forward(h, e, 0);
@@ -420,3 +433,5 @@ extern "C" int g4r_reset_eval_hidden(g4r_handle* h) {
   for (int i = 0; i < h->md.n_layers; i++) CK(cudaMemsetAsync(h->He[i], 0, (size_t)Be * h->md.layer[i].ldL * sizeof(float), h->stream));
   return G4R_OK;
 }
+
+#include "g4r_topk.cuh"

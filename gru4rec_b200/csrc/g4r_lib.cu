@@ -74,6 +74,7 @@ struct g4r_handle {
   GridBar* dGridBar = nullptr; unsigned long long* dStamp = nullptr; int pk_blocks = 0; size_t pk_smem = 0;
   bool mg_alloc = false; MgDev mgdev; std::vector<MgTensor> mg_tensors;
   void* eval_ctx = nullptr;      // EvalCtx* (g4r_eval.cuh), owned by the handle
+  uint64_t wy_version = 0;       // bumped by everything that may change Wy / By (caches derived from them compare it)
   void* mg_host = nullptr;       // MgHost*  (g4r_multi.cuh), owned by the handle
   void* shard = nullptr;         // ShardHost* (g4r_shard.cuh): row-sharded item tables + in-kernel exchange, owned by the handle
   char* shard_ws = nullptr;      // workspace carve-outs of the sharded path (plans, device descriptor, counters, gathered input rows)
@@ -831,6 +832,7 @@ extern "C" int g4r_set_tensor(g4r_handle* h, const char* name, const float* host
   if (!t) FAIL(G4R_ERR_INVALID, std::string("unknown tensor ") + (name ? name : "(null)"));
   if (rows != t->rows || cols != t->cols) FAIL(G4R_ERR_INVALID, std::string("shape mismatch for ") + name);
   cudaSetDevice(h->cfg.device);
+  if (t->ptr == h->md.Wy || t->ptr == h->md.By) h->wy_version++;
   if (t->sharded) return shard_set_tensor(h, *t, host);
   CK(cudaMemcpy2DAsync(t->ptr, t->ld * sizeof(float), host, cols * sizeof(float), cols * sizeof(float), rows, cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -1276,6 +1278,7 @@ extern "C" int g4r_run_uploaded(g4r_handle* h, float* cost_out, float* device_ms
   if (!h) return G4R_ERR_INVALID;
   if (h->win_steps <= 0) FAIL(G4R_ERR_STATE, "no uploaded window");
   cudaSetDevice(h->cfg.device);
+  h->wy_version++;
   const int n = h->win_steps;
   if (h->cfg.world_size > 1 && !mg_is_ready(h)) FAIL(G4R_ERR_STATE, "multi-GPU handle: call g4r_mg_init first");
   if (h->cfg.world_size > 1 && !h->shard) FAIL(G4R_ERR_STATE, "g4r_run_uploaded on a multi-GPU handle needs the row-sharded path");
@@ -1298,6 +1301,7 @@ extern "C" int g4r_profile_uploaded(g4r_handle* h, float* phase_ms, int32_t* pha
   if (h->shard) FAIL(G4R_ERR_STATE, "per-phase profiling is a single-GPU measurement (row-sharded handle)");
   if (h->win_steps <= 0) FAIL(G4R_ERR_STATE, "no uploaded window");
   cudaSetDevice(h->cfg.device);
+  h->wy_version++;
   h->prof = true; h->prof_ev.clear(); h->prof_phase.clear();
   int rc = run_window(h, h->win_steps);
   h->prof = false;
@@ -1339,6 +1343,7 @@ extern "C" int g4r_train_steps(g4r_handle* h, const g4r_schedule* s, int64_t fir
   if (s->B != h->md.B) FAIL(G4R_ERR_INVALID, "schedule batch size != model batch size");
   if (first < 0 || n < 0 || first + n > s->n_steps) FAIL(G4R_ERR_INVALID, "step range out of schedule");
   cudaSetDevice(h->cfg.device);
+  h->wy_version++;
   if (nan_step) *nan_step = -1;
   int64_t done = 0;
   while (done < n) {
@@ -1378,6 +1383,7 @@ extern "C" int g4r_train_step(g4r_handle* h, const int32_t* X, const int32_t* Y,
   if (M <= 0 || M > B) FAIL(G4R_ERR_INVALID, "M out of range");
   if (h->shard) FAIL(G4R_ERR_STATE, "g4r_train_step: not available on a row-sharded multi-GPU handle (use g4r_train_steps)");
   cudaSetDevice(h->cfg.device);
+  h->wy_version++;
   if (h->gen_len > 0 && (!h->have_store || h->sample_ptr >= h->gen_len)) {
     int rc = g4r_generate_samples(h);
     if (rc) return rc;

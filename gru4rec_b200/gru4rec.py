@@ -508,6 +508,33 @@ class GRU4Rec:
         Returns a DataFrame, rows = items, columns = events of the batch.
         '''
         if self.error_during_train: raise Exception
+        eng, reset, in_idxs = self._next_batch_inputs(session_ids, input_item_ids, batch)
+        preds = eng.predict(in_idxs, reset.astype(np.uint8)).T          # items x batch
+        if predict_for_item_ids is not None:
+            iIdxs = self.itemidmap[predict_for_item_ids].values
+            preds = preds[iIdxs]
+            if self.final_act in ('softmax', 'softmax_logit'):
+                preds = preds / preds.sum(axis=0, keepdims=True)          # softmax over the requested subset
+            return pd.DataFrame(data=preds, index=predict_for_item_ids)
+        return pd.DataFrame(data=preds, index=self.itemidmap.index)
+
+    def recommend_next_batch(self, session_ids, input_item_ids, k=20, batch=100):
+        '''
+        The k best next items of every event of the batch, ranked on the device (an addition to the reference's surface).
+        Shares predict_next_batch's per-lane session state, so the two methods can be called alternately.
+        Returns (item_ids [batch, k] of the original item IDs, scores [batch, k] float32), best first.  Order: the score
+        (the pre-activation score for softmax / softmax_logit), then the earlier item of the catalogue; the scores are the
+        values predict_next_batch returns for those items.
+        '''
+        if self.error_during_train: raise Exception
+        k = _lib.check_topk(k, self.n_items)
+        eng, reset, in_idxs = self._next_batch_inputs(session_ids, input_item_ids, batch)
+        items, scores = eng.predict_topk(in_idxs, k, reset.astype(np.uint8))
+        return self.itemidmap.index.to_numpy()[items], scores
+
+    def _next_batch_inputs(self, session_ids, input_item_ids, batch):
+        '''session bookkeeping of predict_next_batch / recommend_next_batch: the hidden state of a lane is
+        kept while its session id stays the same and zeroed when it changes or the batch size changes'''
         eng = self._ensure_engine(batch)
         if getattr(self, 'predict', None) is None or self.predict_batch != batch:
             self.predict_batch = batch
@@ -519,14 +546,7 @@ class GRU4Rec:
         if reset.any():
             self.current_session = session_ids.copy()
         in_idxs = self.itemidmap[input_item_ids].values
-        preds = eng.predict(in_idxs, reset.astype(np.uint8)).T          # items x batch
-        if predict_for_item_ids is not None:
-            iIdxs = self.itemidmap[predict_for_item_ids].values
-            preds = preds[iIdxs]
-            if self.final_act in ('softmax', 'softmax_logit'):
-                preds = preds / preds.sum(axis=0, keepdims=True)          # softmax over the requested subset
-            return pd.DataFrame(data=preds, index=predict_for_item_ids)
-        return pd.DataFrame(data=preds, index=self.itemidmap.index)
+        return eng, reset, in_idxs
 
     # ---- persistence (gru4rec.py:742-781): pickle of the object with NumPy parameters ----
     def __getstate__(self):

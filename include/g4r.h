@@ -207,6 +207,12 @@ int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n);
 /* predict_next_batch's device call: scores of all items for `batch` lanes; reset_mask zeroes lanes first
  * (gru4rec.py:712-717).  out: [batch x n_items] row-major. */
 int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, float* out);
+#define G4R_TOPK_MAX 1024
+/* predict_next_batch's device call, reduced on the device to the k best items of every lane (ranking key and ties: DESIGN §3d).
+ * Advances the scoring-path hidden state like g4r_predict.  out_items / out_scores: [batch x k] row-major, best first.
+ * G4R_ERR_INVALID unless 1 <= k <= min(n_items, G4R_TOPK_MAX); G4R_ERR_INDEX on an out-of-range item. */
+int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
+                     int32_t* out_items, float* out_scores);
 /* Zero the scoring-path hidden state (gru4rec.py:696-697). */
 int g4r_reset_eval_hidden(g4r_handle* h);
 
