@@ -766,10 +766,12 @@ class OracleGRU4Rec:
             sparse.append(('Wx0', self.Wx[0], X, G['dSx'], C['Sx']))
             sparse.append(('Wy', self.Wy, Y, G['dSy'], C['Sy']))
         sparse.append(('By', self.By, Y, G['dSBy'], self.By[Y]))
+        self.last_gscale = dt(1.0)        # the factor grad_cap applied to every gradient of this step
         if self.grad_cap > 0:  # gru4rec.py:386-389
             norm = dt(np.sqrt(sum(np.sum(g * g) for _, _, g in dense) + sum(np.sum(g * g) for _, _, _, g, _ in sparse)))
             if norm >= self.grad_cap:
                 sc = dt(self.grad_cap) / norm
+                self.last_gscale = sc
                 dense = [(n, p, g * sc) for n, p, g in dense]
                 sparse = [(n, p, ix, g * sc, sp) for n, p, ix, g, sp in sparse]
         # all right-hand sides use the OLD parameter values (Theano evaluates updates simultaneously)

@@ -116,9 +116,11 @@ F64_RTOL = 1e-3
 
 def f64_errors(dev, ref, extra_atol=0.0):
     """(max |dev - ref| / max |ref|, max relative error over the elements above 1 % of max |ref|); `extra_atol` (scalar or per
-    element) is an allowance subtracted from |dev - ref| first."""
+    element) is an allowance subtracted from |dev - ref| first.  A non-finite element on either side gives (inf, inf)."""
     dev = np.asarray(dev, np.float64)
     ref = np.asarray(ref, np.float64).reshape(dev.shape)
+    if not (np.isfinite(dev).all() and np.isfinite(ref).all()):
+        return np.inf, np.inf
     scale = max(float(np.abs(ref).max()) if ref.size else 0.0, 1e-30)
     err = np.maximum(np.abs(dev - ref) - extra_atol, 0.0)
     big = np.abs(ref) > 0.01 * scale
@@ -132,6 +134,14 @@ def assert_f64_close(dev, ref, what, extra_atol=0.0):
         what, a, F64_REL, r, F64_RTOL)
 
 
+OPT_SLOTS = {None: (), 'adagrad': ('acc',), 'rmsprop': ('acc',), 'adadelta': ('acc', 'upd'), 'adam': ('acc', 'meang', 'countt')}
+
+
+def opt_slots(m):
+    """optimizer state tensors of every parameter, as g4r_lib.cu layout() registers them ('<param>.<slot>')"""
+    return OPT_SLOTS[m.adapt] + (('vel',) if m.momentum > 0 else ())
+
+
 def oracle_f64(eng, mk, n_items, step_count, P0=None):
     """A float64 oracle holding the device's current float32 weights, hidden state and optimizer state, at dropout step
     `step_count`: the reference for one step of the device, free of the float32 rounding of a second implementation."""
@@ -140,15 +150,29 @@ def oracle_f64(eng, mk, n_items, step_count, P0=None):
     for name in param_names(m):
         p = oracle_param(m, name)
         p[...] = eng.get(name).reshape(p.shape)
-        if m.adapt:
-            m.opt[(name, 'acc')] = eng.get(name + '.acc').reshape(p.shape).astype(np.float64)
-        if m.momentum > 0:
-            m.opt[(name, 'vel')] = eng.get(name + '.vel').reshape(p.shape).astype(np.float64)
+        for slot in opt_slots(m):
+            m.opt[(name, slot)] = eng.get('%s.%s' % (name, slot)).reshape(p.shape).astype(np.float64)
     for i in range(len(m.layers)):
         m.H[i][...] = eng.get('H%d' % i)
     m.step_count = step_count
     m.P0 = None if P0 is None else np.asarray(P0, np.float64)
     return m
+
+
+def random_opt_state(eng, m, rs):
+    """Optimizer state in the range of a trained model: acc and upd positive, meang of both signs, countt small integers that
+    differ per element (so does adam's bias correction), vel of both signs.  From zero state the first Adagrad / rmsprop / adam
+    update is about +-lr whatever the size of the gradient; from this state it depends on the size."""
+    for name in param_names(m):
+        shape = eng.shape(name)
+        for slot in opt_slots(m):
+            if slot in ('acc', 'upd'):
+                v = 10.0 ** rs.uniform(-4.0, -2.0, shape)
+            elif slot == 'countt':
+                v = rs.randint(1, 30, shape)
+            else:
+                v = rs.randn(*shape) * 1e-3
+            eng.set('%s.%s' % (name, slot), v.astype(np.float32))
 
 
 def _tc_mk(L, B, S, loss, fact, **kw):
@@ -180,31 +204,45 @@ TC_CASES = {
 }
 
 
-def tc_step_inputs(n_items, B, S, seed):
+def f64_step_inputs(n_items, B, S, seed, per_item=None, input_in_scores=False, wide_group=0):
     """Sample store and (X, Y, R) of two steps: step 1 with M = B lanes; step 2 with M < B, a reset lane, a duplicated input item,
-    a target that is also one of the samples, and half of the sample row drawn from 8 items (heavy duplicates)."""
+    a target that is also one of the samples, and half of the sample row heavily duplicated -- drawn from 8 items, or, with
+    `per_item`, exactly `per_item` copies of each of S / 2 / per_item items (duplicate groups that fit one chunk of the
+    role-specialised kernels).  `input_in_scores`: step 2 also feeds in the target of another lane and one of its samples
+    (shared embedding: the input-row and the output-row update of one Wy row, once with a target column's large gradient).  `wide_group`: step 1's samples start with that many copies of
+    one item."""
     rs = np.random.RandomState(seed)
     store = rs.randint(0, n_items, size=(4, S)).astype(np.int64)
-    store[1, :S // 2] = rs.randint(0, 8, size=S // 2)
+    if per_item is None:
+        store[1, :S // 2] = rs.randint(0, 8, size=S // 2)
+    else:
+        store[1, :S // 2] = rs.permutation(np.arange(S // 2) // per_item)
     X1, Y1 = rs.randint(0, n_items, B), rs.randint(0, n_items, B)
     M2 = B - max(1, B // 5)
     X2, Y2 = rs.randint(0, n_items, M2), rs.randint(0, n_items, M2)
     X2[-1] = X2[0]
     Y2[1] = store[1, 3]
+    if input_in_scores:
+        X2[2], X2[3] = Y2[4], store[1, S - 5]
+    if wide_group:
+        store[0, :wide_group] = store[0, S - 1]
     R2 = np.zeros(M2, bool)
     R2[M2 // 2] = True
     return store, [(X1, Y1, np.zeros(B, bool)), (X2, Y2, R2)]
 
 
-def tc_setup(mk, n_items, step_mode, seed=0, torch_alloc=True):
-    """Engine with random weights, a random hidden state, biases, logQ support and the sample store of tc_step_inputs."""
+def f64_setup(mk, n_items, step_mode, seed=0, torch_alloc=True, **inputs):
+    """Engine with random weights, a random hidden state, biases, logQ support, random optimizer state and the sample store of
+    f64_step_inputs(**inputs)."""
     rs = np.random.RandomState(seed)
     m = orc.OracleGRU4Rec(**mk)
     m.init(n_items)
-    m.H[0][:] = rs.randn(*m.H[0].shape).astype(np.float32) * 0.5
+    for h in m.H:
+        h[:] = rs.randn(*h.shape).astype(np.float32) * 0.5
     m.By[:] = rs.randn(*m.By.shape).astype(np.float32) * 0.1
-    m.Bh[0][:] = rs.randn(*m.Bh[0].shape).astype(np.float32) * 0.1
-    store, steps = tc_step_inputs(n_items, mk['batch_size'], mk['n_sample'], seed + 1)
+    for b in m.Bh:
+        b[:] = rs.randn(*b.shape).astype(np.float32) * 0.1
+    store, steps = f64_step_inputs(n_items, mk['batch_size'], mk['n_sample'], seed + 1, **inputs)
     eng = _lib.Engine(make_cfg(n_items, mk, sample_store=store.size, step_mode=step_mode), use_torch_allocator=torch_alloc)
     push_weights(eng, m)
     eng.set_sample_store(store)
@@ -212,50 +250,155 @@ def tc_setup(mk, n_items, step_mode, seed=0, torch_alloc=True):
     if mk.get('logq', 0):
         P0 = rs.randint(1, 50, size=n_items).astype(np.float32)
         eng.set_logq_support(P0)
+    random_opt_state(eng, m, np.random.RandomState(seed + 2))
     return eng, store, steps, P0
 
 
-def tc_run_steps(eng, mk, n_items, store, steps, P0):
-    """Runs `steps` through Engine.train_step; before each step a float64 oracle is re-seeded from the device state (errors do not
-    compound), after it every product output the device keeps is paired with the oracle's.  With plain SGD the gradients are
-    recovered from the updates, W0 - W1 = lr * g; otherwise the updated weights and optimizer state are compared.
-    Returns ([(what, dev, ref, extra_atol)], {output name: device array}) -- the second for bitwise comparisons."""
+def dense_grads(m, G):
+    """(name, gradient) of the dense parameters; Wx0 is a row table without an embedding"""
+    nl = len(m.layers)
+    wx0 = 0 if (m.embedding or m.constrained_embedding) else 1
+    return ([('Wx%d' % i, G['dWx'][i]) for i in range(wx0, nl)] + [('Wh%d' % i, G['dWh'][i]) for i in range(nl)] +
+            [('Wrz%d' % i, G['dWrz'][i]) for i in range(nl)] + [('Bh%d' % i, G['dBh'][i]) for i in range(nl)])
+
+
+def sparse_grads(C, G):
+    """(name, rows, per-position gradient) of the row tables a step updates (gru4rec_oracle.apply_updates)"""
+    if C['mode'] == 'shared':
+        out = [('Wy', C['Xc'], np.vstack([G['dSx'], G['dSy']]))]
+    elif C['mode'] == 'embed':
+        out = [('E', C['X'], G['dSx']), ('Wy', C['Y'], G['dSy'])]
+    else:
+        out = [('Wx0', C['X'], G['dSx']), ('Wy', C['Y'], G['dSy'])]
+    return out + [('By', C['Y'], G['dSBy'])]
+
+
+# The kernel a training step runs, told apart by the handle's counters (kernel launches, role-specialised windows, fallback
+# windows) -- and by what it leaves in DSY, the dSy rows of the step:
+#   'tc'          the tensor-core step (uses_tensor_cores()); writes every DSY row
+#   'fast'        k_fast (step_mode 2) or its cluster variant (step_mode 3): one launch after the plan, +1 role-specialised
+#                 window; keeps dSy in shared memory and never writes DSY, so the dSy rows are checked only through the Wy rows
+#   'persistent'  k_persistent: one launch after the plan, +1 fallback window in step_modes 2 / 3
+#   'phases'      the per-phase launch sequence (step_mode 0, and every mode with grad_cap / smoothing)
+# The generic kernels keep the dSy rows of a chunk of <= 16 columns in shared memory (csrc/g4r_kernels.cuh, lossgrad) and write
+# DSY only for wider chunks -- and, with grad_cap, for every chunk (the rows wait for the global norm): DSY is filled with NaN
+# before the step; a row still all NaN was not written, every other row is compared (a partly non-finite row fails).  A chunk
+# never splits a duplicate group, so the rows of a group wider than SC_CT columns must have been written.
+STEP_PATHS = ('tc', 'fast', 'persistent', 'phases')
+SC_CT = 16          # columns of one lossgrad sub tile (csrc/g4r_kernels.cuh)
+
+
+def _counters(eng):
+    return (eng.kernel_launches(),) + tuple(eng.fast_windows())
+
+
+def _assert_path(path, before, after, step_mode, tag):
+    launches, fast, fallback = (a - b for a, b in zip(after, before))
+    if path == 'tc':
+        return
+    if path == 'fast':
+        ok = launches == 2 and fast == 1 and fallback == 0
+    elif path == 'persistent':
+        ok = launches == 2 and fast == 0 and fallback == (1 if step_mode >= 2 else 0)
+    else:
+        ok = launches > 2 and fast == 0 and fallback == 0
+    assert ok, '%sexpected the %s path; kernel launches +%d, role-specialised windows +%d, fallback windows +%d' % (
+        tag, path, launches, fast, fallback)
+
+
+def f64_run_steps(eng, mk, n_items, store, steps, P0, path):
+    """Runs `steps` through Engine.train_step on the kernel `path` (one of STEP_PATHS, or one per step; None: no counters are
+    checked); before each step a float64 oracle is re-seeded from the device state (errors do not compound), after it every
+    product the path keeps is paired with the oracle's: the cost, y, H and dvec = [da_h | da_r | da_z] of every layer, dSx
+    (embedding modes) and the DSY rows the path wrote.  Plain SGD: every gradient is recovered from the update, W0 - W1 =
+    lr * g (* the grad_cap scale): the dense ones, and the rows of Wx0 / E / Wy / By (one fp32 rounding per duplicate).  Any
+    other optimizer: the updates W1 - W0 of every weight and every state tensor against the oracle's, with one fp32 rounding
+    of the result per applied update.  Rows of the row tables that no position touched stay bit-identical (weights and state).
+    Returns ([(what, dev, ref, extra_atol)], {output name: device array} for bitwise comparisons, [grad_cap scale per step])."""
+    paths = [path] * len(steps) if path is None or isinstance(path, str) else list(path)
+    assert eng.uses_tensor_cores() == (paths[0] == 'tc')
     lr = mk['learning_rate']
     sgd = mk.get('adapt', 'adagrad') is None and not mk.get('momentum', 0) and not mk.get('lmbd', 0)
-    checks, outs = [], {}
+    ulp = lambda a, b: 2.0 ** -23 * (np.abs(a) + np.abs(b))        # rounding of one fp32 update
+    checks, outs, scales = [], {}, []
     for k, (X, Y, R) in enumerate(steps):
         m = oracle_f64(eng, mk, n_items, k, P0)
-        names = param_names(m)
+        names, slots = param_names(m), opt_slots(m)
+        nl = len(m.layers)
         W0 = {n: eng.get(n).astype(np.float64) for n in names}
+        S0 = {(n, s): eng.get('%s.%s' % (n, s)).astype(np.float64) for n in names for s in slots}
+        dsy_all = paths[k] == 'tc' or (paths[k] == 'phases' and m.grad_cap > 0)
+        if paths[k] != 'fast' and not dsy_all:
+            eng.set('DSY', np.full(eng.shape('DSY'), np.nan, np.float32))
+        tag = 'step %d (M=%d) ' % (k + 1, len(X))
+        c0 = _counters(eng)
         cost = eng.train_step(X, Y, R)
+        if paths[k] is not None:
+            _assert_path(paths[k], c0, _counters(eng), eng.cfg.step_mode, tag)
         ref_cost = m.train_step(X, Y, R, samples=store[k])
         C, G = m.last_cache, m.last_grads
         M, N = len(X), len(C['Y'])
-        order = np.lexsort((np.arange(N), C['Y']))          # DSY rows: score columns sorted by (item, position) (k_plan)
-        dev = dict(cost=np.float64(cost), y0=eng.get('y0')[:M], H0=eng.get('H0')[:M], dvec0=eng.get('dvec0')[:M], dSx=eng.get('dSx')[:M],
-                   DSY=eng.get('DSY')[:N])
-        ref = dict(cost=ref_cost, y0=C['y_last'], H0=C['H_new'][0], dvec0=G['dvec'][0], dSx=G['dSx'], DSY=G['dSy'][order])
+        ys = [lc['inp'] for lc in C['layers'][1:]] + [C['y_last']]
+        dev, ref = dict(cost=np.float64(cost)), dict(cost=ref_cost)
+        for i in range(nl):
+            for n, r in (('y', ys[i]), ('H', C['H_new'][i]), ('dvec', G['dvec'][i])):
+                dev['%s%d' % (n, i)], ref['%s%d' % (n, i)] = eng.get('%s%d' % (n, i))[:M], r
+        if C['mode'] != 'none':
+            dev['dSx'], ref['dSx'] = eng.get('dSx')[:M], G['dSx']
+        if paths[k] != 'fast':
+            order = np.lexsort((np.arange(N), C['Y']))      # DSY rows: score columns sorted by (item, position) (k_plan)
+            dsy = eng.get('DSY')[:N]
+            wrote = ~np.isnan(dsy).all(axis=1)
+            wide = np.bincount(C['Y'])[C['Y'][order]] > SC_CT
+            assert wrote.all() or not dsy_all, tag + 'DSY: %d of %d rows not written' % ((~wrote).sum(), N)
+            assert wrote[wide].all(), tag + 'DSY: %d rows of duplicate groups wider than a sub tile not written' % (~wrote[wide]).sum()
+            # step 2 has heavy duplicates: some chunk is wider than a sub tile
+            assert wrote.any() or k == 0, tag + 'DSY: no row written'
+            if wrote.any():
+                dev['DSY'], ref['DSY'] = dsy[wrote], G['dSy'][order][wrote]
         W1 = {n: eng.get(n).astype(np.float64) for n in names}
-        tag = 'step %d (M=%d) ' % (k + 1, M)
         checks += [(tag + n, dev[n], ref[n], 0.0) for n in dev]
         outs.update({'%d_%s' % (k, n): v for n, v in dev.items()})
         outs.update({'%d_%s' % (k, n): v for n, v in W1.items()})
+        sc = float(m.last_gscale)
+        scales.append(sc)
+        sparse = sparse_grads(C, G)
+        counts = {n: np.bincount(idx, minlength=W0[n].shape[0]) for n, idx, _ in sparse}
+        for n, cnt in counts.items():
+            assert np.array_equal(W0[n][cnt == 0], W1[n][cnt == 0]), tag + n + ': an untouched row changed'
         if sgd:
-            ulp = lambda n: 2.0 ** -23 * (np.abs(W0[n]) + np.abs(W1[n])) / lr      # rounding of one fp32 update
-            for n, g in (('Wx0', G['dWx'][0]), ('Wh0', G['dWh'][0]), ('Wrz0', G['dWrz'][0]), ('Bh0', G['dBh'][0])):
-                checks.append((tag + 'd' + n + ' recovered', (W0[n] - W1[n]) / lr, g, ulp(n)))
-            # sparse rows: one fp32 update per duplicate; rows nobody scored or fed in stay bit-identical
-            for n, idx, g in (('Wy', C['Xc'], np.vstack([G['dSx'], G['dSy']])), ('By', C['Y'], G['dSBy'])):
-                cnt = np.bincount(idx, minlength=n_items)
+            for n, g in dense_grads(m, G):
+                checks.append((tag + 'd' + n + ' recovered', (W0[n] - W1[n]) / lr, g * sc, ulp(W0[n], W1[n]) / lr))
+            for n, idx, g in sparse:
+                cnt, rows = counts[n], counts[n] > 0
                 gref = np.zeros(W0[n].shape)
-                np.add.at(gref, idx, g)
-                assert np.array_equal(W0[n][cnt == 0], W1[n][cnt == 0]), tag + n + ': an untouched row changed'
-                rows = cnt > 0
-                checks.append((tag + 'd' + n + ' rows recovered', ((W0[n] - W1[n]) / lr)[rows], gref[rows], cnt[rows, None] * ulp(n)[rows]))
+                np.add.at(gref, idx, g * sc)
+                checks.append((tag + 'd' + n + ' rows recovered', ((W0[n] - W1[n]) / lr)[rows], gref[rows],
+                               cnt[rows, None] * (ulp(W0[n], W1[n]) / lr)[rows]))
         else:
-            checks += [(tag + n + ' updated', W1[n], oracle_param(m, n), 0.0) for n in names]
-            checks += [(tag + '%s.%s' % key, eng.get('%s.%s' % key), val, 0.0) for key, val in m.opt.items()]
-    return checks, outs
+            for n in names:
+                rows = counts[n] > 0 if n in counts else slice(None)
+                mult = counts[n][rows, None] if n in counts else 1
+                pairs = [(n, W0[n], W1[n], oracle_param(m, n))]
+                for s in slots:
+                    S1 = eng.get('%s.%s' % (n, s)).astype(np.float64)
+                    if n in counts:
+                        assert np.array_equal(S0[(n, s)][counts[n] == 0], S1[counts[n] == 0]), tag + '%s.%s: an untouched row changed' % (n, s)
+                    pairs.append(('%s.%s' % (n, s), S0[(n, s)], S1, m.opt[(n, s)]))
+                for what, a0, a1, r1 in pairs:
+                    r1 = np.asarray(r1).reshape(a0.shape)
+                    checks.append((tag + what + ' update', (a1 - a0)[rows], (r1 - a0)[rows], mult * ulp(a0, a1)[rows]))
+    return checks, outs, scales
+
+
+def f64_failures(checks):
+    """the checks of f64_run_steps that miss the bar, as 'what: max err / max |ref|  /  max relative err above 1 % of max'"""
+    out = []
+    for what, dev, ref, extra in checks:
+        a, r = f64_errors(dev, ref, extra)
+        if not (a <= F64_REL and r <= F64_RTOL):
+            out.append('%s: %.3g / %.3g' % (what, a, r))
+    return out
 
 
 def assert_step_costs(costs, ref, err_msg=''):

@@ -7,7 +7,7 @@ import sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'oracle')); sys.path.insert(0, os.path.join(ROOT, 'tests'))
-from gpu_utils import TC_CASES, tc_setup, tc_run_steps, f64_errors, F64_REL, F64_RTOL
+from gpu_utils import TC_CASES, f64_setup, f64_run_steps, f64_failures
 
 
 def main():
@@ -15,14 +15,9 @@ def main():
     res = {}
     for name in names:
         mk, n_items, step_mode = TC_CASES[name]
-        eng, store, steps, P0 = tc_setup(mk, n_items, step_mode, torch_alloc=False)
-        assert eng.uses_tensor_cores(), name
-        checks, outs = tc_run_steps(eng, mk, n_items, store, steps, P0)
-        failed = []
-        for what, dev, ref, extra in checks:
-            a, r = f64_errors(dev, ref, extra)
-            if a > F64_REL or r > F64_RTOL:
-                failed.append('%s %s: %.3g / %.3g' % (name, what, a, r))
+        eng, store, steps, P0 = f64_setup(mk, n_items, step_mode, torch_alloc=False)
+        checks, outs, _ = f64_run_steps(eng, mk, n_items, store, steps, P0, 'tc')
+        failed = ['%s %s' % (name, f) for f in f64_failures(checks)]
         res[name + ':failures'] = np.array('\n'.join(failed))
         res.update({'%s:%s' % (name, k): v for k, v in outs.items()})
         eng.close()

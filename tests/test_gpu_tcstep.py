@@ -8,8 +8,7 @@ import pytest
 import gru4rec_oracle as orc
 from gru4rec_b200 import _lib
 from gru4rec_b200.synth import make_sessions, make_session_arrays
-from gpu_utils import (make_cfg, push_weights, compare_weights, assert_step_costs, TC_CASES, tc_setup, tc_run_steps, f64_errors, F64_REL,
-                       F64_RTOL)
+from gpu_utils import make_cfg, push_weights, compare_weights, assert_step_costs, TC_CASES, f64_setup, f64_run_steps, f64_failures
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -91,30 +90,22 @@ def test_tensor_core_step_shipped_shapes(L, B, loss, fact, extra):
     eng.close()
 
 
-def _f64_failures(checks):
-    out = []
-    for what, dev, ref, extra in checks:
-        a, r = f64_errors(dev, ref, extra)
-        if a > F64_REL or r > F64_RTOL:
-            out.append('%s: %.3g / %.3g' % (what, a, r))
-    return out
-
-
 @pytest.mark.parametrize('name', sorted(TC_CASES))
 def test_tc_step_products_match_float64(name):
     """Every product of the tensor-core step against a float64 oracle run on the same float32 inputs, two steps (M = B, then M < B
     with a reset lane and duplicates; the oracle is re-seeded from the device in between): y, H, dvec = [da_h | da_r | da_z], dSx,
     the dSy rows, the cost, and -- plain SGD -- dWx, dWh, dWrz, dBh and the Wy / By row gradients recovered from the updates; the
-    Adagrad case compares the updated weights and optimizer state.  Failures are listed as
-    'max err / max |ref|  /  max relative err above 1 % of max' against the bar of gpu_utils.F64_REL / F64_RTOL (4e-5 / 1e-3).
-    Measured on an H100 80GB HBM3 (400 W power limit), worst tensor over all cases: the device 4.8e-6 / 7.6e-5; a float32 run of
-    the oracle 9.1e-6 / 2.3e-4; the device with the a_lo * b_hi term of every product dropped (2xTF32) at least 2.9e-4 / 1.5e-2 in
-    every case, up to 0.23 / 2.5."""
+    Adagrad case compares the updates W1 - W0 of the weights and the optimizer state, from random non-zero state
+    (gpu_utils.f64_run_steps).  Failures are listed as 'max err / max |ref|  /  max relative err above 1 % of max' against the
+    bar of gpu_utils.F64_REL / F64_RTOL (4e-5 / 1e-3).  Measured on an H100 80GB HBM3 (400 W power limit), worst tensor over all
+    cases: the device 4.8e-6 / 7.6e-5 (the Adagrad case, updates from random state: 2.3e-6 / 4.1e-5); a float32 run of the oracle
+    9.1e-6 / 2.3e-4 (the Adagrad case, updates from random state: 5.5e-6 / 2.1e-4); the device with the a_lo * b_hi term of every
+    product dropped (2xTF32) at least 2.9e-4 / 1.5e-2 in every case, up to 0.23 / 2.5 (the Adagrad case then compared updated
+    weights from zero state)."""
     mk, n_items, step_mode = TC_CASES[name]
-    eng, store, steps, P0 = tc_setup(mk, n_items, step_mode)
-    assert eng.uses_tensor_cores()
-    checks, _ = tc_run_steps(eng, mk, n_items, store, steps, P0)
-    failed = _f64_failures(checks)
+    eng, store, steps, P0 = f64_setup(mk, n_items, step_mode)
+    checks, _, _ = f64_run_steps(eng, mk, n_items, store, steps, P0, 'tc')
+    failed = f64_failures(checks)
     assert not failed, '\n'.join(failed)
     eng.close()
 
@@ -123,8 +114,8 @@ def test_tc_step_bitwise_repeatable():
     """Two engines alive in one process, same inputs: the K splits are summed in a fixed order, so every output is bit for bit
     the same."""
     mk, n_items, step_mode = TC_CASES['L344_B48_xe_logq']
-    runs = [tc_setup(mk, n_items, step_mode) for _ in range(2)]
-    outs = [tc_run_steps(eng, mk, n_items, store, steps, P0)[1] for eng, store, steps, P0 in runs]
+    runs = [f64_setup(mk, n_items, step_mode) for _ in range(2)]
+    outs = [f64_run_steps(eng, mk, n_items, store, steps, P0, 'tc')[1] for eng, store, steps, P0 in runs]
     for k in outs[0]:
         assert np.array_equal(outs[0][k], outs[1][k]), k
     for r in runs:
