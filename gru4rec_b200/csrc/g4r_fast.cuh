@@ -7,7 +7,8 @@
 //    the target rows are PREFETCHED with TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) while the GRU
 //    phases of the previous step run, so the score phase starts with its operands already in shared memory;
 //  * folds the row-statistics combine into the score->gradient barrier (the last CTA to arrive combines);
-//  * runs the GRU phases on a group of G CTAs with group barriers; the other CTAs only wait for `h_ready`;
+//  * runs the GRU phases on a group of G CTAs (step_mode 2: weights resident in shared memory, one group barrier per
+//    mini-batch; see FastSmemR); the other CTAs only wait for `h_ready`;
 //  * uses monotonic release/acquire counters (no resets, no separate fences) for all synchronisation.
 //
 // What is computed (reference hidasib/GRU4Rec, same formulas as the generic phases in g4r_kernels.cuh):
@@ -166,10 +167,10 @@ __device__ __forceinline__ void fk_prefetch_rows(const ModelDev& md, SM& sm, int
   }
 }
 
-__device__ __forceinline__ void fk_group_barrier(FastSync* fs, unsigned int& gepoch) {
+__device__ __forceinline__ void fk_group_barrier(FastSync* fs, unsigned int& gepoch, unsigned int G = FK_G) {
   __syncthreads();
   gepoch += 1;
-  if (threadIdx.x == 0) { red_release_add(&fs->grp, 1u); wait_ge(&fs->grp, gepoch * FK_G); }
+  if (threadIdx.x == 0) { red_release_add(&fs->grp, 1u); wait_ge(&fs->grp, gepoch * G); }
   __syncthreads();
 }
 
@@ -567,13 +568,275 @@ __device__ void fk_b1(const ModelDev& md, SM& sm, int s, int cta, int ncta) {
   }
 }
 
+// ---------------- GRU group of step_mode 2: resident weights, ownership by hidden unit ----------------
+// GRU CTA g owns the four hidden units Kg = [4g, 4g + 4) (one 16-byte quad; the group has ldL / 4 <= 30 CTAs) and keeps,
+// for the whole window, the columns Wh[:, Kg], Wrz[:, Kg], Wrz[:, L + Kg], the rows Wh[Kg, :] and Bh of its units with
+// their Adagrad / momentum state in shared memory.  Every phase then needs only its own units or data every CTA already
+// holds, except F2, which needs Hold * r over all units: one group barrier per mini-batch.  Each Wh element is held by
+// two CTAs (row slab of the owner of its row, column slab of the owner of its column); both copies are updated from the
+// same operands in the same order and stay bitwise identical, and only the column copies are written back.
+constexpr int FR_U = 4;             // hidden units per GRU CTA
+
+struct FastSmemR {
+  // column role (same fields as FastSmem); during the GRU phases sD holds da_h and sPart is the reduction scratch
+  alignas(128) float sY[FK_B * FK_LDS];
+  float sS[FK_CT * FK_LDS];
+  float sAcc[FK_CT * FK_LDS];
+  float sVel[FK_CT * FK_LDS];
+  float sTW[FK_B * FK_LDS];
+  float sD[FK_CT * FK_LDS];
+  float sG[FK_CT * FK_B];
+  float sO[FK_CT * FK_B];
+  float sRS[FK_B * 8];
+  float sPart[FK_NW * FK_B * 8];
+  float sT[FK_B];
+  float sBias[FK_CT], sByP[FK_CT], sByA[FK_CT], sByV[FK_CT], sDby[FK_CT], sTB[FK_B];
+  int sIt[2][FK_CT], sPos[2][FK_CT], sTc[2][FK_B], sYit[2][FK_B], sCb[2][2];
+  int sFlag[4];
+  alignas(8) unsigned long long mbar;
+  int gIdx[3 * FK_B];                            // slot, item, flags of the lanes
+  // GRU role
+  alignas(16) float gH[2][FK_B * FK_LDS];        // H rows of the step's lanes (= Hold) | of the next step, by step parity
+  float gHr[FK_B * FK_LDS];                      // Hold * r of the step, all units
+  float rC[3][3 * FR_U * FK_LDS];                // value | Adagrad | momentum of the resident columns, rows over k: Wh[:, Kg] | Wrz[:, Kg] | Wrz[:, L + Kg]
+  float rR[3][FR_U * FK_LDS];                    // value | Adagrad | momentum of the resident rows Wh[Kg, :]
+  float rB[3][3 * FR_U];                         // value | Adagrad | momentum of Bh[Kg] | Bh[L + Kg] | Bh[2L + Kg]
+  float gR[FK_B * FR_U], gZ[FK_B * FR_U], gDr[FK_B * FR_U], gDz[FK_B * FR_U];   // r, z, da_r, da_z of the own units, [lane][unit]
+};
+static_assert(sizeof(FastSmemR) <= 232448, "FastSmemR exceeds the 227 KB shared memory of one CTA");
+static_assert(FK_NW * FK_B * 8 >= FK_NW * FK_B * 2 * FR_U, "sPart too small for the F1 reduction");
+
+// resident slabs <-> global (once per window each)
+__device__ void fr_load_resident(const ModelDev& md, FastSmemR& sm, int k0) {
+  const LayerDev& ly = md.layer[0];
+  const int L = ly.L, tid = threadIdx.x;
+  for (int i = tid; i < 3 * FR_U * FK_LDS; i += FK_THREADS) {
+    const int q = i / FK_LDS, k = i % FK_LDS, t = q / FR_U, c = k0 + q % FR_U;
+    float p = 0.f, a = 0.f, v = 0.f;
+    if (c < L && k < L) {
+      const size_t o = t == 0 ? (size_t)k * ly.ldL + c : (size_t)k * ly.ld2 + (t == 2 ? L : 0) + c;
+      const float* P = t == 0 ? ly.Wh : ly.Wrz;
+      const float* A = t == 0 ? ly.Wh_acc : ly.Wrz_acc;
+      const float* V = t == 0 ? ly.Wh_vel : ly.Wrz_vel;
+      p = P[o]; if (A) a = A[o]; if (V) v = V[o];
+    }
+    sm.rC[0][i] = p; sm.rC[1][i] = a; sm.rC[2][i] = v;
+  }
+  for (int i = tid; i < FR_U * FK_LDS; i += FK_THREADS) {
+    const int k = k0 + i / FK_LDS, c = i % FK_LDS;
+    float p = 0.f, a = 0.f, v = 0.f;
+    if (k < L && c < L) {
+      const size_t o = (size_t)k * ly.ldL + c;
+      p = ly.Wh[o]; if (ly.Wh_acc) a = ly.Wh_acc[o]; if (ly.Wh_vel) v = ly.Wh_vel[o];
+    }
+    sm.rR[0][i] = p; sm.rR[1][i] = a; sm.rR[2][i] = v;
+  }
+  if (tid < 3 * FR_U) {
+    const int c = k0 + tid % FR_U;
+    float p = 0.f, a = 0.f, v = 0.f;
+    if (c < L) { const int o = (tid / FR_U) * L + c; p = ly.Bh[o]; if (ly.Bh_acc) a = ly.Bh_acc[o]; if (ly.Bh_vel) v = ly.Bh_vel[o]; }
+    sm.rB[0][tid] = p; sm.rB[1][tid] = a; sm.rB[2][tid] = v;
+  }
+  __syncthreads();
+}
+__device__ void fr_store_resident(const ModelDev& md, FastSmemR& sm, int k0) {
+  const LayerDev& ly = md.layer[0];
+  const int L = ly.L, tid = threadIdx.x;
+  __syncthreads();
+  for (int i = tid; i < 3 * FR_U * FK_LDS; i += FK_THREADS) {
+    const int q = i / FK_LDS, k = i % FK_LDS, t = q / FR_U, c = k0 + q % FR_U;
+    if (c < L && k < L) {
+      const size_t o = t == 0 ? (size_t)k * ly.ldL + c : (size_t)k * ly.ld2 + (t == 2 ? L : 0) + c;
+      float* P = t == 0 ? ly.Wh : ly.Wrz;
+      float* A = t == 0 ? ly.Wh_acc : ly.Wrz_acc;
+      float* V = t == 0 ? ly.Wh_vel : ly.Wrz_vel;
+      P[o] = sm.rC[0][i]; if (A) A[o] = sm.rC[1][i]; if (V) V[o] = sm.rC[2][i];
+    }
+  }
+  if (tid < 3 * FR_U) {
+    const int c = k0 + tid % FR_U;
+    if (c < L) { const int o = (tid / FR_U) * L + c; ly.Bh[o] = sm.rB[0][tid]; if (ly.Bh_acc) ly.Bh_acc[o] = sm.rB[1][tid]; if (ly.Bh_vel) ly.Bh_vel[o] = sm.rB[2][tid]; }
+  }
+}
+
+// F1 of step s: r, z of the own units from the staged H rows sH (= Hold); writes r, z, Hold and Hold * r of the own units
+__device__ void fr_f1(const ModelDev& md, FastSmemR& sm, int s, int k0, const float* sH, const unsigned int* wait_ctr, unsigned int wait_target) {
+  const LayerDev& ly = md.layer[0];
+  const int M = md.wM[s], L = ly.L, ldL = ly.ldL, tid = threadIdx.x;
+  // if the helper CTAs' input-row updates are already complete (the usual case), the epilogue operand is fetched before the
+  // product instead of after it
+  if (tid == 0) sm.sFlag[3] = (!wait_ctr || ld_acquire_u32(wait_ctr) >= wait_target) ? 1 : 0;
+  __syncthreads();
+  const bool early = sm.sFlag[3] != 0;
+  const int b = tid & 31, jsel = tid >> 5, j = jsel % FR_U, c = k0 + j;
+  const bool isr = jsel < FR_U;
+  const bool on = jsel < 2 * FR_U && b < M && c < L;
+  const int col = (isr ? L : 2 * L) + c;                 // column of the gate in Wx0 rows and Bh
+  const float bias = sm.rB[0][(isr ? 1 : 2) * FR_U + j];
+  float pre = 0.f;
+  if (early && on) pre = ly.Wx[(size_t)sm.gIdx[FK_B + b] * ly.ld3 + col] + bias;
+  float acc[2 * FR_U];
+  fk_slab_dot<2 * FR_U>(acc, sH, FK_LDS, sm.rC[0] + FR_U * FK_LDS, L);
+  const float v = fk_slab_reduce<2 * FR_U>(acc, sm.sPart, jsel);
+  if (!early) {
+    if (tid == 0) wait_ge(wait_ctr, wait_target);
+    __syncthreads();
+    if (on) pre = ly.Wx[(size_t)sm.gIdx[FK_B + b] * ly.ld3 + col] + bias;
+  }
+  if (jsel < 2 * FR_U) {
+    const float g = on ? sigmoidf_(v + pre) : 0.f;
+    if (isr) {
+      sm.gR[b * FR_U + j] = g;
+      if (on) {
+        const float ho = sH[b * FK_LDS + c];
+        ly.r[(size_t)b * ldL + c] = g;
+        ly.Hold[(size_t)b * ldL + c] = ho;
+        ly.Hr[(size_t)b * ldL + c] = ho * g;
+      }
+    } else {
+      sm.gZ[b * FR_U + j] = g;
+      if (on) ly.z[(size_t)b * ldL + c] = g;
+    }
+  }
+}
+// F2 of step s (after the group barrier that completes Hold * r): h~, h, dropout, H_new of the own units
+__device__ void fr_f2(const ModelDev& md, FastSmemR& sm, int s, int k0, const float* sHo) {
+  const LayerDev& ly = md.layer[0];
+  const int M = md.wM[s], L = ly.L, ldL = ly.ldL, tid = threadIdx.x;
+  const int b = tid & 31, jsel = tid >> 5, c = k0 + jsel;
+  const bool on = jsel < FR_U && b < M && c < L;
+  float pre = 0.f;
+  if (on) pre = ly.Wx[(size_t)sm.gIdx[FK_B + b] * ly.ld3 + c] + sm.rB[0][jsel];
+  stage_rows4(sm.gHr, FK_LDS, FK_B, ldL / 4, [&](int rr) -> const float* { return rr < M ? ly.Hr + (size_t)rr * ldL : nullptr; });
+  __syncthreads();
+  float acc[FR_U];
+  fk_slab_dot<FR_U>(acc, sm.gHr, FK_LDS, sm.rC[0], L);
+  const float v0 = fk_slab_reduce<FR_U>(acc, sm.sPart, jsel);
+  if (on) {
+    const float v = v0 + pre;
+    const float ht = act_fwd(md.hact, v);
+    const float z = sm.gZ[b * FR_U + jsel], ho = sHo[b * FK_LDS + c];
+    float h = (1.0f - z) * ho + z * ht;
+    if (md.p_drop_h > 0.f) h *= drop_scale(md.drop_seed, md.wG[s], 0u, (uint32_t)(b * L + c), 1.0f - md.p_drop_h);
+    ly.ah[(size_t)b * ldL + c] = v;
+    ly.ht[(size_t)b * ldL + c] = ht;
+    ly.y[(size_t)b * ldL + c] = h;
+    ly.H[(size_t)sm.gIdx[b] * ldL + c] = (sm.gIdx[2 * FK_B + b] & 1) ? 0.f : h;
+  }
+}
+// B2 of step s (dL/dh complete): stages da_h (all units) and da_z (own units), then da_r of the own units from the resident
+// rows of Wh; da_r goes to dvec for the helper CTAs and to gDr for the dense update
+__device__ void fr_b2(const ModelDev& md, FastSmemR& sm, int s, int k0, const float* sHo) {
+  const LayerDev& ly = md.layer[0];
+  const int M = md.wM[s], L = ly.L, ld3 = ly.ld3, tid = threadIdx.x;
+  float dz = 0.f;
+  if (tid < FK_B * FR_U && tid / FR_U < M && k0 + tid % FR_U < L) dz = ly.dvec[(size_t)(tid / FR_U) * ld3 + 2 * L + k0 + tid % FR_U];
+  stage_rows4(sm.sD, FK_LDS, FK_B, ly.ldL / 4, [&](int rr) -> const float* { return rr < M ? ly.dvec + (size_t)rr * ld3 : nullptr; });
+  if (tid < FK_B * FR_U) sm.gDz[tid] = dz;
+  __syncthreads();
+  const int b = tid & 31, jsel = tid >> 5, c = k0 + jsel;
+  float acc[FR_U];
+  fk_slab_dot<FR_U>(acc, sm.sD, FK_LDS, sm.rR[0], L);
+  const float v = fk_slab_reduce<FR_U>(acc, sm.sPart, jsel);
+  if (jsel < FR_U) {
+    float dar = 0.f;
+    if (b < M && c < L) {
+      const float ho = sHo[b * FK_LDS + c], r = sm.gR[b * FR_U + jsel];
+      dar = v * ho * r * (1.f - r);
+      ly.dvec[(size_t)b * ld3 + L + c] = dar;
+    }
+    sm.gDr[b * FR_U + jsel] = dar;
+  }
+}
+// Adagrad (+momentum) step of one resident element (same arithmetic as fk_dense)
+__device__ __forceinline__ void fr_upd(const ModelDev& md, bool ada, bool mom, float g, float& p, float& a, float& v) {
+  const float p0 = p;
+  float gs = g;
+  if (ada) { a = a + g * g; gs = __fdiv_rn(g, sqrtf(a + G4R_EPS_ADA)); }
+  if (mom) { v = md.mom * v - md.lr * (gs + md.lmbd * p0); p = p0 + v; }
+  else p = p0 * (1.0f - md.lr * md.lmbd) - md.lr * gs;
+}
+// D of step s: gradients of the resident slabs and Bh from shared memory only (Hold, Hold * r, da_h of all units; da_r,
+// da_z of the own units), summed over the lanes in order with fmaf as fk_dense does, then updated in place.
+// A task is one 16-byte quad of outputs: column tasks (resident column jm, quad q of k), row tasks (resident row j, quad q
+// of the columns), then the 3 * FR_U bias entries.
+__device__ void fr_dense(const ModelDev& md, FastSmemR& sm, int s, int k0, const float* sHo) {
+  const LayerDev& ly = md.layer[0];
+  const int M = md.wM[s], L = ly.L, kw = ly.ldL / 4;
+  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
+  const int ncol = 3 * FR_U * kw, nrow = FR_U * kw;
+  for (int t = threadIdx.x; t < ncol + nrow + 3 * FR_U; t += FK_THREADS) {
+    if (t < ncol + nrow) {
+      const bool colt = t < ncol;
+      const int u = colt ? t : t - ncol, q = u % kw, jm = u / kw, j = jm % FR_U;
+      // g[e] = sum_b vec[b][e] * sc[b]; resident element o + e (o: offset in rC[*] or rR[*])
+      const float* vec; const float* sc; int ss, o;
+      if (colt) {
+        const int m = jm / FR_U;                 // 0: Wh (Hold * r, da_h) | 1: Wrz r-block (Hold, da_r) | 2: z-block (Hold, da_z)
+        vec = (m == 0 ? sm.gHr : sHo) + q * 4;
+        if (m == 0) { sc = sm.sD + k0 + j; ss = FK_LDS; } else { sc = (m == 1 ? sm.gDr : sm.gDz) + j; ss = FR_U; }
+        o = jm * FK_LDS + q * 4;
+      } else {                                   // Wh[k0 + j][4q..]: (Hold * r)[b][k0 + j] * da_h[b][4q..]
+        vec = sm.sD + q * 4; sc = sm.gHr + k0 + j; ss = FK_LDS;
+        o = j * FK_LDS + q * 4;
+      }
+      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+      for (int b = 0; b < M; b++) {
+        const float4 a = ld4(vec + b * FK_LDS);
+        const float d = sc[b * ss];
+        g.x = fmaf(a.x, d, g.x); g.y = fmaf(a.y, d, g.y); g.z = fmaf(a.z, d, g.z); g.w = fmaf(a.w, d, g.w);
+      }
+      // column task: unit k0 + j, rows k = 4q + e; row task: row k0 + j, columns 4q + e
+      if (k0 + j < L) {
+        float* P = colt ? sm.rC[0] : sm.rR[0];
+        float* A = colt ? sm.rC[1] : sm.rR[1];
+        float* V = colt ? sm.rC[2] : sm.rR[2];
+        if (q * 4 + 0 < L) fr_upd(md, ada, mom, g.x, P[o + 0], A[o + 0], V[o + 0]);
+        if (q * 4 + 1 < L) fr_upd(md, ada, mom, g.y, P[o + 1], A[o + 1], V[o + 1]);
+        if (q * 4 + 2 < L) fr_upd(md, ada, mom, g.z, P[o + 2], A[o + 2], V[o + 2]);
+        if (q * 4 + 3 < L) fr_upd(md, ada, mom, g.w, P[o + 3], A[o + 3], V[o + 3]);
+      }
+    } else {
+      const int i = t - ncol - nrow, m = i / FR_U, j = i % FR_U;
+      if (k0 + j < L) {
+        float g = 0.f;
+        for (int b = 0; b < M; b++) g = g + (m == 0 ? sm.sD[b * FK_LDS + k0 + j] : (m == 1 ? sm.gDr : sm.gDz)[b * FR_U + j]);
+        fr_upd(md, ada, mom, g, sm.rB[0][i], sm.rB[1][i], sm.rB[2][i]);
+      }
+    }
+  }
+}
+// sY <- y rows of step s (the column role) and, when hnext != nullptr, hnext <- H rows of the lanes staged in gIdx: one round trip
+template <class SM>
+__device__ __forceinline__ void fk_stage_y(const ModelDev& md, SM& sm, int M, float* hnext) {
+  const LayerDev& ly = md.layer[0];
+  const int ldL = ly.ldL, kw = ldL / 4, n1 = FK_B * kw, total = hnext ? 2 * n1 : n1;
+  for (int i0 = 0; i0 < total; i0 += 4 * FK_THREADS) {
+    float4 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int i = i0 + u * FK_THREADS + (int)threadIdx.x;
+      v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (i < n1) { const int rr = i / kw; if (rr < M) v[u] = ld4(ly.y + (size_t)rr * ldL + (i % kw) * 4); }
+      else if (i < total) { const int sl = sm.gIdx[(i - n1) / kw]; if (sl >= 0) v[u] = ld4(ly.H + (size_t)sl * ldL + ((i - n1) % kw) * 4); }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int i = i0 + u * FK_THREADS + (int)threadIdx.x;
+      if (i < n1) st4(sm.sY + (i / kw) * FK_LDS + (i % kw) * 4, v[u]);
+      else if (i < total) st4(hnext + ((i - n1) / kw) * FK_LDS + ((i - n1) % kw) * 4, v[u]);
+    }
+  }
+}
+
 #include "g4r_fastc.cuh"
 
 // CL = false: GRU phases on a 48-CTA group with global group barriers (step_mode 2).
 // CL = true : launched with thread-block clusters; the GRU phases run on cluster 0 (g4r_fastc.cuh, step_mode 3).
 template <bool CL>
 __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps, FastSync* fs, unsigned long long* tstamp) {
-  using SM = typename std::conditional<CL, FastSmemC, FastSmem>::type;
+  using SM = typename std::conditional<CL, FastSmemC, FastSmemR>::type;
   extern __shared__ __align__(128) unsigned char fk_raw[];
   SM& sm = *reinterpret_cast<SM*>(fk_raw);
   const ModelDev& md = MD;
@@ -582,11 +845,11 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int chunk = cta;                       // CTAs beyond the number of chunks own no columns
   const bool has_chunk = chunk < md.NCH;
-  const int G = CL ? (int)cl_size() : FK_G;    // CTAs of the GRU role
+  const int G = CL ? (int)cl_size() : md.ldL / 4;   // CTAs of the GRU role (step_mode 2: one quad of hidden units each)
   const bool gru = cta < G;
   const bool pw = loss_pairwise(md.loss);
   const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
-  const int L = md.L, ldL = md.ldL, B = md.B;
+  const int ldL = md.ldL, B = md.B;
   const int kw = ldL / 4;
   uint64_t* bar = reinterpret_cast<uint64_t*>(&sm.mbar);
   unsigned int bar_epoch = 0, gepoch = 0, stats_target = 0;
@@ -619,11 +882,16 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
     }
   } else {
     if (gru) {
-      fk_f1(md, sm, 0, cta, nullptr, 0u);
-      fk_group_barrier(fs, gepoch);
-      fk_f2(md, sm, 0, cta);
-      __syncthreads();
-      if (tid == 0) red_release_add(&fs->h_ready, 1u);
+      fr_load_resident(md, sm, 4 * cta);
+      if (n_steps > 0) {
+        fk_stage_lanes(md, sm, 0, md.wM[0]);
+        stage_rows4(sm.gH[0], FK_LDS, FK_B, kw, [&](int rr) -> const float* { const int sl = sm.gIdx[rr]; return sl >= 0 ? ly.H + (size_t)sl * ldL : nullptr; });
+        fr_f1(md, sm, 0, 4 * cta, sm.gH[0], nullptr, 0u);
+        fk_group_barrier(fs, gepoch, G);
+        fr_f2(md, sm, 0, 4 * cta, sm.gH[0]);
+        __syncthreads();
+        if (tid == 0) red_release_add(&fs->h_ready, 1u);
+      }
     }
   }
   for (int s = 0; s < n_steps; s++) {
@@ -634,10 +902,18 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
     FK_STAMP(0);
     // indices of the NEXT step (consumed after this step's last barrier)
     fk_load_idx(md, sm, s + 1, n_steps, chunk, buf ^ 1);
-    // ---- wait for h(s), stage it ----
+    const bool gru_next = !CL && gru && s + 1 < n_steps;
+    if (gru_next && tid < FK_B) {               // lanes of the next step (f2 of this step has used gIdx)
+      const int M1 = md.wM[s + 1];
+      sm.gIdx[tid] = tid < M1 ? md.wSlot[(size_t)(s + 1) * B + tid] : -1;
+      sm.gIdx[FK_B + tid] = tid < M1 ? md.wX[(size_t)(s + 1) * B + tid] : 0;
+      sm.gIdx[2 * FK_B + tid] = tid < M1 ? md.wF[(size_t)(s + 1) * B + tid] : 0;
+    }
+    // ---- wait for h(s), stage it (GRU CTAs of step_mode 2: with the H rows of step s + 1, final once every f2(s) has run) ----
     if (tid == 0) wait_ge(&fs->h_ready, (unsigned int)(s + 1) * (unsigned int)G);
     __syncthreads();
-    stage_rows4(sm.sY, FK_LDS, FK_B, kw, [&](int rr) -> const float* { return rr < M ? ly.y + (size_t)rr * ldL : nullptr; });
+    if constexpr (CL) stage_rows4(sm.sY, FK_LDS, FK_B, kw, [&](int rr) -> const float* { return rr < M ? ly.y + (size_t)rr * ldL : nullptr; });
+    else fk_stage_y(md, sm, M, gru_next ? sm.gH[(s + 1) & 1] : nullptr);
     mbar_wait(bar, (unsigned int)(s & 1));      // prefetched rows of this step have landed
     __syncthreads();
     FK_STAMP(1);
@@ -910,44 +1186,43 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
           cl_wait();                                   // matches the arrive left pending by cf_backward
         }
         FK_STAMP(8);
-      } else if (cta < G + in_ctas) {
-        const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;           // dvec rows of the step complete
-        if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, &fs->grp, tgt);
-        else {
-          if (tid == 0) wait_ge(&fs->grp, tgt);
-          __syncthreads();
-          for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
-        }
-        __syncthreads();
-        if (tid == 0) red_release_add(&fs->in_done, 1u);
       }
     } else if (gru) {
+      const int k0 = 4 * cta;
+      const float* sHo = sm.gH[s & 1];                  // H rows of step s (staged one step earlier)
       if (tid == 0) wait_ge(&fs->b1_done, (unsigned int)(s + 1) * (unsigned int)ncta);
       __syncthreads();
-      fk_b2(md, sm, s, cta);
-      fk_group_barrier(fs, gepoch);      // epoch 3*s + 2: all of dvec (da_r included) is complete -> the helper CTAs poll this counter
+      fr_b2(md, sm, s, k0, sHo);
+      __syncthreads();
+      if (tid == 0) red_release_add(&fs->dvec_done, 1u);   // dvec of the step complete once all G have arrived
       FK_STAMP(5);
-      fk_dense(md, sm, s, cta);
-      fk_group_barrier(fs, gepoch);
+      fr_dense(md, sm, s, k0, sHo);
       FK_STAMP(6);
       if (s + 1 < n_steps) {
-        fk_f1(md, sm, s + 1, cta, &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
-        fk_group_barrier(fs, gepoch);
+        fr_f1(md, sm, s + 1, k0, sm.gH[(s + 1) & 1], &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
+        fk_group_barrier(fs, gepoch, G);                // all-gather of Hold * r
         FK_STAMP(7);
-        fk_f2(md, sm, s + 1, cta);
+        fr_f2(md, sm, s + 1, k0, sm.gH[(s + 1) & 1]);
         __syncthreads();
         if (tid == 0) red_release_add(&fs->h_ready, 1u);
       }
       FK_STAMP(8);
-    } else if (cta < FK_G + in_ctas) {
-      // the GRU group's barrier after B2 is its (3 s + 2)-th group barrier (1 in the prologue, then B2 / dense / f1 per step)
-      if (tid == 0) wait_ge(&fs->grp, (unsigned int)(3 * s + 2) * FK_G);
-      __syncthreads();
-      for (int b = cta - FK_G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
+    }
+    if (!gru && cta < G + in_ctas) {
+      // input-row update of the step's lanes, once dvec is complete: cluster variant = the GRU cluster's grp counter
+      const unsigned int* ctr = CL ? &fs->grp : &fs->dvec_done;
+      const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
+      if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, ctr, tgt);
+      else {
+        if (tid == 0) wait_ge(ctr, tgt);
+        __syncthreads();
+        for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
+      }
       __syncthreads();
       if (tid == 0) red_release_add(&fs->in_done, 1u);
     }
   }
   if constexpr (CL) { if (gru) cf_store_resident(md, sm, cc); }
+  else { if (gru) fr_store_resident(md, sm, 4 * cta); }
 #undef FK_STAMP
 }

@@ -101,6 +101,7 @@ struct FastSync {                   // one counter per 128-byte line
   unsigned int b1_done;  unsigned int p3[31];
   unsigned int grp;      unsigned int p4[31];
   unsigned int in_done;  unsigned int p5[31];
+  unsigned int dvec_done; unsigned int p6[31];   // step_mode 2: GRU CTAs that have written their da_r (dvec of the step complete)
 };
 struct GridBar { unsigned int count; unsigned int gen; unsigned int pad[30]; };   // grid barrier state (persistent mode)
 
@@ -116,6 +117,7 @@ struct LayerDev {
   float *Hold, *r, *z, *ah, *ht, *y;   // forward saves, compact lanes [Bmax x ldL]
   float *dvec;             // [Bmax x ld3]  (da_h | da_r | da_z)
   float *dy;               // [Bmax x ldL]  upstream gradient wrt this layer's (dropped) output
+  float *Hr;               // [Bmax x ldL]  Hold * r, exchanged between the GRU CTAs of k_fast (step_mode 2)
   const float* in;         // [Bmax x ld_in] input activations (layer>0: y of the layer below; layer 0: in0)
 };
 

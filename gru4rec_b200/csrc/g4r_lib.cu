@@ -211,7 +211,7 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     reg("He" + si, he, Be, L, ly.ldL);
     ly.Hold = cv.take<float>((size_t)Bmax * ly.ldL); ly.r = cv.take<float>((size_t)Bmax * ly.ldL); ly.z = cv.take<float>((size_t)Bmax * ly.ldL);
     ly.ah = cv.take<float>((size_t)Bmax * ly.ldL); ly.ht = cv.take<float>((size_t)Bmax * ly.ldL); ly.y = cv.take<float>((size_t)Bmax * ly.ldL);
-    ly.dvec = cv.take<float>((size_t)Bmax * ly.ld3); ly.dy = cv.take<float>((size_t)Bmax * ly.ldL);
+    ly.dvec = cv.take<float>((size_t)Bmax * ly.ld3); ly.dy = cv.take<float>((size_t)Bmax * ly.ldL); ly.Hr = cv.take<float>((size_t)Bmax * ly.ldL);
     reg("y" + si, ly.y, Bmax, L, ly.ldL); reg("dvec" + si, ly.dvec, Bmax, 3 * L, ly.ld3);
   }
   if (mode != 0) {
@@ -782,12 +782,12 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
   }
   {
     const ModelDev& m = h->md;
-    raise_smem_limit((const void*)k_fast_t<false>, sizeof(FastSmem));
+    raise_smem_limit((const void*)k_fast_t<false>, sizeof(FastSmemR));
     int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_t<false>, FK_THREADS, sizeof(FastSmem));
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_t<false>, FK_THREADS, sizeof(FastSmemR));
     const bool plain_opt = m.adapt <= G4R_ADAPT_ADAGRAD && !h->phase_only;    // the role-specialised kernels implement SGD / Adagrad (+momentum) only
     h->fast_ok = plain_opt && h->pk_blocks > 0 && per_sm >= 1 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B && h->n_sm >= FK_G + 1 && m.NCH <= 160 &&
-                 2 * m.L <= FK_W1 * FK_G && m.L <= FK_W2 * FK_G &&     // the 48-CTA GRU group covers FK_W1 gate / FK_W2 candidate columns per CTA (L <= 120)
+                 2 * m.L <= FK_W1 * FK_G && m.L <= FK_W2 * FK_G &&     // L <= 120, the coverage of k_fast_mg's 48-CTA GRU group (k_fast_t<false> uses ldL / 4 CTAs)
                  (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);
     h->fastc_ok = plain_opt && cfg->step_mode == 3 && h->fastc_grid >= FC_CLUSTER * 2 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B &&
                   m.NCH <= h->fastc_grid && (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);
@@ -1232,7 +1232,7 @@ static int run_window(g4r_handle* h, int64_t n) {
     int slot = h->slot, nst = (int)n; FastSync* fsp = h->dFastSync; unsigned long long* ts = h->stamp_on ? h->dStamp : nullptr;
     void* args[] = {&slot, &nst, &fsp, &ts};
     CK(cudaMemsetAsync(h->dFastSync, 0, sizeof(FastSync), h->stream));
-    CK(cudaLaunchCooperativeKernel((void*)k_fast_t<false>, dim3(h->pk_blocks), dim3(FK_THREADS), args, sizeof(FastSmem), h->stream));
+    CK(cudaLaunchCooperativeKernel((void*)k_fast_t<false>, dim3(h->pk_blocks), dim3(FK_THREADS), args, sizeof(FastSmemR), h->stream));
     h->launches += 1; h->fast_windows++;
   } else if (h->cfg.step_mode >= 1 && !h->prof && h->pk_blocks > 0 && !h->phase_only && !h->tc_ok) {
     if (h->cfg.step_mode >= 2) h->slow_windows++;

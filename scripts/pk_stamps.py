@@ -6,14 +6,15 @@ import numpy as np
 import bench
 from gru4rec_b200 import _lib
 import gru4rec as g4
-mk = dict(bench.WORKLOAD['model'])
+WL = bench.WORKLOADS['cfg2']
+mk = dict(WL['model'])
 K = 1000
-cfg = _lib.make_config(bench.WORKLOAD['n_items'], mk, sample_store=bench.WORKLOAD['sample_store'], max_resident_steps=K + 8, step_mode=int(sys.argv[1]) if len(sys.argv) > 1 else 1)
+cfg = _lib.make_config(WL['n_items'], mk, sample_store=bench.SAMPLE_STORE, max_resident_steps=K + 8, step_mode=int(sys.argv[1]) if len(sys.argv) > 1 else 1)
 eng = _lib.Engine(cfg)
-gru = g4.GRU4Rec(**mk); gru.n_items = bench.WORKLOAD['n_items']
+gru = g4.GRU4Rec(**mk); gru.n_items = WL['n_items']
 for name, w in gru._init_host_weights().items():
     eng.set(name, w)
-items, offset, order, supports = bench.build_workload(3 * K)
+items, offset, order, supports = bench.build_workload(WL, 3 * K)
 P = supports.astype(np.float64) ** mk['sample_alpha']; P = P.cumsum() / P.sum(); P[-1] = 1
 eng.set_sampling_cdf(P.astype(np.float32)); eng.generate_samples()
 sched = _lib.Schedule(items, offset, order, mk['batch_size'], mk['n_sample'], mode=0)
@@ -24,7 +25,7 @@ st = eng.persistent_stamps(True, K).astype(np.int64)
 if cfg.step_mode >= 2:
     print('fast windows', eng.fast_windows())
     names = [('wait h + stage', 0, 1), (' targets+scores', 1, 9), (' partial stats', 9, 10), (' B2 + parallel combine', 10, 2), (' RS load + cost', 2, 11), (' g + dby', 11, 12), (' dSy + part', 12, 13), (' sparse update', 13, 14), (' B3', 14, 3),
-             ('b1 (+release)', 3, 15), ('prefetch issue', 15, 4), ('b2 + grp', 4, 5), ('dense + grp', 5, 6), ('f1 + grp', 6, 7), ('f2', 7, 8)]
+             ('b1 (+release)', 3, 15), ('prefetch issue', 15, 4), ('wait b1 + b2 -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 + grp', 6, 7), ('f2', 7, 8)]
     if cfg.step_mode == 3:   # GRU phases on one thread-block cluster
         names[-4:] = [('backward -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 (+in_done, barriers)', 6, 7), ('f2', 7, 8)]
     st = st[:-1]
