@@ -43,7 +43,7 @@ EXPORTS = [
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
     'g4r_eval_schedule', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
-    'g4r_predict_topk',
+    'g4r_predict_topk', 'g4r_predict_topk_filtered',
 ]
 
 _lib = None
@@ -112,6 +112,7 @@ def load():
     lib.g4r_predict.argtypes = [vp, vp, i32, vp, vp]
     lib.g4r_reset_eval_hidden.argtypes = [vp]
     lib.g4r_predict_topk.argtypes = [vp, vp, i32, vp, i32, vp, vp]
+    lib.g4r_predict_topk_filtered.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -501,17 +502,47 @@ class Engine(object):
         self._check(self.lib.g4r_predict(self.h, _ptr(X), len(X), _ptr(rm), _ptr(out)))
         return out
 
-    def predict_topk(self, X, k, reset_mask=None):
+    def predict_topk(self, X, k, reset_mask=None, items=None, exclude=None):
         """predict() reduced on the device to the k best items of every lane: (items int32 [batch, k], scores float32 [batch, k]),
         best first.  Order: the activated score (the pre-activation score for softmax), then the smaller item index; the scores
-        are predict()'s values.  Advances the hidden state exactly as predict() does."""
-        k = check_topk(k, self.cfg.n_items)
+        are predict()'s values.  Advances the hidden state exactly as predict() does.
+
+        Filters (g4r_predict_topk_filtered): `items`, an array of item indices, restricts the ranking to its distinct items (the
+        softmax normaliser then runs over them); `exclude`, one int array (or None) per lane, removes those items from that
+        lane's list.  A lane with fewer than k eligible items gets them best first, then item -1 with score NaN."""
         X = np.ascontiguousarray(X, dtype=np.int32)
         rm = None if reset_mask is None else np.ascontiguousarray(reset_mask, dtype=np.uint8)
-        items = np.empty((len(X), k), dtype=np.int32)
-        scores = np.empty((len(X), k), dtype=np.float32)
-        self._check(self.lib.g4r_predict_topk(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(items), _ptr(scores)))
-        return items, scores
+        if items is None and exclude is None:
+            k = check_topk(k, self.cfg.n_items)
+            out_i = np.empty((len(X), k), dtype=np.int32)
+            out_s = np.empty((len(X), k), dtype=np.float32)
+            self._check(self.lib.g4r_predict_topk(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(out_i), _ptr(out_s)))
+            return out_i, out_s
+        cand = None
+        n_distinct = self.cfg.n_items
+        if items is not None:
+            cand = np.asarray(items, dtype=np.int64).reshape(-1)
+            if cand.size and (cand.min() < 0 or cand.max() >= self.cfg.n_items):
+                raise IndexError('candidate item index out of range')
+            cand = np.ascontiguousarray(cand, dtype=np.int32)
+            n_distinct = int(np.count_nonzero(np.bincount(cand, minlength=self.cfg.n_items)))
+        k = check_topk(k, n_distinct)
+        off = ex = None
+        if exclude is not None:
+            if len(exclude) != len(X):
+                raise ValueError('exclude must hold one entry per lane (%d), got %d' % (len(X), len(exclude)))
+            parts = [np.asarray(e if e is not None else [], dtype=np.int64).reshape(-1) for e in exclude]
+            off = np.zeros(len(X) + 1, dtype=np.int64)
+            off[1:] = np.cumsum([len(p) for p in parts])
+            ex = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+            if ex.size and (ex.min() < 0 or ex.max() >= self.cfg.n_items):
+                raise IndexError('excluded item index out of range')
+            ex = np.ascontiguousarray(ex, dtype=np.int32)
+        out_i = np.empty((len(X), k), dtype=np.int32)
+        out_s = np.empty((len(X), k), dtype=np.float32)
+        self._check(self.lib.g4r_predict_topk_filtered(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(cand), 0 if cand is None else cand.size,
+                                                       _ptr(off), _ptr(ex), _ptr(out_i), _ptr(out_s)))
+        return out_i, out_s
 
     def reset_eval_hidden(self):
         self._check(self.lib.g4r_reset_eval_hidden(self.h))

@@ -12,10 +12,15 @@
 //                survivor list; the softmax normaliser (max, sum of exp) is accumulated per tile on the way
 //   3. select    one CTA per lane rescores its survivors with the fp32 chain of k_eval_tgt, radix-selects the k-th key and sorts
 //                the k winners; a lane whose survivors overflowed its list scores its whole row in fp32 instead (bounded, exact)
+// Filters (g4r_predict_topk_filtered): a candidate set (an n_items-bit mask plus the ascending list of its items, cached between
+// calls by content) and per-lane exclusion lists (sorted CSR, uploaded per call).  The prefix of step 1 is the first P candidates
+// with each lane's exclusions left out of its tau; the fp32 tiles run over the candidate list, the wgmma tiles over the catalogue
+// with the mask; excluded items are never appended; step 3 applies both filters to a fallback row.  When every candidate is in
+// the prefix, the prefix itself is the survivor set and no tile kernel runs.
 #pragma once
 
 constexpr int TOPK_THREADS = 512;          // select / tau kernels: one CTA per lane
-constexpr int TOPK_PREFIX_MIN = 2048;      // items scored exactly for tau: max(k, 2048, n_items / 16), at most n_items
+constexpr int TOPK_PREFIX_MIN = 2048;      // items scored exactly for tau: max(k + exclusions, 2048, n_items / 16), at most n_cand
 constexpr int TOPK_SURV_BASE = 4096;       // survivor list of a lane: min(n_items, 16 k + 4096) item indices
 
 struct TopkCtx {
@@ -32,13 +37,19 @@ struct TopkCtx {
   int *dOvList = nullptr, *dOvRow = nullptr;              // overflowed lanes / row of each lane in the fallback buffer (-1: none)
   int* dItems = nullptr; size_t items_cap = 0;            // [batch x k] results
   float* dScores = nullptr; size_t scores_cap = 0;
+  std::vector<uint32_t> hMask;                            // candidate bitmap last uploaded (the cache key; empty: none)
+  unsigned int* dMask = nullptr; size_t mask_cap = 0;     // its device copy
+  int* dCand = nullptr; size_t cand_cap = 0;              // its items, ascending
+  int* dExOff = nullptr; size_t ex_off_cap = 0;           // [batch + 1] exclusion offsets of this call
+  int* dEx = nullptr; size_t ex_cap = 0;                  // exclusions, sorted and distinct per lane
 };
 
 static void topk_release(EvalCtx& e) {
   if (!e.topk) return;
   TopkCtx& t = *static_cast<TopkCtx*>(e.topk);
   for (void* p : {(void*)t.dAsplit, (void*)t.dBsplit, (void*)t.dAbsMax, (void*)t.dIota, (void*)t.dPre, (void*)t.dTau, (void*)t.dCnt, (void*)t.dSurv,
-                  (void*)t.dSurvPre, (void*)t.dPart, (void*)t.dOvList, (void*)t.dOvRow, (void*)t.dItems, (void*)t.dScores})
+                  (void*)t.dSurvPre, (void*)t.dPart, (void*)t.dOvList, (void*)t.dOvRow, (void*)t.dItems, (void*)t.dScores,
+                  (void*)t.dMask, (void*)t.dCand, (void*)t.dExOff, (void*)t.dEx})
     if (p) cudaFree(p);
   delete static_cast<TopkCtx*>(e.topk);
   e.topk = nullptr;
@@ -74,15 +85,43 @@ __device__ __forceinline__ float topk_score_fp32(const ModelDev& md, int b, int 
   return a + md.By[item];
 }
 
-// candidates of one lane: position j is item idx[j] (idx == nullptr: item j) with fp32 pre-activation pre[j]
-struct TopkSrc { const int* idx; const float* pre; int n; };
+// item at position pos of a tile sweep over `subset` (nullptr: the catalogue)
+__device__ __forceinline__ int topk_item(const int* __restrict__ subset, int pos) { return subset ? subset[pos] : pos; }
+// item in the sorted list l[0 .. n)
+__device__ __forceinline__ bool topk_in(const int* __restrict__ l, int n, int item) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int m = (lo + hi) >> 1; if (l[m] < item) lo = m + 1; else hi = m; }
+  return lo < n && l[lo] == item;
+}
+// item in the candidate bitmap (nullptr: every item)
+__device__ __forceinline__ bool topk_is_cand(const unsigned int* __restrict__ mask, int item) {
+  return !mask || ((mask[item >> 5] >> (item & 31)) & 1u);
+}
+// item on lane b's exclusion list (ex_off == nullptr: no exclusions)
+__device__ __forceinline__ bool topk_excluded(const int* __restrict__ ex_off, const int* __restrict__ ex, int b, int item) {
+  if (!ex_off) return false;
+  const int e0 = ex_off[b];
+  return topk_in(ex + e0, ex_off[b + 1] - e0, item);
+}
+
+// candidates of one lane: position j is item idx[j] (idx == nullptr: item j) with fp32 pre-activation pre[j]; an item outside
+// `cand` (nullptr: none is) or on the sorted list ex[0 .. n_ex) does not compete
+struct TopkSrc { const int* idx; const float* pre; int n; const unsigned int* cand = nullptr; const int* ex = nullptr; int n_ex = 0; };
 __device__ __forceinline__ uint64_t topk_src_key(const ActSpec a, const TopkSrc& s, int j) {
   return topk_key(topk_keyval(a, s.pre[j]), s.idx ? s.idx[j] : j);
 }
+__device__ __forceinline__ bool topk_src_live(const TopkSrc& s, int j) {
+  if (!s.cand && s.n_ex == 0) return true;
+  const int item = s.idx ? s.idx[j] : j;
+  return topk_is_cand(s.cand, item) && !topk_in(s.ex, s.n_ex, item);
+}
+__device__ __forceinline__ void topk_set_excl(TopkSrc& s, const int* ex_off, const int* ex, int b) {
+  if (ex_off) { s.ex = ex + ex_off[b]; s.n_ex = ex_off[b + 1] - ex_off[b]; }
+}
 
-// The k-th largest key among the candidates (keys are distinct, so exactly k candidates are >= it): MSB-first radix select,
-// eight passes of 8 bits with a shared histogram.  With fewer than k candidates (only non-finite weights get there) the result is
-// some key below all of them.  Every thread of the block returns the same value.
+// The k-th largest key among the live candidates (keys are distinct, so exactly k of them are >= it): MSB-first radix select,
+// eight passes of 8 bits with a shared histogram.  With fewer than k live candidates (non-finite weights, or a filtered lane with
+// fewer than k eligible items) the result is 0, below every key.  Every thread of the block returns the same value.
 __device__ uint64_t topk_kth(const ActSpec a, const TopkSrc& s, int k, unsigned int* hist, unsigned int* bc) {
   uint64_t prefix = 0, mask = 0;
   unsigned int kk = (unsigned int)k;
@@ -91,7 +130,7 @@ __device__ uint64_t topk_kth(const ActSpec a, const TopkSrc& s, int k, unsigned 
     __syncthreads();
     for (int j = threadIdx.x; j < s.n; j += blockDim.x) {
       const uint64_t key = topk_src_key(a, s, j);
-      if ((key & mask) == prefix) atomicAdd(&hist[(unsigned int)(key >> shift) & 255u], 1u);
+      if ((key & mask) == prefix && topk_src_live(s, j)) atomicAdd(&hist[(unsigned int)(key >> shift) & 255u], 1u);
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -107,15 +146,29 @@ __device__ uint64_t topk_kth(const ActSpec a, const TopkSrc& s, int k, unsigned 
 
 // pass 1: tau_b = the k-th key of the exact prefix scores, as the two pre-activation thresholds of k_eval_tc (act(x) > key <=>
 // x > hi, act(x) == key <=> lo <= x <= hi) plus its item; delta_b bounds |3xTF32 - fp32| of every score of the lane (absmax !=
-// nullptr, the wgmma tiles): (||y_b||_1 max|Wy| + max|By|) * dscale
+// nullptr, the wgmma tiles): (||y_b||_1 max|Wy| + max|By|) * dscale.  Prefix position j is item pidx[j] (nullptr: item j); the
+// lane's exclusions are left out of the select, so tau_b is the k-th key of its eligible prefix items
+// (FILT = false: pidx / ex_off ignored, the unfiltered instantiation)
+template <bool FILT>
 __global__ void __launch_bounds__(TOPK_THREADS) k_topk_tau(int slot, const float* __restrict__ pre, int P, int k, float* tau,
-                                                          const unsigned int* __restrict__ absmax, float dscale) {
+                                                          const unsigned int* __restrict__ absmax, float dscale, const int* __restrict__ pidx_,
+                                                          const int* __restrict__ ex_off_, const int* __restrict__ ex) {
   const ModelDev& md = MD;
+  const int* pidx = FILT ? pidx_ : nullptr;
+  const int* ex_off = FILT ? ex_off_ : nullptr;
   const int b = blockIdx.x;
   __shared__ unsigned int hist[256], bc[2];
   __shared__ float red[TOPK_THREADS / 32];
-  const TopkSrc s{nullptr, pre + (size_t)b * P, P};
+  __shared__ int tpos;
+  TopkSrc s{pidx, pre + (size_t)b * P, P};
+  topk_set_excl(s, ex_off, ex, b);
+  if (threadIdx.x == 0) tpos = -1;
   const uint64_t T = topk_kth(md.fact, s, k, hist, bc);
+  if (pidx) {                     // the prefix position of tau's item
+    const int ti = (int)~(uint32_t)T;
+    for (int j = threadIdx.x; j < P; j += blockDim.x) if (pidx[j] == ti) tpos = j;
+    __syncthreads();
+  }
   float delta = 0.f;
   if (absmax) {
     const float* yr = md.layer[md.n_layers - 1].y + (size_t)b * md.ldL;
@@ -130,7 +183,8 @@ __global__ void __launch_bounds__(TOPK_THREADS) k_topk_tau(int slot, const float
   }
   if (threadIdx.x == 0) {
     const int ti = (int)~(uint32_t)T;
-    const float t = tc_fkey_inv((uint32_t)(T >> 32)), xt = (ti >= 0 && ti < P) ? s.pre[ti] : t;
+    const int tj = pidx ? tpos : ti;
+    const float t = tc_fkey_inv((uint32_t)(T >> 32)), xt = (tj >= 0 && tj < P) ? s.pre[tj] : t;
     float lo, hi;
     tc_thresholds(md.fact, md.fact.kind <= G4R_ACT_SELU, t, xt, lo, hi);
     tau[b * 4 + 0] = lo; tau[b * 4 + 1] = hi; tau[b * 4 + 2] = delta; tau[b * 4 + 3] = __int_as_float(ti);
@@ -154,14 +208,20 @@ __device__ __forceinline__ float2 topk_smx_merge(float2 p, float2 q) {
 }
 
 // pass 2, fp32 FFMA tiles: k_eval_score's tiles and fma order (scores bitwise equal to the fp32 chain, so delta = 0); partial
-// softmax normaliser per (lane, 64-item tile)
-__global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float* __restrict__ tau, int* cnt, int* surv, int C, float2* part, int n_part) {
+// softmax normaliser per (lane, 64-item tile).  subset != nullptr: the tiles run over the n_comp items subset[0 .. n_comp) instead
+// of the catalogue; items on the lane's exclusion list are not appended (but are summed: exclusions never change a score)
+// FILT = false: the unfiltered instantiation (subset / ex_off ignored), so g4r_predict_topk runs the code it ran before filters
+template <bool FILT>
+__global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float* __restrict__ tau, int* cnt, int* surv, int C, float2* part, int n_part,
+                                                          const int* __restrict__ subset_, int n_comp, const int* __restrict__ ex_off_, const int* __restrict__ ex) {
   const ModelDev& md = MD;
+  const int* subset = FILT ? subset_ : nullptr;
+  const int* ex_off = FILT ? ex_off_ : nullptr;
   extern __shared__ __align__(16) float smem[];
   float* sY = smem;                        // [EV_TB][EV_LDS]
   float* sW = sY + EV_TB * EV_LDS;         // [EV_IT][EV_LDS]
   float2* sP = reinterpret_cast<float2*>(sW + EV_IT * EV_LDS);   // [8 warps][EV_TB]
-  const int M = md.wM[0], I = md.n_items, ldL = md.ldL;
+  const int M = md.wM[0], I = subset ? n_comp : md.n_items, ldL = md.ldL;
   const int i0 = blockIdx.x * EV_IT;
   const int ni = min(EV_IT, I - i0);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -173,7 +233,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
     for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
       const int rr = i / kw, c4 = i % kw;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (rr < ni) v = ld4(md.Wy + (size_t)(i0 + rr) * ldL + c4 * 4);
+      if (rr < ni) v = ld4(md.Wy + (size_t)topk_item(subset, i0 + rr) * ldL + c4 * 4);
       st4(sW + rr * EV_LDS + c4 * 4, v);
     }
   }
@@ -194,7 +254,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
         for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
           const int rr = i / kw, c4 = i % kw;
           float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (rr < ni) v = ld4(md.Wy + (size_t)(i0 + rr) * ldL + k0 + c4 * 4);
+          if (rr < ni) v = ld4(md.Wy + (size_t)topk_item(subset, i0 + rr) * ldL + k0 + c4 * 4);
           st4(sW + rr * EV_LDS + c4 * 4, v);
         }
       }
@@ -214,14 +274,20 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
     if (b < M) {
       const float lo = tau[b * 4 + 0], hi = tau[b * 4 + 1];
       const int ti = __float_as_int(tau[b * 4 + 3]);
+      unsigned int keep = 0u;               // FILT: kept q, tested against the exclusions outside the unrolled loop
 #pragma unroll
       for (int q = 0; q < 8; q++) {
-        const int it = i0 + warp + 8 * q;
         if (warp + 8 * q < ni) {
+          const int it = topk_item(subset, i0 + warp + 8 * q);
           acc[q] += md.By[it];
-          if (topk_keep(acc[q], 0.f, lo, hi, it, ti)) topk_append(cnt, surv, C, b, it);
+          if (topk_keep(acc[q], 0.f, lo, hi, it, ti)) { if (FILT) keep |= 1u << q; else topk_append(cnt, surv, C, b, it); }
           sm.x = fmaxf(sm.x, acc[q]);
         }
+      }
+      while (FILT && keep) {
+        const int q = __ffs(keep) - 1, it = topk_item(subset, i0 + warp + 8 * q);
+        keep &= keep - 1u;
+        if (!topk_excluded(ex_off, ex, b, it)) topk_append(cnt, surv, C, b, it);
       }
       if (soft && sm.x != -INFINITY) {
 #pragma unroll
@@ -243,9 +309,15 @@ static size_t topk_fp32_smem_bytes() { return (size_t)(EV_TB * EV_LDS + EV_IT * 
 
 // pass 2, wgmma 3xTF32 tiles: k_eval_tc's pipeline (persistent CTAs, [A hi | A lo | B hi | B lo] stages fed by bulk copies,
 // four warpgroups of 64 lanes x 128 items) with a filtering epilogue: a thread holds two lanes x 32 items of the tile and keeps
-// those whose score x satisfies x + delta_b >= tau_b (topk_keep); partial softmax normaliser per (lane, tile, column half)
+// those whose score x satisfies x + delta_b >= tau_b (topk_keep); partial softmax normaliser per (lane, tile, column half).
+// Items outside the candidate bitmap `cand` (nullptr: none) are neither kept nor summed; excluded items are summed, not kept.
+// FILT = false: the unfiltered instantiation (cand / ex_off ignored)
+template <bool FILT>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_topk_tc(int slot, const float* __restrict__ tau, int* cnt, int* surv, int C, float2* part, int n_part,
-                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit) {
+                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit,
+                                                           const unsigned int* __restrict__ cand_, const int* __restrict__ ex_off_, const int* __restrict__ ex) {
+  const unsigned int* cand = FILT ? cand_ : nullptr;
+  const int* ex_off = FILT ? ex_off_ : nullptr;
   extern __shared__ __align__(1024) unsigned char tc_raw[];
   TcSmem& sm = *reinterpret_cast<TcSmem*>(tc_raw);
   const ModelDev& md = MD;
@@ -298,15 +370,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_topk_tc(int slot, const float
         if (tid == 0 && it + TC_STAGES < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + TC_STAGES); }
         __syncwarp();
       }
-      // columns past the catalogue (last tile) are neither kept nor summed
+      // columns past the catalogue (last tile) and non-candidates are neither kept nor summed
       const int c0 = t * TC_N + wc + 2 * (lane & 3);                // item of d[0]; d[i] holds item c0 + 8 * (i / 4) + i % 2
       const int n_live = I - c0;
       float2 smx[2] = {make_float2(-INFINITY, 0.f), make_float2(-INFINITY, 0.f)};
 #pragma unroll
       for (int i = 0; i < 64; i++) {
         const int h = (i >> 1) & 1, col = (i >> 2) * 8 + (i & 1);
-        if (col < n_live) {
-          if (vrow[h] && topk_keep(d[i], dl[h], lo[h], hi[h], c0 + col, ti[h])) topk_append(cnt, surv, C, bb[h], c0 + col);
+        if (col < n_live && topk_is_cand(cand, c0 + col)) {
+          if (vrow[h] && topk_keep(d[i], dl[h], lo[h], hi[h], c0 + col, ti[h]) && !topk_excluded(ex_off, ex, bb[h], c0 + col))
+            topk_append(cnt, surv, C, bb[h], c0 + col);
           smx[h].x = fmaxf(smx[h].x, d[i]);
         }
       }
@@ -314,7 +387,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_topk_tc(int slot, const float
 #pragma unroll
         for (int i = 0; i < 64; i++) {
           const int h = (i >> 1) & 1, col = (i >> 2) * 8 + (i & 1);
-          if (col < n_live && smx[h].x != -INFINITY) smx[h].y += expf(d[i] - smx[h].x);
+          if (col < n_live && topk_is_cand(cand, c0 + col) && smx[h].x != -INFINITY) smx[h].y += expf(d[i] - smx[h].x);
         }
 #pragma unroll
         for (int h = 0; h < 2; h++) {                                  // the four threads of a quad share the two lanes
@@ -338,23 +411,35 @@ __global__ void __launch_bounds__(128) k_topk_rows(int slot, const int* __restri
 
 // pass 3: per lane (one CTA) the exact fp32 pre-activations of the candidates -- the survivors, rescored with the fp32 chain, or
 // the lane's whole fallback row -- then the k-th key, the k winners sorted best first, and their scores: the activated score for
-// the elementwise activations, exp(x - m) / z with the catalogue's normaliser merged from the tile partials for softmax
+// the elementwise activations, exp(x - m) / z with the catalogue's normaliser merged from the tile partials for softmax.
+// cnt == nullptr (every candidate is in the prefix, no tile ran): the candidates are the prefix pidx[0 .. P) (nullptr: items
+// 0 .. P-1) with pre-activations ppre, and the softmax normaliser is summed over them here (part unused).  The lane's exclusions
+// never win; a fallback row is also restricted to the candidate bitmap `cand`.  Slots past the lane's eligible items: key 0,
+// i.e. item -1 and a NaN score.
+// (FILT = false: cnt != nullptr, and cand / ex_off ignored, the unfiltered instantiation)
+template <bool FILT>
 __global__ void __launch_bounds__(TOPK_THREADS) k_topk_final(int slot, int k, const int* __restrict__ cnt, const int* __restrict__ surv, float* surv_pre, int C,
                                                             const int* __restrict__ ov_row, const float* __restrict__ rows, const float2* __restrict__ part, int n_part,
-                                                            int* out_items, float* out_scores) {
+                                                            int* out_items, float* out_scores, const int* __restrict__ pidx, const float* __restrict__ ppre, int P,
+                                                            const unsigned int* __restrict__ cand_, const int* __restrict__ ex_off_, const int* __restrict__ ex) {
   const ModelDev& md = MD;
+  const unsigned int* cand = FILT ? cand_ : nullptr;
+  const int* ex_off = FILT ? ex_off_ : nullptr;
+  const bool from_prefix = FILT && !cnt;
   const int b = blockIdx.x, tid = threadIdx.x;
   __shared__ unsigned int hist[256], bc[2], n_got;
   __shared__ unsigned long long keys[G4R_TOPK_MAX];
   __shared__ float redf[TOPK_THREADS / 32];
   __shared__ double redd[TOPK_THREADS / 32];
   TopkSrc s;
-  if (ov_row && ov_row[b] >= 0) s = TopkSrc{nullptr, rows + (size_t)ov_row[b] * md.n_items, md.n_items};
+  if (from_prefix) s = TopkSrc{pidx, ppre + (size_t)b * P, P};
+  else if (ov_row && ov_row[b] >= 0) s = TopkSrc{nullptr, rows + (size_t)ov_row[b] * md.n_items, md.n_items, cand};
   else {
     s = TopkSrc{surv + (size_t)b * C, surv_pre + (size_t)b * C, min(cnt[b], C)};
     for (int j = tid; j < s.n; j += blockDim.x) surv_pre[(size_t)b * C + j] = topk_score_fp32(md, b, s.idx[j]);
     __syncthreads();
   }
+  topk_set_excl(s, ex_off, ex, b);
   const uint64_t T = topk_kth(md.fact, s, k, hist, bc);
   int kp = 1;
   while (kp < k) kp <<= 1;
@@ -362,10 +447,10 @@ __global__ void __launch_bounds__(TOPK_THREADS) k_topk_final(int slot, int k, co
   __syncthreads();
   for (int j = tid; j < s.n; j += blockDim.x) {
     const uint64_t key = topk_src_key(md.fact, s, j);
-    if (key >= T) { const unsigned int p = atomicAdd(&n_got, 1u); if (p < (unsigned)k) keys[p] = key; }
+    if (key >= T && topk_src_live(s, j)) { const unsigned int p = atomicAdd(&n_got, 1u); if (p < (unsigned)k) keys[p] = key; }
   }
   __syncthreads();
-  for (int i = min(n_got, (unsigned)k) + tid; i < kp; i += blockDim.x) keys[i] = 0ull;   // (fewer than k only with non-finite weights)
+  for (int i = min(n_got, (unsigned)k) + tid; i < kp; i += blockDim.x) keys[i] = 0ull;   // fewer than k eligible (or non-finite weights)
   // bitonic sort, descending
   for (int size = 2; size <= kp; size <<= 1) {
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
@@ -382,15 +467,21 @@ __global__ void __launch_bounds__(TOPK_THREADS) k_topk_final(int slot, int k, co
   __syncthreads();
   float m = -INFINITY, z = 0.f;
   if (md.fact.kind > G4R_ACT_SELU) {
-    const float2* pr = part + (size_t)b * n_part;
-    for (int j = tid; j < n_part; j += blockDim.x) m = fmaxf(m, pr[j].x);
+    // the partials (max, sum exp(x - max)) of the tiles, or one (x, 1) per prefix candidate
+    const float2* pr = from_prefix ? nullptr : part + (size_t)b * n_part;
+    const int n_pr = from_prefix ? s.n : n_part;
+    auto part_at = [&](int j) -> float2 { return pr ? pr[j] : make_float2(s.pre[j], 1.f); };
+    for (int j = tid; j < n_pr; j += blockDim.x) m = fmaxf(m, part_at(j).x);
     m = warp_max(m);
     if ((tid & 31) == 0) redf[tid >> 5] = m;
     __syncthreads();
     m = redf[0];
     for (int w = 1; w < (int)(blockDim.x >> 5); w++) m = fmaxf(m, redf[w]);
     double zz = 0.0;
-    for (int j = tid; j < n_part; j += blockDim.x) if (pr[j].x != -INFINITY) zz += (double)pr[j].y * exp((double)pr[j].x - (double)m);
+    for (int j = tid; j < n_pr; j += blockDim.x) {
+      const float2 p = part_at(j);
+      if (p.x != -INFINITY) zz += (double)p.y * exp((double)p.x - (double)m);
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) zz += __shfl_xor_sync(0xffffffffu, zz, o);
     if ((tid & 31) == 0) redd[tid >> 5] = zz;
@@ -429,20 +520,63 @@ static int topk_ctx(g4r_handle* h, EvalCtx* e, TopkCtx** out) {
     CK(cudaMalloc(&t.dCnt, (size_t)e->Be * sizeof(int)));
     CK(cudaMalloc(&t.dOvList, (size_t)e->Be * sizeof(int)));
     CK(cudaMalloc(&t.dOvRow, (size_t)e->Be * sizeof(int)));
-    CK(cudaFuncSetAttribute(k_topk_fp32, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)topk_fp32_smem_bytes()));
-    if (cudaFuncSetAttribute(k_topk_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
+    CK(cudaFuncSetAttribute(k_topk_fp32<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)topk_fp32_smem_bytes()));
+    CK(cudaFuncSetAttribute(k_topk_fp32<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)topk_fp32_smem_bytes()));
+    if (cudaFuncSetAttribute(k_topk_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
+    if (cudaFuncSetAttribute(k_topk_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
     e->topk = new TopkCtx(t);
   }
   *out = static_cast<TopkCtx*>(e->topk);
   return G4R_OK;
 }
 
-extern "C" int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
-                                int32_t* out_items, float* out_scores) {
+extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
+                                         const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
+                                         int32_t* out_items, float* out_scores) {
   if (!h || !X || !out_items || !out_scores) return G4R_ERR_INVALID;
   const int I = h->md.n_items;
-  if (k < 1 || k > I || k > G4R_TOPK_MAX) FAIL(G4R_ERR_INVALID, "k must be in 1 .. min(n_items, G4R_TOPK_MAX)");
+  // candidates: a bitmap of the distinct items (the cache key of the device copy)
+  std::vector<uint32_t> cmask;
+  int n_distinct = I;
+  if (cand) {
+    if (n_cand < 0) FAIL(G4R_ERR_INVALID, "n_cand must be >= 0");
+    cmask.assign((size_t)(I + 31) / 32, 0u);
+    for (int64_t i = 0; i < n_cand; i++) {
+      const int32_t c = cand[i];
+      if (c < 0 || c >= I) FAIL(G4R_ERR_INDEX, "candidate item out of bounds");
+      cmask[(size_t)c >> 5] |= 1u << (c & 31);
+    }
+    n_distinct = 0;
+    for (const uint32_t w : cmask) n_distinct += __builtin_popcount(w);
+  }
+  if (k < 1 || k > n_distinct || k > G4R_TOPK_MAX)
+    FAIL(G4R_ERR_INVALID, cand ? "k must be in 1 .. min(distinct candidates, G4R_TOPK_MAX)" : "k must be in 1 .. min(n_items, G4R_TOPK_MAX)");
   if (h->shard) FAIL(G4R_ERR_STATE, "g4r_predict_topk: not available on a row-sharded multi-GPU handle");
+  const bool use_cand = cand && n_distinct < I;          // every item a candidate: the unfiltered catalogue
+  // exclusions: per lane sorted and distinct, restricted to the candidates (no other item can win anyway)
+  std::vector<int> ex_off, ex;
+  int max_ex = 0;
+  if (excl_off) {
+    if (batch <= 0) FAIL(G4R_ERR_INVALID, "predict batch exceeds eval_batch_size");
+    if (excl_off[0] != 0) FAIL(G4R_ERR_INVALID, "excl_off[0] must be 0");
+    for (int b = 0; b < batch; b++) if (excl_off[b + 1] < excl_off[b]) FAIL(G4R_ERR_INVALID, "excl_off must be non-decreasing");
+    if (excl_off[batch] > 0 && !excl_items) FAIL(G4R_ERR_INVALID, "excl_items is NULL");
+    ex_off.assign((size_t)batch + 1, 0);
+    for (int b = 0; b < batch; b++) {
+      const size_t e0 = ex.size();
+      for (int64_t j = excl_off[b]; j < excl_off[b + 1]; j++) {
+        const int32_t v = excl_items[j];
+        if (v < 0 || v >= I) FAIL(G4R_ERR_INDEX, "excluded item out of bounds");
+        if (!use_cand || ((cmask[(size_t)v >> 5] >> (v & 31)) & 1u)) ex.push_back(v);
+      }
+      std::sort(ex.begin() + e0, ex.end());
+      ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
+      if (ex.size() > (size_t)INT32_MAX) FAIL(G4R_ERR_INVALID, "too many exclusions");
+      ex_off[(size_t)b + 1] = (int)ex.size();
+      max_ex = std::max(max_ex, (int)(ex.size() - e0));
+    }
+  }
+  const bool use_ex = !ex.empty();
   cudaSetDevice(h->cfg.device);
   EvalCtx* e = nullptr;
   int rc = eval_ctx(h, &e);
@@ -454,14 +588,41 @@ extern "C" int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, 
   if (rc) return rc;
   cudaStream_t st = h->stream;
   const int Be = e->Be, L = h->md.L;
-  const int P = std::min(I, std::max(k, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
-  const int C = std::min(I, 16 * k + TOPK_SURV_BASE);
+  if (use_cand && t->hMask != cmask) {                    // a candidate set other than the cached one
+    t->hMask.clear();
+    std::vector<int> list;
+    list.reserve((size_t)n_distinct);
+    for (int i = 0; i < I; i++) if ((cmask[(size_t)i >> 5] >> (i & 31)) & 1u) list.push_back(i);
+    CK(topk_grow(&t->dMask, &t->mask_cap, cmask.size()));
+    CK(topk_grow(&t->dCand, &t->cand_cap, list.size()));
+    CK(cudaMemcpyAsync(t->dMask, cmask.data(), cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(t->dCand, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    t->hMask.swap(cmask);
+  }
+  if (use_ex) {
+    CK(topk_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
+    CK(topk_grow(&t->dEx, &t->ex_cap, ex.size()));
+    CK(cudaMemcpyAsync(t->dExOff, ex_off.data(), ex_off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(t->dEx, ex.data(), ex.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  }
+  const unsigned int* dmask = use_cand ? t->dMask : nullptr;
+  const int* dcand = use_cand ? t->dCand : nullptr;
+  const int* dexoff = use_ex ? t->dExOff : nullptr;
+  const int* dex = use_ex ? t->dEx : nullptr;
+  // the prefix is the first P candidates; P covers k eligible items of every lane, or every candidate (then it is the survivor
+  // set and no tile runs)
+  const int n_comp = use_cand ? n_distinct : I;
+  const int P = std::min(n_comp, std::max(k + max_ex, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
+  const bool no_tile = (use_cand || use_ex) && P == n_comp;
+  const int C = std::min(n_comp, 16 * k + TOPK_SURV_BASE);
   // tile kind: the rule of g4r_eval_schedule (cfg.eval_tc 1 = fp32 FFMA tiles, 2 = wgmma tiles, 0 = wgmma for >= 64 lanes and
-  // >= 2048 items, where the split table is amortised over enough lanes)
-  const bool tc = h->cfg.eval_tc == 2 || (h->cfg.eval_tc == 0 && batch >= 64 && I >= 2048);
+  // >= 2048 items, where the split table is amortised over enough lanes).  The wgmma tiles cover the whole catalogue whatever
+  // the candidates, so the automatic choice also asks for at least a quarter of the catalogue as candidates.
+  const bool tc = !no_tile && (h->cfg.eval_tc == 2 || (h->cfg.eval_tc == 0 && batch >= 64 && n_comp >= 2048 && 4 * (int64_t)n_comp >= I));
   const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
-  const int n_part = tc ? 2 * tc_tiles : (I + EV_IT - 1) / EV_IT;
-  if (t->iota_n < P) {
+  const int n_part = no_tile ? 0 : tc ? 2 * tc_tiles : (n_comp + EV_IT - 1) / EV_IT;
+  if (!use_cand && t->iota_n < P) {
     if (t->dIota) cudaFree(t->dIota);
     t->dIota = nullptr; t->iota_n = 0;
     CK(cudaMalloc(&t->dIota, (size_t)P * sizeof(int)));
@@ -469,9 +630,11 @@ extern "C" int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, 
     t->iota_n = P;
   }
   CK(topk_grow(&t->dPre, &t->pre_cap, (size_t)batch * P));
-  CK(topk_grow(&t->dSurv, &t->surv_cap, (size_t)batch * C));
-  CK(topk_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)batch * C));
-  CK(topk_grow(&t->dPart, &t->part_cap, (size_t)batch * n_part));
+  if (!no_tile) {
+    CK(topk_grow(&t->dSurv, &t->surv_cap, (size_t)batch * C));
+    CK(topk_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)batch * C));
+    CK(topk_grow(&t->dPart, &t->part_cap, (size_t)batch * n_part));
+  }
   CK(topk_grow(&t->dItems, &t->items_cap, (size_t)batch * k));
   CK(topk_grow(&t->dScores, &t->scores_cap, (size_t)batch * k));
   if (tc && (!t->dBsplit || t->split_version != h->wy_version)) {        // the cached item-table split is stale
@@ -483,43 +646,57 @@ extern "C" int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, 
     t->split_version = h->wy_version;
   }
   eval_forward(h, e, 0);
-  // 1. exact fp32 scores of the prefix [0, P) (the predict kernel over the item list 0 .. P-1) and tau_b
-  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, t->dIota, P);
-  // delta_b = (||y_b||_1 max|Wy| + max|By|) (L + 3) 2^-18: four times the worst case of |3xTF32 - fp32| (DESIGN §3d)
-  k_topk_tau<<<batch, TOPK_THREADS, 0, st>>>(e->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18));
-  CK(cudaMemsetAsync(t->dCnt, 0, (size_t)batch * sizeof(int), st));
-  // 2. the catalogue in tiles: survivors and softmax partials
-  if (tc) {
-    if (!t->dAsplit) CK(cudaMalloc(&t->dAsplit, (size_t)((Be + TC_M - 1) / TC_M) * tc_chunks * 2 * TC_A_BYTES));
-    k_tc_split<TC_M><<<dim3((batch + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(h->md.layer[h->md.n_layers - 1].y, batch, h->md.ldL, L, t->dAsplit, tc_chunks, nullptr, 1.0f);
-    k_topk_tc<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part, t->dAsplit, t->dBsplit);
-    h->launches += 2;
-  } else {
-    k_topk_fp32<<<(I + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part);
+  // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the item list 0 .. P-1) and tau_b
+  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, use_cand ? dcand : t->dIota, P);
+  h->launches++;
+  int n_ov = 0;
+  if (!no_tile) {
+    // delta_b = (||y_b||_1 max|Wy| + max|By|) (L + 3) 2^-18: four times the worst case of |3xTF32 - fp32| (DESIGN §3d)
+    (use_cand || use_ex ? k_topk_tau<true> : k_topk_tau<false>)<<<batch, TOPK_THREADS, 0, st>>>(e->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18), dcand, dexoff, dex);
+    CK(cudaMemsetAsync(t->dCnt, 0, (size_t)batch * sizeof(int), st));
+    // 2. the candidates in tiles: survivors and softmax partials
+    if (tc) {
+      if (!t->dAsplit) CK(cudaMalloc(&t->dAsplit, (size_t)((Be + TC_M - 1) / TC_M) * tc_chunks * 2 * TC_A_BYTES));
+      k_tc_split<TC_M><<<dim3((batch + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(h->md.layer[h->md.n_layers - 1].y, batch, h->md.ldL, L, t->dAsplit, tc_chunks, nullptr, 1.0f);
+      auto kern = (use_cand || use_ex) ? k_topk_tc<true> : k_topk_tc<false>;
+      kern<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part, t->dAsplit, t->dBsplit,
+                                                                            dmask, dexoff, dex);
+      h->launches += 2;
+    } else {
+      auto kern = (use_cand || use_ex) ? k_topk_fp32<true> : k_topk_fp32<false>;
+      kern<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part,
+                                                                                    dcand, n_comp, dexoff, dex);
+      h->launches++;
+    }
     h->launches++;
+    CK(cudaGetLastError());
+    // 3. overflowed lanes (more survivors than their list holds) take their whole fp32 row, in g4r_predict's score buffer
+    std::vector<int> cnt((size_t)batch), ov_row((size_t)batch, -1), ov_list;
+    CK(cudaMemcpyAsync(cnt.data(), t->dCnt, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int b = 0; b < batch; b++) if (cnt[(size_t)b] > C) { ov_row[(size_t)b] = (int)ov_list.size(); ov_list.push_back(b); }
+    n_ov = (int)ov_list.size();
+    if (n_ov > 0) {
+      const size_t need = (size_t)n_ov * I;
+      if (e->out_cap < need) { if (e->dOut) cudaFree(e->dOut); e->dOut = nullptr; e->out_cap = 0; CK(cudaMalloc(&e->dOut, need * sizeof(float))); e->out_cap = need; }
+      CK(cudaMemcpyAsync(t->dOvList, ov_list.data(), (size_t)n_ov * sizeof(int), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(t->dOvRow, ov_row.data(), (size_t)batch * sizeof(int), cudaMemcpyHostToDevice, st));
+      k_topk_rows<<<dim3((I + 127) / 128, n_ov), 128, 0, st>>>(e->slot, t->dOvList, e->dOut);
+      h->launches++;
+    }
   }
-  h->launches += 2;
-  CK(cudaGetLastError());
-  // 3. overflowed lanes (more survivors than their list holds) take their whole fp32 row, in g4r_predict's score buffer
-  std::vector<int> cnt((size_t)batch), ov_row((size_t)batch, -1), ov_list;
-  CK(cudaMemcpyAsync(cnt.data(), t->dCnt, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  for (int b = 0; b < batch; b++) if (cnt[(size_t)b] > C) { ov_row[(size_t)b] = (int)ov_list.size(); ov_list.push_back(b); }
-  const int n_ov = (int)ov_list.size();
-  if (n_ov > 0) {
-    const size_t need = (size_t)n_ov * I;
-    if (e->out_cap < need) { if (e->dOut) cudaFree(e->dOut); e->dOut = nullptr; e->out_cap = 0; CK(cudaMalloc(&e->dOut, need * sizeof(float))); e->out_cap = need; }
-    CK(cudaMemcpyAsync(t->dOvList, ov_list.data(), (size_t)n_ov * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(t->dOvRow, ov_row.data(), (size_t)batch * sizeof(int), cudaMemcpyHostToDevice, st));
-    k_topk_rows<<<dim3((I + 127) / 128, n_ov), 128, 0, st>>>(e->slot, t->dOvList, e->dOut);
-    h->launches++;
-  }
-  k_topk_final<<<batch, TOPK_THREADS, 0, st>>>(e->slot, k, t->dCnt, t->dSurv, t->dSurvPre, C, n_ov > 0 ? t->dOvRow : nullptr, e->dOut, t->dPart, n_part,
-                                               t->dItems, t->dScores);
+  // select: from the survivors (or a fallback row), or from the prefix when it holds every candidate
+  (use_cand || use_ex ? k_topk_final<true> : k_topk_final<false>)<<<batch, TOPK_THREADS, 0, st>>>(e->slot, k, no_tile ? nullptr : t->dCnt, t->dSurv, t->dSurvPre, C, n_ov > 0 ? t->dOvRow : nullptr, e->dOut,
+                                               t->dPart, n_part, t->dItems, t->dScores, dcand, t->dPre, P, dmask, dexoff, dex);
   h->launches++;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out_items, t->dItems, (size_t)batch * k * sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(out_scores, t->dScores, (size_t)batch * k * sizeof(float), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return G4R_OK;
+}
+
+extern "C" int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
+                                int32_t* out_items, float* out_scores) {
+  return g4r_predict_topk_filtered(h, X, batch, reset_mask, k, nullptr, 0, nullptr, nullptr, out_items, out_scores);
 }

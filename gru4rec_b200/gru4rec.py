@@ -518,34 +518,79 @@ class GRU4Rec:
             return pd.DataFrame(data=preds, index=predict_for_item_ids)
         return pd.DataFrame(data=preds, index=self.itemidmap.index)
 
-    def recommend_next_batch(self, session_ids, input_item_ids, k=20, batch=100):
+    def recommend_next_batch(self, session_ids, input_item_ids, k=20, batch=100, items=None, exclude=None, exclude_seen=False):
         '''
         The k best next items of every event of the batch, ranked on the device (an addition to the reference's surface).
         Shares predict_next_batch's per-lane session state, so the two methods can be called alternately.
         Returns (item_ids [batch, k] of the original item IDs, scores [batch, k] float32), best first.  Order: the score
         (the pre-activation score for softmax / softmax_logit), then the earlier item of the catalogue; the scores are the
         values predict_next_batch returns for those items.
+
+        Filters, applied on the device:
+          items         original item IDs: only these compete (as predict_for_item_ids; unknown IDs raise KeyError, duplicates
+                        are ignored; softmax scores are normalised over them); k must not exceed their number
+          exclude       one iterable of original item IDs (or None) per lane, never recommended to that lane (unknown IDs
+                        are ignored)
+          exclude_seen  also exclude every item fed into the lane since its session began, this call's input included
+        With a filter, a lane with fewer than k eligible items is padded with item None and score NaN (the ID array is then
+        of object dtype).
         '''
         if self.error_during_train: raise Exception
         k = _lib.check_topk(k, self.n_items)
+        cand = None
+        if items is not None:
+            cand = self.itemidmap[items].values
+            n_cand = len(np.unique(cand))
+            if k > n_cand:
+                raise ValueError('k = %d exceeds the %d distinct candidate items' % (k, n_cand))
+        if exclude is not None and len(exclude) != batch:
+            raise ValueError('exclude must hold one entry per lane (%d), got %d' % (batch, len(exclude)))
         eng, reset, in_idxs = self._next_batch_inputs(session_ids, input_item_ids, batch)
-        items, scores = eng.predict_topk(in_idxs, k, reset.astype(np.uint8))
-        return self.itemidmap.index.to_numpy()[items], scores
+        if cand is None and exclude is None and not exclude_seen:
+            out, scores = eng.predict_topk(in_idxs, k, reset.astype(np.uint8))
+            return self.itemidmap.index.to_numpy()[out], scores
+        excl = [self._item_indices(e) for e in exclude] if exclude is not None else [np.zeros(0, np.int64)] * batch
+        if exclude_seen:
+            excl = [np.concatenate([e, self._seen[b, :self._seen_n[b]]]) for b, e in enumerate(excl)]
+        out, scores = eng.predict_topk(in_idxs, k, reset.astype(np.uint8), items=cand, exclude=excl)
+        ids = self.itemidmap.index.to_numpy()
+        miss = out < 0
+        if not miss.any():
+            return ids[out], scores
+        res = ids[np.where(miss, 0, out)].astype(object)
+        res[miss] = None
+        return res, scores
+
+    def _item_indices(self, item_ids):
+        '''item indices of the known IDs among item_ids (unknown IDs are dropped)'''
+        if item_ids is None:
+            return np.zeros(0, np.int64)
+        pos = self.itemidmap.index.get_indexer(pd.Index(list(item_ids)))
+        return self.itemidmap.values[pos[pos >= 0]].astype(np.int64)
 
     def _next_batch_inputs(self, session_ids, input_item_ids, batch):
         '''session bookkeeping of predict_next_batch / recommend_next_batch: the hidden state of a lane is
-        kept while its session id stays the same and zeroed when it changes or the batch size changes'''
+        kept while its session id stays the same and zeroed when it changes or the batch size changes.  The items fed
+        into each lane since its session began are kept alongside (_seen [batch, cap] + _seen_n, for exclude_seen) and
+        cleared at the same points.'''
         eng = self._ensure_engine(batch)
         if getattr(self, 'predict', None) is None or self.predict_batch != batch:
             self.predict_batch = batch
             eng.reset_eval_hidden()
             self.current_session = np.ones(batch) * -1
             self.predict = True
+            self._seen = np.zeros((batch, 8), dtype=np.int64)
+            self._seen_n = np.zeros(batch, dtype=np.int64)
         session_ids = np.asarray(session_ids)
         reset = (session_ids != self.current_session)
         if reset.any():
             self.current_session = session_ids.copy()
         in_idxs = self.itemidmap[input_item_ids].values
+        self._seen_n[reset] = 0
+        if self._seen_n.max() >= self._seen.shape[1]:          # grow by doubling
+            self._seen = np.concatenate([self._seen, np.zeros_like(self._seen)], axis=1)
+        self._seen[np.arange(batch), self._seen_n] = in_idxs
+        self._seen_n += 1
         return eng, reset, in_idxs
 
     # ---- persistence (gru4rec.py:742-781): pickle of the object with NumPy parameters ----
@@ -570,7 +615,8 @@ class GRU4Rec:
                                              'top1-max': 'top1_max', 'xe_logit': 'cross_entropy_logits'}[self.loss])
         st['final_activation'] = self._act_object(self.final_act)
         st['hidden_activation'] = self._act_object(self.hidden_act)
-        for k in ('device', 'dropout_seed', 'eval_lanes', 'step_mode', '_engine_eval_lanes', 'predict', 'predict_batch', 'current_session'):
+        for k in ('device', 'dropout_seed', 'eval_lanes', 'step_mode', '_engine_eval_lanes', 'predict', 'predict_batch', 'current_session',
+                  '_seen', '_seen_n'):
             st.pop(k, None)
         st['predict'] = None
         return st

@@ -213,6 +213,16 @@ int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* r
  * G4R_ERR_INVALID unless 1 <= k <= min(n_items, G4R_TOPK_MAX); G4R_ERR_INDEX on an out-of-range item. */
 int g4r_predict_topk(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
                      int32_t* out_items, float* out_scores);
+/* g4r_predict_topk with filters (DESIGN §3d).  Only the distinct items of cand[0 .. n_cand) compete (cand == NULL: the whole
+ * catalogue; duplicates ignored); lane b never receives items excl_items[excl_off[b] .. excl_off[b+1]) (excl_off == NULL: no
+ * exclusions; lists need not be sorted, duplicates allowed).  Ranking key, tie rule and scores as g4r_predict_topk, except that
+ * the softmax / softmax_logit normaliser runs over the distinct candidates; exclusions never change a score.  Slots past a
+ * lane's eligible items: item -1, score NaN.  G4R_ERR_INVALID unless 1 <= k <= min(distinct candidates, G4R_TOPK_MAX) and
+ * excl_off is non-decreasing from 0; G4R_ERR_INDEX on an out-of-range item.  Any error leaves the hidden state untouched.
+ * The candidate set is kept on the device between calls and re-uploaded only when its content changes. */
+int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
+                              const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
+                              int32_t* out_items, float* out_scores);
 /* Zero the scoring-path hidden state (gru4rec.py:696-697). */
 int g4r_reset_eval_hidden(g4r_handle* h);
 
