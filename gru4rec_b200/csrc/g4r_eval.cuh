@@ -20,13 +20,9 @@ __device__ __forceinline__ float tie_noise(unsigned int seed, int s, int b, unsi
   return (float)(mix32(k + col) >> 8) * (1.0f / 16777216.0f) * 1e-10f;
 }
 
-// target score of every lane, computed with the same sequential k order as the tile kernel (bitwise equal)
-__global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, int* cnt, unsigned int tie, int subset_mode, int lohi_stride) {
-  const ModelDev& md = MD;
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  const int M = md.wM[s];
-  if (b >= M) return;
-  const int item = md.wY[(size_t)s * md.B + b];
+// fp32 score y_b . Wy[item] + By[item] of one (lane, item): the sequential k order of the tile loop (ev_tiles), so bitwise equal
+// to the tile's score
+__device__ __forceinline__ float ev_score_fp32(const ModelDev& md, int b, int item) {
   const float* yr = md.layer[md.n_layers - 1].y + (size_t)b * md.ldL;
   const float* wr = md.Wy + (size_t)item * md.ldL;
   float a = 0.f;
@@ -35,33 +31,22 @@ __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, i
     const float4 y = ld4(yr + c4 * 4), w = ld4(wr + c4 * 4);
     a = fmaf(y.x, w.x, a); a = fmaf(y.y, w.y, a); a = fmaf(y.z, w.z, a); a = fmaf(y.w, w.w, a);
   }
-  float sc = a + md.By[item];
-  const float pre = sc;
-  if (md.fact.kind <= G4R_ACT_SELU) sc = act_fwd(md.fact, sc);
-  if (lohi_stride > 0) {      // tensor-core ranking: the two pre-activation thresholds of this lane (g4r_eval_tc.cuh)
-    float lo, hi;
-    tc_thresholds(md.fact, md.fact.kind <= G4R_ACT_SELU, sc, pre, lo, hi);
-    tgt[lohi_stride + b] = lo; tgt[2 * lohi_stride + b] = hi;
-  }
-  if (tie) sc += tie_noise(tie, s, b, subset_mode ? 0x40000000U + (unsigned int)b : (unsigned int)item);
-  tgt[b] = sc;
-  cnt[b * 2 + 0] = 0; cnt[b * 2 + 1] = 0;
+  return a + md.By[item];
 }
 
-// `subset` (evaluate_gpu(items=...), evaluation.py:52-56): the competitors are the n_cand listed items instead of the catalogue
-template <bool WRITE>
-__global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, const float* __restrict__ tgt, int* cnt, float* out,
-                                                           const int* __restrict__ subset, int n_cand, unsigned int tie = 0u) {
-  const ModelDev& md = MD;
-  extern __shared__ __align__(16) float smem[];
+// item at position pos of a tile sweep over `subset` (nullptr: item pos)
+__device__ __forceinline__ int ev_item(const int* __restrict__ subset, int pos) { return subset ? subset[pos] : pos; }
+
+// fp32 FFMA tiles (k_eval_score, k_topk_fp32): the CTA scores positions i0 .. i0 + ni - 1 (item ev_item(subset, pos)) against
+// every lane, in row blocks of EV_TB lanes.  Lane l of warp w accumulates lane b0 + l x position i0 + w + 8 q in acc[q], one
+// sequential fma chain over k.  The Wy rows are staged once when ldL <= EV_KT, else per EV_KT-column slab together with Y.
+// smem: [EV_TB][EV_LDS] Y, then [EV_IT][EV_LDS] Wy rows (EV_TILE_FLOATS).  epi(b0, acc): after every row block, on every thread.
+constexpr int EV_TILE_FLOATS = (EV_TB + EV_IT) * EV_LDS;
+template <class Epi>
+__device__ __forceinline__ void ev_tiles(const ModelDev& md, float* smem, int M, int i0, int ni, const int* __restrict__ subset, Epi&& epi) {
   float* sY = smem;                        // [EV_TB][EV_LDS]
   float* sW = sY + EV_TB * EV_LDS;         // [EV_IT][EV_LDS]
-  int* sCnt = reinterpret_cast<int*>(sW + EV_IT * EV_LDS);   // [EV_TB][2]
-  const int M = md.wM[s];
-  const int I = subset ? n_cand : md.n_items, ldL = md.ldL;
-  const int i0 = blockIdx.x * EV_IT;
-  const int ni = min(EV_IT, I - i0);
-  auto item_of = [&](int pos) -> int { return subset ? subset[pos] : pos; };
+  const int ldL = md.ldL;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* Y = md.layer[md.n_layers - 1].y;
   const bool hoist = ldL <= EV_KT;
@@ -70,7 +55,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
     for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
       const int rr = i / kw, c4 = i % kw;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (rr < ni) v = ld4(md.Wy + (size_t)item_of(i0 + rr) * ldL + c4 * 4);
+      if (rr < ni) v = ld4(md.Wy + (size_t)ev_item(subset, i0 + rr) * ldL + c4 * 4);
       st4(sW + rr * EV_LDS + c4 * 4, v);
     }
   }
@@ -78,7 +63,6 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
     float acc[8];
 #pragma unroll
     for (int q = 0; q < 8; q++) acc[q] = 0.f;
-    if (tid < EV_TB * 2) sCnt[tid] = 0;
     for (int k0 = 0; k0 < ldL; k0 += EV_KT) {
       const int kw = min(EV_KT, ldL - k0) / 4;
       __syncthreads();
@@ -92,7 +76,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
         for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
           const int rr = i / kw, c4 = i % kw;
           float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (rr < ni) v = ld4(md.Wy + (size_t)item_of(i0 + rr) * ldL + k0 + c4 * 4);
+          if (rr < ni) v = ld4(md.Wy + (size_t)ev_item(subset, i0 + rr) * ldL + k0 + c4 * 4);
           st4(sW + rr * EV_LDS + c4 * 4, v);
         }
       }
@@ -107,16 +91,56 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
         }
       }
     }
+    epi(b0, acc);
+  }
+}
+
+// target score of every lane, computed with the same sequential k order as the tile kernel (bitwise equal)
+__global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, int* cnt, unsigned int tie, int subset_mode, int lohi_stride) {
+  const ModelDev& md = MD;
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  const int M = md.wM[s];
+  if (b >= M) return;
+  const int item = md.wY[(size_t)s * md.B + b];
+  float sc = ev_score_fp32(md, b, item);
+  const float pre = sc;
+  if (md.fact.kind <= G4R_ACT_SELU) sc = act_fwd(md.fact, sc);
+  if (lohi_stride > 0) {      // tensor-core ranking: the two pre-activation thresholds of this lane (g4r_eval_tc.cuh)
+    float lo, hi;
+    tc_thresholds(md.fact, md.fact.kind <= G4R_ACT_SELU, sc, pre, lo, hi);
+    tgt[lohi_stride + b] = lo; tgt[2 * lohi_stride + b] = hi;
+  }
+  if (tie) sc += tie_noise(tie, s, b, subset_mode ? 0x40000000U + (unsigned int)b : (unsigned int)item);
+  tgt[b] = sc;
+  cnt[b * 2 + 0] = 0; cnt[b * 2 + 1] = 0;
+}
+
+// Competitors: `subset` (evaluate_gpu(items=...), evaluation.py:52-56) lists the n_cand items that compete instead of the catalogue;
+// without a subset, n_cand > 0 scores the leading items 0 .. n_cand - 1 and 0 the catalogue.  WRITE: out[b * n_comp + pos] = score.
+template <bool WRITE>
+__global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, const float* __restrict__ tgt, int* cnt, float* out,
+                                                           const int* __restrict__ subset, int n_cand, unsigned int tie = 0u) {
+  const ModelDev& md = MD;
+  extern __shared__ __align__(16) float smem[];
+  int* sCnt = reinterpret_cast<int*>(smem + EV_TILE_FLOATS);   // [EV_TB][2]
+  const int M = md.wM[s];
+  const int I = n_cand > 0 ? n_cand : md.n_items;
+  const int i0 = blockIdx.x * EV_IT;
+  const int ni = min(EV_IT, I - i0);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid < EV_TB * 2) sCnt[tid] = 0;
+  ev_tiles(md, smem, M, i0, ni, subset, [&](int b0, const float (&acc)[8]) {
     const int b = b0 + lane;
     if (b < M) {
       int gt = 0, eq = 0;
       const float t = WRITE ? 0.f : tgt[b];
+      float* orow = WRITE ? out + (size_t)b * I + i0 + warp : nullptr;   // one row pointer keeps the kernel free of spills
 #pragma unroll
       for (int q = 0; q < 8; q++) {
         const int it = i0 + warp + 8 * q;
         if (warp + 8 * q < ni) {
-          float sc = acc[q] + md.By[item_of(it)];
-          if (WRITE) out[(size_t)b * I + it] = sc;
+          float sc = acc[q] + md.By[ev_item(subset, it)];
+          if (WRITE) orow[8 * q] = sc;
           else {
             if (md.fact.kind <= G4R_ACT_SELU) sc = act_fwd(md.fact, sc);
             if (tie) sc += tie_noise(tie, s, b, (unsigned int)it);
@@ -127,13 +151,14 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
       if (!WRITE) { if (gt) atomicAdd(&sCnt[lane * 2], gt); if (eq) atomicAdd(&sCnt[lane * 2 + 1], eq); }
     }
     __syncthreads();
-    if (!WRITE && tid < EV_TB * 2) {
+    if (!WRITE && tid < EV_TB * 2) {             // flush and clear for the next row block (the tile loop syncs before its epilogue)
       const int bb = b0 + tid / 2;
       if (bb < M && sCnt[tid]) atomicAdd(&cnt[bb * 2 + (tid & 1)], sCnt[tid]);
+      sCnt[tid] = 0;
     }
-  }
+  });
 }
-static size_t eval_smem_bytes() { return (size_t)(EV_TB * EV_LDS + EV_IT * EV_LDS) * sizeof(float) + EV_TB * 2 * sizeof(int) + 64; }
+static size_t eval_smem_bytes() { return (size_t)EV_TILE_FLOATS * sizeof(float) + EV_TB * 2 * sizeof(int) + 64; }
 
 // ranks + per-cutoff sums (evaluation.py:60-75), accumulated in double on the device
 __global__ void __launch_bounds__(256) k_eval_rank(int slot, int s, const int* cnt, const int* cut, int n_cut, int mode, double* sums) {
@@ -204,10 +229,45 @@ struct EvalCtx {
   int cap = 0;
   int slot = -1;
   int* dCand = nullptr; int n_cand = 0; size_t cand_cap = 0;     // candidate subset of evaluate_gpu(items=...), item indices
-  unsigned char *dAsplit = nullptr, *dBsplit = nullptr;           // tensor-core path: hi / lo TF32 operand blocks (g4r_eval_tc.cuh)
+  // wgmma tiles (g4r_eval_tc.cuh): [hi | lo] TF32 operand blocks of the hidden states (per call) and of the item table, which
+  // is kept between calls and tagged with the handle's wy_version it was made from
+  unsigned char *dAsplit = nullptr, *dBsplit = nullptr;
+  uint64_t split_version = ~0ull;
   void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
 };
 static void topk_release(EvalCtx& e);
+
+// device buffer of at least n elements (contents not kept)
+template <class T>
+static cudaError_t dev_grow(T** p, size_t* cap, size_t n) {
+  if (*cap >= n && *p) return cudaSuccess;
+  if (*p) cudaFree(*p);
+  *p = nullptr; *cap = 0;
+  const cudaError_t r = cudaMalloc(p, n * sizeof(T));
+  if (r == cudaSuccess) *cap = n;
+  return r;
+}
+
+// Tile kind of a scoring call of `lanes` lanes against n_comp competing items: cfg.eval_tc 1 = fp32 FFMA tiles, 2 = wgmma
+// 3xTF32 tiles, 0 = wgmma from 64 lanes and 2048 competitors on (the split item table is amortised over enough lanes; at one lane
+// it is twice the bytes of Wy) and only when the competitors are at least a quarter of the catalogue (the wgmma tiles cover the
+// whole catalogue)
+static bool wgmma_tiles(const g4r_config& cfg, int lanes, int n_comp, int n_items) {
+  return cfg.eval_tc == 2 || (cfg.eval_tc == 0 && lanes >= 64 && n_comp >= 2048 && 4 * (int64_t)n_comp >= n_items);
+}
+
+// operand buffers of the wgmma tiles, and the item-table split made again only if Wy / By may have changed since (wy_version)
+static int tc_operands(g4r_handle* h, EvalCtx* e) {
+  const int chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tiles = (h->md.n_items + TC_N - 1) / TC_N;   // + the bias column
+  if (!e->dAsplit) CK(cudaMalloc(&e->dAsplit, (size_t)((e->Be + TC_M - 1) / TC_M) * chunks * 2 * TC_A_BYTES));   // blocks of 128 lanes
+  if (!e->dBsplit) CK(cudaMalloc(&e->dBsplit, (size_t)tiles * chunks * 2 * TC_B_BYTES));                         // blocks of 256 items
+  if (e->split_version != h->wy_version) {
+    k_tc_split<TC_N><<<dim3(tiles, chunks), 256, 0, h->stream>>>(h->md.Wy, h->md.n_items, h->md.ldL, h->md.L, e->dBsplit, chunks, h->md.By, 0.f);
+    h->launches++;
+    e->split_version = h->wy_version;
+  }
+  return G4R_OK;
+}
 
 static void eval_release(g4r_handle* h) {
   if (!h->eval_ctx) return;
@@ -275,16 +335,13 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
   for (int i = 0; i < h->md.n_layers; i++) CK(cudaMemsetAsync(h->He[i], 0, (size_t)Be * h->md.layer[i].ldL * sizeof(float), st));   // gru4rec.py:731-733
   CK(cudaMemcpyAsync(e->dCut, cut_off, n_cut * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(e->dSums, 0, 128 * sizeof(double), st));
-  // tensor-core scoring (full-catalogue ranking of a wide batch): the item table is split once per evaluation into hi / lo
-  // TF32 operand blocks; cfg.eval_tc: 1 forces the fp32 FFMA tiles, 2 forces the wgmma 3xTF32 tiles
-  const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC,      // + the bias column
-             tc_tiles = (I + TC_N - 1) / TC_N, tc_lblocks = (Be + TC_M - 1) / TC_M;
-  const bool tc_possible = e->n_cand == 0 && mode != 3 && h->cfg.eval_tc != 1 && (h->cfg.eval_tc == 2 || (Bs >= 64 && I >= 2048));
+  // wgmma tiles (full-catalogue ranking of a wide batch; candidate subsets and tiebreaking take the fp32 tiles): decided once
+  // with the schedule's batch, then per mini-batch with its lanes
+  const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;   // + the bias column
+  const bool tc_possible = e->n_cand == 0 && mode != 3 && wgmma_tiles(h->cfg, Bs, I, I);
   if (tc_possible) {
-    if (!e->dAsplit) CK(cudaMalloc(&e->dAsplit, (size_t)tc_lblocks * tc_chunks * 2 * TC_A_BYTES));     // hidden states: blocks of 128 lanes
-    if (!e->dBsplit) CK(cudaMalloc(&e->dBsplit, (size_t)tc_tiles * tc_chunks * 2 * TC_B_BYTES));       // item table: blocks of 256 items
-    k_tc_split<TC_N><<<dim3(tc_tiles, tc_chunks), 256, 0, st>>>(h->md.Wy, I, h->md.ldL, h->md.L, e->dBsplit, tc_chunks, h->md.By, 0.f);
-    h->launches++;
+    rc = tc_operands(h, e);
+    if (rc) return rc;
   }
   int64_t done = 0;
   while (done < s->n_steps) {
@@ -323,7 +380,7 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
       k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
       const int n_comp = e->n_cand > 0 ? e->n_cand : I;
       const int M_i = e->hM[i];
-      const bool tc = tc_possible && (h->cfg.eval_tc == 2 || M_i >= 64);
+      const bool tc = tc_possible && wgmma_tiles(h->cfg, M_i, I, I);
       if (tc) {
         k_tc_split<TC_M><<<dim3((M_i + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(h->md.layer[h->md.n_layers - 1].y, M_i, h->md.ldL, h->md.L, e->dAsplit, tc_chunks, nullptr, 1.0f);
         CK(cudaEventRecord(h->ts_ev[1], rk));
@@ -374,7 +431,7 @@ extern "C" int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n
     if (items[i] < 0 || items[i] >= h->md.n_items) FAIL(G4R_ERR_INDEX, "Index out of bounds");
     tmp[(size_t)i] = (int)items[i];
   }
-  if (e->cand_cap < (size_t)n) { if (e->dCand) cudaFree(e->dCand); e->dCand = nullptr; e->cand_cap = 0; CK(cudaMalloc(&e->dCand, (size_t)n * sizeof(int))); e->cand_cap = (size_t)n; }
+  CK(dev_grow(&e->dCand, &e->cand_cap, (size_t)n));
   CK(cudaMemcpyAsync(e->dCand, tmp.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   e->n_cand = (int)n;
@@ -414,7 +471,7 @@ extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const
   const int I = h->md.n_items;
   cudaStream_t st = h->stream;
   const size_t need = (size_t)batch * I;
-  if (e->out_cap < need) { if (e->dOut) cudaFree(e->dOut); CK(cudaMalloc(&e->dOut, need * sizeof(float))); e->out_cap = need; }
+  CK(dev_grow(&e->dOut, &e->out_cap, need));
   eval_forward(h, e, 0);
   k_eval_score<true><<<(I + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, e->dOut, nullptr, 0);
   k_predict_act<<<batch, 256, 0, st>>>(e->slot, e->dOut, batch);

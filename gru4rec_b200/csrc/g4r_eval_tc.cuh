@@ -13,7 +13,7 @@
 //
 // Structure (one CTA per SM, 512 threads = four warpgroups, persistent over its item tiles):
 //   pre-pass   k_tc_split writes the operands as hi / lo TF32 blocks in the K-major 128-byte-swizzle layout: the item table
-//              once per evaluation, the hidden states once per mini-batch; one extra K column carries the item bias (1.0 on the
+//              when Wy / By have changed (kept between calls), the hidden states once per mini-batch; one extra K column carries the item bias (1.0 on the
 //              hidden-state side), so the accumulator is the complete pre-activation score
 //   loads      thread 0: two bulk copies (cp.async.bulk -> mbarrier complete_tx) per 32-wide K chunk fill a 96 KB stage
 //              [A hi | A lo | B hi | B lo]; two stages, a stage is refilled once all four warpgroups have released it
@@ -123,7 +123,7 @@ __device__ __forceinline__ void wg_chunk_3xtf32(float (&d)[NR], uint32_t a_hi, u
   wg_fence_acc(d);
 }
 
-// Pre-split operand blocks in global memory (written once per evaluation for the item table, once per mini-batch for the hidden
+// Pre-split operand blocks in global memory (written for the item table whenever it has changed, once per mini-batch for the hidden
 // states): block (rb, c) = rows [rb * RB, +RB) x k [32 c, +32) as [hi | lo], each in the K-major 128-byte-swizzle layout
 // (tc_block_off).  The scoring kernel then feeds the tensor cores with plain bulk copies (TMA) -- no register staging on the
 // critical path.
@@ -194,19 +194,20 @@ __device__ __forceinline__ void tc_thresholds(const ActSpec a, bool elem_act, fl
   lo = tc_fkey_inv(r2);
 }
 
-// cnt[b*2 + 0] += #items with score > target score of lane b; cnt[b*2 + 1] += #items with score == target (the target itself
-// counts as one tie, exactly as in the fp32 kernel where its score equals the target score bit for bit).
-// Tile = 128 evaluation lanes x 256 items; warpgroup wg accumulates rows (wg & 1) * 64 .. + 63 x columns (wg >> 1) * 128 .. + 127 in
-// registers, so a thread holds two lanes x 32 items and counts them thread-locally.  Asplit: hidden-state blocks of 128 lanes,
-// Bsplit: item-table blocks of 256 items (k_tc_split).  Thread 0 also feeds the stages: it issues the bulk copies of a stage as
-// soon as all four warpgroups have finished the MMAs that read it.
-__global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, const float* __restrict__ tgt, int tgt_stride, int* cnt,
-                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit) {
+// The wgmma sweep of the scoring kernels (k_eval_tc, k_topk_tc): one persistent CTA per SM loops over (lane block of 128) x (its
+// item tiles of 256) x (32-wide K chunks).  Asplit: hidden-state blocks of 128 lanes, Bsplit: item-table blocks of 256 items
+// (k_tc_split), K = L + 1 with the bias column.  Warpgroup wg accumulates rows (wg & 1) * 64 .. + 63 x columns (wg >> 1) * 128
+// .. + 127 of the tile in registers, so a thread holds two lanes x 32 items.  Thread 0 also feeds the stages: it issues the bulk
+// copies of a stage as soon as all four warpgroups have finished the MMAs that read it.
+//   lane_block(b)      at the start of every lane block: b is the thread's first lane, b + 8 its second
+//   tile(d, c0, last)  after every tile: d[i] holds lane b + 8 * ((i / 2) % 2) x item c0 + 8 * (i / 4) + i % 2 (columns past the
+//                      catalogue included); last: the CTA's last tile of the lane block
+template <class LaneBlock, class Tile>
+__device__ __forceinline__ void tc_sweep(int M, int I, int K, const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit,
+                                         LaneBlock&& lane_block, Tile&& tile) {
   extern __shared__ __align__(1024) unsigned char tc_raw[];
   TcSmem& sm = *reinterpret_cast<TcSmem*>(tc_raw);
-  const ModelDev& md = MD;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-  const int M = md.wM[s], I = md.n_items, K = md.L + 1;        // + the bias column
   const int n_tiles = (I + TC_N - 1) / TC_N;         // item tiles
   const int n_lb = (M + TC_M - 1) / TC_M;            // lane blocks
   const int n_chunk = (K + TC_KC - 1) / TC_KC;
@@ -231,15 +232,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, cons
   const int rq = (warp & 3) * 16 + (lane >> 2);                 // first of the thread's two rows inside the warpgroup's 64
   unsigned int it = 0;
   for (int lb = 0; lb < n_lb; lb++) {
-    int bb[2], yit[2]; bool vrow[2]; float lo[2], hi[2];
-    int cgt[2] = {0, 0}, cge[2] = {0, 0};
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      bb[h] = lb * TC_M + wr + rq + 8 * h;
-      vrow[h] = bb[h] < M;
-      yit[h] = vrow[h] ? md.wY[(size_t)s * md.B + bb[h]] : -1;
-      lo[h] = vrow[h] ? tgt[tgt_stride + bb[h]] : INFINITY; hi[h] = vrow[h] ? tgt[2 * tgt_stride + bb[h]] : INFINITY;   // k_eval_tgt
-    }
+    lane_block(lb * TC_M + wr + rq);
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
       float d[64];
 #pragma unroll
@@ -254,35 +247,60 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, cons
         if (tid == 0 && it + TC_STAGES < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + TC_STAGES); }
         __syncwarp();
       }
-      // two compares per item against the lane's pre-activation thresholds; columns past the catalogue (last tile) do not count
-      const int c0 = t * TC_N + wc + 2 * (lane & 3);                // item of d[0]
-      const int n_live = I - c0;                                    // d[i] holds item c0 + 8 * (i / 4) + i % 2
+      tile(d, t * TC_N + wc + 2 * (lane & 3), t + (int)gridDim.x >= n_tiles);
+    }
+  }
+}
+
+// cnt[b*2 + 0] += #items with score > target score of lane b; cnt[b*2 + 1] += #items with score == target (the target itself
+// counts as one tie, exactly as in the fp32 kernel where its score equals the target score bit for bit).  Each thread counts its
+// two lanes x 32 items of a tile thread-locally; the four threads of a quad sum their counts after the lane block's last tile.
+__global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, const float* __restrict__ tgt, int tgt_stride, int* cnt,
+                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit) {
+  const ModelDev& md = MD;
+  const int M = md.wM[s], I = md.n_items, lane = threadIdx.x & 31;
+  int bb[2], yit[2]; bool vrow[2]; float lo[2], hi[2];
+  int cgt[2], cge[2];
+  auto lane_block = [&](int b) {
 #pragma unroll
-      for (int i = 0; i < 64; i++) {
-        const int h = (i >> 1) & 1;
-        const bool live = (i >> 2) * 8 + (i & 1) < n_live;
-        cgt[h] += (live && d[i] > hi[h]) ? 1 : 0;
-        cge[h] += (live && d[i] >= lo[h]) ? 1 : 0;
-      }
+    for (int h = 0; h < 2; h++) {
+      bb[h] = b + 8 * h;
+      vrow[h] = bb[h] < M;
+      yit[h] = vrow[h] ? md.wY[(size_t)s * md.B + bb[h]] : -1;
+      lo[h] = vrow[h] ? tgt[tgt_stride + bb[h]] : INFINITY; hi[h] = vrow[h] ? tgt[2 * tgt_stride + bb[h]] : INFINITY;   // k_eval_tgt
+      cgt[h] = 0; cge[h] = 0;
+    }
+  };
+  auto tile = [&](const float (&d)[64], int c0, bool last) {
+    // two compares per item against the lane's pre-activation thresholds; columns past the catalogue (last tile) do not count
+    const int n_live = I - c0;
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int rel = yit[h] - c0;                                 // the target's own column, if this thread holds it
-        if (rel >= 0 && rel < 128 && (rel & 7) < 2) {               // rare: take it back out, it counts as exactly one tie
-          float xs = 0.f;
-#pragma unroll
-          for (int i = 0; i < 64; i++) if (((i >> 1) & 1) == h && (i >> 2) * 8 + (i & 1) == rel) xs = d[i];
-          cgt[h] -= (xs > hi[h]) ? 1 : 0;
-          cge[h] -= (xs >= lo[h]) ? 1 : 0;
-          cge[h] += 1;                                               // == (self: not above) + one tie
-        }
-      }
+    for (int i = 0; i < 64; i++) {
+      const int h = (i >> 1) & 1;
+      const bool live = (i >> 2) * 8 + (i & 1) < n_live;
+      cgt[h] += (live && d[i] > hi[h]) ? 1 : 0;
+      cge[h] += (live && d[i] >= lo[h]) ? 1 : 0;
     }
 #pragma unroll
-    for (int h = 0; h < 2; h++) {                                    // the four threads of a quad share the two rows
-      int g = cgt[h], e = cge[h] - cgt[h];                           // lo <= x <= hi
+    for (int h = 0; h < 2; h++) {
+      const int rel = yit[h] - c0;                                 // the target's own column, if this thread holds it
+      if (rel >= 0 && rel < 128 && (rel & 7) < 2) {               // rare: take it back out, it counts as exactly one tie
+        float xs = 0.f;
+#pragma unroll
+        for (int i = 0; i < 64; i++) if (((i >> 1) & 1) == h && (i >> 2) * 8 + (i & 1) == rel) xs = d[i];
+        cgt[h] -= (xs > hi[h]) ? 1 : 0;
+        cge[h] -= (xs >= lo[h]) ? 1 : 0;
+        cge[h] += 1;                                               // == (self: not above) + one tie
+      }
+    }
+    if (!last) return;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {                                  // the four threads of a quad share the two rows
+      int g = cgt[h], e = cge[h] - cgt[h];                         // lo <= x <= hi
       g += __shfl_xor_sync(0xffffffffu, g, 1); g += __shfl_xor_sync(0xffffffffu, g, 2);
       e += __shfl_xor_sync(0xffffffffu, e, 1); e += __shfl_xor_sync(0xffffffffu, e, 2);
       if ((lane & 3) == 0 && vrow[h]) { if (g) atomicAdd(&cnt[bb[h] * 2], g); if (e) atomicAdd(&cnt[bb[h] * 2 + 1], e); }
     }
-  }
+  };
+  tc_sweep(M, I, md.L + 1, Asplit, Bsplit, lane_block, tile);
 }

@@ -1,5 +1,6 @@
 // g4r_topk.cuh -- predict_next_batch reduced on the device to the k best items of every lane (g4r_predict_topk, DESIGN §3d).
-// Included at the end of g4r_eval.cuh (uses EvalCtx, eval_forward, k_eval_score and the k_eval_tc pipeline pieces).
+// Included at the end of g4r_eval.cuh (uses EvalCtx and its operand split, eval_forward, k_eval_score, the tile loops ev_tiles /
+// tc_sweep and the score chain ev_score_fp32).
 //
 // Ranking key of item i in lane b: act(x) for the elementwise final activations, the pre-activation x = y_b . Wy[i] + By[i] for
 // softmax / softmax_logit; equal keys put the smaller index first.  Both are folded into one 64-bit key
@@ -7,7 +8,7 @@
 // so the order is total and the list unique.  The [lanes x items] score matrix is never written:
 //   1. tau       exact fp32 scores of a catalogue prefix (k_eval_score, the predict kernel) and, per lane, their k-th key tau_b:
 //                the k-th key of any subset bounds the k-th key of the catalogue from below
-//   2. filter    the catalogue in tiles -- fp32 FFMA tiles (the very fma chain of k_eval_score, so exact) or wgmma 3xTF32 tiles
+//   2. filter    the catalogue in tiles -- fp32 FFMA tiles (k_eval_score's tile loop, so exact) or wgmma 3xTF32 tiles
 //                (within delta_b of fp32) -- keeps an item only if its key can still reach tau_b and appends its index to the lane's
 //                survivor list; the softmax normaliser (max, sum of exp) is accumulated per tile on the way
 //   3. select    one CTA per lane rescores its survivors with the fp32 chain of k_eval_tgt, radix-selects the k-th key and sorts
@@ -24,10 +25,8 @@ constexpr int TOPK_PREFIX_MIN = 2048;      // items scored exactly for tau: max(
 constexpr int TOPK_SURV_BASE = 4096;       // survivor list of a lane: min(n_items, 16 k + 4096) item indices
 
 struct TopkCtx {
-  unsigned char *dAsplit = nullptr, *dBsplit = nullptr;   // hidden-state / item-table [hi | lo] TF32 blocks (k_tc_split)
-  uint64_t split_version = ~0ull;                         // handle's wy_version the item-table split was made from
-  unsigned int* dAbsMax = nullptr;                        // max |Wy|, max |By| as fp32 bits (with the split)
-  int* dIota = nullptr; int iota_n = 0;                   // 0, 1, 2, ...: the prefix as a k_eval_score item list
+  unsigned int* dAbsMax = nullptr;                        // max |Wy|, max |By| as fp32 bits
+  uint64_t absmax_version = ~0ull;                        // handle's wy_version they were taken from (as EvalCtx::split_version)
   float* dPre = nullptr; size_t pre_cap = 0;              // [batch x P] prefix pre-activations
   float* dTau = nullptr;                                  // [Be x 4] lo, hi, delta, tau item (int bits)
   int* dCnt = nullptr;                                    // [Be] survivors appended (may exceed the list)
@@ -47,22 +46,12 @@ struct TopkCtx {
 static void topk_release(EvalCtx& e) {
   if (!e.topk) return;
   TopkCtx& t = *static_cast<TopkCtx*>(e.topk);
-  for (void* p : {(void*)t.dAsplit, (void*)t.dBsplit, (void*)t.dAbsMax, (void*)t.dIota, (void*)t.dPre, (void*)t.dTau, (void*)t.dCnt, (void*)t.dSurv,
+  for (void* p : {(void*)t.dAbsMax, (void*)t.dPre, (void*)t.dTau, (void*)t.dCnt, (void*)t.dSurv,
                   (void*)t.dSurvPre, (void*)t.dPart, (void*)t.dOvList, (void*)t.dOvRow, (void*)t.dItems, (void*)t.dScores,
                   (void*)t.dMask, (void*)t.dCand, (void*)t.dExOff, (void*)t.dEx})
     if (p) cudaFree(p);
   delete static_cast<TopkCtx*>(e.topk);
   e.topk = nullptr;
-}
-
-template <class T>
-static cudaError_t topk_grow(T** p, size_t* cap, size_t n) {
-  if (*cap >= n && *p) return cudaSuccess;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  const cudaError_t r = cudaMalloc(p, n * sizeof(T));
-  if (r == cudaSuccess) *cap = n;
-  return r;
 }
 
 // -0 and +0 are the same key (the index decides between them)
@@ -72,21 +61,6 @@ __device__ __forceinline__ uint64_t topk_key(float kf, int item) {
 }
 __device__ __forceinline__ float topk_keyval(const ActSpec a, float pre) { return a.kind <= G4R_ACT_SELU ? act_fwd(a, pre) : pre; }
 
-// fp32 score of (lane b, item): the sequential fma chain of k_eval_tgt / k_eval_score (bitwise equal to g4r_predict's value)
-__device__ __forceinline__ float topk_score_fp32(const ModelDev& md, int b, int item) {
-  const float* yr = md.layer[md.n_layers - 1].y + (size_t)b * md.ldL;
-  const float* wr = md.Wy + (size_t)item * md.ldL;
-  float a = 0.f;
-#pragma unroll 8
-  for (int c4 = 0; c4 < md.ldL / 4; c4++) {
-    const float4 y = ld4(yr + c4 * 4), w = ld4(wr + c4 * 4);
-    a = fmaf(y.x, w.x, a); a = fmaf(y.y, w.y, a); a = fmaf(y.z, w.z, a); a = fmaf(y.w, w.w, a);
-  }
-  return a + md.By[item];
-}
-
-// item at position pos of a tile sweep over `subset` (nullptr: the catalogue)
-__device__ __forceinline__ int topk_item(const int* __restrict__ subset, int pos) { return subset ? subset[pos] : pos; }
 // item in the sorted list l[0 .. n)
 __device__ __forceinline__ bool topk_in(const int* __restrict__ l, int n, int item) {
   int lo = 0, hi = n;
@@ -218,57 +192,13 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
   const int* subset = FILT ? subset_ : nullptr;
   const int* ex_off = FILT ? ex_off_ : nullptr;
   extern __shared__ __align__(16) float smem[];
-  float* sY = smem;                        // [EV_TB][EV_LDS]
-  float* sW = sY + EV_TB * EV_LDS;         // [EV_IT][EV_LDS]
-  float2* sP = reinterpret_cast<float2*>(sW + EV_IT * EV_LDS);   // [8 warps][EV_TB]
-  const int M = md.wM[0], I = subset ? n_comp : md.n_items, ldL = md.ldL;
+  float2* sP = reinterpret_cast<float2*>(smem + EV_TILE_FLOATS);   // [8 warps][EV_TB]
+  const int M = md.wM[0], I = subset ? n_comp : md.n_items;
   const int i0 = blockIdx.x * EV_IT;
   const int ni = min(EV_IT, I - i0);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool soft = md.fact.kind > G4R_ACT_SELU;
-  const float* Y = md.layer[md.n_layers - 1].y;
-  const bool hoist = ldL <= EV_KT;
-  if (hoist) {
-    const int kw = ldL / 4;
-    for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
-      const int rr = i / kw, c4 = i % kw;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (rr < ni) v = ld4(md.Wy + (size_t)topk_item(subset, i0 + rr) * ldL + c4 * 4);
-      st4(sW + rr * EV_LDS + c4 * 4, v);
-    }
-  }
-  for (int b0 = 0; b0 < M; b0 += EV_TB) {
-    float acc[8];
-#pragma unroll
-    for (int q = 0; q < 8; q++) acc[q] = 0.f;
-    for (int k0 = 0; k0 < ldL; k0 += EV_KT) {
-      const int kw = min(EV_KT, ldL - k0) / 4;
-      __syncthreads();
-      for (int i = tid; i < EV_TB * kw; i += EV_THREADS) {
-        const int rr = i / kw, c4 = i % kw;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (b0 + rr < M) v = ld4(Y + (size_t)(b0 + rr) * ldL + k0 + c4 * 4);
-        st4(sY + rr * EV_LDS + c4 * 4, v);
-      }
-      if (!hoist) {
-        for (int i = tid; i < EV_IT * kw; i += EV_THREADS) {
-          const int rr = i / kw, c4 = i % kw;
-          float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (rr < ni) v = ld4(md.Wy + (size_t)topk_item(subset, i0 + rr) * ldL + k0 + c4 * 4);
-          st4(sW + rr * EV_LDS + c4 * 4, v);
-        }
-      }
-      __syncthreads();
-      const float* yr = sY + lane * EV_LDS;
-      for (int c4 = 0; c4 < kw; c4++) {
-        const float4 y = ld4(yr + c4 * 4);
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 w = ld4(sW + (warp + 8 * q) * EV_LDS + c4 * 4);
-          acc[q] = fmaf(y.x, w.x, acc[q]); acc[q] = fmaf(y.y, w.y, acc[q]); acc[q] = fmaf(y.z, w.z, acc[q]); acc[q] = fmaf(y.w, w.w, acc[q]);
-        }
-      }
-    }
+  ev_tiles(md, smem, M, i0, ni, subset, [&](int b0, float (&acc)[8]) {
     const int b = b0 + lane;
     float2 sm = make_float2(-INFINITY, 0.f);
     if (b < M) {
@@ -278,14 +208,14 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
 #pragma unroll
       for (int q = 0; q < 8; q++) {
         if (warp + 8 * q < ni) {
-          const int it = topk_item(subset, i0 + warp + 8 * q);
+          const int it = ev_item(subset, i0 + warp + 8 * q);
           acc[q] += md.By[it];
           if (topk_keep(acc[q], 0.f, lo, hi, it, ti)) { if (FILT) keep |= 1u << q; else topk_append(cnt, surv, C, b, it); }
           sm.x = fmaxf(sm.x, acc[q]);
         }
       }
       while (FILT && keep) {
-        const int q = __ffs(keep) - 1, it = topk_item(subset, i0 + warp + 8 * q);
+        const int q = __ffs(keep) - 1, it = ev_item(subset, i0 + warp + 8 * q);
         keep &= keep - 1u;
         if (!topk_excluded(ex_off, ex, b, it)) topk_append(cnt, surv, C, b, it);
       }
@@ -303,102 +233,62 @@ __global__ void __launch_bounds__(EV_THREADS) k_topk_fp32(int slot, const float*
         part[(size_t)b * n_part + blockIdx.x] = r;
       }
     }
-  }
+  });
 }
-static size_t topk_fp32_smem_bytes() { return (size_t)(EV_TB * EV_LDS + EV_IT * EV_LDS) * sizeof(float) + (EV_THREADS / 32) * EV_TB * sizeof(float2) + 64; }
+static size_t topk_fp32_smem_bytes() { return (size_t)EV_TILE_FLOATS * sizeof(float) + (EV_THREADS / 32) * EV_TB * sizeof(float2) + 64; }
 
-// pass 2, wgmma 3xTF32 tiles: k_eval_tc's pipeline (persistent CTAs, [A hi | A lo | B hi | B lo] stages fed by bulk copies,
-// four warpgroups of 64 lanes x 128 items) with a filtering epilogue: a thread holds two lanes x 32 items of the tile and keeps
-// those whose score x satisfies x + delta_b >= tau_b (topk_keep); partial softmax normaliser per (lane, tile, column half).
-// Items outside the candidate bitmap `cand` (nullptr: none) are neither kept nor summed; excluded items are summed, not kept.
-// FILT = false: the unfiltered instantiation (cand / ex_off ignored)
+// pass 2, wgmma 3xTF32 tiles: the sweep of k_eval_tc (tc_sweep) with a filtering epilogue: a thread keeps those of its two lanes
+// x 32 items of the tile whose score x satisfies x + delta_b >= tau_b (topk_keep); partial softmax normaliser per (lane, tile,
+// column half).  Items outside the candidate bitmap `cand` (nullptr: none) are neither kept nor summed; excluded items are summed,
+// not kept.  FILT = false: the unfiltered instantiation (cand / ex_off ignored)
 template <bool FILT>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_topk_tc(int slot, const float* __restrict__ tau, int* cnt, int* surv, int C, float2* part, int n_part,
                                                            const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit,
                                                            const unsigned int* __restrict__ cand_, const int* __restrict__ ex_off_, const int* __restrict__ ex) {
   const unsigned int* cand = FILT ? cand_ : nullptr;
   const int* ex_off = FILT ? ex_off_ : nullptr;
-  extern __shared__ __align__(1024) unsigned char tc_raw[];
-  TcSmem& sm = *reinterpret_cast<TcSmem*>(tc_raw);
   const ModelDev& md = MD;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-  const int M = md.wM[0], I = md.n_items, K = md.L + 1;       // + the bias column
+  const int M = md.wM[0], I = md.n_items, lane = threadIdx.x & 31;
   const bool soft = md.fact.kind > G4R_ACT_SELU;
-  const int n_tiles = (I + TC_N - 1) / TC_N;
-  const int n_lb = (M + TC_M - 1) / TC_M;
-  const int n_chunk = (K + TC_KC - 1) / TC_KC;
-  const int my_tiles = blockIdx.x < n_tiles ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const unsigned int total = (unsigned int)(n_lb * my_tiles * n_chunk);
-  if (tid == 0) {
-    for (int i = 0; i < TC_STAGES; i++) { tc_mbar_init(&sm.stage_free[i], 4); tc_mbar_init(&sm.stage_full[i], 1); }
-    sm.err = 0;
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  auto issue = [&](unsigned int it) {
-    const int c = (int)(it % n_chunk), q = (int)(it / n_chunk), t = blockIdx.x + (q % my_tiles) * gridDim.x, lb = q / my_tiles;
-    const uint32_t st = it % TC_STAGES;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(tc_smem_u32(&sm.stage_full[st])), "r"(TC_STAGE_BYTES) : "memory");
-    tc_bulk_copy(sm.stage[st], Asplit + ((size_t)lb * n_chunk + c) * 2 * TC_A_BYTES, 2 * TC_A_BYTES, &sm.stage_full[st]);
-    tc_bulk_copy(sm.stage[st] + 2 * TC_A_BYTES, Bsplit + ((size_t)t * n_chunk + c) * 2 * TC_B_BYTES, 2 * TC_B_BYTES, &sm.stage_full[st]);
-  };
-  if (tid == 0) for (unsigned int it = 0; it < total && it < (unsigned)TC_STAGES; it++) issue(it);
-  __syncwarp();
-  const int wr = (wg & 1) * 64, wc = (wg >> 1) * 128;
-  const int rq = (warp & 3) * 16 + (lane >> 2);
-  unsigned int it = 0;
-  for (int lb = 0; lb < n_lb; lb++) {
-    int bb[2], ti[2]; bool vrow[2]; float lo[2], hi[2], dl[2];
+  int bb[2], ti[2]; bool vrow[2]; float lo[2], hi[2], dl[2];
+  auto lane_block = [&](int b) {
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      bb[h] = lb * TC_M + wr + rq + 8 * h;
+      bb[h] = b + 8 * h;
       vrow[h] = bb[h] < M;
       lo[h] = vrow[h] ? tau[bb[h] * 4 + 0] : INFINITY; hi[h] = vrow[h] ? tau[bb[h] * 4 + 1] : INFINITY;
       dl[h] = vrow[h] ? tau[bb[h] * 4 + 2] : 0.f; ti[h] = vrow[h] ? __float_as_int(tau[bb[h] * 4 + 3]) : -1;
     }
-    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-      float d[64];
+  };
+  auto tile = [&](const float (&d)[64], int c0, bool) {
+    // columns past the catalogue (last tile) and non-candidates are neither kept nor summed
+    const int n_live = I - c0;
+    float2 smx[2] = {make_float2(-INFINITY, 0.f), make_float2(-INFINITY, 0.f)};
 #pragma unroll
-      for (int i = 0; i < 64; i++) d[i] = 0.f;
-      for (int c = 0; c < n_chunk; c++, it++) {
-        const uint32_t st = it % TC_STAGES, use = it / TC_STAGES;
-        tc_mbar_wait(&sm.stage_full[st], use & 1u, &sm.err);
-        const uint32_t a_hi = tc_smem_u32(sm.stage[st]) + wr * 128, a_lo = a_hi + TC_A_BYTES;
-        const uint32_t b_hi = tc_smem_u32(sm.stage[st]) + 2 * TC_A_BYTES + wc * 128, b_lo = b_hi + TC_B_BYTES;
-        wg_chunk_3xtf32(d, a_hi, a_lo, b_hi, b_lo);
-        if ((tid & 127) == 0) tc_mbar_arrive(&sm.stage_free[st]);
-        if (tid == 0 && it + TC_STAGES < total) { tc_mbar_wait(&sm.stage_free[st], use & 1u, &sm.err); issue(it + TC_STAGES); }
-        __syncwarp();
+    for (int i = 0; i < 64; i++) {
+      const int h = (i >> 1) & 1, col = (i >> 2) * 8 + (i & 1);
+      if (col < n_live && topk_is_cand(cand, c0 + col)) {
+        if (vrow[h] && topk_keep(d[i], dl[h], lo[h], hi[h], c0 + col, ti[h]) && !topk_excluded(ex_off, ex, bb[h], c0 + col))
+          topk_append(cnt, surv, C, bb[h], c0 + col);
+        smx[h].x = fmaxf(smx[h].x, d[i]);
       }
-      // columns past the catalogue (last tile) and non-candidates are neither kept nor summed
-      const int c0 = t * TC_N + wc + 2 * (lane & 3);                // item of d[0]; d[i] holds item c0 + 8 * (i / 4) + i % 2
-      const int n_live = I - c0;
-      float2 smx[2] = {make_float2(-INFINITY, 0.f), make_float2(-INFINITY, 0.f)};
+    }
+    if (soft) {
 #pragma unroll
       for (int i = 0; i < 64; i++) {
         const int h = (i >> 1) & 1, col = (i >> 2) * 8 + (i & 1);
-        if (col < n_live && topk_is_cand(cand, c0 + col)) {
-          if (vrow[h] && topk_keep(d[i], dl[h], lo[h], hi[h], c0 + col, ti[h]) && !topk_excluded(ex_off, ex, bb[h], c0 + col))
-            topk_append(cnt, surv, C, bb[h], c0 + col);
-          smx[h].x = fmaxf(smx[h].x, d[i]);
-        }
+        if (col < n_live && topk_is_cand(cand, c0 + col) && smx[h].x != -INFINITY) smx[h].y += expf(d[i] - smx[h].x);
       }
-      if (soft) {
 #pragma unroll
-        for (int i = 0; i < 64; i++) {
-          const int h = (i >> 1) & 1, col = (i >> 2) * 8 + (i & 1);
-          if (col < n_live && topk_is_cand(cand, c0 + col) && smx[h].x != -INFINITY) smx[h].y += expf(d[i] - smx[h].x);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; h++) {                                  // the four threads of a quad share the two lanes
-          float2 r = smx[h];
-          r = topk_smx_merge(r, make_float2(__shfl_xor_sync(0xffffffffu, r.x, 1), __shfl_xor_sync(0xffffffffu, r.y, 1)));
-          r = topk_smx_merge(r, make_float2(__shfl_xor_sync(0xffffffffu, r.x, 2), __shfl_xor_sync(0xffffffffu, r.y, 2)));
-          if ((lane & 3) == 0 && vrow[h]) part[(size_t)bb[h] * n_part + 2 * t + (wg >> 1)] = r;
-        }
+      for (int h = 0; h < 2; h++) {                                  // the four threads of a quad share the two lanes
+        float2 r = smx[h];
+        r = topk_smx_merge(r, make_float2(__shfl_xor_sync(0xffffffffu, r.x, 1), __shfl_xor_sync(0xffffffffu, r.y, 1)));
+        r = topk_smx_merge(r, make_float2(__shfl_xor_sync(0xffffffffu, r.x, 2), __shfl_xor_sync(0xffffffffu, r.y, 2)));
+        if ((lane & 3) == 0 && vrow[h]) part[(size_t)bb[h] * n_part + c0 / 128] = r;   // c0 / 128 = 2 * tile + column half
       }
     }
-  }
+  };
+  tc_sweep(M, I, md.L + 1, Asplit, Bsplit, lane_block, tile);
 }
 
 // overflow fallback: the fp32 row of every overflowed lane (blockIdx.y-th entry of ov_list) into rows[y * n_items ...]
@@ -406,7 +296,7 @@ __global__ void __launch_bounds__(128) k_topk_rows(int slot, const int* __restri
   const ModelDev& md = MD;
   const int item = blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= md.n_items) return;
-  rows[(size_t)blockIdx.y * md.n_items + item] = topk_score_fp32(md, ov_list[blockIdx.y], item);
+  rows[(size_t)blockIdx.y * md.n_items + item] = ev_score_fp32(md, ov_list[blockIdx.y], item);
 }
 
 // pass 3: per lane (one CTA) the exact fp32 pre-activations of the candidates -- the survivors, rescored with the fp32 chain, or
@@ -436,7 +326,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) k_topk_final(int slot, int k, co
   else if (ov_row && ov_row[b] >= 0) s = TopkSrc{nullptr, rows + (size_t)ov_row[b] * md.n_items, md.n_items, cand};
   else {
     s = TopkSrc{surv + (size_t)b * C, surv_pre + (size_t)b * C, min(cnt[b], C)};
-    for (int j = tid; j < s.n; j += blockDim.x) surv_pre[(size_t)b * C + j] = topk_score_fp32(md, b, s.idx[j]);
+    for (int j = tid; j < s.n; j += blockDim.x) surv_pre[(size_t)b * C + j] = ev_score_fp32(md, b, s.idx[j]);
     __syncthreads();
   }
   topk_set_excl(s, ex_off, ex, b);
@@ -506,10 +396,6 @@ __global__ void __launch_bounds__(256) k_topk_absmax(const float* __restrict__ W
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)I; i += stride) mb = max(mb, __float_as_uint(fabsf(By[i])));
   mw = __reduce_max_sync(0xffffffffu, mw); mb = __reduce_max_sync(0xffffffffu, mb);
   if ((threadIdx.x & 31) == 0) { atomicMax(&out[0], mw); atomicMax(&out[1], mb); }
-}
-__global__ void k_topk_iota(int* p, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = i;
 }
 
 static int topk_ctx(g4r_handle* h, EvalCtx* e, TopkCtx** out) {
@@ -587,22 +473,22 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
   rc = topk_ctx(h, e, &t);
   if (rc) return rc;
   cudaStream_t st = h->stream;
-  const int Be = e->Be, L = h->md.L;
+  const int L = h->md.L;
   if (use_cand && t->hMask != cmask) {                    // a candidate set other than the cached one
     t->hMask.clear();
     std::vector<int> list;
     list.reserve((size_t)n_distinct);
     for (int i = 0; i < I; i++) if ((cmask[(size_t)i >> 5] >> (i & 31)) & 1u) list.push_back(i);
-    CK(topk_grow(&t->dMask, &t->mask_cap, cmask.size()));
-    CK(topk_grow(&t->dCand, &t->cand_cap, list.size()));
+    CK(dev_grow(&t->dMask, &t->mask_cap, cmask.size()));
+    CK(dev_grow(&t->dCand, &t->cand_cap, list.size()));
     CK(cudaMemcpyAsync(t->dMask, cmask.data(), cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(t->dCand, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
     t->hMask.swap(cmask);
   }
   if (use_ex) {
-    CK(topk_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
-    CK(topk_grow(&t->dEx, &t->ex_cap, ex.size()));
+    CK(dev_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
+    CK(dev_grow(&t->dEx, &t->ex_cap, ex.size()));
     CK(cudaMemcpyAsync(t->dExOff, ex_off.data(), ex_off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(t->dEx, ex.data(), ex.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   }
@@ -616,38 +502,30 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
   const int P = std::min(n_comp, std::max(k + max_ex, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
   const bool no_tile = (use_cand || use_ex) && P == n_comp;
   const int C = std::min(n_comp, 16 * k + TOPK_SURV_BASE);
-  // tile kind: the rule of g4r_eval_schedule (cfg.eval_tc 1 = fp32 FFMA tiles, 2 = wgmma tiles, 0 = wgmma for >= 64 lanes and
-  // >= 2048 items, where the split table is amortised over enough lanes).  The wgmma tiles cover the whole catalogue whatever
-  // the candidates, so the automatic choice also asks for at least a quarter of the catalogue as candidates.
-  const bool tc = !no_tile && (h->cfg.eval_tc == 2 || (h->cfg.eval_tc == 0 && batch >= 64 && n_comp >= 2048 && 4 * (int64_t)n_comp >= I));
+  const bool tc = !no_tile && wgmma_tiles(h->cfg, batch, n_comp, I);
   const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
   const int n_part = no_tile ? 0 : tc ? 2 * tc_tiles : (n_comp + EV_IT - 1) / EV_IT;
-  if (!use_cand && t->iota_n < P) {
-    if (t->dIota) cudaFree(t->dIota);
-    t->dIota = nullptr; t->iota_n = 0;
-    CK(cudaMalloc(&t->dIota, (size_t)P * sizeof(int)));
-    k_topk_iota<<<(P + 255) / 256, 256, 0, st>>>(t->dIota, P);
-    t->iota_n = P;
-  }
-  CK(topk_grow(&t->dPre, &t->pre_cap, (size_t)batch * P));
+  CK(dev_grow(&t->dPre, &t->pre_cap, (size_t)batch * P));
   if (!no_tile) {
-    CK(topk_grow(&t->dSurv, &t->surv_cap, (size_t)batch * C));
-    CK(topk_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)batch * C));
-    CK(topk_grow(&t->dPart, &t->part_cap, (size_t)batch * n_part));
+    CK(dev_grow(&t->dSurv, &t->surv_cap, (size_t)batch * C));
+    CK(dev_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)batch * C));
+    CK(dev_grow(&t->dPart, &t->part_cap, (size_t)batch * n_part));
   }
-  CK(topk_grow(&t->dItems, &t->items_cap, (size_t)batch * k));
-  CK(topk_grow(&t->dScores, &t->scores_cap, (size_t)batch * k));
-  if (tc && (!t->dBsplit || t->split_version != h->wy_version)) {        // the cached item-table split is stale
-    if (!t->dBsplit) CK(cudaMalloc(&t->dBsplit, (size_t)tc_tiles * tc_chunks * 2 * TC_B_BYTES));
-    k_tc_split<TC_N><<<dim3(tc_tiles, tc_chunks), 256, 0, st>>>(h->md.Wy, I, h->md.ldL, L, t->dBsplit, tc_chunks, h->md.By, 0.f);
-    CK(cudaMemsetAsync(t->dAbsMax, 0, 2 * sizeof(unsigned int), st));
-    k_topk_absmax<<<2 * h->n_sm, 256, 0, st>>>(h->md.Wy, h->md.By, I, h->md.ldL, L, t->dAbsMax);
-    h->launches += 2;
-    t->split_version = h->wy_version;
+  CK(dev_grow(&t->dItems, &t->items_cap, (size_t)batch * k));
+  CK(dev_grow(&t->dScores, &t->scores_cap, (size_t)batch * k));
+  if (tc) {
+    rc = tc_operands(h, e);
+    if (rc) return rc;
+    if (t->absmax_version != h->wy_version) {
+      CK(cudaMemsetAsync(t->dAbsMax, 0, 2 * sizeof(unsigned int), st));
+      k_topk_absmax<<<2 * h->n_sm, 256, 0, st>>>(h->md.Wy, h->md.By, I, h->md.ldL, L, t->dAbsMax);
+      h->launches++;
+      t->absmax_version = h->wy_version;
+    }
   }
   eval_forward(h, e, 0);
-  // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the item list 0 .. P-1) and tau_b
-  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, use_cand ? dcand : t->dIota, P);
+  // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the items 0 .. P-1) and tau_b
+  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, dcand, P);
   h->launches++;
   int n_ov = 0;
   if (!no_tile) {
@@ -656,10 +534,9 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
     CK(cudaMemsetAsync(t->dCnt, 0, (size_t)batch * sizeof(int), st));
     // 2. the candidates in tiles: survivors and softmax partials
     if (tc) {
-      if (!t->dAsplit) CK(cudaMalloc(&t->dAsplit, (size_t)((Be + TC_M - 1) / TC_M) * tc_chunks * 2 * TC_A_BYTES));
-      k_tc_split<TC_M><<<dim3((batch + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(h->md.layer[h->md.n_layers - 1].y, batch, h->md.ldL, L, t->dAsplit, tc_chunks, nullptr, 1.0f);
+      k_tc_split<TC_M><<<dim3((batch + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(h->md.layer[h->md.n_layers - 1].y, batch, h->md.ldL, L, e->dAsplit, tc_chunks, nullptr, 1.0f);
       auto kern = (use_cand || use_ex) ? k_topk_tc<true> : k_topk_tc<false>;
-      kern<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part, t->dAsplit, t->dBsplit,
+      kern<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part, e->dAsplit, e->dBsplit,
                                                                             dmask, dexoff, dex);
       h->launches += 2;
     } else {
@@ -678,7 +555,7 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
     n_ov = (int)ov_list.size();
     if (n_ov > 0) {
       const size_t need = (size_t)n_ov * I;
-      if (e->out_cap < need) { if (e->dOut) cudaFree(e->dOut); e->dOut = nullptr; e->out_cap = 0; CK(cudaMalloc(&e->dOut, need * sizeof(float))); e->out_cap = need; }
+      CK(dev_grow(&e->dOut, &e->out_cap, need));
       CK(cudaMemcpyAsync(t->dOvList, ov_list.data(), (size_t)n_ov * sizeof(int), cudaMemcpyHostToDevice, st));
       CK(cudaMemcpyAsync(t->dOvRow, ov_row.data(), (size_t)batch * sizeof(int), cudaMemcpyHostToDevice, st));
       k_topk_rows<<<dim3((I + 127) / 128, n_ov), 128, 0, st>>>(e->slot, t->dOvList, e->dOut);

@@ -1,10 +1,12 @@
 """Serving leg with filters: per-call time of Engine.predict_topk with a candidate set and per-lane exclusions
-(g4r_predict_topk_filtered), and the unfiltered call of this build against a parent build.
+(g4r_predict_topk_filtered), each against a parent build.
 
-  filtered       Engine.predict_topk(X, k, items=..., exclude=...) on the automatic tile choice (eval_tc=0), candidates
+  filtered       Engine.predict_topk(X, k, items=..., exclude=...) on the tile choice of --tiles (auto: eval_tc=0), candidates
                  100 % / 50 % / 1 % of the catalogue (random, fixed per shape), 0 / 20 / 1000 random exclusions per lane
-  unfiltered     Engine.predict_topk(X, k) of this build and of --parent-lib (a libg4r.so built from the parent commit), timed
-                 in alternating windows in the same process
+  unfiltered     Engine.predict_topk(X, k)
+  --parent-lib   a libg4r.so built from the parent commit runs every row too: its predict() and its top-k (unfiltered and
+                 filtered) must equal this build's bit for bit, and the two builds are timed in alternating windows in the
+                 same process
 
 at the RSC15 shape (37,483 items, GRU(100)) and the Rees46 shape (172,000 items, GRU(512)), batch 1 / 32 / 512, k = 20 / 100.
 Every filtered configuration first checks each row against predict() plus the mask and a sort (items exactly, scores bitwise,
@@ -12,7 +14,8 @@ Every filtered configuration first checks each row against predict() plus the ma
 every call does the same work.  Timing: one warm-up call, then windows of n calls (host clock around calls that end in a device
 synchronise); the median window is reported with the min / max.  Prints the card name and power limit first.  Writes nothing.
 
-  python scripts/serve_filter_bench.py [--shapes rsc15,rees46] [--batches 1,32,512] [--k 20,100] [--parent-lib PATH]
+  python scripts/serve_filter_bench.py [--shapes rsc15,rees46] [--batches 1,32,512] [--k 20,100] [--tiles auto|fp32|wgmma]
+                                       [--parent-lib PATH]
 """
 import argparse
 import ctypes as C
@@ -57,12 +60,12 @@ def parent_lib(path):
     return lib
 
 
-def make_engine(I, mk, Be, w, lib=None):
+def make_engine(I, mk, Be, w, lib=None, eval_tc=None):
     saved = _lib._lib
     if lib is not None:
         _lib._lib = lib
     try:
-        eng = _lib.Engine(_lib.make_config(I, mk, sample_store=0, eval_lanes=Be, step_mode=1, eval_tc=None))
+        eng = _lib.Engine(_lib.make_config(I, mk, sample_store=0, eval_lanes=Be, step_mode=1, eval_tc=eval_tc))
     finally:
         _lib._lib = saved
     for n, v in w.items():
@@ -95,8 +98,10 @@ def main(argv=None):
     ap.add_argument('--shapes', default='rsc15,rees46')
     ap.add_argument('--batches', default='1,32,512')
     ap.add_argument('--k', default='20,100')
+    ap.add_argument('--tiles', default='auto', choices=['auto', 'fp32', 'wgmma'])
     ap.add_argument('--parent-lib', default=None)
     a = ap.parse_args(argv)
+    eval_tc = {'auto': None, 'fp32': False, 'wgmma': True}[a.tiles]
     batches = [int(x) for x in a.batches.split(',')]
     ks = [int(x) for x in a.k.split(',')]
     name, q = card()
@@ -109,8 +114,8 @@ def main(argv=None):
         gru = g4.GRU4Rec(**mk); gru.n_items = I
         w = gru._init_host_weights()
         Be = max(batches)
-        eng = make_engine(I, mk, Be, w)
-        par = make_engine(I, mk, Be, w, plib) if plib is not None else None
+        eng = make_engine(I, mk, Be, w, eval_tc=eval_tc)
+        par = make_engine(I, mk, Be, w, plib, eval_tc=eval_tc) if plib is not None else None
         rs = np.random.RandomState(0)
         cands = {f: (None if f == 1.0 else np.sort(rs.choice(I, int(f * I), replace=False)).astype(np.int32)) for f in FRACS}
         for B in batches:
@@ -118,6 +123,8 @@ def main(argv=None):
             ones = np.ones(B, np.uint8)
             excls = {n: [rs.randint(0, I, n).astype(np.int32) for _ in range(B)] for n in N_EXCL}
             p = eng.predict(X, ones)
+            if par is not None and not np.array_equal(p.view(np.uint32), par.predict(X, ones).view(np.uint32)):
+                raise SystemExit('MISMATCH: predict differs from the parent build at %s batch %d' % (sh, B))
             for k in ks:
                 if par is not None:         # unfiltered: parent and this build, alternating windows
                     i0, s0 = par.predict_topk(X, k, ones)
@@ -129,8 +136,9 @@ def main(argv=None):
                     for _ in range(4):
                         wp += timed(lambda: par.predict_topk(X, k, ones), 0.15, 2)
                         wn += timed(lambda: eng.predict_topk(X, k, ones), 0.15, 2)
-                    r = dict(shape=sh, batch=B, k=k, parent_ms=float(np.median(wp)) * 1e3, parent_spread_ms=[min(wp) * 1e3, max(wp) * 1e3],
-                             pr_ms=float(np.median(wn)) * 1e3, pr_spread_ms=[min(wn) * 1e3, max(wn) * 1e3], same_result=same)
+                    r = dict(shape=sh, batch=B, k=k, cand_frac=1.0, excl_per_lane=0, filtered=False, parent_ms=float(np.median(wp)) * 1e3,
+                             parent_spread_ms=[min(wp) * 1e3, max(wp) * 1e3], pr_ms=float(np.median(wn)) * 1e3,
+                             pr_spread_ms=[min(wn) * 1e3, max(wn) * 1e3], same_result=same)
                     cmp_rows.append(r)
                     print(json.dumps(r), flush=True)
                 for f in FRACS:
@@ -139,12 +147,27 @@ def main(argv=None):
                         excl = excls[ne] if ne else None
                         if cand is not None and k > len(cand):
                             continue
-                        call = lambda: eng.predict_topk(X, k, ones, items=cand if cand is not None else np.arange(I, dtype=np.int32),
-                                                        exclude=excl)
+                        items = cand if cand is not None else np.arange(I, dtype=np.int32)
+                        call = lambda e=eng: e.predict_topk(X, k, ones, items=items, exclude=excl)
                         it, sc = call()
                         if not check(p, it, sc, k, cand, excl):
                             raise SystemExit('MISMATCH: filtered top-k differs from the masked sort of predict() at %s batch %d k %d '
                                              'candidates %g exclusions %d' % (sh, B, k, f, ne))
+                        if par is not None:     # parent and this build, alternating windows
+                            i0, s0 = call(par)
+                            same = bool(np.array_equal(i0, it) and np.array_equal(s0.view(np.uint32), sc.view(np.uint32)))
+                            if not same:
+                                raise SystemExit('MISMATCH: filtered top-k differs from the parent build at %s batch %d k %d '
+                                                 'candidates %g exclusions %d' % (sh, B, k, f, ne))
+                            wp, wn = [], []
+                            for _ in range(4):
+                                wp += timed(lambda: call(par), 0.15, 2)
+                                wn += timed(call, 0.15, 2)
+                            r = dict(shape=sh, batch=B, k=k, cand_frac=f, excl_per_lane=ne, filtered=True, parent_ms=float(np.median(wp)) * 1e3,
+                                     parent_spread_ms=[min(wp) * 1e3, max(wp) * 1e3], pr_ms=float(np.median(wn)) * 1e3,
+                                     pr_spread_ms=[min(wn) * 1e3, max(wn) * 1e3], same_result=same)
+                            cmp_rows.append(r)
+                            print(json.dumps(r), flush=True)
                         wins = timed(call)
                         r = dict(shape=sh, batch=B, k=k, cand_frac=f, excl_per_lane=ne, checked=True,
                                  ms=float(np.median(wins)) * 1e3, spread_ms=[min(wins) * 1e3, max(wins) * 1e3])
@@ -154,11 +177,12 @@ def main(argv=None):
         if par is not None:
             par.close()
     if cmp_rows:
-        print('\n| shape | batch | k | parent (ms) | parent min-max | this build (ms) | this build min-max |')
-        print('|---|---|---|---|---|---|---|')
+        print('\n| shape | batch | k | candidates | exclusions / lane | parent (ms) | parent min-max | this build (ms) | this build min-max |')
+        print('|---|---|---|---|---|---|---|---|---|')
         for r in cmp_rows:
-            print('| %s | %d | %d | %.3f | %.3f-%.3f | %.3f | %.3f-%.3f |' % (r['shape'], r['batch'], r['k'], r['parent_ms'], *r['parent_spread_ms'],
-                                                                        r['pr_ms'], *r['pr_spread_ms']))
+            print('| %s | %d | %d | %g %% | %d | %.3f | %.3f-%.3f | %.3f | %.3f-%.3f |' % (
+                r['shape'], r['batch'], r['k'], 100 * r['cand_frac'], r['excl_per_lane'], r['parent_ms'], *r['parent_spread_ms'],
+                r['pr_ms'], *r['pr_spread_ms']))
     print('\n| shape | batch | k | candidates | exclusions / lane | filtered top-k (ms) | min-max |')
     print('|---|---|---|---|---|---|---|')
     for r in rows:

@@ -145,33 +145,47 @@ def test_topk_alternates_with_predict(tc):
 
 
 def test_topk_split_cache_follows_the_weights():
-    """the wgmma tiles keep the split item table between calls: set('Wy'), set('By') and training must all be seen"""
+    """the wgmma tiles of top-k and evaluation share one split item table, kept between calls: set('Wy'), set('By') and training
+    must all be seen, also when an evaluation made the split that top-k then uses"""
     n_items, lanes, k = 3000, 128, 20
     mk, m = _model(n_items, 'linear', [32], seed=10)
     a = _engine(n_items, mk, m, lanes, True)
     b = _engine(n_items, mk, m, lanes)
     rs = np.random.RandomState(11)
     ones = np.ones(lanes, np.uint8)
+    d = orc.prepare_fit_data(make_sessions(n_items=n_items, n_events=3000, seed=12))
+    esched = _lib.Schedule(d['data_items'] % n_items, d['offset_sessions'], None, lanes, 0, mode=1)
+    m_last = int(esched.export()['M'][-1])
 
     def check(what):
         X = _inputs(rs, n_items, lanes)
         items, scores = a.predict_topk(X, k, ones)
         _assert_topk(items, scores, b.predict(X, ones), k, what)
 
+    def check_eval(what):
+        twin = _engine(n_items, mk, m, lanes, True)     # a fresh engine: its split is made from the current weights
+        for name in param_names(m):
+            twin.set(name, a.get(name))
+        for call in range(2):                           # the first call on `a` splits the new table, the second reuses it
+            got = [tuple(e.eval_schedule(esched, [1, 5, 20], 0)) + (e.eval_counts(m_last),) for e in (a, twin)]
+            for x, y in zip(*got):
+                np.testing.assert_array_equal(x, y, err_msg='%s, call %d' % (what, call))
+        twin.close()
+
     check('initial')
     Wy = (rs.randn(*m.Wy.shape) * 0.2).astype(np.float32)
     a.set('Wy', Wy); b.set('Wy', Wy)
-    check('after set Wy')
+    check_eval('evaluation after set Wy')
+    check('after set Wy and an evaluation')
     By = (rs.randn(*m.By.shape) * 0.5).astype(np.float32)
     a.set('By', By); b.set('By', By)
     check('after set By')
-    df = make_sessions(n_items=n_items, n_events=3000, seed=12)
-    d = orc.prepare_fit_data(df)
     sched = _lib.Schedule(d['data_items'] % n_items, d['offset_sessions'], None, 8, 0, mode=0)
     a.train_steps(sched)
     for name in param_names(m):                # the twin takes the trained weights (its own split is never cached)
         b.set(name, a.get(name))
-    check('after train_steps')
+    check_eval('evaluation after train_steps')
+    check('after train_steps and an evaluation')
 
 
 @pytest.mark.parametrize('tc', [False, True])
