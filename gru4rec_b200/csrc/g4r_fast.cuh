@@ -7,6 +7,8 @@
 //    the target rows are PREFETCHED with TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) while the GRU
 //    phases of the previous step run, so the score phase starts with its operands already in shared memory;
 //  * folds the row-statistics combine into the score->gradient barrier (the last CTA to arrive combines);
+//  * (step_mode 2) puts only the partial dL/dh before the b1 barrier: dSy and the update of the chunk's rows follow b1, gated for
+//    the next prefetch by `rows_done`, and a GRU CTA's chunk is updated by a partner CTA with no GRU or helper role;
 //  * runs the GRU phases on a group of G CTAs (step_mode 2: weights resident in shared memory, one group barrier per
 //    mini-batch; see FastSmemR); the other CTAs only wait for `h_ready`;
 //  * uses monotonic release/acquire counters (no resets, no separate fences) for all synchronisation.
@@ -126,11 +128,13 @@ __device__ __forceinline__ void fk_prefetch_rows(const ModelDev& md, SM& sm, int
   const int ncopy = nj * ntab + (pw ? M : 0);
   if (tid == 0) {
     const unsigned int total = rowb * (unsigned int)ncopy;
-    asm volatile("fence.proxy.async.global;" ::: "memory");
     if (total > 0) mbar_expect_tx(bar, total);
     else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
   }
   if ((tid & 31) == 0) {
+    // every issuing thread orders the rows' generic-proxy stores (other CTAs' after the caller's acquire, this CTA's after
+    // its __syncthreads) before its bulk copies
+    asm volatile("fence.proxy.async.global;" ::: "memory");
     for (int i = tid >> 5; i < ncopy; i += FK_NW) {
       if (i < nj * ntab) {
         const int j = i / ntab, t = i % ntab;
@@ -807,27 +811,143 @@ __device__ void fr_dense(const ModelDev& md, FastSmemR& sm, int s, int k0, const
     }
   }
 }
-// sY <- y rows of step s (the column role) and, when hnext != nullptr, hnext <- H rows of the lanes staged in gIdx: one round trip
+// ---------------- loss-gradient tail of the column role (dL/do in sG, the chunk's rows in sS / sAcc / sVel) ----------------
+// partial dL/dh[b][quad] = sum_j g[b][j] Sy_j[quad] of this chunk: one thread per (lane, quad)
 template <class SM>
-__device__ __forceinline__ void fk_stage_y(const ModelDev& md, SM& sm, int M, float* hnext) {
-  const LayerDev& ly = md.layer[0];
-  const int ldL = ly.ldL, kw = ldL / 4, n1 = FK_B * kw, total = hnext ? 2 * n1 : n1;
-  for (int i0 = 0; i0 < total; i0 += 4 * FK_THREADS) {
-    float4 v[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-      const int i = i0 + u * FK_THREADS + (int)threadIdx.x;
-      v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (i < n1) { const int rr = i / kw; if (rr < M) v[u] = ld4(ly.y + (size_t)rr * ldL + (i % kw) * 4); }
-      else if (i < total) { const int sl = sm.gIdx[(i - n1) / kw]; if (sl >= 0) v[u] = ld4(ly.H + (size_t)sl * ldL + ((i - n1) % kw) * 4); }
+__device__ __forceinline__ void fk_part(SM& sm, float* part, int M, int nj, int ldL) {
+  const int kw = ldL / 4;
+  for (int t = threadIdx.x; t < M * kw; t += FK_THREADS) {
+    const int bb = t / kw, q4 = t % kw;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int jj = 0; jj < nj; jj++) {
+      const float g = sm.sG[jj * FK_B + bb];
+      const float4 w = ld4(sm.sS + jj * FK_LDS + q4 * 4);
+      a.x = fmaf(g, w.x, a.x); a.y = fmaf(g, w.y, a.y); a.z = fmaf(g, w.z, a.z); a.w = fmaf(g, w.w, a.w);
     }
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-      const int i = i0 + u * FK_THREADS + (int)threadIdx.x;
-      if (i < n1) st4(sm.sY + (i / kw) * FK_LDS + (i % kw) * 4, v[u]);
-      else if (i < total) st4(hnext + ((i - n1) / kw) * FK_LDS + ((i - n1) % kw) * 4, v[u]);
+    st4(part + (size_t)bb * ldL + q4 * 4, a);
+  }
+}
+// dSy[j][quad] = sum_b g[b][j] y[b][quad] into sD: one thread per (column, 16-byte feature quad), all nj*kw pairs in parallel
+template <class SM>
+__device__ __forceinline__ void fk_dsy(SM& sm, int M, int nj, int kw) {
+  for (int t = threadIdx.x; t < nj * kw; t += FK_THREADS) {
+    const int jj = t / kw, q4 = t % kw;
+    float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int bb = 0; bb < M; bb++) {
+      const float4 y = ld4(sm.sY + bb * FK_LDS + q4 * 4);
+      const float g = sm.sG[jj * FK_B + bb];
+      d.x = fmaf(g, y.x, d.x); d.y = fmaf(g, y.y, d.y); d.z = fmaf(g, y.z, d.z); d.w = fmaf(g, y.w, d.w);
+    }
+    st4(sm.sD + jj * FK_LDS + q4 * 4, d);
+  }
+}
+// sparse update of the chunk's Wy / By rows and their Adagrad / momentum state from shared memory (rows prefetched before
+// the step, dSy in sD, dby in sDby): one warp per duplicate group
+template <class SM>
+__device__ __forceinline__ void fk_update_rows(const ModelDev& md, SM& sm, int buf, int nj, int kw) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, ldL = md.ldL;
+  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
+  for (int j = warp; j < nj; j += FK_NW) {
+    const int item = sm.sIt[buf][j];
+    if (j > 0 && sm.sIt[buf][j - 1] == item) continue;
+    int je = j + 1;
+    while (je < nj && sm.sIt[buf][je] == item) je++;
+    if (lane < kw) {
+      const float4 p0 = ld4(sm.sS + j * FK_LDS + lane * 4);
+      float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0;
+      if (ada) a0 = ld4(sm.sAcc + j * FK_LDS + lane * 4);
+      if (mom) v0 = ld4(sm.sVel + j * FK_LDS + lane * 4);
+      float4 ps = p0;
+      for (int k = j; k < je; k++) {
+        const float4 g = ld4(sm.sD + k * FK_LDS + lane * 4);
+        float4 gs = g;
+        if (ada) {
+          al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
+          gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
+          gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
+        }
+        float4 d;
+        if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
+        else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
+        if (mom) {
+          vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
+          ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
+        } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
+      }
+      const size_t off = (size_t)item * ldL + lane * 4;
+      st4(md.Wy + off, ps);
+      if (ada) st4(md.Wy_acc + off, al);
+      if (mom) st4(md.Wy_vel + off, vl);
+    }
+    if (lane == 0) {
+      const float p0 = sm.sByP[j];
+      float a0 = sm.sByA[j], v0 = sm.sByV[j], al = 0.f, vl = 0.f, ps = p0;
+      for (int k = j; k < je; k++) {
+        const float g = sm.sDby[k];
+        float gs = g;
+        if (ada) { al = a0 + g * g; gs = __fdiv_rn(g, sqrtf(al + G4R_EPS_ADA)); }
+        const float d = md.lmbd > 0.f ? md.lr * (gs + md.lmbd * p0) : md.lr * gs;
+        if (mom) { vl = md.mom * v0 - d; ps += vl; } else ps -= d;
+      }
+      md.By[item] = ps;
+      if (ada) md.By_acc[item] = al;
+      if (mom) md.By_vel[item] = vl;
     }
   }
+}
+// dby of the chunk's columns from sG (fixed shuffle order)
+template <class SM>
+__device__ __forceinline__ void fk_dby(SM& sm, int M, int nj) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int jj = warp; jj < nj; jj += FK_NW) {
+    float a = (lane < M) ? sm.sG[jj * FK_B + lane] : 0.f;
+    a = warp_sum(a);
+    if (lane == 0) sm.sDby[jj] = a;
+  }
+}
+// step_mode 2: GRU CTA g's chunk is updated by its partner CTA (one with no GRU or helper role) after the partner's own chunk.
+// The chunk's dL/do columns come from md.O, where CTA g put them before B3; its items, rows and bias entries are read from
+// global memory, where nothing has written them since the previous step's rows_done.  These are the operands CTA g holds,
+// and dby / dSy / the update run the same code.  fk_partner_fetch issues the loads that do not depend on one another (chunk
+// bounds, items, dL/do) into registers before the own chunk is processed; fk_partner_stage puts them and the chunk's rows into
+// the shared-memory slots of the own chunk once that is done, and returns the chunk's column count.
+struct FkPartner { int nj, it; float g[2]; };
+__device__ __forceinline__ FkPartner fk_partner_fetch(const ModelDev& md, int s, int g, int M) {
+  const int tid = threadIdx.x;
+  const int* cbeg = md.pCbeg + (size_t)s * (md.NCH + 1);
+  const int cb = g < md.NCH ? cbeg[g] : 0;
+  FkPartner r;
+  r.nj = g < md.NCH ? cbeg[g + 1] - cb : 0;
+  r.it = (tid < r.nj) ? md.pItem[(size_t)s * md.NP + cb + tid] : 0;
+#pragma unroll
+  for (int u = 0; u < 2; u++) {
+    const int i = u * FK_THREADS + tid, jj = i / FK_B, b = i % FK_B;
+    r.g[u] = (jj < r.nj && b < M) ? md.O[(size_t)(cb + jj) * md.Bld + b] : 0.f;
+  }
+  return r;
+}
+template <class SM>
+__device__ int fk_partner_stage(const ModelDev& md, SM& sm, const FkPartner& r, int buf, int M, int kw) {
+  static_assert(FK_CT * FK_B == 2 * FK_THREADS, "fk_partner_fetch: two dL/do entries per thread");
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nj = r.nj;
+  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
+  __syncthreads();                                     // the own chunk's update has finished reading these slots
+  if (tid < FK_CT) sm.sIt[buf][tid] = r.it;
+  sm.sG[tid] = r.g[0]; sm.sG[FK_THREADS + tid] = r.g[1];
+  __syncthreads();
+  for (int j = warp; j < nj; j += FK_NW) {
+    const int it = sm.sIt[buf][j];
+    const size_t off = (size_t)it * md.ldL + lane * 4;
+    if (lane < kw) {
+      st4(sm.sS + j * FK_LDS + lane * 4, ld4(md.Wy + off));
+      if (ada) st4(sm.sAcc + j * FK_LDS + lane * 4, ld4(md.Wy_acc + off));
+      if (mom) st4(sm.sVel + j * FK_LDS + lane * 4, ld4(md.Wy_vel + off));
+    }
+    if (lane == 0) { sm.sByP[j] = md.By[it]; sm.sByA[j] = ada ? md.By_acc[it] : 0.f; sm.sByV[j] = mom ? md.By_vel[it] : 0.f; }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these generic stores precede the next TMA writes of the slots
+  fk_dby(sm, M, nj);
+  return nj;
 }
 
 #include "g4r_fastc.cuh"
@@ -848,12 +968,14 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
   const int G = CL ? (int)cl_size() : md.ldL / 4;   // CTAs of the GRU role (step_mode 2: one quad of hidden units each)
   const bool gru = cta < G;
   const bool pw = loss_pairwise(md.loss);
-  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
   const int ldL = md.ldL, B = md.B;
   const int kw = ldL / 4;
   uint64_t* bar = reinterpret_cast<uint64_t*>(&sm.mbar);
   unsigned int bar_epoch = 0, gepoch = 0, stats_target = 0;
   const int in_ctas = min(B, ncta - G);        // helper CTAs [G, G + in_ctas) update the gathered input rows
+  // step_mode 2: CTA G + in_ctas + g updates the rows of GRU CTA g's chunk, off the GRU CTAs' chain (the host launches
+  // k_fast_t<false> only on grids with room for these partners)
+  const int partner_of = (!CL && cta >= G + in_ctas && cta < 2 * G + in_ctas) ? cta - G - in_ctas : -1;
 #ifdef G4R_CF_FINE
 #define FK_FTS(s_) ((tstamp && cta == 0 && (s_) < 500 && n_steps >= 1000) ? tstamp + (size_t)((s_) + 500) * 16 : nullptr)
 #define FK_STAMP_OK(s_) ((s_) < 500)
@@ -909,11 +1031,10 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
       sm.gIdx[FK_B + tid] = tid < M1 ? md.wX[(size_t)(s + 1) * B + tid] : 0;
       sm.gIdx[2 * FK_B + tid] = tid < M1 ? md.wF[(size_t)(s + 1) * B + tid] : 0;
     }
-    // ---- wait for h(s), stage it (GRU CTAs of step_mode 2: with the H rows of step s + 1, final once every f2(s) has run) ----
+    // ---- wait for h(s), stage it ----
     if (tid == 0) wait_ge(&fs->h_ready, (unsigned int)(s + 1) * (unsigned int)G);
     __syncthreads();
-    if constexpr (CL) stage_rows4(sm.sY, FK_LDS, FK_B, kw, [&](int rr) -> const float* { return rr < M ? ly.y + (size_t)rr * ldL : nullptr; });
-    else fk_stage_y(md, sm, M, gru_next ? sm.gH[(s + 1) & 1] : nullptr);
+    stage_rows4(sm.sY, FK_LDS, FK_B, kw, [&](int rr) -> const float* { return rr < M ? ly.y + (size_t)rr * ldL : nullptr; });
     mbar_wait(bar, (unsigned int)(s & 1));      // prefetched rows of this step have landed
     __syncthreads();
     FK_STAMP(1);
@@ -1074,104 +1195,38 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
       sm.sG[i] = (jj < nj && b < M) ? loss_grad_elem(md, sm.sRS + (size_t)b * 8, sm.sO[i], sm.sTc[buf][b] == cb + jj, M, N) : 0.f;
     }
     __syncthreads();
-    for (int jj = warp; jj < nj; jj += FK_THREADS / 32) {
-      float a = (lane < M) ? sm.sG[jj * FK_B + lane] : 0.f;
-      a = warp_sum(a);
-      if (lane == 0) sm.sDby[jj] = a;
+    if (!CL && gru) {                           // the partner CTA updates this chunk's rows (B3 publishes these columns)
+      for (int i = tid; i < nj * FK_B; i += FK_THREADS) {
+        const int jj = i / FK_B, b = i % FK_B;
+        if (b < M) md.O[(size_t)(cb + jj) * md.Bld + b] = sm.sG[i];
+      }
+    } else {
+      fk_dby(sm, M, nj);
     }
     FK_STAMP(12);
     float* part = md.part + (size_t)(has_chunk ? chunk : 0) * md.B * ldL;
-    if (has_chunk) {
-      // dSy[j][quad] = sum_b g[b][j] y[b][quad]: one thread per (column, 16-byte feature quad), all nj*kw pairs in parallel
-      for (int t = tid; t < nj * kw; t += FK_THREADS) {
-        const int jj = t / kw, q4 = t % kw;
-        float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int bb = 0; bb < M; bb++) {
-          const float4 y = ld4(sm.sY + bb * FK_LDS + q4 * 4);
-          const float g = sm.sG[jj * FK_B + bb];
-          d.x = fmaf(g, y.x, d.x); d.y = fmaf(g, y.y, d.y); d.z = fmaf(g, y.z, d.z); d.w = fmaf(g, y.w, d.w);
-        }
-        st4(sm.sD + jj * FK_LDS + q4 * 4, d);
-      }
-      // partial dL/dh[b][quad] = sum_j g[b][j] Sy_j[quad]: one thread per (lane, quad)
-      for (int t = tid; t < M * kw; t += FK_THREADS) {
-        const int bb = t / kw, q4 = t % kw;
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int jj = 0; jj < nj; jj++) {
-          const float g = sm.sG[jj * FK_B + bb];
-          const float4 w = ld4(sm.sS + jj * FK_LDS + q4 * 4);
-          a.x = fmaf(g, w.x, a.x); a.y = fmaf(g, w.y, a.y); a.z = fmaf(g, w.z, a.z); a.w = fmaf(g, w.w, a.w);
-        }
-        st4(part + (size_t)bb * ldL + q4 * 4, a);
-      }
-    }
-    __syncthreads();
-    FK_STAMP(13);
-    // sparse update from shared memory (rows prefetched before the step): one warp per duplicate group
-    for (int j = warp; j < nj; j += FK_THREADS / 32) {
-      const int item = sm.sIt[buf][j];
-      if (j > 0 && sm.sIt[buf][j - 1] == item) continue;
-      int je = j + 1;
-      while (je < nj && sm.sIt[buf][je] == item) je++;
-      if (lane < kw) {
-        const float4 p0 = ld4(sm.sS + j * FK_LDS + lane * 4);
-        float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0;
-        if (ada) a0 = ld4(sm.sAcc + j * FK_LDS + lane * 4);
-        if (mom) v0 = ld4(sm.sVel + j * FK_LDS + lane * 4);
-        float4 ps = p0;
-        for (int k = j; k < je; k++) {
-          const float4 g = ld4(sm.sD + k * FK_LDS + lane * 4);
-          float4 gs = g;
-          if (ada) {
-            al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-            gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-            gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-          }
-          float4 d;
-          if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-          else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-          if (mom) {
-            vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-            ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-          } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
-        }
-        const size_t off = (size_t)item * ldL + lane * 4;
-        st4(md.Wy + off, ps);
-        if (ada) st4(md.Wy_acc + off, al);
-        if (mom) st4(md.Wy_vel + off, vl);
-      }
-      if (lane == 0) {
-        const float p0 = sm.sByP[j];
-        float a0 = sm.sByA[j], v0 = sm.sByV[j], al = 0.f, vl = 0.f, ps = p0;
-        for (int k = j; k < je; k++) {
-          const float g = sm.sDby[k];
-          float gs = g;
-          if (ada) { al = a0 + g * g; gs = __fdiv_rn(g, sqrtf(al + G4R_EPS_ADA)); }
-          const float d = md.lmbd > 0.f ? md.lr * (gs + md.lmbd * p0) : md.lr * gs;
-          if (mom) { vl = md.mom * v0 - d; ps += vl; } else ps -= d;
-        }
-        md.By[item] = ps;
-        if (ada) md.By_acc[item] = al;
-        if (mom) md.By_vel[item] = vl;
-      }
-    }
-    if (has_chunk && nj == 0) for (int i = tid; i < M * ldL; i += FK_THREADS) part[i] = 0.f;
-    // ---- barrier B3: all updates and partial dL/dh complete ----
-    __syncthreads();
-    FK_STAMP(14);
-    bar_epoch += 1;
-    if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncta); }
-    __syncthreads();
-    FK_STAMP(3);
-    // ---- b1 on every CTA, then prefetch the next step's rows ----
-    fk_b1<CL>(md, sm, s, cta, ncta);
-    __syncthreads();
-    if (tid == 0) red_release_add(&fs->b1_done, 1u);
-    FK_STAMP(15);
-    fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
-    FK_STAMP(4);
-    // ---- GRU role: backward, dense update, forward of the next step ----
     if constexpr (CL) {
+      // cluster variant: dSy, partial dL/dh and the row update before B3, then b1 and the prefetch of the next step's rows
+      if (has_chunk) { fk_dsy(sm, M, nj, kw); fk_part(sm, part, M, nj, ldL); }
+      __syncthreads();
+      FK_STAMP(13);
+      fk_update_rows(md, sm, buf, nj, kw);
+      if (has_chunk && nj == 0) for (int i = tid; i < M * ldL; i += FK_THREADS) part[i] = 0.f;
+      // ---- barrier B3: all updates and partial dL/dh complete ----
+      __syncthreads();
+      FK_STAMP(14);
+      bar_epoch += 1;
+      if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncta); }
+      __syncthreads();
+      FK_STAMP(3);
+      // ---- b1 on every CTA, then prefetch the next step's rows ----
+      fk_b1<CL>(md, sm, s, cta, ncta);
+      __syncthreads();
+      if (tid == 0) red_release_add(&fs->b1_done, 1u);
+      FK_STAMP(15);
+      fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
+      FK_STAMP(4);
+      // ---- GRU role: backward, dense update, forward of the next step ----
       if (gru) {
         if (s + 1 < n_steps) fk_stage_lanes(md, sm, s + 1, md.wM[s + 1]);
         cf_backward(md, sm, cc, fs, s, ncta, s + 1 < n_steps, (tstamp && cta == 0 && FK_STAMP_OK(s)) ? tstamp + (size_t)s * 16 : nullptr, FK_FTS(s));
@@ -1187,39 +1242,99 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
         }
         FK_STAMP(8);
       }
-    } else if (gru) {
-      const int k0 = 4 * cta;
-      const float* sHo = sm.gH[s & 1];                  // H rows of step s (staged one step earlier)
-      if (tid == 0) wait_ge(&fs->b1_done, (unsigned int)(s + 1) * (unsigned int)ncta);
-      __syncthreads();
-      fr_b2(md, sm, s, k0, sHo);
-      __syncthreads();
-      if (tid == 0) red_release_add(&fs->dvec_done, 1u);   // dvec of the step complete once all G have arrived
-      FK_STAMP(5);
-      fr_dense(md, sm, s, k0, sHo);
-      FK_STAMP(6);
-      if (s + 1 < n_steps) {
-        fr_f1(md, sm, s + 1, k0, sm.gH[(s + 1) & 1], &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
-        fk_group_barrier(fs, gepoch, G);                // all-gather of Hold * r
-        FK_STAMP(7);
-        fr_f2(md, sm, s + 1, k0, sm.gH[(s + 1) & 1]);
+      if (!gru && cta < G + in_ctas) {
+        // input-row update of the step's lanes, once dvec is complete (the GRU cluster's grp counter)
+        const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
+        if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, &fs->grp, tgt);
+        else {
+          if (tid == 0) wait_ge(&fs->grp, tgt);
+          __syncthreads();
+          for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
+        }
         __syncthreads();
-        if (tid == 0) red_release_add(&fs->h_ready, 1u);
+        if (tid == 0) red_release_add(&fs->in_done, 1u);
       }
-      FK_STAMP(8);
-    }
-    if (!gru && cta < G + in_ctas) {
-      // input-row update of the step's lanes, once dvec is complete: cluster variant = the GRU cluster's grp counter
-      const unsigned int* ctr = CL ? &fs->grp : &fs->dvec_done;
-      const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
-      if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, ctr, tgt);
-      else {
-        if (tid == 0) wait_ge(ctr, tgt);
-        __syncthreads();
-        for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
-      }
+    } else {
+      // partial dL/dh first: b1 and the GRU phases after it need nothing else from the column role
+      if (has_chunk) fk_part(sm, part, M, nj, ldL);
+      if (has_chunk && nj == 0) for (int i = tid; i < M * ldL; i += FK_THREADS) part[i] = 0.f;
+      // ---- barrier B3: partial dL/dh complete ----
       __syncthreads();
-      if (tid == 0) red_release_add(&fs->in_done, 1u);
+      FK_STAMP(13);
+      bar_epoch += 1;
+      if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncta); }
+      __syncthreads();
+      FK_STAMP(3);
+      fk_b1<CL>(md, sm, s, cta, ncta);
+      __syncthreads();
+      if (tid == 0) red_release_add(&fs->b1_done, 1u);
+      FK_STAMP(15);
+      // ---- off the chain: dSy and the update of the chunk's Wy / By rows.  Only the TMA prefetch of the next step reads the
+      // updated rows; it waits for rows_done (every CTA's update) ----
+      const bool nxt = s + 1 < n_steps;
+      const unsigned int rows_target = (unsigned int)(s + 1) * (unsigned int)ncta;
+      if (gru) {
+        const int k0 = 4 * cta;
+        const float* sHo = sm.gH[s & 1];                  // H rows of step s (staged one step earlier)
+        float* hnext = sm.gH[(s + 1) & 1];
+        // in the b1_done wait: the H rows of step s + 1 (final since every f2(s) has run).  This CTA's chunk rows are updated
+        // by its partner CTA.
+        if (nxt) stage_rows4(hnext, FK_LDS, FK_B, kw, [&](int rr) -> const float* { const int sl = sm.gIdx[rr]; return sl >= 0 ? ly.H + (size_t)sl * ldL : nullptr; });
+        __syncthreads();
+        FK_STAMP(14);
+        if (tid == 0) { red_release_add(&fs->rows_done, 1u); wait_ge(&fs->b1_done, (unsigned int)(s + 1) * (unsigned int)ncta); }
+        __syncthreads();
+        FK_STAMP(4);
+        // ---- GRU role: backward, dense update, forward of the next step ----
+        fr_b2(md, sm, s, k0, sHo);
+        __syncthreads();
+        if (tid == 0) red_release_add(&fs->dvec_done, 1u);   // dvec of the step complete once all G have arrived
+        FK_STAMP(5);
+        fr_dense(md, sm, s, k0, sHo);
+        FK_STAMP(6);
+        if (nxt) {
+          fr_f1(md, sm, s + 1, k0, hnext, &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
+          fk_group_barrier(fs, gepoch, G);                // all-gather of Hold * r
+          FK_STAMP(7);
+          fr_f2(md, sm, s + 1, k0, hnext);
+          __syncthreads();
+          if (tid == 0) red_release_add(&fs->h_ready, 1u);
+          // the prefetch of the next step's rows, once h(s + 1) is out: it overlaps the h_ready wait and the staging of y
+          // that open the next step
+          if (tid == 0) wait_ge(&fs->rows_done, rows_target);
+          __syncthreads();
+          fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
+        }
+        FK_STAMP(8);
+      } else {
+        // the own chunk, then on a partner CTA the chunk of GRU CTA partner_of, through the same dSy / update code
+        const FkPartner pc = partner_of >= 0 ? fk_partner_fetch(md, s, partner_of, M) : FkPartner{0, 0, {0.f, 0.f}};
+        for (int pass = 0, njp = nj; pass < (partner_of >= 0 ? 2 : 1); pass++) {
+          if (pass == 1) njp = fk_partner_stage(md, sm, pc, buf, M, kw);
+          fk_dsy(sm, M, njp, kw);
+          __syncthreads();
+          fk_update_rows(md, sm, buf, njp, kw);
+        }
+        __syncthreads();
+        if (tid == 0) red_release_add(&fs->rows_done, 1u);
+        if (cta < G + in_ctas) {
+          // input-row update of the step's lanes, once dvec is complete
+          const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
+          if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, &fs->dvec_done, tgt);
+          else {
+            if (tid == 0) wait_ge(&fs->dvec_done, tgt);
+            __syncthreads();
+            for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
+          }
+          __syncthreads();
+          if (tid == 0) red_release_add(&fs->in_done, 1u);
+        }
+        if (nxt) {
+          if (tid == 0) wait_ge(&fs->rows_done, rows_target);
+          __syncthreads();
+          fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
+        }
+      }
     }
   }
   if constexpr (CL) { if (gru) cf_store_resident(md, sm, cc); }

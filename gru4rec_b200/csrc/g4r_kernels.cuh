@@ -102,6 +102,7 @@ struct FastSync {                   // one counter per 128-byte line
   unsigned int grp;      unsigned int p4[31];
   unsigned int in_done;  unsigned int p5[31];
   unsigned int dvec_done; unsigned int p6[31];   // step_mode 2: GRU CTAs that have written their da_r (dvec of the step complete)
+  unsigned int rows_done; unsigned int p7[31];   // step_mode 2: CTAs that have updated their chunk's Wy / By rows (gates the next prefetch)
 };
 struct GridBar { unsigned int count; unsigned int gen; unsigned int pad[30]; };   // grid barrier state (persistent mode)
 

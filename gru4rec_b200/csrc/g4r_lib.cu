@@ -788,6 +788,10 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
     const bool plain_opt = m.adapt <= G4R_ADAPT_ADAGRAD && !h->phase_only;    // the role-specialised kernels implement SGD / Adagrad (+momentum) only
     h->fast_ok = plain_opt && h->pk_blocks > 0 && per_sm >= 1 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B && h->n_sm >= FK_G + 1 && m.NCH <= 160 &&
                  2 * m.L <= FK_W1 * FK_G && m.L <= FK_W2 * FK_G &&     // L <= 120, the coverage of k_fast_mg's 48-CTA GRU group (k_fast_t<false> uses ldL / 4 CTAs)
+                 // k_fast_t<false>: ldL / 4 GRU CTAs, up to B helper CTAs, and one partner CTA per GRU CTA for its chunk's row update.
+                 // At most 96 CTAs (ldL <= 128, B <= 32): every shape k_fast takes fits a 132-SM H100.  A smaller grid runs these
+                 // shapes on k_persistent; g4r_fast_windows() reports such windows as slow ones.
+                 h->pk_blocks >= 2 * (m.ldL / 4) + std::min(m.B, h->pk_blocks - m.ldL / 4) &&
                  (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);
     h->fastc_ok = plain_opt && cfg->step_mode == 3 && h->fastc_grid >= FC_CLUSTER * 2 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B &&
                   m.NCH <= h->fastc_grid && (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);

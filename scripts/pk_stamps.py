@@ -24,10 +24,12 @@ eng.upload_steps(sched, K, K); c, ms = eng.run_uploaded(K, True)
 st = eng.persistent_stamps(True, K).astype(np.int64)
 if cfg.step_mode >= 2:
     print('fast windows', eng.fast_windows())
-    names = [('wait h + stage', 0, 1), (' targets+scores', 1, 9), (' partial stats', 9, 10), (' B2 + parallel combine', 10, 2), (' RS load + cost', 2, 11), (' g + dby', 11, 12), (' dSy + part', 12, 13), (' sparse update', 13, 14), (' B3', 14, 3),
-             ('b1 (+release)', 3, 15), ('prefetch issue', 15, 4), ('wait b1 + b2 -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 + grp', 6, 7), ('f2', 7, 8)]
-    if cfg.step_mode == 3:   # GRU phases on one thread-block cluster
-        names[-4:] = [('backward -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 (+in_done, barriers)', 6, 7), ('f2', 7, 8)]
+    # step_mode 2 (CTA 0 is a GRU CTA): dSy and the update of its chunk's rows run on a partner CTA after b1
+    names = [('wait h + stage', 0, 1), (' targets+scores', 1, 9), (' partial stats', 9, 10), (' B2 + parallel combine', 10, 2), (' RS load + cost', 2, 11), (' g + dby', 11, 12), (' part', 12, 13), (' B3', 13, 3),
+             ('b1 (+release)', 3, 15), ('stage H(s+1)', 15, 14), ('wait b1_done', 14, 4), ('b2 -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 + grp', 6, 7), ('f2 + prefetch issue', 7, 8)]
+    if cfg.step_mode == 3:   # GRU phases on one thread-block cluster; dSy and the row update before B3
+        names = names[:6] + [(' dSy + part', 12, 13), (' sparse update', 13, 14), (' B3', 14, 3), ('b1 (+release)', 3, 15), ('prefetch issue', 15, 4),
+                             ('backward -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 (+in_done, barriers)', 6, 7), ('f2', 7, 8)]
     st = st[:-1]
 else:
   names = [('gru_rz(f1)', 0, 6), ('gru_h(f2)', 6, 1), ('score', 1, 2), ('stats', 2, 3), ('lossgrad', 3, 4), ('b1', 4, 7), ('b2', 7, 8), ('dense+sparse_in', 8, 5)]
