@@ -348,84 +348,6 @@ __device__ void fk_b2(const ModelDev& md, FastSmem& sm, int s, int cta) {
   const float v = fk_slab_reduce<FK_W2>(acc, sm.gW + 8 * FK_LDS, jsel);
   if (jsel < W && b < M) ly.dvec[(size_t)b * ly.ld3 + L + c0 + jsel] = v * ho * r * (1.f - r);
 }
-// D: dense gradients of this CTA's row slab of Wh / Wrz (and a slice of Bh) fused with their Adagrad(+momentum) update
-__device__ void fk_dense(const ModelDev& md, FastSmem& sm, int s, int cta) {
-  const LayerDev& ly = md.layer[0];
-  const int M = md.wM[s], L = ly.L, ldL = ly.ldL, ld3 = ly.ld3, tid = threadIdx.x;
-  const int R = (L + FK_G - 1) / FK_G;            // rows of Wh / Wrz per CTA
-  const int k0 = cta * R;
-  const int nr = max(0, min(R, L - k0));
-  const int CB = (3 * L + FK_G - 1) / FK_G;       // Bh entries per CTA
-  const int cb0 = cta * CB, ncb = max(0, min(CB, 3 * L - cb0));
-  if (nr == 0 && ncb == 0) return;
-  float* sHo = sm.gW;                  // [R][32]
-  float* sHr = sm.gW + 8 * FK_B;       // [R][32]
-  // outputs: nr x L (Wh), nr x 2L (Wrz), ncb (Bh).  Each thread owns U outputs at a time: their parameter / Adagrad /
-  // momentum values are loaded first, the U batch reductions (<= 32 lanes) run interleaved, then the updates are stored.
-  const int nWh = nr * L, nWrz = nr * 2 * L, total = nWh + nWrz + ncb;
-  constexpr int U = 2;
-  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
-  float* p[U]; float* pa[U]; float* pv[U]; const float* av[U]; const float* bv[U]; bool ok[U]; bool bias[U];
-  float p0[U], a0[U], v0[U], g[U];
-  auto load_ops = [&](int o0) {
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int o = o0 + u * FK_THREADS + tid;
-      ok[u] = o < total; bias[u] = false; p[u] = nullptr; pa[u] = nullptr; pv[u] = nullptr; av[u] = sHo; bv[u] = sm.gA;
-      if (ok[u]) {
-        if (o < nWh) {
-          const int rr = o / L, c = o % L;
-          const size_t off = (size_t)(k0 + rr) * ldL + c;
-          p[u] = ly.Wh + off; pa[u] = ly.Wh_acc ? ly.Wh_acc + off : nullptr; pv[u] = ly.Wh_vel ? ly.Wh_vel + off : nullptr;
-          av[u] = sHr + rr * FK_B; bv[u] = sm.gA + c;
-        } else if (o < nWh + nWrz) {
-          const int q = o - nWh, rr = q / (2 * L), c = q % (2 * L);
-          const size_t off = (size_t)(k0 + rr) * ly.ld2 + c;
-          p[u] = ly.Wrz + off; pa[u] = ly.Wrz_acc ? ly.Wrz_acc + off : nullptr; pv[u] = ly.Wrz_vel ? ly.Wrz_vel + off : nullptr;
-          av[u] = sHo + rr * FK_B; bv[u] = sm.gA + L + c;
-        } else {
-          const int c = cb0 + (o - nWh - nWrz);
-          p[u] = ly.Bh + c; pa[u] = ly.Bh_acc ? ly.Bh_acc + c : nullptr; pv[u] = ly.Bh_vel ? ly.Bh_vel + c : nullptr;
-          bias[u] = true; bv[u] = sm.gA + c;
-        }
-      }
-      p0[u] = ok[u] ? *p[u] : 0.f;
-      a0[u] = (ok[u] && ada && pa[u]) ? *pa[u] : 0.f;
-      v0[u] = (ok[u] && mom && pv[u]) ? *pv[u] : 0.f;
-      g[u] = 0.f;
-    }
-  };
-  // this CTA's rows of Wh / Wrz / Bh are written by nobody else: the operands of the first pass are fetched before the
-  // dvec rows are staged, so the two global round trips overlap
-  load_ops(0);
-  __syncthreads();
-  // stage dvec [32 x 3L] and the (Hold, Hold*r) columns of this slab
-  // 32 x 75 quads at L = 100: five loads in flight per thread cover the whole block in one round trip
-  stage_rows_n<5>(sm.gA, 388, FK_B, ld3 / 4, [&](int rr) -> const float* { return rr < M ? ly.dvec + (size_t)rr * ld3 : nullptr; });
-  for (int i = tid; i < nr * FK_B; i += FK_THREADS) {
-    const int rr = i / FK_B, b = i % FK_B;
-    float ho = 0.f, r = 0.f;
-    if (b < M) { ho = ly.Hold[(size_t)b * ldL + k0 + rr]; r = ly.r[(size_t)b * ldL + k0 + rr]; }
-    sHo[i] = ho; sHr[i] = ho * r;
-  }
-  __syncthreads();
-  for (int o0 = 0; o0 < total; o0 += U * FK_THREADS) {
-    if (o0 > 0) load_ops(o0);
-    for (int b = 0; b < M; b++) {
-#pragma unroll
-      for (int u = 0; u < U; u++) g[u] = bias[u] ? g[u] + bv[u][b * 388] : fmaf(av[u][b], bv[u][b * 388], g[u]);
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (!ok[u]) continue;
-      float gs = g[u];
-      if (ada) { const float a = a0[u] + g[u] * g[u]; *pa[u] = a; gs = __fdiv_rn(g[u], sqrtf(a + G4R_EPS_ADA)); }
-      if (mom) { const float v2 = md.mom * v0[u] - md.lr * (gs + md.lmbd * p0[u]); *pv[u] = v2; *p[u] = p0[u] + v2; }
-      else *p[u] = p0[u] * (1.0f - md.lr * md.lmbd) - md.lr * gs;
-    }
-  }
-}
-
 // Input-row update of lane b on a helper (non-GRU) CTA, concurrent with the dense update of the GRU group: it starts when
 // the GRU group has passed its B2 barrier (dvec complete) and only touches Wx0 rows, which the dense phase never reads.
 template <class SM>
@@ -444,30 +366,13 @@ __device__ void fk_sparse_in(const ModelDev& md, SM& sm, int s, int b) {
   const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
   float* prow = ly.Wx + (size_t)item * ld3;
   for (int c4 = tid; c4 < ld3 / 4; c4 += FK_THREADS) {
-    const float4 p0 = ld4(prow + c4 * 4);
-    float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0;
-    if (ada) a0 = ld4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4);
-    if (mom) v0 = ld4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4);
-    float4 ps = p0;
-    for (int k = 0; k < nmem; k++) {
-      const float4 g = ld4(ly.dvec + (size_t)sm.gIdx[k] * ld3 + c4 * 4);
-      float4 gs = g;
-      if (ada) {
-        al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-        gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-        gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-      }
-      float4 d;
-      if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-      else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-      if (mom) {
-        vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-        ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-      } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
-    }
-    st4(prow + c4 * 4, ps);
-    if (ada) st4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4, al);
-    if (mom) st4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4, vl);
+    const float4 p0 = ld4(prow + c4 * 4), z = make_float4(0.f, 0.f, 0.f, 0.f);
+    RowChain<float4> u;
+    u.begin(p0, p0, ada ? ld4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4) : z, mom ? ld4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4) : z);
+    for (int k = 0; k < nmem; k++) u.add(md, ld4(ly.dvec + (size_t)sm.gIdx[k] * ld3 + c4 * 4), ada, mom);
+    st4(prow + c4 * 4, u.ps);
+    if (ada) st4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4, u.al);
+    if (mom) st4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4, u.vl);
   }
 }
 
@@ -498,26 +403,12 @@ __device__ void fk_sparse_in_one(const ModelDev& md, SM& sm, int s, int b, const
   __syncthreads();
   if (mine) {
     const int nmem = sm.gIdx[FK_B];
-    float4 al = a0, vl = v0, ps = p0;
-    for (int k = 0; k < nmem; k++) {
-      const float4 g = ld4(ly.dvec + (size_t)sm.gIdx[k] * ld3 + c4 * 4);
-      float4 gs = g;
-      if (ada) {
-        al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-        gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-        gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-      }
-      float4 d;
-      if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-      else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-      if (mom) {
-        vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-        ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-      } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
-    }
-    st4(prow + c4 * 4, ps);
-    if (ada) st4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4, al);
-    if (mom) st4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4, vl);
+    RowChain<float4> u;
+    u.begin(p0, p0, a0, v0);
+    for (int k = 0; k < nmem; k++) u.add(md, ld4(ly.dvec + (size_t)sm.gIdx[k] * ld3 + c4 * 4), ada, mom);
+    st4(prow + c4 * 4, u.ps);
+    if (ada) st4(ly.Wx_acc + (size_t)item * ld3 + c4 * 4, u.al);
+    if (mom) st4(ly.Wx_vel + (size_t)item * ld3 + c4 * 4, u.vl);
   }
 }
 
@@ -752,16 +643,8 @@ __device__ void fr_b2(const ModelDev& md, FastSmemR& sm, int s, int k0, const fl
     sm.gDr[b * FR_U + jsel] = dar;
   }
 }
-// Adagrad (+momentum) step of one resident element (same arithmetic as fk_dense)
-__device__ __forceinline__ void fr_upd(const ModelDev& md, bool ada, bool mom, float g, float& p, float& a, float& v) {
-  const float p0 = p;
-  float gs = g;
-  if (ada) { a = a + g * g; gs = __fdiv_rn(g, sqrtf(a + G4R_EPS_ADA)); }
-  if (mom) { v = md.mom * v - md.lr * (gs + md.lmbd * p0); p = p0 + v; }
-  else p = p0 * (1.0f - md.lr * md.lmbd) - md.lr * gs;
-}
 // D of step s: gradients of the resident slabs and Bh from shared memory only (Hold, Hold * r, da_h of all units; da_r,
-// da_z of the own units), summed over the lanes in order with fmaf as fk_dense does, then updated in place.
+// da_z of the own units), summed over the lanes in order with fmaf, then updated in place.
 // A task is one 16-byte quad of outputs: column tasks (resident column jm, quad q of k), row tasks (resident row j, quad q
 // of the columns), then the 3 * FR_U bias entries.
 __device__ void fr_dense(const ModelDev& md, FastSmemR& sm, int s, int k0, const float* sHo) {
@@ -796,17 +679,17 @@ __device__ void fr_dense(const ModelDev& md, FastSmemR& sm, int s, int k0, const
         float* P = colt ? sm.rC[0] : sm.rR[0];
         float* A = colt ? sm.rC[1] : sm.rR[1];
         float* V = colt ? sm.rC[2] : sm.rR[2];
-        if (q * 4 + 0 < L) fr_upd(md, ada, mom, g.x, P[o + 0], A[o + 0], V[o + 0]);
-        if (q * 4 + 1 < L) fr_upd(md, ada, mom, g.y, P[o + 1], A[o + 1], V[o + 1]);
-        if (q * 4 + 2 < L) fr_upd(md, ada, mom, g.z, P[o + 2], A[o + 2], V[o + 2]);
-        if (q * 4 + 3 < L) fr_upd(md, ada, mom, g.w, P[o + 3], A[o + 3], V[o + 3]);
+        if (q * 4 + 0 < L) dense_elem(md, ada, mom, g.x, P + o + 0, A + o + 0, V + o + 0);
+        if (q * 4 + 1 < L) dense_elem(md, ada, mom, g.y, P + o + 1, A + o + 1, V + o + 1);
+        if (q * 4 + 2 < L) dense_elem(md, ada, mom, g.z, P + o + 2, A + o + 2, V + o + 2);
+        if (q * 4 + 3 < L) dense_elem(md, ada, mom, g.w, P + o + 3, A + o + 3, V + o + 3);
       }
     } else {
       const int i = t - ncol - nrow, m = i / FR_U, j = i % FR_U;
       if (k0 + j < L) {
         float g = 0.f;
         for (int b = 0; b < M; b++) g = g + (m == 0 ? sm.sD[b * FK_LDS + k0 + j] : (m == 1 ? sm.gDr : sm.gDz)[b * FR_U + j]);
-        fr_upd(md, ada, mom, g, sm.rB[0][i], sm.rB[1][i], sm.rB[2][i]);
+        dense_elem(md, ada, mom, g, sm.rB[0] + i, sm.rB[1] + i, sm.rB[2] + i);
       }
     }
   }
@@ -853,45 +736,22 @@ __device__ __forceinline__ void fk_update_rows(const ModelDev& md, SM& sm, int b
     int je = j + 1;
     while (je < nj && sm.sIt[buf][je] == item) je++;
     if (lane < kw) {
-      const float4 p0 = ld4(sm.sS + j * FK_LDS + lane * 4);
-      float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0;
-      if (ada) a0 = ld4(sm.sAcc + j * FK_LDS + lane * 4);
-      if (mom) v0 = ld4(sm.sVel + j * FK_LDS + lane * 4);
-      float4 ps = p0;
-      for (int k = j; k < je; k++) {
-        const float4 g = ld4(sm.sD + k * FK_LDS + lane * 4);
-        float4 gs = g;
-        if (ada) {
-          al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-          gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-          gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-        }
-        float4 d;
-        if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-        else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-        if (mom) {
-          vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-          ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-        } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
-      }
+      const float4 p0 = ld4(sm.sS + j * FK_LDS + lane * 4), z = make_float4(0.f, 0.f, 0.f, 0.f);
+      RowChain<float4> u;
+      u.begin(p0, p0, ada ? ld4(sm.sAcc + j * FK_LDS + lane * 4) : z, mom ? ld4(sm.sVel + j * FK_LDS + lane * 4) : z);
+      for (int k = j; k < je; k++) u.add(md, ld4(sm.sD + k * FK_LDS + lane * 4), ada, mom);
       const size_t off = (size_t)item * ldL + lane * 4;
-      st4(md.Wy + off, ps);
-      if (ada) st4(md.Wy_acc + off, al);
-      if (mom) st4(md.Wy_vel + off, vl);
+      st4(md.Wy + off, u.ps);
+      if (ada) st4(md.Wy_acc + off, u.al);
+      if (mom) st4(md.Wy_vel + off, u.vl);
     }
     if (lane == 0) {
-      const float p0 = sm.sByP[j];
-      float a0 = sm.sByA[j], v0 = sm.sByV[j], al = 0.f, vl = 0.f, ps = p0;
-      for (int k = j; k < je; k++) {
-        const float g = sm.sDby[k];
-        float gs = g;
-        if (ada) { al = a0 + g * g; gs = __fdiv_rn(g, sqrtf(al + G4R_EPS_ADA)); }
-        const float d = md.lmbd > 0.f ? md.lr * (gs + md.lmbd * p0) : md.lr * gs;
-        if (mom) { vl = md.mom * v0 - d; ps += vl; } else ps -= d;
-      }
-      md.By[item] = ps;
-      if (ada) md.By_acc[item] = al;
-      if (mom) md.By_vel[item] = vl;
+      RowChain<float> u;
+      u.begin(sm.sByP[j], sm.sByP[j], sm.sByA[j], sm.sByV[j]);
+      for (int k = j; k < je; k++) u.add(md, sm.sDby[k], ada, mom);
+      md.By[item] = u.ps;
+      if (ada) md.By_acc[item] = u.al;
+      if (mom) md.By_vel[item] = u.vl;
     }
   }
 }

@@ -372,13 +372,7 @@ __device__ void cf_backward(const ModelDev& md, FastSmemC& sm, const ClusterCtx&
       const int o = (t * FC_PH + j) * FK_LDS + lane * 4;
       const float ge[4] = {g4.x, g4.y, g4.z, g4.w};
 #pragma unroll
-      for (int e = 0; e < 4; e++) {
-        const float g = ge[e], p0 = sm.rP[o + e];
-        float gs = g;
-        if (ada) { const float a = sm.rA[o + e] + g * g; sm.rA[o + e] = a; gs = __fdiv_rn(g, sqrtf(a + G4R_EPS_ADA)); }
-        if (mom) { const float v2 = md.mom * sm.rV[o + e] - md.lr * (gs + md.lmbd * p0); sm.rV[o + e] = v2; sm.rP[o + e] = p0 + v2; }
-        else sm.rP[o + e] = p0 * (1.0f - md.lr * md.lmbd) - md.lr * gs;
-      }
+      for (int e = 0; e < 4; e++) dense_elem(md, ada, mom, ge[e], sm.rP + o + e, sm.rA + o + e, sm.rV + o + e);
     }
   }
   CF_T(6);
@@ -390,11 +384,7 @@ __device__ void cf_backward(const ModelDev& md, FastSmemC& sm, const ClusterCtx&
       for (int bb = 0; bb < M; bb++) g += d[bb * FC_SL + j];
     }
     const int o = lane * FC_PH + j;
-    const float p0 = sm.rB[0][o];
-    float gs = g;
-    if (ada) { const float a = sm.rB[1][o] + g * g; sm.rB[1][o] = a; gs = __fdiv_rn(g, sqrtf(a + G4R_EPS_ADA)); }
-    if (mom) { const float v2 = md.mom * sm.rB[2][o] - md.lr * (gs + md.lmbd * p0); sm.rB[2][o] = v2; sm.rB[0][o] = p0 + v2; }
-    else sm.rB[0][o] = p0 * (1.0f - md.lr * md.lmbd) - md.lr * gs;
+    dense_elem(md, ada, mom, g, sm.rB[0] + o, sm.rB[1] + o, sm.rB[2] + o);
   }
   __syncthreads();
   cl_arrive();          // this CTA no longer reads H*r of step s

@@ -18,7 +18,6 @@
 #include <stdint.h>
 #include "../../include/g4r.h"
 
-#define G4R_EPS_ADA 1e-6f
 #define G4R_EPS_LOG 1e-24f
 #define G4R_NSTAT 8
 
@@ -326,87 +325,9 @@ __device__ __forceinline__ void stage_rows4(float* sdst, int sld, int nrows, int
     }
   }
 }
-// ------------------------------------------------------------------------------------------------
-// Adaptive scalers other than Adagrad (gru4rec.py:300-329 adam, 341-366 adadelta, 367-381 rmsprop) and the update that follows
-// (gru4rec.py:390-431), for ONE element of a parameter with n gradient contributions in position order (n = 1: dense).
-// Sparse ("sampled") parameters use the reference's duplicate-accurate forms: the decayed state receives the squared
-// gradients of ALL duplicates, every duplicate is scaled with that common state (and adam's sparse first moment accumulates
-// grad**2 -- sic, gru4rec.py:325); velocity: last duplicate wins; parameter: all duplicates accumulate.
-// States of an element: s0 = acc, s1 = upd (adadelta) | meang (adam), s2 = countt (adam).
-// ------------------------------------------------------------------------------------------------
-struct OptE { float p, s0, s1, s2, v; };
-__device__ __forceinline__ float grad_scale(const ModelDev& md) { return md.gscale ? *md.gscale : 1.0f; }
-template <bool SPARSE, class FG>
-__device__ __forceinline__ void opt_elem(const ModelDev& md, OptE& e, float p0l, int n, FG gk) {
-  const float gsc = grad_scale(md);
-  const int ad = md.adapt;
-  const bool mom = md.mom > 0.f;
-  float A = e.s0, sclr = 1.f, common = 0.f;
-  if (ad == G4R_ADAPT_RMSPROP || ad == G4R_ADAPT_ADADELTA) {
-    A = e.s0 * md.ap1;
-    for (int k = 0; k < n; k++) { const float g = gk(k) * gsc; A += md.ap1c * g * g; }
-    if (ad == G4R_ADAPT_ADADELTA) {
-      sclr = __fdiv_rn(e.s1 + G4R_EPS_ADA, A + G4R_EPS_ADA);
-      float U = e.s1 * md.ap1;
-      for (int k = 0; k < n; k++) { const float g = gk(k) * gsc; U += md.ap1c * sclr * g * g; }
-      e.s1 = U;
-      sclr = sqrtf(sclr);
-    } else sclr = __fdiv_rn(1.0f, sqrtf(A + G4R_EPS_ADA));
-    e.s0 = A;
-  } else if (ad == G4R_ADAPT_ADAM) {
-    A = e.s0 * md.ap2;
-    float Mg = e.s1 * md.ap1;
-    for (int k = 0; k < n; k++) { const float g = gk(k) * gsc; A += md.ap2c * g * g; Mg += md.ap1c * (SPARSE ? g * g : g); }
-    const float ct = e.s2 + 1.0f;
-    const float bias = 1.0f - powf(md.ap1, ct);
-    common = __fdiv_rn(__fdiv_rn(Mg, bias), sqrtf(__fdiv_rn(A, bias)) + G4R_EPS_ADA);
-    e.s0 = A; e.s1 = Mg; e.s2 = ct;
-  }
-  const float v0 = e.v, a0 = e.s0;
-  float ps = e.p, vl = e.v, al = e.s0;
-  for (int k = 0; k < n; k++) {
-    const float g = gk(k) * gsc;
-    float gs;
-    if (ad == G4R_ADAPT_ADAGRAD) { al = a0 + g * g; gs = __fdiv_rn(g, sqrtf(al + G4R_EPS_ADA)); }
-    else if (ad == G4R_ADAPT_RMSPROP) gs = g * sclr;
-    else if (ad == G4R_ADAPT_ADADELTA) gs = g * sclr;
-    else if (ad == G4R_ADAPT_ADAM) gs = common;
-    else gs = g;
-    if (SPARSE) {
-      const float d = md.lmbd > 0.f ? md.lr * (gs + md.lmbd * p0l) : md.lr * gs;
-      if (mom) { vl = md.mom * v0 - d; ps += vl; } else ps -= d;
-    } else {
-      if (mom) { vl = md.mom * v0 - md.lr * (gs + md.lmbd * e.p); ps = e.p + vl; }
-      else ps = e.p * (1.0f - md.lr * md.lmbd) - md.lr * gs;
-    }
-  }
-  if (ad == G4R_ADAPT_ADAGRAD) e.s0 = al;
-  e.p = ps; e.v = vl;
-}
-// number of adaptive state arrays per parameter (they sit one after the other, `stride` elements apart, behind `*.acc`)
-__host__ __device__ inline int opt_states(int adapt) { return adapt == G4R_ADAPT_ADAM ? 3 : (adapt == G4R_ADAPT_ADADELTA ? 2 : (adapt == G4R_ADAPT_NONE ? 0 : 1)); }
-// generic (any scaler) row update: one row of `ld` elements, n members, element-wise over the lanes of a warp / threads of a CTA
-template <class FG>
-__device__ __forceinline__ void opt_row_generic(const ModelDev& md, float* prow, float* arow, size_t ast, float* vrow, const float* p0row, int ld,
-                                                int n, int t0, int tstep, bool write_state, FG grow /* (member k, column c) -> gradient */) {
-  const int ns = opt_states(md.adapt);
-  for (int c = t0; c < ld; c += tstep) {
-    OptE e;
-    e.p = prow[c];
-    e.s0 = ns > 0 ? arow[c] : 0.f; e.s1 = ns > 1 ? arow[ast + c] : 0.f; e.s2 = ns > 2 ? arow[2 * ast + c] : 0.f;
-    e.v = vrow ? vrow[c] : 0.f;
-    opt_elem<true>(md, e, p0row ? p0row[c] : e.p, n, [&](int k) { return grow(k, c); });
-    prow[c] = e.p;
-    if (write_state) {
-      if (ns > 0) arow[c] = e.s0;
-      if (ns > 1) arow[ast + c] = e.s1;
-      if (ns > 2) arow[2 * ast + c] = e.s2;
-      if (vrow) vrow[c] = e.v;
-    }
-  }
-}
+#include "g4r_opt.cuh"
 
-// dense Adagrad(+momentum) on one element (gru4rec.py:330-340,390-406)
+// dense update of one element (gru4rec.py:330-406)
 __device__ __forceinline__ void dense_update(const ModelDev& md, float* p, float* acc, float* vel, float g, size_t ast = 0) {
   if (md.adapt > G4R_ADAPT_ADAGRAD) {
     const int ns = opt_states(md.adapt);
@@ -419,21 +340,7 @@ __device__ __forceinline__ void dense_update(const ModelDev& md, float* p, float
     if (vel) *vel = e.v;
     return;
   }
-  g *= grad_scale(md);
-  float gs = g;
-  if (md.adapt == G4R_ADAPT_ADAGRAD) {
-    float a = *acc + g * g;
-    *acc = a;
-    gs = __fdiv_rn(g, sqrtf(a + G4R_EPS_ADA));
-  }
-  float pv = *p;
-  if (md.mom > 0.f) {
-    float v2 = md.mom * (*vel) - md.lr * (gs + md.lmbd * pv);
-    *vel = v2;
-    *p = pv + v2;
-  } else {
-    *p = pv * (1.0f - md.lr * md.lmbd) - md.lr * gs;
-  }
+  dense_elem(md, md.adapt == G4R_ADAPT_ADAGRAD, md.mom > 0.f, g * grad_scale(md), p, acc, vel);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1036,31 +943,17 @@ __device__ __forceinline__ void sparse_row_update(const ModelDev& md, float* __r
   }
   const float gsc = grad_scale(md);
   for (int c4 = lane; c4 < ld / 4; c4 += 32) {
-    const float4 p0 = ld4(prow + c4 * 4);
-    float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0;
-    if (ada) a0 = ld4(arow + c4 * 4);
-    if (mom) v0 = ld4(vrow + c4 * 4);
-    float4 ps = p0;
+    const float4 p0 = ld4(prow + c4 * 4), z = make_float4(0.f, 0.f, 0.f, 0.f);
+    RowChain<float4> u;
+    u.begin(p0, p0, ada ? ld4(arow + c4 * 4) : z, mom ? ld4(vrow + c4 * 4) : z);
     for (int k = 0; k < n_members; k++) {
       float4 g = ld4(gsrc + (size_t)k * gstride + c4 * 4);
       g.x *= gsc; g.y *= gsc; g.z *= gsc; g.w *= gsc;
-      float4 gs = g;
-      if (ada) {
-        al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-        gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-        gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-      }
-      float4 d;
-      if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-      else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-      if (mom) {
-        vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-        ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-      } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
+      u.add(md, g, ada, mom);
     }
-    st4(prow + c4 * 4, ps);
-    if (ada) st4(arow + c4 * 4, al);
-    if (mom) st4(vrow + c4 * 4, vl);
+    st4(prow + c4 * 4, u.ps);
+    if (ada) st4(arow + c4 * 4, u.al);
+    if (mom) st4(vrow + c4 * 4, u.vl);
   }
 }
 
@@ -1087,17 +980,12 @@ __device__ __forceinline__ void chunk_rows_update(const ModelDev& md, const int*
     } else if (lane == 0) {   // By (gru4rec.py:486-489)
       const float gsc = grad_scale(md);
       const float p0 = md.By[item];
-      float a0 = ada ? md.By_acc[item] : 0.f, v0 = mom ? md.By_vel[item] : 0.f, al = 0.f, vl = 0.f, ps = p0;
-      for (int jj = j; jj < je; jj++) {
-        const float g = gDby[jj - gDoff] * gsc;
-        float gs = g;
-        if (ada) { al = a0 + g * g; gs = __fdiv_rn(g, sqrtf(al + G4R_EPS_ADA)); }
-        const float d = md.lmbd > 0.f ? md.lr * (gs + md.lmbd * p0) : md.lr * gs;
-        if (mom) { vl = md.mom * v0 - d; ps += vl; } else ps -= d;
-      }
-      md.By[item] = ps;
-      if (ada) md.By_acc[item] = al;
-      if (mom) md.By_vel[item] = vl;
+      RowChain<float> u;
+      u.begin(p0, p0, ada ? md.By_acc[item] : 0.f, mom ? md.By_vel[item] : 0.f);
+      for (int jj = j; jj < je; jj++) u.add(md, gDby[jj - gDoff] * gsc, ada, mom);
+      md.By[item] = u.ps;
+      if (ada) md.By_acc[item] = u.al;
+      if (mom) md.By_vel[item] = u.vl;
     }
   }
 }
@@ -1448,7 +1336,7 @@ __device__ void phase_sparse_in(const ModelDev& md, int s, int b, bool apply_pas
   const float gsc = grad_scale(md);
   for (int c4 = threadIdx.x; c4 < ld / 4; c4 += blockDim.x) {
     const float4 pcur = ld4(prow + c4 * 4);
-    float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, al = a0, vl = a0, p0 = pcur;
+    float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), v0 = a0, p0 = pcur;
     if (shared) {
       p0 = ld4(md.Sx + (size_t)b * ldg + c4 * 4);         // row value before the Wy update (sparam)
       if (ada) a0 = ld4(md.snapAcc + (size_t)b * ldg + c4 * 4);
@@ -1457,28 +1345,17 @@ __device__ void phase_sparse_in(const ModelDev& md, int s, int b, bool apply_pas
       if (ada) a0 = ld4(tacc + (size_t)item * ld + c4 * 4);
       if (mom) v0 = ld4(tvel + (size_t)item * ld + c4 * 4);
     }
-    float4 ps = pcur;
+    RowChain<float4> u;
+    u.begin(pcur, p0, a0, v0);
     for (int bb = b; bb >= 0; bb = xnext[bb]) {
       float4 g = ld4(G + (size_t)bb * ldg + c4 * 4);
       g.x *= gsc; g.y *= gsc; g.z *= gsc; g.w *= gsc;
-      float4 gs = g;
-      if (ada) {
-        al.x = a0.x + g.x * g.x; al.y = a0.y + g.y * g.y; al.z = a0.z + g.z * g.z; al.w = a0.w + g.w * g.w;
-        gs.x = __fdiv_rn(g.x, sqrtf(al.x + G4R_EPS_ADA)); gs.y = __fdiv_rn(g.y, sqrtf(al.y + G4R_EPS_ADA));
-        gs.z = __fdiv_rn(g.z, sqrtf(al.z + G4R_EPS_ADA)); gs.w = __fdiv_rn(g.w, sqrtf(al.w + G4R_EPS_ADA));
-      }
-      float4 d;
-      if (md.lmbd > 0.f) { d.x = md.lr * (gs.x + md.lmbd * p0.x); d.y = md.lr * (gs.y + md.lmbd * p0.y); d.z = md.lr * (gs.z + md.lmbd * p0.z); d.w = md.lr * (gs.w + md.lmbd * p0.w); }
-      else { d.x = md.lr * gs.x; d.y = md.lr * gs.y; d.z = md.lr * gs.z; d.w = md.lr * gs.w; }
-      if (mom) {
-        vl.x = md.mom * v0.x - d.x; vl.y = md.mom * v0.y - d.y; vl.z = md.mom * v0.z - d.z; vl.w = md.mom * v0.w - d.w;
-        ps.x += vl.x; ps.y += vl.y; ps.z += vl.z; ps.w += vl.w;
-      } else { ps.x -= d.x; ps.y -= d.y; ps.z -= d.z; ps.w -= d.w; }
+      u.add(md, g, ada, mom);
     }
-    st4(prow + c4 * 4, ps);
+    st4(prow + c4 * 4, u.ps);
     if (write_state) {
-      if (ada) st4(tacc + (size_t)item * ld + c4 * 4, al);
-      if (mom) st4(tvel + (size_t)item * ld + c4 * 4, vl);
+      if (ada) st4(tacc + (size_t)item * ld + c4 * 4, u.al);
+      if (mom) st4(tvel + (size_t)item * ld + c4 * 4, u.vl);
     }
   }
 }
