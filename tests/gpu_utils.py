@@ -306,9 +306,12 @@ def _assert_path(path, before, after, step_mode, tag):
         tag, path, launches, fast, fallback)
 
 
-def f64_run_steps(eng, mk, n_items, store, steps, P0, path):
+def f64_run_steps(eng, mk, n_items, store, steps, P0, path, run=None):
     """Runs `steps` through Engine.train_step on the kernel `path` (one of STEP_PATHS, or one per step; None: no counters are
-    checked); before each step a float64 oracle is re-seeded from the device state (errors do not compound), after it every
+    checked).  A step is (X, Y, R), or a step of orc.build_train_schedule (a dict that also holds `slots`, the H row of each
+    lane: H is compared at those rows and the oracle runs with them); `run(k, X, Y, R)`, if given, runs step k on the device
+    instead of Engine.train_step and returns its cost.  Step k takes sample-store row k and dropout step k.
+    Before each step a float64 oracle is re-seeded from the device state (errors do not compound), after it every
     product the path keeps is paired with the oracle's: the cost, y, H and dvec = [da_h | da_r | da_z] of every layer, dSx
     (embedding modes) and the DSY rows the path wrote.  Plain SGD: every gradient is recovered from the update, W0 - W1 =
     lr * g (* the grad_cap scale): the dense ones, and the rows of Wx0 / E / Wy / By (one fp32 rounding per duplicate).  Any
@@ -321,7 +324,8 @@ def f64_run_steps(eng, mk, n_items, store, steps, P0, path):
     sgd = mk.get('adapt', 'adagrad') is None and not mk.get('momentum', 0) and not mk.get('lmbd', 0)
     ulp = lambda a, b: 2.0 ** -23 * (np.abs(a) + np.abs(b))        # rounding of one fp32 update
     checks, outs, scales = [], {}, []
-    for k, (X, Y, R) in enumerate(steps):
+    for k, st in enumerate(steps):
+        X, Y, R, lanes = (st['X'], st['Y'], st['R'], st['slots']) if isinstance(st, dict) else tuple(st) + (None,)
         m = oracle_f64(eng, mk, n_items, k, P0)
         names, slots = param_names(m), opt_slots(m)
         nl = len(m.layers)
@@ -332,17 +336,18 @@ def f64_run_steps(eng, mk, n_items, store, steps, P0, path):
             eng.set('DSY', np.full(eng.shape('DSY'), np.nan, np.float32))
         tag = 'step %d (M=%d) ' % (k + 1, len(X))
         c0 = _counters(eng)
-        cost = eng.train_step(X, Y, R)
+        cost = eng.train_step(X, Y, R) if run is None else run(k, X, Y, R)
         if paths[k] is not None:
             _assert_path(paths[k], c0, _counters(eng), eng.cfg.step_mode, tag)
-        ref_cost = m.train_step(X, Y, R, samples=store[k])
+        ref_cost = m.train_step(X, Y, R, samples=store[k], slots=lanes)
         C, G = m.last_cache, m.last_grads
         M, N = len(X), len(C['Y'])
         ys = [lc['inp'] for lc in C['layers'][1:]] + [C['y_last']]
         dev, ref = dict(cost=np.float64(cost)), dict(cost=ref_cost)
+        hrows = slice(None, M) if lanes is None else np.asarray(lanes)
         for i in range(nl):
             for n, r in (('y', ys[i]), ('H', C['H_new'][i]), ('dvec', G['dvec'][i])):
-                dev['%s%d' % (n, i)], ref['%s%d' % (n, i)] = eng.get('%s%d' % (n, i))[:M], r
+                dev['%s%d' % (n, i)], ref['%s%d' % (n, i)] = eng.get('%s%d' % (n, i))[hrows if n == 'H' else slice(None, M)], r
         if C['mode'] != 'none':
             dev['dSx'], ref['dSx'] = eng.get('dSx')[:M], G['dSx']
         if paths[k] != 'fast':
