@@ -44,6 +44,8 @@ EXPORTS = [
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
     'g4r_eval_schedule', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
+    'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
+    'g4r_sessions_export', 'g4r_sessions_import',
 ]
 
 _lib = None
@@ -113,6 +115,13 @@ def load():
     lib.g4r_reset_eval_hidden.argtypes = [vp]
     lib.g4r_predict_topk.argtypes = [vp, vp, i32, vp, i32, vp, vp]
     lib.g4r_predict_topk_filtered.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp, vp]
+    lib.g4r_sessions_open.argtypes = [vp, i64]
+    lib.g4r_sessions_count.argtypes = [vp, C.POINTER(i64)]; lib.g4r_sessions_count.restype = i64
+    lib.g4r_sessions_feed.argtypes = [vp, vp, vp, i64]
+    lib.g4r_sessions_topk.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, vp, i32, vp, vp]
+    lib.g4r_sessions_end.argtypes = [vp, vp, i64]
+    lib.g4r_sessions_export.argtypes = [vp, vp, vp, vp, vp]
+    lib.g4r_sessions_import.argtypes = [vp, vp, vp, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -518,6 +527,16 @@ class Engine(object):
             out_s = np.empty((len(X), k), dtype=np.float32)
             self._check(self.lib.g4r_predict_topk(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(out_i), _ptr(out_s)))
             return out_i, out_s
+        k, cand, off, ex = self._topk_filters(len(X), k, items, exclude)
+        out_i = np.empty((len(X), k), dtype=np.int32)
+        out_s = np.empty((len(X), k), dtype=np.float32)
+        self._check(self.lib.g4r_predict_topk_filtered(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(cand), 0 if cand is None else cand.size,
+                                                       _ptr(off), _ptr(ex), _ptr(out_i), _ptr(out_s)))
+        return out_i, out_s
+
+    def _topk_filters(self, n, k, items, exclude):
+        """k checked against the candidates, and the filter arrays of g4r_predict_topk_filtered / g4r_sessions_topk: candidate
+        item indices (or None), exclusion offsets [n + 1] and items (or None)"""
         cand = None
         n_distinct = self.cfg.n_items
         if items is not None:
@@ -529,20 +548,81 @@ class Engine(object):
         k = check_topk(k, n_distinct)
         off = ex = None
         if exclude is not None:
-            if len(exclude) != len(X):
-                raise ValueError('exclude must hold one entry per lane (%d), got %d' % (len(X), len(exclude)))
+            if len(exclude) != n:
+                raise ValueError('exclude must hold one entry per lane (%d), got %d' % (n, len(exclude)))
             parts = [np.asarray(e if e is not None else [], dtype=np.int64).reshape(-1) for e in exclude]
-            off = np.zeros(len(X) + 1, dtype=np.int64)
+            off = np.zeros(n + 1, dtype=np.int64)
             off[1:] = np.cumsum([len(p) for p in parts])
             ex = np.concatenate(parts) if parts else np.zeros(0, np.int64)
             if ex.size and (ex.min() < 0 or ex.max() >= self.cfg.n_items):
                 raise IndexError('excluded item index out of range')
             ex = np.ascontiguousarray(ex, dtype=np.int32)
-        out_i = np.empty((len(X), k), dtype=np.int32)
-        out_s = np.empty((len(X), k), dtype=np.float32)
-        self._check(self.lib.g4r_predict_topk_filtered(self.h, _ptr(X), len(X), _ptr(rm), k, _ptr(cand), 0 if cand is None else cand.size,
-                                                       _ptr(off), _ptr(ex), _ptr(out_i), _ptr(out_s)))
-        return out_i, out_s
+        return k, cand, off, ex
 
     def reset_eval_hidden(self):
         self._check(self.lib.g4r_reset_eval_hidden(self.h))
+
+    # ---- session store (g4r_sessions_*, DESIGN §3e) ----
+    session_capacity = None       # capacity of the open store (None: not opened)
+
+    def sessions_open(self, capacity):
+        """(Re)creates an empty session store of `capacity` sessions."""
+        self._check(self.lib.g4r_sessions_open(self.h, int(capacity)))
+        self.session_capacity = int(capacity)
+
+    def sessions_count(self):
+        """(number of sessions, total length of their histories)"""
+        nh = C.c_int64()
+        n = self.lib.g4r_sessions_count(self.h, C.byref(nh))
+        self._check(int(n) if n < 0 else 0)
+        return int(n), nh.value
+
+    def sessions_feed(self, keys, X):
+        """Advances session keys[i] by item index X[i] without scoring (keys may repeat; a key's events apply in order)."""
+        keys = np.ascontiguousarray(keys, dtype=np.int64); X = np.ascontiguousarray(X, dtype=np.int32)
+        if keys.shape != X.shape:
+            raise ValueError('keys and X differ in length')
+        self._check(self.lib.g4r_sessions_feed(self.h, _ptr(keys), _ptr(X), keys.size))
+
+    def sessions_topk(self, keys, X, k, items=None, exclude=None, exclude_seen=False):
+        """predict_topk for sessions addressed by key (distinct within a call): advances session keys[i] by item index X[i] and
+        returns its k best next items (items int32 [n, k], scores float32 [n, k]).  Filters as in predict_topk; exclude_seen
+        also excludes the items fed to the session since it entered the store, this input included."""
+        keys = np.ascontiguousarray(keys, dtype=np.int64); X = np.ascontiguousarray(X, dtype=np.int32)
+        if keys.shape != X.shape:
+            raise ValueError('keys and X differ in length')
+        k, cand, off, ex = self._topk_filters(keys.size, k, items, exclude)
+        out_i = np.empty((keys.size, k), dtype=np.int32)
+        out_s = np.empty((keys.size, k), dtype=np.float32)
+        self._check(self.lib.g4r_sessions_topk(self.h, _ptr(keys), _ptr(X), keys.size, k, _ptr(cand), 0 if cand is None else cand.size,
+                                               _ptr(off), _ptr(ex), 1 if exclude_seen else 0, _ptr(out_i), _ptr(out_s)))
+        return out_i, out_s
+
+    def sessions_end(self, keys=None):
+        """Drops the given sessions (unknown keys ignored), or every session."""
+        if keys is None:
+            self._check(self.lib.g4r_sessions_end(self.h, None, 0))
+            return
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        self._check(self.lib.g4r_sessions_end(self.h, _ptr(keys), keys.size))
+
+    def sessions_export(self):
+        """Every session, least recently used first: keys int64 [n], states float32 [n, sum of layer widths], history offsets
+        int64 [n + 1] and items int32."""
+        n, nh = self.sessions_count()
+        Lsum = int(sum(self.cfg.layers[i] for i in range(self.cfg.n_layers)))
+        keys = np.empty(n, np.int64); states = np.empty((n, Lsum), np.float32)
+        off = np.empty(n + 1, np.int64); items = np.empty(nh, np.int32)
+        self._check(self.lib.g4r_sessions_export(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(items)))
+        return keys, states, off, items
+
+    def sessions_import(self, keys, states, hist_off=None, hist_items=None):
+        """Inserts sessions in order as the most recently used (layouts of sessions_export); existing keys are overwritten."""
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        Lsum = int(sum(self.cfg.layers[i] for i in range(self.cfg.n_layers)))
+        states = np.ascontiguousarray(np.asarray(states, dtype=np.float32).reshape(keys.size, Lsum))
+        off = None if hist_off is None else np.ascontiguousarray(hist_off, dtype=np.int64)
+        it = None if hist_items is None else np.ascontiguousarray(hist_items, dtype=np.int32)
+        if off is not None and off.size != keys.size + 1:
+            raise ValueError('hist_off must have %d entries' % (keys.size + 1))
+        self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))

@@ -307,14 +307,16 @@ static int eval_ctx(g4r_handle* h, EvalCtx** out) {
   return G4R_OK;
 }
 
-static int eval_forward(g4r_handle* h, EvalCtx* e, int s) {
+// GRU forward of step s of the scoring window; Hst[li]: the hidden-state array of layer li that the staged slots address (the
+// handle's lanes He, or a session table)
+static int eval_forward(g4r_handle* h, EvalCtx* e, int s, float* const* Hst) {
   const ModelDev& md = e->mde;
   cudaStream_t st = h->stream;
   if (md.mode != 0) { k_gather_in<<<std::max(1, (e->Be + 7) / 8), 256, 0, st>>>(e->slot, nullptr, s, 0); h->launches++; }
   for (int li = 0; li < md.n_layers; li++) {
     const LayerDev& ly = md.layer[li];
-    k_f1<<<tiles2(2 * ly.L, e->Be), GEMM_THREADS, 0, st>>>(e->slot, nullptr, s, li, h->He[li]);
-    k_f2<<<tiles2(ly.L, e->Be), GEMM_THREADS, 0, st>>>(e->slot, nullptr, s, li, h->He[li], 0);
+    k_f1<<<tiles2(2 * ly.L, e->Be), GEMM_THREADS, 0, st>>>(e->slot, nullptr, s, li, Hst[li]);
+    k_f2<<<tiles2(ly.L, e->Be), GEMM_THREADS, 0, st>>>(e->slot, nullptr, s, li, Hst[li], 0);
     h->launches += 2;
   }
   return G4R_OK;
@@ -375,7 +377,7 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
     // sums) is ordered by the ranking stream itself, so the sums accumulate in mini-batch order as before.
     cudaStream_t rk = h->side;
     for (int64_t i = 0; i < w; i++) {
-      eval_forward(h, e, (int)i);
+      eval_forward(h, e, (int)i, h->He);
       CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
       k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
       const int n_comp = e->n_cand > 0 ? e->n_cand : I;
@@ -472,7 +474,7 @@ extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const
   cudaStream_t st = h->stream;
   const size_t need = (size_t)batch * I;
   CK(dev_grow(&e->dOut, &e->out_cap, need));
-  eval_forward(h, e, 0);
+  eval_forward(h, e, 0, h->He);
   k_eval_score<true><<<(I + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, e->dOut, nullptr, 0);
   k_predict_act<<<batch, 256, 0, st>>>(e->slot, e->dOut, batch);
   h->launches += 2;
@@ -492,3 +494,4 @@ extern "C" int g4r_reset_eval_hidden(g4r_handle* h) {
 }
 
 #include "g4r_topk.cuh"
+#include "g4r_sessions.cuh"

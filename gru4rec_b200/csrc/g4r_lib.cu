@@ -17,6 +17,7 @@
 static thread_local std::string g_create_error;
 struct g4r_handle;
 static void eval_release(g4r_handle* h);
+static void sessions_release(g4r_handle* h);
 static void mg_release(g4r_handle* h);
 static void shard_release(g4r_handle* h);
 static bool shard_eligible(const g4r_config& c, int n_sm);
@@ -74,6 +75,7 @@ struct g4r_handle {
   GridBar* dGridBar = nullptr; unsigned long long* dStamp = nullptr; int pk_blocks = 0; size_t pk_smem = 0;
   bool mg_alloc = false; MgDev mgdev; std::vector<MgTensor> mg_tensors;
   void* eval_ctx = nullptr;      // EvalCtx* (g4r_eval.cuh), owned by the handle
+  void* sessions = nullptr;      // SessStore* (g4r_sessions.cuh), owned by the handle
   uint64_t wy_version = 0;       // bumped by everything that may change Wy / By (caches derived from them compare it)
   void* mg_host = nullptr;       // MgHost*  (g4r_multi.cuh), owned by the handle
   void* shard = nullptr;         // ShardHost* (g4r_shard.cuh): row-sharded item tables + in-kernel exchange, owned by the handle
@@ -680,6 +682,7 @@ extern "C" int g4r_destroy(g4r_handle* h) {
   if (!h) return G4R_OK;
   cudaSetDevice(h->cfg.device);
   if (h->stream) cudaStreamSynchronize(h->stream);
+  sessions_release(h);
   eval_release(h);
   if (h->ts_buf) { delete static_cast<TsBuf*>(h->ts_buf); h->ts_buf = nullptr; }
   shard_release(h);

@@ -416,75 +416,121 @@ static int topk_ctx(g4r_handle* h, EvalCtx* e, TopkCtx** out) {
   return G4R_OK;
 }
 
+// The candidate filter of a top-k call, validated with k: a bitmap of the distinct candidate items (the cache key of the device
+// copy; empty: the whole catalogue)
+struct TopkFilter {
+  std::vector<uint32_t> cmask;
+  int n_distinct = 0;
+  bool use_cand = false;                                  // false when every item is a candidate: the unfiltered catalogue
+  bool is_cand(int v) const { return !use_cand || ((cmask[(size_t)v >> 5] >> (v & 31)) & 1u); }
+};
+
+static int topk_filter(g4r_handle* h, int32_t k, const int32_t* cand, int64_t n_cand, TopkFilter* f) {
+  const int I = h->md.n_items;
+  f->n_distinct = I;
+  if (cand) {
+    if (n_cand < 0) FAIL(G4R_ERR_INVALID, "n_cand must be >= 0");
+    f->cmask.assign((size_t)(I + 31) / 32, 0u);
+    for (int64_t i = 0; i < n_cand; i++) {
+      const int32_t c = cand[i];
+      if (c < 0 || c >= I) FAIL(G4R_ERR_INDEX, "candidate item out of bounds");
+      f->cmask[(size_t)c >> 5] |= 1u << (c & 31);
+    }
+    f->n_distinct = 0;
+    for (const uint32_t w : f->cmask) f->n_distinct += __builtin_popcount(w);
+  }
+  if (k < 1 || k > f->n_distinct || k > G4R_TOPK_MAX)
+    FAIL(G4R_ERR_INVALID, cand ? "k must be in 1 .. min(distinct candidates, G4R_TOPK_MAX)" : "k must be in 1 .. min(n_items, G4R_TOPK_MAX)");
+  if (h->shard) FAIL(G4R_ERR_STATE, "g4r_predict_topk: not available on a row-sharded multi-GPU handle");
+  f->use_cand = cand && f->n_distinct < I;
+  if (!f->use_cand) f->cmask.clear();
+  return G4R_OK;
+}
+
+// excl_off[0 .. n] of a call with n lanes: non-decreasing from 0, items in range
+static int topk_check_excl(g4r_handle* h, int64_t n, const int64_t* excl_off, const int32_t* excl_items) {
+  if (excl_off[0] != 0) FAIL(G4R_ERR_INVALID, "excl_off[0] must be 0");
+  for (int64_t b = 0; b < n; b++) if (excl_off[b + 1] < excl_off[b]) FAIL(G4R_ERR_INVALID, "excl_off must be non-decreasing");
+  if (excl_off[n] > 0 && !excl_items) FAIL(G4R_ERR_INVALID, "excl_items is NULL");
+  for (int64_t j = 0; j < excl_off[n]; j++)
+    if (excl_items[j] < 0 || excl_items[j] >= h->md.n_items) FAIL(G4R_ERR_INDEX, "excluded item out of bounds");
+  return G4R_OK;
+}
+
+// exclusions of one lane: the (validated) items v[0 .. n) that are candidates (no other item can win anyway) appended to ex
+static void topk_add_excl(const TopkFilter& f, const int32_t* v, int64_t n, std::vector<int>& ex) {
+  for (int64_t j = 0; j < n; j++) if (f.is_cand(v[j])) ex.push_back(v[j]);
+}
+// ends the lane whose exclusions start at ex[e0]: sorted and distinct, its end offset appended to ex_off
+static int topk_close_lane(g4r_handle* h, std::vector<int>& ex_off, std::vector<int>& ex, size_t e0) {
+  std::sort(ex.begin() + e0, ex.end());
+  ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
+  if (ex.size() > (size_t)INT32_MAX) FAIL(G4R_ERR_INVALID, "too many exclusions");
+  ex_off.push_back((int)ex.size());
+  return G4R_OK;
+}
+
+static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, int32_t k, const TopkFilter& f,
+                     const std::vector<int>& ex_off, const std::vector<int>& ex, int32_t* out_items, float* out_scores);
+
 extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
                                          const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
                                          int32_t* out_items, float* out_scores) {
   if (!h || !X || !out_items || !out_scores) return G4R_ERR_INVALID;
-  const int I = h->md.n_items;
-  // candidates: a bitmap of the distinct items (the cache key of the device copy)
-  std::vector<uint32_t> cmask;
-  int n_distinct = I;
-  if (cand) {
-    if (n_cand < 0) FAIL(G4R_ERR_INVALID, "n_cand must be >= 0");
-    cmask.assign((size_t)(I + 31) / 32, 0u);
-    for (int64_t i = 0; i < n_cand; i++) {
-      const int32_t c = cand[i];
-      if (c < 0 || c >= I) FAIL(G4R_ERR_INDEX, "candidate item out of bounds");
-      cmask[(size_t)c >> 5] |= 1u << (c & 31);
-    }
-    n_distinct = 0;
-    for (const uint32_t w : cmask) n_distinct += __builtin_popcount(w);
-  }
-  if (k < 1 || k > n_distinct || k > G4R_TOPK_MAX)
-    FAIL(G4R_ERR_INVALID, cand ? "k must be in 1 .. min(distinct candidates, G4R_TOPK_MAX)" : "k must be in 1 .. min(n_items, G4R_TOPK_MAX)");
-  if (h->shard) FAIL(G4R_ERR_STATE, "g4r_predict_topk: not available on a row-sharded multi-GPU handle");
-  const bool use_cand = cand && n_distinct < I;          // every item a candidate: the unfiltered catalogue
-  // exclusions: per lane sorted and distinct, restricted to the candidates (no other item can win anyway)
+  TopkFilter f;
+  int rc = topk_filter(h, k, cand, n_cand, &f);
+  if (rc) return rc;
+  // exclusions: per lane sorted and distinct, restricted to the candidates
   std::vector<int> ex_off, ex;
-  int max_ex = 0;
   if (excl_off) {
     if (batch <= 0) FAIL(G4R_ERR_INVALID, "predict batch exceeds eval_batch_size");
-    if (excl_off[0] != 0) FAIL(G4R_ERR_INVALID, "excl_off[0] must be 0");
-    for (int b = 0; b < batch; b++) if (excl_off[b + 1] < excl_off[b]) FAIL(G4R_ERR_INVALID, "excl_off must be non-decreasing");
-    if (excl_off[batch] > 0 && !excl_items) FAIL(G4R_ERR_INVALID, "excl_items is NULL");
-    ex_off.assign((size_t)batch + 1, 0);
+    rc = topk_check_excl(h, batch, excl_off, excl_items);
+    if (rc) return rc;
+    ex_off.push_back(0);
     for (int b = 0; b < batch; b++) {
       const size_t e0 = ex.size();
-      for (int64_t j = excl_off[b]; j < excl_off[b + 1]; j++) {
-        const int32_t v = excl_items[j];
-        if (v < 0 || v >= I) FAIL(G4R_ERR_INDEX, "excluded item out of bounds");
-        if (!use_cand || ((cmask[(size_t)v >> 5] >> (v & 31)) & 1u)) ex.push_back(v);
-      }
-      std::sort(ex.begin() + e0, ex.end());
-      ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
-      if (ex.size() > (size_t)INT32_MAX) FAIL(G4R_ERR_INVALID, "too many exclusions");
-      ex_off[(size_t)b + 1] = (int)ex.size();
-      max_ex = std::max(max_ex, (int)(ex.size() - e0));
+      topk_add_excl(f, excl_items + excl_off[b], excl_off[b + 1] - excl_off[b], ex);
+      rc = topk_close_lane(h, ex_off, ex, e0);
+      if (rc) return rc;
     }
   }
-  const bool use_ex = !ex.empty();
   cudaSetDevice(h->cfg.device);
   EvalCtx* e = nullptr;
-  int rc = eval_ctx(h, &e);
+  rc = eval_ctx(h, &e);
   if (rc) return rc;
   rc = predict_stage(h, e, X, batch, reset_mask);
   if (rc) return rc;
+  return topk_rank(h, e, h->He, batch, k, f, ex_off, ex, out_items, out_scores);
+}
+
+// The shared ranking of g4r_predict_topk_filtered and g4r_sessions_topk: the GRU forward of the lanes staged at step 0 of the
+// scoring window, reading and writing hidden states in Hst (one array per layer, addressed by the staged slots), then the k best
+// items of every lane under the filter f and the per-lane exclusions ex_off / ex (empty: none; built by topk_add_excl /
+// topk_close_lane) into out_items / out_scores [batch x k] (host)
+static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, int32_t k, const TopkFilter& f,
+                     const std::vector<int>& ex_off, const std::vector<int>& ex, int32_t* out_items, float* out_scores) {
+  const int I = h->md.n_items;
+  const bool use_cand = f.use_cand;
+  const int n_distinct = f.n_distinct;
+  const bool use_ex = !ex.empty();
+  int max_ex = 0;
+  for (size_t b = 1; b < ex_off.size(); b++) max_ex = std::max(max_ex, ex_off[b] - ex_off[b - 1]);
   TopkCtx* t = nullptr;
-  rc = topk_ctx(h, e, &t);
+  int rc = topk_ctx(h, e, &t);
   if (rc) return rc;
   cudaStream_t st = h->stream;
   const int L = h->md.L;
-  if (use_cand && t->hMask != cmask) {                    // a candidate set other than the cached one
+  if (use_cand && t->hMask != f.cmask) {                  // a candidate set other than the cached one
     t->hMask.clear();
     std::vector<int> list;
     list.reserve((size_t)n_distinct);
-    for (int i = 0; i < I; i++) if ((cmask[(size_t)i >> 5] >> (i & 31)) & 1u) list.push_back(i);
-    CK(dev_grow(&t->dMask, &t->mask_cap, cmask.size()));
+    for (int i = 0; i < I; i++) if (f.is_cand(i)) list.push_back(i);
+    CK(dev_grow(&t->dMask, &t->mask_cap, f.cmask.size()));
     CK(dev_grow(&t->dCand, &t->cand_cap, list.size()));
-    CK(cudaMemcpyAsync(t->dMask, cmask.data(), cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(t->dMask, f.cmask.data(), f.cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(t->dCand, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
-    t->hMask.swap(cmask);
+    t->hMask = f.cmask;
   }
   if (use_ex) {
     CK(dev_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
@@ -523,7 +569,7 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
       t->absmax_version = h->wy_version;
     }
   }
-  eval_forward(h, e, 0);
+  eval_forward(h, e, 0, Hst);
   // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the items 0 .. P-1) and tau_b
   k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, dcand, P);
   h->launches++;

@@ -97,6 +97,7 @@ class GRU4Rec:
         self.dropout_seed = 0
         self.eval_lanes = 512            # run.py evaluates with batch_size=512 (run.py:127)
         self.step_mode = 2               # role-specialised persistent kernel where the shape allows, else generic persistent
+        self.session_capacity = 100000   # sessions kept by recommend_sessions / feed_sessions (least recently used evicted)
         self._engine = None
         self._host = None                # numpy copies of the parameters when no engine is alive
 
@@ -274,11 +275,15 @@ class GRU4Rec:
             pass
         return 1, 0
 
-    def _build_engine(self, sample_store=0, eval_lanes=None, training=True, single=False):
-        """`single`: a one-GPU engine even under torchrun (the scoring path of every rank works on a full replica)."""
+    def _build_engine(self, sample_store=0, eval_lanes=None, training=True, single=False, keep_sessions=True):
+        """`single`: a one-GPU engine even under torchrun (the scoring path of every rank works on a full replica).
+        `keep_sessions`: the session store of the old engine (recommend_sessions) moves to the new one."""
         eval_lanes = self.eval_lanes if eval_lanes is None else eval_lanes
         host = self._host if self._host is not None else self._pull_host()
+        sessions = None
         if self._engine is not None:
+            if keep_sessions and getattr(self._engine, 'session_capacity', None) is not None:
+                sessions = (self._engine.session_capacity, self._engine.sessions_export())
             self._engine.close()
             self._engine = None
         world, rank = (1, 0) if single else self._world()
@@ -291,6 +296,9 @@ class GRU4Rec:
         if world > 1:
             import torch.distributed as dist
             eng.init_multi_gpu(dist)
+        if sessions is not None:
+            eng.sessions_open(sessions[0])
+            eng.sessions_import(*sessions[1])
         self._engine = eng
         self._engine_eval_lanes = eval_lanes
         self._host = None
@@ -406,7 +414,8 @@ class GRU4Rec:
             raise NotImplementedError("store_type='cpu' is not available for multi-GPU training; use the device sample store")
         # the training engine carries no scoring lanes: the step scratch keeps the leading dimension of the mini-batch
         # (the scoring engine with `eval_lanes` lanes is created on the first evaluate_gpu / predict_next_batch call)
-        eng = self._build_engine(sample_store=(sample_store if use_store else (2 * self.n_sample if per_step_sampling else 0)), eval_lanes=0)
+        eng = self._build_engine(sample_store=(sample_store if use_store else (2 * self.n_sample if per_step_sampling else 0)), eval_lanes=0,
+                                 keep_sessions=False)
         if P0 is not None:
             eng.set_logq_support(P0)
         if use_store:
@@ -593,6 +602,130 @@ class GRU4Rec:
         self._seen_n += 1
         return eng, reset, in_idxs
 
+    # ---- serving by session key (an addition to the reference surface; DESIGN §3e) ----
+    # The hidden state of every session lives in a device-resident store of the scoring engine, addressed by session id: events
+    # of any number of interleaved sessions can arrive in any order and any call size.  Session ids are integers (the store's
+    # keys are int64); string ids must be factorized by the caller.  The store holds `session_capacity` sessions; when a new
+    # session needs room, the least recently used session not named in the call is dropped (its next event starts afresh).
+    # The store survives rebuilds of the scoring engine and set_value(); fit() and loadmodel() start without sessions, and it
+    # is never pickled.
+    def recommend_sessions(self, session_ids, input_item_ids, k=20, items=None, exclude=None, exclude_seen=False):
+        '''
+        Session session_ids[i] has just seen item input_item_ids[i]: advances its state and returns its k best next items.
+        A session id may appear at most once per call (ValueError); a session not in the store starts from a zero state.
+        Returns (item_ids [n, k] of the original item IDs, scores [n, k] float32), best first, ranked as recommend_next_batch ranks
+        a lane.  Filters as in recommend_next_batch, per event: `items` (original item IDs competing), `exclude` (one iterable of
+        original item IDs or None per event), `exclude_seen` (every item fed to the session since it entered the store, this
+        input included).  With a filter, missing places are padded with item None and score NaN.
+        '''
+        if self.error_during_train: raise Exception
+        keys = self._session_keys(session_ids)
+        k = _lib.check_topk(k, self.n_items)
+        in_idxs = self._session_inputs(keys, input_item_ids)
+        if len(np.unique(keys)) != len(keys):
+            raise ValueError('a session id appears more than once in the call (feed_sessions takes repeated ids)')
+        cand = None
+        if items is not None:
+            cand = self.itemidmap[items].values
+            n_cand = len(np.unique(cand))
+            if k > n_cand:
+                raise ValueError('k = %d exceeds the %d distinct candidate items' % (k, n_cand))
+        if exclude is not None and len(exclude) != len(keys):
+            raise ValueError('exclude must hold one entry per event (%d), got %d' % (len(keys), len(exclude)))
+        excl = None if exclude is None else [self._item_indices(e) for e in exclude]
+        eng = self._session_engine()
+        out, scores = eng.sessions_topk(keys, in_idxs, k, items=cand, exclude=excl, exclude_seen=exclude_seen)
+        ids = self.itemidmap.index.to_numpy()
+        miss = out < 0
+        if not miss.any():
+            return ids[out], scores
+        res = ids[np.where(miss, 0, out)].astype(object)
+        res[miss] = None
+        return res, scores
+
+    def feed_sessions(self, session_ids, input_item_ids):
+        '''Advances sessions by their events without scoring; session ids may repeat (a session's events apply in order).'''
+        if self.error_during_train: raise Exception
+        keys = self._session_keys(session_ids)
+        in_idxs = self._session_inputs(keys, input_item_ids)
+        self._session_engine().sessions_feed(keys, in_idxs)
+
+    def end_sessions(self, session_ids=None):
+        '''Drops the given sessions from the store (unknown ids are ignored), or every session.'''
+        keys = None if session_ids is None else self._session_keys(session_ids)
+        if self._engine is not None and self._engine.session_capacity is not None:
+            self._engine.sessions_end(keys)
+
+    def export_sessions(self):
+        '''
+        Every session in the store, least recently used first: (session_ids int64 [n], states float32 [n, sum(layers)] -- the
+        layers' hidden states concatenated --, history: a list of n arrays of the original item IDs fed since the session entered).
+        '''
+        width = int(sum(self.layers))
+        if self._engine is None or self._engine.session_capacity is None:
+            return np.zeros(0, np.int64), np.zeros((0, width), np.float32), []
+        keys, states, off, items = self._engine.sessions_export()
+        ids = self.itemidmap.index.to_numpy()
+        return keys, states, [ids[items[off[i]:off[i + 1]]] for i in range(len(keys))]
+
+    def import_sessions(self, session_ids, states, history=None):
+        '''
+        Inserts sessions as the most recently used, in order (the layout of export_sessions); a session id already in the store is
+        overwritten.  history: one iterable of original item IDs per session (unknown IDs raise KeyError), or None.
+        '''
+        keys = self._session_keys(session_ids)
+        if len(np.unique(keys)) != len(keys):
+            raise ValueError('a session id appears more than once')
+        states = np.asarray(states, dtype=np.float32)
+        width = int(sum(self.layers))
+        if states.shape != (len(keys), width):
+            raise ValueError('states must have shape (%d, %d), got %s' % (len(keys), width, states.shape))
+        if len(keys) > int(self.session_capacity):
+            raise ValueError('%d sessions exceed session_capacity = %d' % (len(keys), int(self.session_capacity)))
+        off = items = None
+        if history is not None:
+            if len(history) != len(keys):
+                raise ValueError('history must hold one entry per session (%d), got %d' % (len(keys), len(history)))
+            parts = [self.itemidmap[list(h)].values.astype(np.int64) if len(h) else np.zeros(0, np.int64) for h in history]
+            off = np.zeros(len(keys) + 1, np.int64)
+            off[1:] = np.cumsum([len(p) for p in parts])
+            items = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+        self._session_engine().sessions_import(keys, states, off, items)
+
+    @staticmethod
+    def _session_keys(session_ids):
+        '''session ids as int64 keys; TypeError unless they are integers'''
+        a = np.asarray(session_ids)
+        if a.ndim != 1:
+            a = a.reshape(-1)
+        if a.size == 0:
+            return np.zeros(0, np.int64)
+        if a.dtype.kind not in 'iu' or (a.dtype.kind == 'u' and a.max() > np.iinfo(np.int64).max):
+            raise TypeError('session ids must be integers that fit int64 (factorize other ids first), got dtype %s' % a.dtype)
+        return a.astype(np.int64)
+
+    def _session_inputs(self, keys, input_item_ids):
+        '''item indices of the inputs (KeyError for an unknown item ID)'''
+        if len(input_item_ids) != len(keys):
+            raise ValueError('session_ids and input_item_ids differ in length (%d, %d)' % (len(keys), len(input_item_ids)))
+        if len(keys) == 0:
+            return np.zeros(0, np.int64)
+        return self.itemidmap[input_item_ids].values
+
+    def _session_engine(self):
+        '''the scoring engine with its session store open at session_capacity (a changed capacity keeps the most recent
+        sessions that fit)'''
+        eng = self._ensure_engine(1)
+        cap = int(self.session_capacity)
+        if eng.session_capacity != cap:
+            old = eng.sessions_export() if eng.session_capacity is not None else None
+            eng.sessions_open(cap)
+            if old is not None:
+                keys, states, off, items = old
+                first = max(0, len(keys) - cap)
+                eng.sessions_import(keys[first:], states[first:], off[first:] - off[first], items[off[first]:])
+        return eng
+
     # ---- persistence (gru4rec.py:742-781): pickle of the object with NumPy parameters ----
     def __getstate__(self):
         st = dict(self.__dict__)
@@ -615,8 +748,8 @@ class GRU4Rec:
                                              'top1-max': 'top1_max', 'xe_logit': 'cross_entropy_logits'}[self.loss])
         st['final_activation'] = self._act_object(self.final_act)
         st['hidden_activation'] = self._act_object(self.hidden_act)
-        for k in ('device', 'dropout_seed', 'eval_lanes', 'step_mode', '_engine_eval_lanes', 'predict', 'predict_batch', 'current_session',
-                  '_seen', '_seen_n'):
+        for k in ('device', 'dropout_seed', 'eval_lanes', 'step_mode', 'session_capacity', '_engine_eval_lanes', 'predict', 'predict_batch',
+                  'current_session', '_seen', '_seen_n'):
             st.pop(k, None)
         st['predict'] = None
         return st
@@ -646,7 +779,7 @@ class GRU4Rec:
         self._host = host
         self._engine = None
         self.predict = None
-        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2)):
+        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2), ('session_capacity', 100000)):
             if not hasattr(self, k):
                 setattr(self, k, v)
 

@@ -226,6 +226,40 @@ int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, co
 /* Zero the scoring-path hidden state (gru4rec.py:696-697). */
 int g4r_reset_eval_hidden(g4r_handle* h);
 
+/* ---- session store: scoring-path state addressed by session key (DESIGN §3e; no reference counterpart) ----------------------
+ * An int64 session key maps to a row of a device table of `capacity` hidden states per layer, separate from the lanes of
+ * g4r_predict / g4r_predict_topk and from the training state.  Every event that names a session makes it the most recently used,
+ * in call order.  A key not in the store takes a free row, else the row of the least recently used session that the call does
+ * not name; that session's state and history are dropped, and the new session starts from a zero state.  The store also keeps
+ * each session's input items since it entered (exclude_seen).  Every argument is checked before the store changes: after an
+ * error, keys, recency order, states and histories are as they were.  G4R_ERR_INVALID when a call names more distinct keys than
+ * the capacity; G4R_ERR_INDEX on an out-of-range item; G4R_ERR_STATE on a row-sharded multi-GPU handle or before
+ * g4r_sessions_open.  The results do not depend on how the events of a session are spread over calls. */
+/* (Re)creates an empty store of `capacity` sessions (1 .. 2^31 - 1); an existing store is dropped. */
+int g4r_sessions_open(g4r_handle* h, int64_t capacity);
+/* Number of sessions in the store (0 if none is open); *n_history_items (may be NULL): total length of their histories. */
+int64_t g4r_sessions_count(const g4r_handle* h, int64_t* n_history_items);
+/* Advances sessions without scoring: event i feeds item X[i] to session keys[i].  Keys may repeat; the events of one key apply
+ * in call order.  The whole call runs on the device without host round trips. */
+int g4r_sessions_feed(g4r_handle* h, const int64_t* keys, const int32_t* X, int64_t n);
+/* Advances session keys[i] by item X[i] and ranks its next items as g4r_predict_topk_filtered ranks a lane (same ranking key,
+ * ties, scores, filters and empty slots): out_items / out_scores [n x k].  Each key at most once per call (G4R_ERR_INVALID
+ * otherwise); any n (the call runs in chunks of the scoring lanes).  excl_off / excl_items: per-event exclusions as in
+ * g4r_predict_topk_filtered (excl_off has n + 1 entries).  exclude_seen != 0: the session's history, this input included, is
+ * excluded too. */
+int g4r_sessions_topk(g4r_handle* h, const int64_t* keys, const int32_t* X, int64_t n, int32_t k,
+                      const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
+                      int32_t exclude_seen, int32_t* out_items, float* out_scores);
+/* Drops the sessions keys[0 .. n) (unknown keys ignored); keys == NULL: every session. */
+int g4r_sessions_end(g4r_handle* h, const int64_t* keys, int64_t n);
+/* Every session, least recently used first (sizes from g4r_sessions_count): keys [n], states [n x sum of layer widths] (the
+ * layers' states concatenated), histories as CSR: hist_off [n + 1], hist_items [n_history_items].  Any pointer may be NULL. */
+int g4r_sessions_export(g4r_handle* h, int64_t* keys, float* states, int64_t* hist_off, int32_t* hist_items);
+/* Inserts n sessions in order as the most recently used (layouts of g4r_sessions_export; hist_off == NULL: empty histories).
+ * A key already in the store is overwritten; keys must be distinct, and at most the capacity.  Other sessions may be evicted. */
+int g4r_sessions_import(g4r_handle* h, const int64_t* keys, const float* states, const int64_t* hist_off,
+                        const int32_t* hist_items, int64_t n);
+
 #ifdef __cplusplus
 }
 #endif
