@@ -8,6 +8,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libg4r.so')
 G4R_MAX_LAYERS = 8
 G4R_TOPK_MAX = 1024
+SCHED_POSITIONS = 2          # Schedule(mode=1 | SCHED_POSITIONS): an evaluation schedule that records input positions
 
 G4R_OK, G4R_ERR_INVALID, G4R_ERR_INDEX, G4R_ERR_CUDA, G4R_ERR_NAN, G4R_ERR_STATE = 0, -1, -2, -3, -4, -5
 LOSS = {'cross-entropy': 0, 'bpr-max': 1, 'top1-max': 2, 'bpr': 3, 'top1': 4, 'xe_logit': 5}
@@ -38,11 +39,11 @@ EXPORTS = [
     'g4r_set_sampling_cdf', 'g4r_set_logq_support', 'g4r_generate_samples', 'g4r_generate_samples_from_uniform',
     'g4r_set_sample_store', 'g4r_get_sample_store', 'g4r_sample_store_rows', 'g4r_set_sample_pointer', 'g4r_get_sample_pointer',
     'g4r_mrg_uniform', 'g4r_searchsorted', 'g4r_gather_rows',
-    'g4r_schedule_build', 'g4r_schedule_free', 'g4r_schedule_steps', 'g4r_schedule_events', 'g4r_schedule_export',
+    'g4r_schedule_build', 'g4r_schedule_free', 'g4r_schedule_steps', 'g4r_schedule_events', 'g4r_schedule_export', 'g4r_schedule_positions',
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
-    'g4r_eval_schedule', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
+    'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
     'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
     'g4r_sessions_export', 'g4r_sessions_import',
@@ -88,6 +89,7 @@ def load():
     lib.g4r_schedule_steps.argtypes = [vp]; lib.g4r_schedule_steps.restype = i64
     lib.g4r_schedule_events.argtypes = [vp]; lib.g4r_schedule_events.restype = i64
     lib.g4r_schedule_export.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.g4r_schedule_positions.argtypes = [vp, vp]
     lib.g4r_train_step.argtypes = [vp, vp, vp, i32, vp, C.POINTER(C.c_float)]
     lib.g4r_train_steps.argtypes = [vp, vp, i64, i64, vp, C.POINTER(i64)]
     lib.g4r_upload_steps.argtypes = [vp, vp, i64, i64]
@@ -109,6 +111,7 @@ def load():
     lib.g4r_mg_shard_rows.argtypes = [i64, i32, i32]; lib.g4r_mg_shard_rows.restype = i64
     lib.g4r_mg_segment_bytes.argtypes = [C.POINTER(G4RConfig), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.g4r_eval_schedule.argtypes = [vp, vp, vp, i32, i32, vp, vp, C.POINTER(i64)]
+    lib.g4r_eval_events.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, C.POINTER(i64), vp, vp, vp]
     lib.g4r_eval_counts.argtypes = [vp, vp, i64]
     lib.g4r_set_eval_items.argtypes = [vp, vp, i64]
     lib.g4r_predict.argtypes = [vp, vp, i32, vp, vp]
@@ -237,6 +240,15 @@ class Schedule(object):
         M = np.empty(n, np.int32); S = np.empty((n, B), np.int32)
         self._lib.g4r_schedule_export(self.h, _ptr(X), _ptr(Y), _ptr(F), _ptr(M), _ptr(S))
         return dict(X=X, Y=Y, F=F, M=M, slots=S)
+
+    def positions(self):
+        """[n_steps, batch_size] int64 (schedules built with mode=1 | SCHED_POSITIONS): index in data_items of every lane's input,
+        -1 on unused lanes; the lane's target is the next entry."""
+        P = np.empty((self.n_steps, self.batch_size), np.int64)
+        rc = self._lib.g4r_schedule_positions(self.h, _ptr(P))
+        if rc != 0:
+            raise RuntimeError(self._lib.g4r_last_error(None).decode())
+        return P
 
     def batch_sizes(self):
         """M of every mini-batch (the weights of the epoch loss, gru4rec.py:654) without copying the index arrays."""
@@ -488,6 +500,23 @@ class Engine(object):
         n = C.c_int64()
         self._check(self.lib.g4r_eval_schedule(self.h, sched.h, _ptr(cut), len(cut), mode, _ptr(rec), _ptr(mrr), C.byref(n)))
         return rec, mrr, n.value
+
+    def eval_events(self, sched, cut_off, mode=0, k=0):
+        """eval_schedule with per-event outputs, events in the order the schedule consumes them (Schedule.positions maps them to
+        the data): (recall sums, mrr sums, n_events, counts int32 [n_events, 2], items int32 [n_events, k], scores float32
+        [n_events, k]).  The sums equal eval_schedule's bit for bit; counts are (#greater, #equal) as eval_counts gives them; with
+        k > 0 every event's top-k list as predict_topk ranks the lane after the input (with set_eval_items, among those items);
+        k = 0: items / scores are None."""
+        cut = np.ascontiguousarray(cut_off, dtype=np.int32)
+        rec = np.zeros(len(cut), dtype=np.float64); mrr = np.zeros(len(cut), dtype=np.float64)
+        n = C.c_int64()
+        counts = np.empty((sched.n_events, 2), dtype=np.int32)
+        items = scores = None
+        if k:
+            items = np.empty((sched.n_events, k), dtype=np.int32); scores = np.empty((sched.n_events, k), dtype=np.float32)
+        self._check(self.lib.g4r_eval_events(self.h, sched.h, _ptr(cut), len(cut), mode, int(k), _ptr(rec), _ptr(mrr), C.byref(n),
+                                             _ptr(counts), _ptr(items), _ptr(scores)))
+        return rec, mrr, n.value, counts, items, scores
 
     def eval_counts(self, n_lanes):
         """[n_lanes x 2] int32: (#items scoring above the target, #items tied with it incl. the target) of every lane of the last

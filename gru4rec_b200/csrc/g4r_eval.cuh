@@ -229,13 +229,16 @@ struct EvalCtx {
   int cap = 0;
   int slot = -1;
   int* dCand = nullptr; int n_cand = 0; size_t cand_cap = 0;     // candidate subset of evaluate_gpu(items=...), item indices
+  std::vector<int32_t> hCand;                                     // its host copy (the top-k filter of g4r_eval_events)
   // wgmma tiles (g4r_eval_tc.cuh): [hi | lo] TF32 operand blocks of the hidden states (per call) and of the item table, which
   // is kept between calls and tagged with the handle's wy_version it was made from
   unsigned char *dAsplit = nullptr, *dBsplit = nullptr;
   uint64_t split_version = ~0ull;
   void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
+  void* events = nullptr;                                         // EventsCtx* of g4r_eval_events (g4r_events.cuh)
 };
 static void topk_release(EvalCtx& e);
+static void events_release(EvalCtx& e);
 
 // device buffer of at least n elements (contents not kept)
 template <class T>
@@ -273,6 +276,7 @@ static void eval_release(g4r_handle* h) {
   if (!h->eval_ctx) return;
   EvalCtx& e = *static_cast<EvalCtx*>(h->eval_ctx);
   topk_release(e);
+  events_release(e);
   cudaFreeHost(e.hX); cudaFreeHost(e.hY); cudaFreeHost(e.hSlot); cudaFreeHost(e.hF); cudaFreeHost(e.hM); cudaFreeHost(e.hSti); cudaFreeHost(e.hG);
   cudaFree(e.dX); cudaFree(e.dY); cudaFree(e.dSlot); cudaFree(e.dF); cudaFree(e.dM); cudaFree(e.dSti); cudaFree(e.dG);
   cudaFree(e.dCut); cudaFree(e.dSums); if (e.dOut) cudaFree(e.dOut); if (e.dCand) cudaFree(e.dCand);
@@ -322,9 +326,18 @@ static int eval_forward(g4r_handle* h, EvalCtx* e, int s, float* const* Hst) {
   return G4R_OK;
 }
 
-extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
-                                 double* recall_sum, double* mrr_sum, int64_t* n_events) {
-  if (!h || !s || !cut_off || n_cut <= 0 || n_cut > 64 || !recall_sum || !mrr_sum) return G4R_ERR_INVALID;
+// g4r_eval_events' per-event outputs (g4r_events.cuh); nullptr on g4r_eval_schedule's path
+struct EventsRun;
+static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev);
+static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
+static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
+static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t rk);
+
+// The evaluation schedule in staging windows of e->cap mini-batches (g4r_eval_schedule); ev != nullptr adds g4r_eval_events'
+// per-event work on the ranking stream, after the kernels of g4r_eval_schedule, which stay as they are and see the same step
+// indices (the tiebreaking noise hashes them) whatever the per-event window
+static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
+                    double* recall_sum, double* mrr_sum, int64_t* n_events, EventsRun* ev) {
   if (mode < 0 || mode > 3) FAIL(G4R_ERR_INVALID, "eval mode must be 0 (standard), 1 (conservative), 2 (median) or 3 (tiebreaking)");
   const unsigned int tie = mode == 3 ? 0x5bd1e995u : 0u;
   cudaSetDevice(h->cfg.device);
@@ -332,6 +345,10 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
   int rc = eval_ctx(h, &e);
   if (rc) return rc;
   if (s->B > e->Be) FAIL(G4R_ERR_INVALID, "schedule batch size exceeds eval_batch_size");
+  if (ev) {
+    rc = events_begin(h, e, s, ev);
+    if (rc) return rc;
+  }
   const int Be = e->Be, Bs = s->B, I = h->md.n_items;
   cudaStream_t st = h->stream;
   for (int i = 0; i < h->md.n_layers; i++) CK(cudaMemsetAsync(h->He[i], 0, (size_t)Be * h->md.layer[i].ldL * sizeof(float), st));   // gru4rec.py:731-733
@@ -380,6 +397,10 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
       eval_forward(h, e, (int)i, h->He);
       CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
       k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
+      if (ev) {
+        rc = events_stage(h, e, ev, (int)i, rk);     // saves this mini-batch's y before the forward may move on
+        if (rc) return rc;
+      }
       const int n_comp = e->n_cand > 0 ? e->n_cand : I;
       const int M_i = e->hM[i];
       const bool tc = tc_possible && wgmma_tiles(h->cfg, M_i, I, I);
@@ -395,6 +416,14 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
       CK(cudaStreamWaitEvent(st, h->ts_ev[1], 0));        // the hidden output of this mini-batch has been consumed
       k_eval_rank<<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums);
       h->launches += 3;
+      if (ev) {
+        rc = events_step(h, e, ev, (int)i, rk);
+        if (rc) return rc;
+      }
+    }
+    if (ev) {
+      rc = events_flush(h, e, ev, rk);         // the rest of the per-event window before the staging is reused
+      if (rc) return rc;
     }
     CK(cudaEventRecord(h->ts_ev[2], rk)); CK(cudaStreamWaitEvent(st, h->ts_ev[2], 0));   // window complete before its staging is reused
     CK(cudaGetLastError());
@@ -406,6 +435,12 @@ extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int
   for (int j = 0; j < n_cut; j++) { recall_sum[j] = sums[j]; mrr_sum[j] = sums[n_cut + j]; }
   if (n_events) *n_events = s->n_events;
   return G4R_OK;
+}
+
+extern "C" int g4r_eval_schedule(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
+                                 double* recall_sum, double* mrr_sum, int64_t* n_events) {
+  if (!h || !s || !cut_off || n_cut <= 0 || n_cut > 64 || !recall_sum || !mrr_sum) return G4R_ERR_INVALID;
+  return eval_run(h, s, cut_off, n_cut, mode, recall_sum, mrr_sum, n_events, nullptr);
 }
 
 extern "C" int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes) {
@@ -437,6 +472,7 @@ extern "C" int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n
   CK(cudaMemcpyAsync(e->dCand, tmp.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   e->n_cand = (int)n;
+  e->hCand = std::move(tmp);
   return G4R_OK;
 }
 
@@ -495,3 +531,4 @@ extern "C" int g4r_reset_eval_hidden(g4r_handle* h) {
 
 #include "g4r_topk.cuh"
 #include "g4r_sessions.cuh"
+#include "g4r_events.cuh"

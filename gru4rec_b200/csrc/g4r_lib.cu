@@ -38,6 +38,8 @@ struct g4r_schedule {
   int64_t n_steps = 0, n_events = 0;
   std::vector<int32_t> X, Y, slots, M;
   std::vector<uint8_t> F;
+  std::vector<int64_t> P;       // recorded on request (mode | 2): index in data_items of every input X (target at P + 1), -1 on unused lanes
+  bool has_pos = false;
 };
 
 struct g4r_handle {
@@ -1048,8 +1050,10 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
                                   const int64_t* order, int32_t B, int32_t n_sample, int32_t mode, g4r_schedule** out) {
   if (!data_items || !offs || !out || B <= 0 || n_sessions < 0) return G4R_ERR_INVALID;
   if (n_sessions < B) { g_create_error = "index out of bounds: fewer sessions than batch_size (reference: IndexError at gru4rec.py:596)"; return G4R_ERR_INDEX; }
+  const bool want_pos = mode == (1 | G4R_SCHED_POSITIONS);   // evaluation schedule that also records input positions
+  if (want_pos) mode = 1;
   g4r_schedule* s = new g4r_schedule();
-  s->B = B; s->mode = mode;
+  s->B = B; s->mode = mode; s->has_pos = want_pos;
   auto sess_of = [&](int64_t it) -> int64_t { return order ? order[it] : it; };
   std::vector<int64_t> iters(B), start(B), end(B);
   std::vector<int32_t> slots(B);
@@ -1068,6 +1072,7 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
     }
     const size_t guess = (size_t)(pairs / B + max_len + 2);
     s->X.reserve(guess * B); s->Y.reserve(guess * B); s->slots.reserve(guess * B); s->F.reserve(guess * B); s->M.reserve(guess);
+    if (want_pos) s->P.reserve(guess * B);
   }
   int64_t maxiter = B - 1;
   int M = B;
@@ -1088,6 +1093,10 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
           x[b] = (int32_t)data_items[p]; y[b] = (int32_t)data_items[p + 1]; sl[b] = slots[b];
         }
         for (int b = M; b < B; b++) { x[b] = -1; y[b] = -1; }
+      }
+      if (want_pos) {
+        s->P.resize(base + add, -1);
+        for (int64_t i = 0; i < nst; i++) for (int b = 0; b < M; b++) s->P[base + i * B + b] = start[b] + i;
       }
       if (mode == 0) {       // bit 0: the step that consumes a session's last event -- the lane's state is reset after it (gru4rec.py:647-651)
         uint8_t* f = F + (nst - 1) * B;
@@ -1133,6 +1142,12 @@ extern "C" int g4r_schedule_export(const g4r_schedule* s, int32_t* X, int32_t* Y
   if (flags) memcpy(flags, s->F.data(), n);
   if (slots) memcpy(slots, s->slots.data(), n * sizeof(int32_t));
   if (M) memcpy(M, s->M.data(), s->M.size() * sizeof(int32_t));
+  return G4R_OK;
+}
+extern "C" int g4r_schedule_positions(const g4r_schedule* s, int64_t* pos) {
+  if (!s || !pos) return G4R_ERR_INVALID;
+  if (!s->has_pos) { g_create_error = "g4r_schedule_positions: the schedule was not built with mode 1 | G4R_SCHED_POSITIONS"; return G4R_ERR_STATE; }
+  memcpy(pos, s->P.data(), s->P.size() * sizeof(int64_t));
   return G4R_OK;
 }
 

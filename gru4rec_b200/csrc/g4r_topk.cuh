@@ -473,6 +473,36 @@ static int topk_close_lane(g4r_handle* h, std::vector<int>& ex_off, std::vector<
 static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, int32_t k, const TopkFilter& f,
                      const std::vector<int>& ex_off, const std::vector<int>& ex, int32_t* out_items, float* out_scores);
 
+// operands of the wgmma filter tiles: tc_operands' split item table and max |Wy|, max |By| (both remade only after Wy / By changed)
+static int topk_tc_operands(g4r_handle* h, EvalCtx* e, TopkCtx* t) {
+  int rc = tc_operands(h, e);
+  if (rc) return rc;
+  if (t->absmax_version != h->wy_version) {
+    CK(cudaMemsetAsync(t->dAbsMax, 0, 2 * sizeof(unsigned int), h->stream));
+    k_topk_absmax<<<2 * h->n_sm, 256, 0, h->stream>>>(h->md.Wy, h->md.By, h->md.n_items, h->md.ldL, h->md.L, t->dAbsMax);
+    h->launches++;
+    t->absmax_version = h->wy_version;
+  }
+  return G4R_OK;
+}
+
+// the device copy of f's candidate set (bitmap and ascending item list), uploaded only when it differs from the cached one
+static int topk_upload_cand(g4r_handle* h, TopkCtx* t, const TopkFilter& f) {
+  if (!f.use_cand || t->hMask == f.cmask) return G4R_OK;
+  cudaStream_t st = h->stream;
+  t->hMask.clear();
+  std::vector<int> list;
+  list.reserve((size_t)f.n_distinct);
+  for (int i = 0; i < h->md.n_items; i++) if (f.is_cand(i)) list.push_back(i);
+  CK(dev_grow(&t->dMask, &t->mask_cap, f.cmask.size()));
+  CK(dev_grow(&t->dCand, &t->cand_cap, list.size()));
+  CK(cudaMemcpyAsync(t->dMask, f.cmask.data(), f.cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(t->dCand, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaStreamSynchronize(st));
+  t->hMask = f.cmask;
+  return G4R_OK;
+}
+
 extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
                                          const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
                                          int32_t* out_items, float* out_scores) {
@@ -520,18 +550,8 @@ static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, in
   if (rc) return rc;
   cudaStream_t st = h->stream;
   const int L = h->md.L;
-  if (use_cand && t->hMask != f.cmask) {                  // a candidate set other than the cached one
-    t->hMask.clear();
-    std::vector<int> list;
-    list.reserve((size_t)n_distinct);
-    for (int i = 0; i < I; i++) if (f.is_cand(i)) list.push_back(i);
-    CK(dev_grow(&t->dMask, &t->mask_cap, f.cmask.size()));
-    CK(dev_grow(&t->dCand, &t->cand_cap, list.size()));
-    CK(cudaMemcpyAsync(t->dMask, f.cmask.data(), f.cmask.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(t->dCand, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
-    t->hMask = f.cmask;
-  }
+  rc = topk_upload_cand(h, t, f);
+  if (rc) return rc;
   if (use_ex) {
     CK(dev_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
     CK(dev_grow(&t->dEx, &t->ex_cap, ex.size()));
@@ -560,14 +580,8 @@ static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, in
   CK(dev_grow(&t->dItems, &t->items_cap, (size_t)batch * k));
   CK(dev_grow(&t->dScores, &t->scores_cap, (size_t)batch * k));
   if (tc) {
-    rc = tc_operands(h, e);
+    rc = topk_tc_operands(h, e, t);
     if (rc) return rc;
-    if (t->absmax_version != h->wy_version) {
-      CK(cudaMemsetAsync(t->dAbsMax, 0, 2 * sizeof(unsigned int), st));
-      k_topk_absmax<<<2 * h->n_sm, 256, 0, st>>>(h->md.Wy, h->md.By, I, h->md.ldL, L, t->dAbsMax);
-      h->launches++;
-      t->absmax_version = h->wy_version;
-    }
   }
   eval_forward(h, e, 0, Hst);
   // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the items 0 .. P-1) and tau_b

@@ -9,6 +9,21 @@ from . import _lib
 _MODES = {'standard': 0, 'conservative': 1, 'median': 2, 'tiebreaking': 3}
 
 
+def _prepare(gru, test_data, session_key, item_key, time_key):
+    """evaluate_gpu's test data (evaluation.py:84-89): merged with the item map (unknown items dropped) and sorted by session,
+    time and item; returns (frame, item indices, session offsets)"""
+    test_data = pd.merge(test_data, pd.DataFrame({'ItemIdx': gru.itemidmap.values, item_key: gru.itemidmap.index}), on=item_key, how='inner')
+    test_data.sort_values([session_key, time_key, item_key], inplace=True)
+    offset_sessions = np.zeros(test_data[session_key].nunique() + 1, dtype=np.int32)
+    offset_sessions[1:] = test_data.groupby(session_key).size().cumsum()
+    return test_data, test_data.ItemIdx.values, offset_sessions
+
+
+def _cuts(cut_off):
+    multi_cut_off = (type(cut_off) == list) or (type(cut_off) == tuple)
+    return list(cut_off) if multi_cut_off else [cut_off]
+
+
 def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard'):
     '''
     Recall@N and MRR@N of next-item prediction, session-parallel (evaluation.py:15-147).
@@ -22,14 +37,9 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     if gru.error_during_train: raise Exception
     if mode not in _MODES:
         raise NotImplementedError
-    multi_cut_off = (type(cut_off) == list) or (type(cut_off) == tuple)
-    cuts = list(cut_off) if multi_cut_off else [cut_off]
+    cuts = _cuts(cut_off)
     print('Measuring Recall@{} and MRR@{}'.format(','.join([str(c) for c in cuts]), ','.join([str(c) for c in cuts])))
-    test_data = pd.merge(test_data, pd.DataFrame({'ItemIdx': gru.itemidmap.values, item_key: gru.itemidmap.index}), on=item_key, how='inner')
-    test_data.sort_values([session_key, time_key, item_key], inplace=True)
-    test_data_items = test_data.ItemIdx.values
-    offset_sessions = np.zeros(test_data[session_key].nunique() + 1, dtype=np.int32)
-    offset_sessions[1:] = test_data.groupby(session_key).size().cumsum()
+    test_data, test_data_items, offset_sessions = _prepare(gru, test_data, session_key, item_key, time_key)
     n_sessions = len(offset_sessions) - 1
     world, rank = gru._world()
     if world > 1 and os.environ.get('G4R_EVAL_SHARD', '1') == '0':
@@ -64,3 +74,74 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     recall = [float(r) / n for r in rec]
     mrrs = [float(m) / n for m in mrr]
     return recall, mrrs
+
+
+def _ranks(counts, mode):
+    """rank of every event from its (#greater, #equal) counts, by the formula of `mode` (evaluation.py:60-63)"""
+    gt, eq = counts[:, 0].astype(np.float64), counts[:, 1].astype(np.float64)
+    if mode == 'conservative':
+        return gt + eq
+    if mode == 'median':
+        return gt + 0.5 * (eq - 1.0) + 1.0
+    return gt + 1.0
+
+
+def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard', k=0):
+    '''
+    evaluate_gpu with per-event outputs, from one evaluation pass on the device.  The test data is prepared, batched and ranked
+    exactly as evaluate_gpu does it (same arguments, modes and `items` semantics).  Returns a dict:
+
+    - 'events': DataFrame with one row per scored event (every event but the first of its session), in the order of the sorted
+      test data: session id, time, input item id (column 'input_item'), target item id (column `item_key`) and 'rank' (float64,
+      by the formula of `mode`, so 'median' gives halves).
+    - 'recall', 'mrr': lists, one entry per cut-off, equal to evaluate_gpu's for the same arguments.
+    - 'ndcg': NDCG@N per cut-off, mean(1 / log2(rank + 1) if rank <= N else 0) over the events.  With `items` in
+      'conservative' mode a target outside the items can get rank 0 (as in evaluate_gpu, where MRR is then inf): its
+      1 / log2(1) makes NDCG inf too.
+    - k > 0: 'topk_items' [n_events, k] (original item ids, best first), 'topk_scores' [n_events, k] float32 and 'coverage'
+      (distinct recommended items / n_items): the list recommend_next_batch would return for the event's session after its input
+      (ranking key, the smaller item index first on equal keys, predict_next_batch's scores; with `items`, only those items
+      compete and the softmax normaliser runs over them).  The lists do not tie-break like 'rank' does: the rank of a target
+      that ties other items depends on `mode`, its place in the list on the item index.
+
+    Single process only: under a torch.distributed job it raises NotImplementedError.
+    '''
+    if gru.error_during_train: raise Exception
+    if mode not in _MODES:
+        raise NotImplementedError
+    if k != 0:
+        k = _lib.check_topk(k, gru.n_items if items is None else len(set(gru.itemidmap[items].values)))
+    if gru._world()[0] > 1:
+        raise NotImplementedError('evaluate_events runs in a single process (evaluate_gpu shards sessions over the ranks)')
+    cuts = _cuts(cut_off)
+    test_data, test_data_items, offset_sessions = _prepare(gru, test_data, session_key, item_key, time_key)
+    eng = gru._ensure_engine(batch_size)
+    if items is not None:
+        eng.set_eval_items(gru.itemidmap[items].values)
+    try:
+        sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS)
+        rec, mrr, n, counts, top_i, top_s = eng.eval_events(sched, cuts, _MODES[mode], k)
+        pos = sched.positions()
+    finally:
+        if items is not None:
+            eng.set_eval_items(None)
+    gru.predict = None                                     # the scoring hidden state is shared with predict_next_batch
+    # events in schedule order -> rows of the sorted frame (the target's row), then frame order
+    M = sched.batch_sizes()
+    row = (pos[np.arange(pos.shape[1])[None, :] < M[:, None]] + 1).astype(np.int64)
+    order = np.argsort(row, kind='stable')
+    row = row[order]
+    rank = _ranks(counts[order], mode)
+    tgt, inp = test_data.iloc[row], test_data.iloc[row - 1]
+    events = pd.DataFrame({session_key: tgt[session_key].values, time_key: tgt[time_key].values, 'input_item': inp[item_key].values,
+                           item_key: tgt[item_key].values, 'rank': rank})
+    with np.errstate(divide='ignore'):
+        ndcg = [float(np.where(rank <= c, 1.0 / np.log2(rank + 1.0), 0.0).mean()) if n else float('nan') for c in cuts]
+    out = {'events': events, 'recall': [float(r) / n for r in rec], 'mrr': [float(m) / n for m in mrr], 'ndcg': ndcg}
+    if k:
+        top_i = top_i[order]
+        ids = gru.itemidmap.index.values
+        out['topk_items'] = ids[top_i]
+        out['topk_scores'] = top_s[order]
+        out['coverage'] = len(np.unique(top_i)) / gru.n_items
+    return out

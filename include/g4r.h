@@ -122,7 +122,8 @@ int g4r_gather_rows(g4r_handle* h, const float* table, int64_t rows, int64_t col
 
 /* ---- session-parallel schedule (gru4rec.py:585-651; evaluation.py:90-139) -------------------------- */
 /* Builds every mini-batch of one epoch on the host: X/Y item indices, reset flags, batch sizes, lane slots.
- * mode 0 = training order semantics (reset-after flags), 1 = evaluation (zero-before flags).
+ * mode 0 = training order semantics (reset-after flags), 1 = evaluation (zero-before flags), 1 | G4R_SCHED_POSITIONS = evaluation
+ * that also records every lane's input position (g4r_schedule_positions).
  * session_order: n_sessions session ids (gru4rec.py:585/593; a rank's shard in the multi-GPU path) or NULL for identity;
  * offset_sessions must cover every id that occurs in it. */
 int g4r_schedule_build(const int64_t* data_items, int64_t n_events, const int32_t* offset_sessions, int64_t n_sessions,
@@ -132,6 +133,11 @@ int64_t g4r_schedule_steps(const g4r_schedule* s);
 int64_t g4r_schedule_events(const g4r_schedule* s);       /* sum of batch sizes */
 /* Copies out step arrays (each step padded to batch_size entries; unused lanes = -1 / 0). Any pointer may be NULL. */
 int g4r_schedule_export(const g4r_schedule* s, int32_t* X, int32_t* Y, uint8_t* flags, int32_t* M, int32_t* slots);
+/* Evaluation schedules built with mode 1 | G4R_SCHED_POSITIONS: pos[step * batch_size + b] = index in data_items of the input X
+ * of lane b (its target is at pos + 1), -1 on unused lanes.  This maps the events of g4r_eval_events back to the test data.
+ * G4R_ERR_STATE for a schedule built without the flag (other schedules do not spend the memory). */
+#define G4R_SCHED_POSITIONS 2
+int g4r_schedule_positions(const g4r_schedule* s, int64_t* pos);
 
 /* ---- the compiled step: train_function(X, Y, M, R) -> cost (gru4rec.py:584,623) ------------------- */
 /* One mini-batch from host arrays; returns the cost (D2H) like the reference call. */
@@ -203,6 +209,18 @@ int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes);
  * the whole catalogue for subsequent g4r_eval_schedule calls (the target's own score competes only if the target is listed,
  * as in the reference); n = 0 restores the full-catalogue ranking.  G4R_ERR_INDEX on an out-of-range index. */
 int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n);
+/* g4r_eval_schedule with per-event outputs (DESIGN §3f).  Events are numbered in the order the schedule consumes them: mini-batch
+ * by mini-batch, lanes 0 .. M-1 of each (g4r_schedule_positions maps them to the test data).  recall_sum / mrr_sum / n_events
+ * are bit for bit those of g4r_eval_schedule with the same arguments.  out_counts [n_events x 2]: (#items scoring above the
+ * target, #items tied with it, the target included), as g4r_eval_counts, under the same mode and candidate items.  k > 0: the
+ * k best items of every event, as g4r_predict_topk_filtered ranks the lane after the event's input (ranking key, ties, scores;
+ * with g4r_set_eval_items only the distinct candidates compete, softmax normaliser over them), into out_items / out_scores
+ * [n_events x k]; k = 0: no lists (out_items / out_scores may be NULL).  The lists and the counts follow different tie rules.
+ * Runs in windows of mini-batches with no host round trip inside a window; the window is shortened to bound its device buffers
+ * (G4R_EVENTS_WINDOW in the environment, read when a handle first runs this, caps it further).  G4R_ERR_INVALID unless
+ * 0 <= k <= min(distinct candidates, G4R_TOPK_MAX). */
+int g4r_eval_events(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode, int32_t k,
+                    double* recall_sum, double* mrr_sum, int64_t* n_events, int32_t* out_counts, int32_t* out_items, float* out_scores);
 
 /* predict_next_batch's device call: scores of all items for `batch` lanes; reset_mask zeroes lanes first
  * (gru4rec.py:712-717).  out: [batch x n_items] row-major. */

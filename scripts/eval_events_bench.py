@@ -1,0 +1,79 @@
+"""Time of per-event evaluation (Engine.eval_events, g4r_eval_events, DESIGN §3f) against evaluate_gpu's device call
+(Engine.eval_schedule) and against the only way to get per-event top-k lists without it, a Python loop of predict_topk
+(recommend_next_batch's device call) over the same schedule.  Shapes: RSC15 (37,483 items, GRU(100)) and Rees46 (172,000 items,
+GRU(512)), 100 and 512 lanes.  Before timing, the loop's lists must equal eval_events' lists.  The engine calls are timed, not
+the public functions: the pandas preparation of evaluate_gpu / evaluate_events, the events frame and recommend_next_batch's item
+id mapping are left out.
+
+  python scripts/eval_events_bench.py [--rounds R]
+
+Env: EE_EVENTS (test events per shape, default 100,000, at least twice the items), EE_SHAPES (e.g. 'rsc15,rees46'), EE_LANES (e.g. '100,512')."""
+import argparse, os, sys, time
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'scripts'))
+import numpy as np
+import torch
+from gru4rec_b200 import _lib
+from gru4rec_b200.synth import make_session_arrays
+import gru4rec as g4
+from serve_bench import card
+from serve_filter_bench import make_engine
+
+SHAPES = {'rsc15': (37483, 100), 'rees46': (172000, 512)}
+
+ap = argparse.ArgumentParser()
+ap.add_argument('--rounds', type=int, default=3)
+a = ap.parse_args()
+print('card: %s | nvidia-smi name, power.limit, clocks.max.sm: %s' % card(), flush=True)
+n_ev = int(os.environ.get('EE_EVENTS', 100000))
+CUTS = [1, 5, 20]
+
+
+def timed(f):
+    ts = []
+    for _ in range(a.rounds):
+        torch.cuda.synchronize(); t0 = time.time()
+        f()
+        torch.cuda.synchronize(); ts.append(time.time() - t0)
+    return float(np.median(ts))
+
+
+def loop_topk(eng, sched, e, k):
+    """the per-event lists by predict_topk, one call per mini-batch of the schedule (lanes = state slots)"""
+    B = sched.batch_size
+    out = []
+    eng.reset_eval_hidden()
+    for s in range(sched.n_steps):
+        M = int(e['M'][s]); sl = e['slots'][s, :M]
+        X = np.zeros(B, np.int32); X[sl] = e['X'][s, :M]
+        R = np.zeros(B, np.uint8); R[sl] = (e['F'][s, :M] & 2) != 0
+        out.append(eng.predict_topk(X, k, R)[0][sl])
+    return np.concatenate(out)
+
+
+for shape in os.environ.get('EE_SHAPES', 'rsc15,rees46').split(','):
+    I, L = SHAPES[shape]
+    mk = dict(layers=[L], loss='bpr-max', final_act='elu-0.5', batch_size=32, n_sample=2048)
+    gru = g4.GRU4Rec(**mk); gru.n_items = I
+    w = gru._init_host_weights()
+    items, offset, _, _ = make_session_arrays(I, max(n_ev, 2 * I), seed=1)
+    for lanes in [int(x) for x in os.environ.get('EE_LANES', '100,512').split(',')]:
+        eng = make_engine(I, mk, lanes, w)
+        sched = _lib.Schedule(items, offset, None, lanes, 0, mode=1)
+        e = sched.export()
+        ref = loop_topk(eng, sched, e, 20)
+        got = eng.eval_events(sched, CUTS, 0, k=20)
+        if not np.array_equal(ref, got[4]):
+            raise SystemExit('MISMATCH: predict_topk loop and eval_events lists differ (%s, %d lanes)' % (shape, lanes))
+        rec = eng.eval_schedule(sched, CUTS, 0)
+        if not (np.array_equal(rec[0], got[0]) and np.array_equal(rec[1], got[1])):
+            raise SystemExit('MISMATCH: eval_events sums differ from eval_schedule (%s, %d lanes)' % (shape, lanes))
+        t = {'evaluate_gpu (eval_schedule)': timed(lambda: eng.eval_schedule(sched, CUTS, 0))}
+        for k in (0, 20, 100):
+            t['eval_events k=%d' % k] = timed(lambda: eng.eval_events(sched, CUTS, 0, k=k))
+        t['predict_topk loop k=20'] = timed(lambda: loop_topk(eng, sched, e, 20))
+        for name, dt in t.items():
+            print('%-7s I=%d GRU(%d) lanes=%3d %-30s %8.3f s  %8.1f us / mini-batch  (%d mini-batches, %d events)'
+                  % (shape, I, L, lanes, name, dt, dt / sched.n_steps * 1e6, sched.n_steps, sched.n_events), flush=True)
+        eng.close()
