@@ -3,12 +3,13 @@
 // (step_mode 2; anything else runs k_persistent / the per-phase kernels, which share all numerics.)
 //
 // Why: at B=32, L=100 a mini-batch is ~8 dependent phases over ~6 MB; time is memory/barrier latency.  This kernel
-//  * keeps every CTA a "column CTA" owning one chunk of score columns; the chunk's Wy / Adagrad / momentum rows and
-//    the target rows are PREFETCHED with TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) while the GRU
-//    phases of the previous step run, so the score phase starts with its operands already in shared memory;
-//  * folds the row-statistics combine into the score->gradient barrier (the last CTA to arrive combines);
+//  * gives each "column CTA" one chunk of score columns (step_mode 2: the CTAs after the G GRU CTAs, chunk c on CTA G + c;
+//    step_mode 3: every CTA, chunk c on CTA c); the chunk's Wy / Adagrad / momentum rows and the target rows are
+//    PREFETCHED with TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) while the GRU phases of the previous step
+//    run, so the score phase starts with its operands already in shared memory;
+//  * combines the row statistics of lane b on column CTA b right after the score->gradient barrier;
 //  * (step_mode 2) puts only the partial dL/dh before the b1 barrier: dSy and the update of the chunk's rows follow b1, gated for
-//    the next prefetch by `rows_done`, and a GRU CTA's chunk is updated by a partner CTA with no GRU or helper role;
+//    the next prefetch by `rows_done`; the GRU CTAs take no part in the column phases, so none of this is on their chain;
 //  * runs the GRU phases on a group of G CTAs (step_mode 2: weights resident in shared memory, one group barrier per
 //    mini-batch; see FastSmemR); the other CTAs only wait for `h_ready`;
 //  * uses monotonic release/acquire counters (no resets, no separate fences) for all synchronisation.
@@ -412,7 +413,7 @@ __device__ void fk_sparse_in_one(const ModelDev& md, SM& sm, int s, int b, const
   }
 }
 
-// B1 (fast kernel): every CTA reduces a contiguous run of dL/dh elements; lanes = consecutive elements (coalesced),
+// B1 (fast kernel): every column CTA (cta of ncta) reduces a contiguous run of dL/dh elements; lanes = consecutive elements (coalesced),
 // warps = slices of the chunk partials, cross-warp sum in shared memory in fixed order; then da_h / da_z.
 template <bool CL, class SM>
 __device__ void fk_b1(const ModelDev& md, SM& sm, int s, int cta, int ncta) {
@@ -422,7 +423,7 @@ __device__ void fk_b1(const ModelDev& md, SM& sm, int s, int cta, int ncta) {
   const int E = M * ldL;                                  // padded elements (padding columns are zero everywhere)
   const int per = ((E + ncta - 1) / ncta + 31) / 32 * 32; // elements per CTA, multiple of 32
   const int e0 = cta * per;
-  float* red = sm.sPart;                                  // [FK_NW][per]  (per <= 128 for M*ldL <= 4096*... checked on host)
+  float* red = sm.sPart;                                  // [FK_NW][per]  (per <= 256: M * ldL <= 4096 elements over >= 16 CTAs)
   const size_t cs = (size_t)md.B * ldL;
   // forward saves of this thread's output element (per <= 128 <= FK_THREADS: at most one element per thread), fetched up
   // front so that their round trip overlaps the loads of the chunk partials
@@ -765,51 +766,6 @@ __device__ __forceinline__ void fk_dby(SM& sm, int M, int nj) {
     if (lane == 0) sm.sDby[jj] = a;
   }
 }
-// step_mode 2: GRU CTA g's chunk is updated by its partner CTA (one with no GRU or helper role) after the partner's own chunk.
-// The chunk's dL/do columns come from md.O, where CTA g put them before B3; its items, rows and bias entries are read from
-// global memory, where nothing has written them since the previous step's rows_done.  These are the operands CTA g holds,
-// and dby / dSy / the update run the same code.  fk_partner_fetch issues the loads that do not depend on one another (chunk
-// bounds, items, dL/do) into registers before the own chunk is processed; fk_partner_stage puts them and the chunk's rows into
-// the shared-memory slots of the own chunk once that is done, and returns the chunk's column count.
-struct FkPartner { int nj, it; float g[2]; };
-__device__ __forceinline__ FkPartner fk_partner_fetch(const ModelDev& md, int s, int g, int M) {
-  const int tid = threadIdx.x;
-  const int* cbeg = md.pCbeg + (size_t)s * (md.NCH + 1);
-  const int cb = g < md.NCH ? cbeg[g] : 0;
-  FkPartner r;
-  r.nj = g < md.NCH ? cbeg[g + 1] - cb : 0;
-  r.it = (tid < r.nj) ? md.pItem[(size_t)s * md.NP + cb + tid] : 0;
-#pragma unroll
-  for (int u = 0; u < 2; u++) {
-    const int i = u * FK_THREADS + tid, jj = i / FK_B, b = i % FK_B;
-    r.g[u] = (jj < r.nj && b < M) ? md.O[(size_t)(cb + jj) * md.Bld + b] : 0.f;
-  }
-  return r;
-}
-template <class SM>
-__device__ int fk_partner_stage(const ModelDev& md, SM& sm, const FkPartner& r, int buf, int M, int kw) {
-  static_assert(FK_CT * FK_B == 2 * FK_THREADS, "fk_partner_fetch: two dL/do entries per thread");
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nj = r.nj;
-  const bool ada = md.adapt == G4R_ADAPT_ADAGRAD, mom = md.mom > 0.f;
-  __syncthreads();                                     // the own chunk's update has finished reading these slots
-  if (tid < FK_CT) sm.sIt[buf][tid] = r.it;
-  sm.sG[tid] = r.g[0]; sm.sG[FK_THREADS + tid] = r.g[1];
-  __syncthreads();
-  for (int j = warp; j < nj; j += FK_NW) {
-    const int it = sm.sIt[buf][j];
-    const size_t off = (size_t)it * md.ldL + lane * 4;
-    if (lane < kw) {
-      st4(sm.sS + j * FK_LDS + lane * 4, ld4(md.Wy + off));
-      if (ada) st4(sm.sAcc + j * FK_LDS + lane * 4, ld4(md.Wy_acc + off));
-      if (mom) st4(sm.sVel + j * FK_LDS + lane * 4, ld4(md.Wy_vel + off));
-    }
-    if (lane == 0) { sm.sByP[j] = md.By[it]; sm.sByA[j] = ada ? md.By_acc[it] : 0.f; sm.sByV[j] = mom ? md.By_vel[it] : 0.f; }
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these generic stores precede the next TMA writes of the slots
-  fk_dby(sm, M, nj);
-  return nj;
-}
-
 #include "g4r_fastc.cuh"
 
 // CL = false: GRU phases on a 48-CTA group with global group barriers (step_mode 2).
@@ -823,19 +779,20 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
   const LayerDev& ly = md.layer[0];
   const int cta = blockIdx.x, ncta = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int chunk = cta;                       // CTAs beyond the number of chunks own no columns
-  const bool has_chunk = chunk < md.NCH;
   const int G = CL ? (int)cl_size() : md.ldL / 4;   // CTAs of the GRU role (step_mode 2: one quad of hidden units each)
   const bool gru = cta < G;
+  // column CTAs: step_mode 2 the CTAs after the GRU group (the host sized NCH <= ncta - G), step_mode 3 every CTA.  Column CTA
+  // `chunk` owns chunk `chunk` (those beyond NCH own no columns) and combines the row statistics of lane `chunk`.
+  const bool col = CL || !gru;
+  const int chunk = CL ? cta : cta - G;
+  const int ncol = CL ? ncta : ncta - G;       // arrivals at B2 / B3, rows_done and b1_done per step
+  const bool has_chunk = col && chunk < md.NCH;
   const bool pw = loss_pairwise(md.loss);
   const int ldL = md.ldL, B = md.B;
   const int kw = ldL / 4;
   uint64_t* bar = reinterpret_cast<uint64_t*>(&sm.mbar);
   unsigned int bar_epoch = 0, gepoch = 0, stats_target = 0;
   const int in_ctas = min(B, ncta - G);        // helper CTAs [G, G + in_ctas) update the gathered input rows
-  // step_mode 2: CTA G + in_ctas + g updates the rows of GRU CTA g's chunk, off the GRU CTAs' chain (the host launches
-  // k_fast_t<false> only on grids with room for these partners)
-  const int partner_of = (!CL && cta >= G + in_ctas && cta < 2 * G + in_ctas) ? cta - G - in_ctas : -1;
 #ifdef G4R_CF_FINE
 #define FK_FTS(s_) ((tstamp && cta == 0 && (s_) < 500 && n_steps >= 1000) ? tstamp + (size_t)((s_) + 500) * 16 : nullptr)
 #define FK_STAMP_OK(s_) ((s_) < 500)
@@ -843,11 +800,13 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
 #define FK_FTS(s_) ((unsigned long long*)nullptr)
 #define FK_STAMP_OK(s_) true
 #endif
-#define FK_STAMP(k) do { if (tstamp && cta == 0 && tid == 0 && FK_STAMP_OK(s)) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); tstamp[(size_t)s * 16 + (k)] = t_; } } while (0)
+  // one row of 16 stamps per step: the GRU-phase slots 4-8 from CTA 0, the column-phase slots from the first column CTA
+  // (step_mode 3: CTA 0 for both)
+#define FK_STAMP(k) do { if (tstamp && cta == ((CL || ((k) >= 4 && (k) <= 8)) ? 0 : G) && tid == 0 && FK_STAMP_OK(s)) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); tstamp[(size_t)s * 16 + (k)] = t_; } } while (0)
   if (tid == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  fk_load_idx(md, sm, 0, n_steps, chunk, 0);
+  if (col) fk_load_idx(md, sm, 0, n_steps, chunk, 0);
   __syncthreads();
-  fk_prefetch_rows(md, sm, 0, n_steps, 0, pw);
+  if (col) fk_prefetch_rows(md, sm, 0, n_steps, 0, pw);
   // GRU forward of step 0
   ClusterCtx cc = {0, 1, 0, 0};
   if constexpr (CL) {
@@ -883,7 +842,7 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
     const int N = M + (sti >= 0 ? md.S : 0);
     FK_STAMP(0);
     // indices of the NEXT step (consumed after this step's last barrier)
-    fk_load_idx(md, sm, s + 1, n_steps, chunk, buf ^ 1);
+    if (col) fk_load_idx(md, sm, s + 1, n_steps, chunk, buf ^ 1);
     const bool gru_next = !CL && gru && s + 1 < n_steps;
     if (gru_next && tid < FK_B) {               // lanes of the next step (f2 of this step has used gIdx)
       const int M1 = md.wM[s + 1];
@@ -891,9 +850,41 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
       sm.gIdx[FK_B + tid] = tid < M1 ? md.wX[(size_t)(s + 1) * B + tid] : 0;
       sm.gIdx[2 * FK_B + tid] = tid < M1 ? md.wF[(size_t)(s + 1) * B + tid] : 0;
     }
-    // ---- wait for h(s), stage it ----
+    // ---- wait for h(s) ----
     if (tid == 0) wait_ge(&fs->h_ready, (unsigned int)(s + 1) * (unsigned int)G);
     __syncthreads();
+    if constexpr (!CL) {
+      if (!col) {
+        // ---- step_mode 2 GRU role (no score columns): backward of step s once b1 is done, dense update, forward of s + 1 ----
+        const bool nxt = s + 1 < n_steps;
+        const int k0 = 4 * cta;
+        const float* sHo = sm.gH[s & 1];                  // H rows of step s (staged one step earlier)
+        float* hnext = sm.gH[(s + 1) & 1];
+        // while the column CTAs run the step: the H rows of step s + 1 (final since every f2(s) has run)
+        if (nxt) stage_rows4(hnext, FK_LDS, FK_B, kw, [&](int rr) -> const float* { const int sl = sm.gIdx[rr]; return sl >= 0 ? ly.H + (size_t)sl * ldL : nullptr; });
+        __syncthreads();
+        if (tid == 0) wait_ge(&fs->b1_done, (unsigned int)(s + 1) * (unsigned int)ncol);
+        __syncthreads();
+        FK_STAMP(4);
+        fr_b2(md, sm, s, k0, sHo);
+        __syncthreads();
+        if (tid == 0) red_release_add(&fs->dvec_done, 1u);   // dvec of the step complete once all G have arrived
+        FK_STAMP(5);
+        fr_dense(md, sm, s, k0, sHo);
+        FK_STAMP(6);
+        if (nxt) {
+          fr_f1(md, sm, s + 1, k0, hnext, &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
+          fk_group_barrier(fs, gepoch, G);                // all-gather of Hold * r
+          FK_STAMP(7);
+          fr_f2(md, sm, s + 1, k0, hnext);
+          __syncthreads();
+          if (tid == 0) red_release_add(&fs->h_ready, 1u);
+        }
+        FK_STAMP(8);
+        continue;
+      }
+    }
+    // ---- column role: stage h(s) ----
     stage_rows4(sm.sY, FK_LDS, FK_B, kw, [&](int rr) -> const float* { return rr < M ? ly.y + (size_t)rr * ldL : nullptr; });
     mbar_wait(bar, (unsigned int)(s & 1));      // prefetched rows of this step have landed
     __syncthreads();
@@ -981,15 +972,15 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
         }
       }
     }
-    // ---- barrier B2, then lane b's statistics are combined by CTA b (all lanes in parallel, fixed merge order) ----
+    // ---- barrier B2, then lane b's statistics are combined by column CTA b (all lanes in parallel, fixed merge order) ----
     __syncthreads();
     FK_STAMP(10);
     bar_epoch += 1;
-    if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncta); }
+    if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncol); }
     __syncthreads();
-    if (cta < M) {
-      // lane b = cta: row max over the chunk maxima, one rescale exp per chunk, then plain sums (fixed shuffle / warp order)
-      const int b = cta;
+    if (chunk < M) {
+      // lane b = chunk: row max over the chunk maxima, one rescale exp per chunk, then plain sums (fixed shuffle / warp order)
+      const int b = chunk;
       const bool maxed = !(md.loss == G4R_LOSS_BPR || md.loss == G4R_LOSS_TOP1);
       float mc = -INFINITY, Z = 0.f, A = 0.f, Q = 0.f, D = 0.f, T = 0.f, has = 0.f, tt = 0.f;
       if (tid < md.NCH) {
@@ -1055,14 +1046,7 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
       sm.sG[i] = (jj < nj && b < M) ? loss_grad_elem(md, sm.sRS + (size_t)b * 8, sm.sO[i], sm.sTc[buf][b] == cb + jj, M, N) : 0.f;
     }
     __syncthreads();
-    if (!CL && gru) {                           // the partner CTA updates this chunk's rows (B3 publishes these columns)
-      for (int i = tid; i < nj * FK_B; i += FK_THREADS) {
-        const int jj = i / FK_B, b = i % FK_B;
-        if (b < M) md.O[(size_t)(cb + jj) * md.Bld + b] = sm.sG[i];
-      }
-    } else {
-      fk_dby(sm, M, nj);
-    }
+    fk_dby(sm, M, nj);
     FK_STAMP(12);
     float* part = md.part + (size_t)(has_chunk ? chunk : 0) * md.B * ldL;
     if constexpr (CL) {
@@ -1122,78 +1106,39 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
       __syncthreads();
       FK_STAMP(13);
       bar_epoch += 1;
-      if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncta); }
+      if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncol); }
       __syncthreads();
       FK_STAMP(3);
-      fk_b1<CL>(md, sm, s, cta, ncta);
+      fk_b1<CL>(md, sm, s, chunk, ncol);
       __syncthreads();
       if (tid == 0) red_release_add(&fs->b1_done, 1u);
       FK_STAMP(15);
       // ---- off the chain: dSy and the update of the chunk's Wy / By rows.  Only the TMA prefetch of the next step reads the
-      // updated rows; it waits for rows_done (every CTA's update) ----
-      const bool nxt = s + 1 < n_steps;
-      const unsigned int rows_target = (unsigned int)(s + 1) * (unsigned int)ncta;
-      if (gru) {
-        const int k0 = 4 * cta;
-        const float* sHo = sm.gH[s & 1];                  // H rows of step s (staged one step earlier)
-        float* hnext = sm.gH[(s + 1) & 1];
-        // in the b1_done wait: the H rows of step s + 1 (final since every f2(s) has run).  This CTA's chunk rows are updated
-        // by its partner CTA.
-        if (nxt) stage_rows4(hnext, FK_LDS, FK_B, kw, [&](int rr) -> const float* { const int sl = sm.gIdx[rr]; return sl >= 0 ? ly.H + (size_t)sl * ldL : nullptr; });
-        __syncthreads();
-        FK_STAMP(14);
-        if (tid == 0) { red_release_add(&fs->rows_done, 1u); wait_ge(&fs->b1_done, (unsigned int)(s + 1) * (unsigned int)ncta); }
-        __syncthreads();
-        FK_STAMP(4);
-        // ---- GRU role: backward, dense update, forward of the next step ----
-        fr_b2(md, sm, s, k0, sHo);
-        __syncthreads();
-        if (tid == 0) red_release_add(&fs->dvec_done, 1u);   // dvec of the step complete once all G have arrived
-        FK_STAMP(5);
-        fr_dense(md, sm, s, k0, sHo);
-        FK_STAMP(6);
-        if (nxt) {
-          fr_f1(md, sm, s + 1, k0, hnext, &fs->in_done, (unsigned int)(s + 1) * (unsigned int)in_ctas);   // waits for the helper CTAs' input-row updates
-          fk_group_barrier(fs, gepoch, G);                // all-gather of Hold * r
-          FK_STAMP(7);
-          fr_f2(md, sm, s + 1, k0, hnext);
+      // updated rows; it waits for rows_done (every column CTA's update) ----
+      fk_dsy(sm, M, nj, kw);
+      __syncthreads();
+      if (chunk < in_ctas) {
+        // helper CTA: the input-row update of the step's lanes first, once dvec is complete -- F1 of the next step waits for
+        // it (in_done), the chunk's row update only gates the next prefetch.  Wx0 and Wy / By are separate tables here, so
+        // the order changes no result.
+        const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
+        if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, chunk, &fs->dvec_done, tgt);
+        else {
+          if (tid == 0) wait_ge(&fs->dvec_done, tgt);
           __syncthreads();
-          if (tid == 0) red_release_add(&fs->h_ready, 1u);
-          // the prefetch of the next step's rows, once h(s + 1) is out: it overlaps the h_ready wait and the staging of y
-          // that open the next step
-          if (tid == 0) wait_ge(&fs->rows_done, rows_target);
-          __syncthreads();
-          fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
-        }
-        FK_STAMP(8);
-      } else {
-        // the own chunk, then on a partner CTA the chunk of GRU CTA partner_of, through the same dSy / update code
-        const FkPartner pc = partner_of >= 0 ? fk_partner_fetch(md, s, partner_of, M) : FkPartner{0, 0, {0.f, 0.f}};
-        for (int pass = 0, njp = nj; pass < (partner_of >= 0 ? 2 : 1); pass++) {
-          if (pass == 1) njp = fk_partner_stage(md, sm, pc, buf, M, kw);
-          fk_dsy(sm, M, njp, kw);
-          __syncthreads();
-          fk_update_rows(md, sm, buf, njp, kw);
+          for (int b = chunk; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
         }
         __syncthreads();
-        if (tid == 0) red_release_add(&fs->rows_done, 1u);
-        if (cta < G + in_ctas) {
-          // input-row update of the step's lanes, once dvec is complete
-          const unsigned int tgt = (unsigned int)(s + 1) * (unsigned int)G;
-          if (in_ctas == B && ly.ld3 / 4 <= FK_THREADS) fk_sparse_in_one(md, sm, s, cta - G, &fs->dvec_done, tgt);
-          else {
-            if (tid == 0) wait_ge(&fs->dvec_done, tgt);
-            __syncthreads();
-            for (int b = cta - G; b < B; b += in_ctas) { fk_sparse_in(md, sm, s, b); __syncthreads(); }
-          }
-          __syncthreads();
-          if (tid == 0) red_release_add(&fs->in_done, 1u);
-        }
-        if (nxt) {
-          if (tid == 0) wait_ge(&fs->rows_done, rows_target);
-          __syncthreads();
-          fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
-        }
+        if (tid == 0) red_release_add(&fs->in_done, 1u);
+      }
+      fk_update_rows(md, sm, buf, nj, kw);
+      __syncthreads();
+      FK_STAMP(14);
+      if (tid == 0) red_release_add(&fs->rows_done, 1u);
+      if (s + 1 < n_steps) {
+        if (tid == 0) wait_ge(&fs->rows_done, (unsigned int)(s + 1) * (unsigned int)ncol);
+        __syncthreads();
+        fk_prefetch_rows(md, sm, s + 1, n_steps, buf ^ 1, pw);
       }
     }
   }

@@ -404,6 +404,19 @@ __global__ void k_advance(int* base, int n) { if (threadIdx.x == 0 && blockIdx.x
 #include "g4r_persistent.cuh"
 #include "g4r_fast.cuh"
 
+// The shapes k_fast_t<false> (step_mode 2) takes, from the configuration alone: no-embedding mode, one GRU layer with
+// L <= 120, batch <= 32, SGD / Adagrad (+momentum), none of the phases only the per-phase sequence has.  Its ldL / 4 GRU
+// CTAs own no score columns, so this decides the chunk geometry before the workspace is laid out: such a handle has
+// n_sm - ldL / 4 chunks (chunk c on CTA ldL / 4 + c) in every window, whichever kernel runs it, and needs at least one
+// column CTA per lane (column CTA b combines the row statistics of lane b).
+static bool fast_shape(const g4r_config& c, int n_sm) {
+  const int L = c.layers[0], ldL = round4(L);
+  const bool smoothing = (c.loss == G4R_LOSS_XE || c.loss == G4R_LOSS_XE_LOGIT) && c.smoothing > 0.f;
+  return c.step_mode == 2 && c.adapt <= G4R_ADAPT_ADAGRAD && !(c.grad_cap > 0.f) && !smoothing && model_mode(c) == 0 && c.n_layers == 1 &&
+         ldL <= 128 && c.batch_size <= FK_B && 2 * L <= FK_W1 * FK_G && L <= FK_W2 * FK_G && n_sm >= FK_G + 1 &&
+         n_sm - ldL / 4 >= c.batch_size && !tc_eligible(c) && !shard_eligible(c, n_sm);
+}
+
 // ---- cluster launch of the role-specialised kernel (step_mode 3) ----
 constexpr int FC_CLUSTER = 8;      // portable cluster size; cRed in FastSmemC is sized for <= 8 ranks
 static cudaError_t fastc_config(cudaLaunchConfig_t& lc, cudaLaunchAttribute* attrs, int n_attr_coop, int grid, cudaStream_t st) {
@@ -738,6 +751,7 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
     h->fastc_grid = fastc_max_grid(h->n_sm);
     if (h->fastc_grid >= FC_CLUSTER * 2) chunk_cap = std::min(chunk_cap, h->fastc_grid);
   }
+  if (fast_shape(*cfg, h->n_sm)) chunk_cap = h->n_sm - round4(cfg->layers[0]) / 4;   // step_mode 2: no chunks on the GRU CTAs
   size_t need = 0;
   { Carver cv{nullptr, 0, true}; layout(*cfg, cv, nullptr, chunk_cap); need = align_up(cv.off, 256) + 256; }
   if (device_workspace) {
@@ -791,12 +805,11 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_t<false>, FK_THREADS, sizeof(FastSmemR));
     const bool plain_opt = m.adapt <= G4R_ADAPT_ADAGRAD && !h->phase_only;    // the role-specialised kernels implement SGD / Adagrad (+momentum) only
-    h->fast_ok = plain_opt && h->pk_blocks > 0 && per_sm >= 1 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B && h->n_sm >= FK_G + 1 && m.NCH <= 160 &&
-                 2 * m.L <= FK_W1 * FK_G && m.L <= FK_W2 * FK_G &&     // L <= 120, the coverage of k_fast_mg's 48-CTA GRU group (k_fast_t<false> uses ldL / 4 CTAs)
-                 // k_fast_t<false>: ldL / 4 GRU CTAs, up to B helper CTAs, and one partner CTA per GRU CTA for its chunk's row update.
-                 // At most 96 CTAs (ldL <= 128, B <= 32): every shape k_fast takes fits a 132-SM H100.  A smaller grid runs these
-                 // shapes on k_persistent; g4r_fast_windows() reports such windows as slow ones.
-                 h->pk_blocks >= 2 * (m.ldL / 4) + std::min(m.B, h->pk_blocks - m.ldL / 4) &&
+    // k_fast_t<false>: ldL / 4 GRU CTAs, then one column CTA per chunk (the grid is n_sm CTAs, fast_shape chose
+    // NCH = n_sm - ldL / 4); the first B of them also update the input rows.  fk_b1 sums at most 160 chunk
+    // partials.  Otherwise these shapes run on the generic kernels with the same chunks; g4r_fast_windows() reports such
+    // windows as slow ones.
+    h->fast_ok = plain_opt && fast_shape(*cfg, h->n_sm) && h->pk_blocks == h->n_sm && per_sm >= 1 && m.NCH <= h->pk_blocks - m.ldL / 4 && m.NCH <= 160 &&
                  (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);
     h->fastc_ok = plain_opt && cfg->step_mode == 3 && h->fastc_grid >= FC_CLUSTER * 2 && m.mode == 0 && m.n_layers == 1 && m.ldL <= 128 && m.B <= FK_B &&
                   m.NCH <= h->fastc_grid && (m.adapt == G4R_ADAPT_ADAGRAD ? m.Wy_acc != nullptr : true);

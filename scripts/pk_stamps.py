@@ -24,9 +24,10 @@ eng.upload_steps(sched, K, K); c, ms = eng.run_uploaded(K, True)
 st = eng.persistent_stamps(True, K).astype(np.int64)
 if cfg.step_mode >= 2:
     print('fast windows', eng.fast_windows())
-    # step_mode 2 (CTA 0 is a GRU CTA): dSy and the update of its chunk's rows run on a partner CTA after b1
+    # step_mode 2: the column-phase slots come from the first column CTA (dSy and its chunk's row update after b1), the GRU
+    # slots 4-8 from GRU CTA 0 (b1_done reached, then backward, dense update and forward of the next step)
     names = [('wait h + stage', 0, 1), (' targets+scores', 1, 9), (' partial stats', 9, 10), (' B2 + parallel combine', 10, 2), (' RS load + cost', 2, 11), (' g + dby', 11, 12), (' part', 12, 13), (' B3', 13, 3),
-             ('b1 (+release)', 3, 15), ('stage H(s+1)', 15, 14), ('wait b1_done', 14, 4), ('b2 -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 + grp', 6, 7), ('f2 + prefetch issue', 7, 8)]
+             ('b1 (+release)', 3, 15), (' dSy + row update', 15, 14), ('b1 end -> GRU past b1_done', 15, 4), ('b2 -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 + grp', 6, 7), ('f2', 7, 8)]
     if cfg.step_mode == 3:   # GRU phases on one thread-block cluster; dSy and the row update before B3
         names = names[:6] + [(' dSy + part', 12, 13), (' sparse update', 13, 14), (' B3', 14, 3), ('b1 (+release)', 3, 15), ('prefetch issue', 15, 4),
                              ('backward -> dvec', 4, 5), ('dense (resident)', 5, 6), ('f1 (+in_done, barriers)', 6, 7), ('f2', 7, 8)]
