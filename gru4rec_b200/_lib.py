@@ -43,7 +43,7 @@ EXPORTS = [
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
-    'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_predict', 'g4r_reset_eval_hidden',
+    'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_set_eval_exclude_seen', 'g4r_predict', 'g4r_reset_eval_hidden',
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
     'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
     'g4r_sessions_export', 'g4r_sessions_import',
@@ -114,6 +114,7 @@ def load():
     lib.g4r_eval_events.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, C.POINTER(i64), vp, vp, vp]
     lib.g4r_eval_counts.argtypes = [vp, vp, i64]
     lib.g4r_set_eval_items.argtypes = [vp, vp, i64]
+    lib.g4r_set_eval_exclude_seen.argtypes = [vp, i32]
     lib.g4r_predict.argtypes = [vp, vp, i32, vp, vp]
     lib.g4r_reset_eval_hidden.argtypes = [vp]
     lib.g4r_predict_topk.argtypes = [vp, vp, i32, vp, i32, vp, vp]
@@ -151,6 +152,15 @@ def parse_act(name):
         p = [float(x) for x in name.split('-')[1:]]
         return ACT['selu'], p[0], p[1]
     raise NotImplementedError
+
+
+SEEN_BUDGET = 256 << 20     # bytes of exclude_seen's device lists per evaluation call (g4r_set_eval_exclude_seen)
+
+
+def seen_budget():
+    """the library's budget for exclude_seen's lists: SEEN_BUDGET, lowered by G4R_SEEN_BUDGET in the environment (for tests)"""
+    env = os.environ.get('G4R_SEEN_BUDGET')
+    return SEEN_BUDGET if env is None else min(SEEN_BUDGET, max(0, int(env)))
 
 
 def check_topk(k, n_items):
@@ -506,7 +516,8 @@ class Engine(object):
         the data): (recall sums, mrr sums, n_events, counts int32 [n_events, 2], items int32 [n_events, k], scores float32
         [n_events, k]).  The sums equal eval_schedule's bit for bit; counts are (#greater, #equal) as eval_counts gives them; with
         k > 0 every event's top-k list as predict_topk ranks the lane after the input (with set_eval_items, among those items);
-        k = 0: items / scores are None."""
+        k = 0: items / scores are None.  With set_eval_exclude_seen(True) an event whose target its session has already input
+        counts (-1, -1), and the lists leave out the session's inputs (item -1, score NaN past the eligible items)."""
         cut = np.ascontiguousarray(cut_off, dtype=np.int32)
         rec = np.zeros(len(cut), dtype=np.float64); mrr = np.zeros(len(cut), dtype=np.float64)
         n = C.c_int64()
@@ -532,6 +543,12 @@ class Engine(object):
             return
         it = np.ascontiguousarray(items, dtype=np.int64)
         self._check(self.lib.g4r_set_eval_items(self.h, _ptr(it), it.size))
+
+    def set_eval_exclude_seen(self, on):
+        """exclude_seen for later eval_schedule / eval_events calls: each event is ranked without the items its session has
+        input so far (the current input included); a target among them is a miss.  A schedule whose seen lists (lanes x longest
+        session - 1 int32) exceed 256 MiB is refused (NotImplementedError from G4R_ERR_INVALID) before any device work."""
+        self._check(self.lib.g4r_set_eval_exclude_seen(self.h, 1 if on else 0))
 
     def predict(self, X, reset_mask=None):
         X = np.ascontiguousarray(X, dtype=np.int32)

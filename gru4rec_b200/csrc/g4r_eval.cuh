@@ -3,6 +3,7 @@
 // consecutive items against all lanes and counts how many beat / tie the lane's target score.
 // Included at the end of g4r_lib.cu (uses its handle type and helper macros).
 #pragma once
+#include "g4r_seen.cuh"
 #include "g4r_eval_tc.cuh"
 
 constexpr int EV_IT = 64;     // items per CTA tile
@@ -95,8 +96,11 @@ __device__ __forceinline__ void ev_tiles(const ModelDev& md, float* smem, int M,
   }
 }
 
-// target score of every lane, computed with the same sequential k order as the tile kernel (bitwise equal)
-__global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, int* cnt, unsigned int tie, int subset_mode, int lohi_stride) {
+// target score of every lane, computed with the same sequential k order as the tile kernel (bitwise equal); SEEN: also adds the
+// lane's input to its seen list (seen_insert) and flags the lanes whose target is in it (sd.miss)
+template <bool SEEN = false>
+__global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, int* cnt, unsigned int tie, int subset_mode, int lohi_stride,
+                                                  SeenDev sd = SeenDev{}) {
   const ModelDev& md = MD;
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int M = md.wM[s];
@@ -113,13 +117,18 @@ __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, i
   if (tie) sc += tie_noise(tie, s, b, subset_mode ? 0x40000000U + (unsigned int)b : (unsigned int)item);
   tgt[b] = sc;
   cnt[b * 2 + 0] = 0; cnt[b * 2 + 1] = 0;
+  if (SEEN) sd.miss[b] = seen_insert(md, sd, s, b, item) ? 1 : 0;
 }
 
 // Competitors: `subset` (evaluate_gpu(items=...), evaluation.py:52-56) lists the n_cand items that compete instead of the catalogue;
 // without a subset, n_cand > 0 scores the leading items 0 .. n_cand - 1 and 0 the catalogue.  WRITE: out[b * n_comp + pos] = score.
-template <bool WRITE>
+// SEEN (counting only): an item on the lane's seen list is never compared -- a bit per held position, set from the list (a walk
+// of the list's items inside the tile for the catalogue, a binary search per position for a subset, whose every occurrence of a
+// seen item goes)
+template <bool WRITE, bool SEEN = false>
 __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, const float* __restrict__ tgt, int* cnt, float* out,
-                                                           const int* __restrict__ subset, int n_cand, unsigned int tie = 0u) {
+                                                           const int* __restrict__ subset, int n_cand, unsigned int tie = 0u,
+                                                           SeenDev sd = SeenDev{}) {
   const ModelDev& md = MD;
   extern __shared__ __align__(16) float smem[];
   int* sCnt = reinterpret_cast<int*>(smem + EV_TILE_FLOATS);   // [EV_TB][2]
@@ -134,11 +143,25 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
     if (b < M) {
       int gt = 0, eq = 0;
       const float t = WRITE ? 0.f : tgt[b];
+      unsigned int xq = 0u;                      // SEEN: held positions i0 + warp + 8 q whose item is seen
+      if (SEEN) {
+        const int sl = md.wSlot[(size_t)s * md.B + b], n = sd.n[sl];
+        const int* l = sd.list + (size_t)sl * sd.cap;
+        if (subset) {
+#pragma unroll
+          for (int q = 0; q < 8; q++) if (warp + 8 * q < ni && sorted_has(l, n, subset[i0 + warp + 8 * q])) xq |= 1u << q;
+        } else {
+          for (int p = sorted_lb(l, n, i0); p < n && l[p] < i0 + ni; p++) {
+            const int rel = l[p] - i0;
+            if ((rel & 7) == warp) xq |= 1u << (rel >> 3);
+          }
+        }
+      }
       float* orow = WRITE ? out + (size_t)b * I + i0 + warp : nullptr;   // one row pointer keeps the kernel free of spills
 #pragma unroll
       for (int q = 0; q < 8; q++) {
         const int it = i0 + warp + 8 * q;
-        if (warp + 8 * q < ni) {
+        if (warp + 8 * q < ni && !((xq >> q) & 1u)) {
           float sc = acc[q] + md.By[ev_item(subset, it)];
           if (WRITE) orow[8 * q] = sc;
           else {
@@ -160,8 +183,11 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
 }
 static size_t eval_smem_bytes() { return (size_t)EV_TILE_FLOATS * sizeof(float) + EV_TB * 2 * sizeof(int) + 64; }
 
-// ranks + per-cutoff sums (evaluation.py:60-75), accumulated in double on the device
-__global__ void __launch_bounds__(256) k_eval_rank(int slot, int s, const int* cnt, const int* cut, int n_cut, int mode, double* sums) {
+// ranks + per-cutoff sums (evaluation.py:60-75), accumulated in double on the device; SEEN: a lane flagged in miss (target
+// already seen) is a miss, rank +inf, whatever its counts
+template <bool SEEN = false>
+__global__ void __launch_bounds__(256) k_eval_rank(int slot, int s, const int* cnt, const int* cut, int n_cut, int mode, double* sums,
+                                                   const int* __restrict__ miss = nullptr) {
   const ModelDev& md = MD;
   if (blockIdx.x != 0) return;
   const int M = md.wM[s];
@@ -171,6 +197,7 @@ __global__ void __launch_bounds__(256) k_eval_rank(int slot, int s, const int* c
   for (int j = 0; j < n_cut; j++) {
     double hit = 0.0, rr = 0.0;
     for (int b = tid; b < M; b += blockDim.x) {
+      if (SEEN && miss[b]) continue;
       const int gt = cnt[b * 2], eq = cnt[b * 2 + 1];
       double rank;
       if (mode == 1) rank = (double)(gt + eq);
@@ -236,6 +263,12 @@ struct EvalCtx {
   uint64_t split_version = ~0ull;
   void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
   void* events = nullptr;                                         // EventsCtx* of g4r_eval_events (g4r_events.cuh)
+  // exclude_seen (g4r_set_eval_exclude_seen, g4r_seen.cuh): per state slot the seen list, its length, the lanes' miss flags, and
+  // the per-mini-batch CSR copy the top-k kernels of g4r_eval_events read as their exclusions
+  bool seen_on = false;
+  int* dSeen = nullptr; size_t seen_cap = 0;
+  int *dSeenN = nullptr, *dMiss = nullptr;
+  int* dSeenOff = nullptr; int* dSeenEx = nullptr; size_t seen_ex_cap = 0;
 };
 static void topk_release(EvalCtx& e);
 static void events_release(EvalCtx& e);
@@ -281,6 +314,7 @@ static void eval_release(g4r_handle* h) {
   cudaFree(e.dX); cudaFree(e.dY); cudaFree(e.dSlot); cudaFree(e.dF); cudaFree(e.dM); cudaFree(e.dSti); cudaFree(e.dG);
   cudaFree(e.dCut); cudaFree(e.dSums); if (e.dOut) cudaFree(e.dOut); if (e.dCand) cudaFree(e.dCand);
   if (e.dAsplit) cudaFree(e.dAsplit); if (e.dBsplit) cudaFree(e.dBsplit);
+  for (void* p : {(void*)e.dSeen, (void*)e.dSeenN, (void*)e.dMiss, (void*)e.dSeenOff, (void*)e.dSeenEx}) if (p) cudaFree(p);
   slot_free(e.slot);
   delete static_cast<EvalCtx*>(h->eval_ctx);
   h->eval_ctx = nullptr;
@@ -305,7 +339,9 @@ static int eval_ctx(g4r_handle* h, EvalCtx** out) {
   CK(slot_upload(e.slot, e.mde, h->stream));
   cudaFuncSetAttribute(k_eval_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
   cudaFuncSetAttribute(k_eval_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
-  if (cudaFuncSetAttribute(k_eval_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
+  cudaFuncSetAttribute(k_eval_score<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
+  if (cudaFuncSetAttribute(k_eval_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
+  if (cudaFuncSetAttribute(k_eval_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
   h->eval_ctx = new EvalCtx(e);
   *out = static_cast<EvalCtx*>(h->eval_ctx);
   return G4R_OK;
@@ -328,10 +364,38 @@ static int eval_forward(g4r_handle* h, EvalCtx* e, int s, float* const* Hst) {
 
 // g4r_eval_events' per-event outputs (g4r_events.cuh); nullptr on g4r_eval_schedule's path
 struct EventsRun;
-static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev);
+static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev, const SeenDev* sd);
+static bool events_lists(const EventsRun* ev);      // k > 0
+static void events_window(EventsRun* ev, int64_t done);
 static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
 static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
 static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t rk);
+
+// exclude_seen: lists of capacity cap = the schedule's longest session - 1 for every scoring slot (eval_run empties them);
+// refused before any device work when B x cap x 4 bytes (B: the schedule's lanes) exceed SEEN_BYTES, the 256 MiB budget of g4r_eval_events' window
+// buffers (G4R_SEEN_BUDGET in the environment lowers it, for tests)
+constexpr size_t SEEN_BYTES = (size_t)256 << 20;
+static int seen_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, bool csr, SeenDev* sd) {
+  const int64_t cap = std::max<int64_t>(1, s->max_len - 1);
+  size_t budget = SEEN_BYTES;
+  if (const char* b = getenv("G4R_SEEN_BUDGET")) budget = std::min<size_t>(budget, (size_t)std::max(0LL, atoll(b)));
+  if ((size_t)s->B * (size_t)cap * sizeof(int) > budget) {
+    char msg[256];
+    snprintf(msg, sizeof msg, "exclude_seen: the longest session (%lld events) needs seen lists of %d lanes x %lld items, over the %zu-byte budget",
+             (long long)s->max_len, s->B, (long long)cap, budget);
+    FAIL(G4R_ERR_INVALID, msg);
+  }
+  const size_t n = (size_t)s->B * (size_t)cap;             // state slots of the schedule: 0 .. B - 1
+  CK(dev_grow(&e->dSeen, &e->seen_cap, n));
+  if (!e->dSeenN) CK(cudaMalloc(&e->dSeenN, (size_t)e->Be * sizeof(int)));
+  if (!e->dMiss) CK(cudaMalloc(&e->dMiss, (size_t)e->Be * sizeof(int)));
+  if (csr) {
+    if (!e->dSeenOff) CK(cudaMalloc(&e->dSeenOff, (size_t)(e->Be + 1) * sizeof(int)));
+    CK(dev_grow(&e->dSeenEx, &e->seen_ex_cap, n));
+  }
+  sd->list = e->dSeen; sd->n = e->dSeenN; sd->cap = (int)cap; sd->miss = e->dMiss;
+  return G4R_OK;
+}
 
 // The evaluation schedule in staging windows of e->cap mini-batches (g4r_eval_schedule); ev != nullptr adds g4r_eval_events'
 // per-event work on the ranking stream, after the kernels of g4r_eval_schedule, which stay as they are and see the same step
@@ -345,8 +409,14 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
   int rc = eval_ctx(h, &e);
   if (rc) return rc;
   if (s->B > e->Be) FAIL(G4R_ERR_INVALID, "schedule batch size exceeds eval_batch_size");
+  const bool seen = e->seen_on;
+  SeenDev sd;
+  if (seen) {
+    rc = seen_begin(h, e, s, ev && events_lists(ev), &sd);
+    if (rc) return rc;
+  }
   if (ev) {
-    rc = events_begin(h, e, s, ev);
+    rc = events_begin(h, e, s, ev, seen ? &sd : nullptr);
     if (rc) return rc;
   }
   const int Be = e->Be, Bs = s->B, I = h->md.n_items;
@@ -354,6 +424,7 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
   for (int i = 0; i < h->md.n_layers; i++) CK(cudaMemsetAsync(h->He[i], 0, (size_t)Be * h->md.layer[i].ldL * sizeof(float), st));   // gru4rec.py:731-733
   CK(cudaMemcpyAsync(e->dCut, cut_off, n_cut * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(e->dSums, 0, 128 * sizeof(double), st));
+  if (seen) CK(cudaMemsetAsync(sd.n, 0, (size_t)Be * sizeof(int), st));   // every lane starts a session with the schedule
   // wgmma tiles (full-catalogue ranking of a wide batch; candidate subsets and tiebreaking take the fp32 tiles): decided once
   // with the schedule's batch, then per mini-batch with its lanes
   const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;   // + the bias column
@@ -393,10 +464,20 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
     // forward stream may overwrite it; everything the ranking kernels share (target scores, counters, operand blocks, metric
     // sums) is ordered by the ranking stream itself, so the sums accumulate in mini-batch order as before.
     cudaStream_t rk = h->side;
+    if (ev) events_window(ev, done);
     for (int64_t i = 0; i < w; i++) {
       eval_forward(h, e, (int)i, h->He);
       CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
-      k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
+      if (seen) {       // inserts this mini-batch's inputs on the ranking stream: after i-1's ranking has read the lists, while
+                        // i+1's forward runs
+        k_eval_tgt<true><<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0, sd);
+        if (ev && events_lists(ev)) {
+          k_seen_csr<<<1, SEEN_CSR_THREADS, 0, rk>>>(e->slot, (int)i, sd, e->dSeenOff, e->dSeenEx);
+          h->launches++;
+        }
+      } else {
+        k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
+      }
       if (ev) {
         rc = events_stage(h, e, ev, (int)i, rk);     // saves this mini-batch's y before the forward may move on
         if (rc) return rc;
@@ -407,14 +488,17 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
       if (tc) {
         k_tc_split<TC_M><<<dim3((M_i + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(h->md.layer[h->md.n_layers - 1].y, M_i, h->md.ldL, h->md.L, e->dAsplit, tc_chunks, nullptr, 1.0f);
         CK(cudaEventRecord(h->ts_ev[1], rk));
-        k_eval_tc<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(e->slot, (int)i, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit);
+        if (seen) k_eval_tc<true><<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(e->slot, (int)i, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit, sd);
+        else k_eval_tc<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(e->slot, (int)i, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit);
         h->launches++;
       } else {
-        k_eval_score<false><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, tie);
+        if (seen) k_eval_score<false, true><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, tie, sd);
+        else k_eval_score<false><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, tie);
         CK(cudaEventRecord(h->ts_ev[1], rk));
       }
       CK(cudaStreamWaitEvent(st, h->ts_ev[1], 0));        // the hidden output of this mini-batch has been consumed
-      k_eval_rank<<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums);
+      if (seen) k_eval_rank<true><<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums, sd.miss);
+      else k_eval_rank<<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums);
       h->launches += 3;
       if (ev) {
         rc = events_step(h, e, ev, (int)i, rk);
@@ -450,6 +534,18 @@ extern "C" int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes) {
   cudaSetDevice(h->cfg.device);
   CK(cudaStreamSynchronize(h->stream));
   CK(cudaMemcpy(out, h->dRankCnt, (size_t)n_lanes * 2 * sizeof(int), cudaMemcpyDeviceToHost));
+  return G4R_OK;
+}
+
+// evaluate_gpu(exclude_seen=True): later g4r_eval_schedule / g4r_eval_events calls rank each target without the items its session
+// has input so far (the current input included); a target among them is a miss (g4r_seen.cuh, DESIGN §3g)
+extern "C" int g4r_set_eval_exclude_seen(g4r_handle* h, int32_t on) {
+  if (!h) return G4R_ERR_INVALID;
+  cudaSetDevice(h->cfg.device);
+  EvalCtx* e = nullptr;
+  int rc = eval_ctx(h, &e);
+  if (rc) return rc;
+  e->seen_on = on != 0;
   return G4R_OK;
 }
 

@@ -255,12 +255,20 @@ __device__ __forceinline__ void tc_sweep(int M, int I, int K, const unsigned cha
 // cnt[b*2 + 0] += #items with score > target score of lane b; cnt[b*2 + 1] += #items with score == target (the target itself
 // counts as one tie, exactly as in the fp32 kernel where its score equals the target score bit for bit).  Each thread counts its
 // two lanes x 32 items of a tile thread-locally; the four threads of a quad sum their counts after the lane block's last tile.
+// SEEN: the items of a lane's seen list are taken back out the way the target's column is -- the seen items among the columns the
+// thread holds become a bit mask, and the same d[i] that was counted is uncounted, so no seen item is ever counted, exactly.  The
+// CTA visits a lane block's tiles in increasing column order, so each lane keeps a cursor into its list with the next seen item
+// already loaded: a tile without a seen item costs no load, a cursor behind the tile jumps by a binary search (O(log cap + seen
+// items in the tile) per lane and tile at worst)
+template <bool SEEN = false>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, const float* __restrict__ tgt, int tgt_stride, int* cnt,
-                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit) {
+                                                           const unsigned char* __restrict__ Asplit, const unsigned char* __restrict__ Bsplit,
+                                                           SeenDev sd = SeenDev{}) {
   const ModelDev& md = MD;
   const int M = md.wM[s], I = md.n_items, lane = threadIdx.x & 31;
   int bb[2], yit[2]; bool vrow[2]; float lo[2], hi[2];
   int cgt[2], cge[2];
+  const int* sl_l[2]; int sl_n[2], sl_p[2], sl_nx[2];              // SEEN: the two lanes' lists, cursors and next seen items
   auto lane_block = [&](int b) {
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -269,6 +277,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, cons
       yit[h] = vrow[h] ? md.wY[(size_t)s * md.B + bb[h]] : -1;
       lo[h] = vrow[h] ? tgt[tgt_stride + bb[h]] : INFINITY; hi[h] = vrow[h] ? tgt[2 * tgt_stride + bb[h]] : INFINITY;   // k_eval_tgt
       cgt[h] = 0; cge[h] = 0;
+      if (SEEN) {
+        const int sl = vrow[h] ? md.wSlot[(size_t)s * md.B + bb[h]] : 0;
+        sl_l[h] = sd.list + (size_t)sl * sd.cap; sl_n[h] = vrow[h] ? sd.n[sl] : 0;
+        sl_p[h] = 0; sl_nx[h] = sl_n[h] > 0 ? sl_l[h][0] : INT_MAX;
+      }
     }
   };
   auto tile = [&](const float (&d)[64], int c0, bool last) {
@@ -291,6 +304,30 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_eval_tc(int slot, int s, cons
         cgt[h] -= (xs > hi[h]) ? 1 : 0;
         cge[h] -= (xs >= lo[h]) ? 1 : 0;
         cge[h] += 1;                                               // == (self: not above) + one tie
+      }
+    }
+    if (SEEN) {
+      unsigned int xm[2];                                          // bit 2 (i / 4) + i % 2: column of d[i] is a seen item
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        xm[h] = 0u;
+        if (sl_nx[h] < c0) {                                       // seen items in other CTAs' tiles: jump past them
+          sl_p[h] += sorted_lb(sl_l[h] + sl_p[h], sl_n[h] - sl_p[h], c0);
+          sl_nx[h] = sl_p[h] < sl_n[h] ? sl_l[h][sl_p[h]] : INT_MAX;
+        }
+        while (sl_nx[h] < c0 + 128) {
+          const int rel = sl_nx[h] - c0;
+          if ((rel & 7) < 2) xm[h] |= 1u << ((rel >> 3) * 2 + (rel & 1));
+          sl_p[h]++;
+          sl_nx[h] = sl_p[h] < sl_n[h] ? sl_l[h][sl_p[h]] : INT_MAX;
+        }
+      }
+      if (xm[0] | xm[1]) {
+#pragma unroll
+        for (int i = 0; i < 64; i++) {
+          const int h = (i >> 1) & 1;
+          if ((xm[h] >> ((i >> 2) * 2 + (i & 1))) & 1u) { cgt[h] -= (d[i] > hi[h]) ? 1 : 0; cge[h] -= (d[i] >= lo[h]) ? 1 : 0; }
+        }
       }
     }
     if (!last) return;

@@ -12,6 +12,9 @@
 //           normaliser and is redone at the end of the window
 //   flush   one read of the window's survivor counters; every overflowed lane is rescored over the whole catalogue in fp32 from
 //           the saved y (k_topk_rows / k_topk_final, in chunks of rows), then the window's outputs go to the host
+// exclude_seen (g4r_seen.cuh): the lanes' seen lists, gathered per mini-batch into the CSR exclusions the top-k kernels read
+// (k_seen_csr), with a prefix of at least k + cap items; an overflowed lane's seen set at its own mini-batch (the lists have moved
+// on by the flush) is rebuilt from the schedule on the host
 // The per-event window (w mini-batches, bounded by the size of its buffers) is separate from eval_run's staging window: eval_run
 // stages the schedule in windows of e->cap mini-batches exactly as g4r_eval_schedule does, so every kernel of the evaluation sees
 // the same step index (the tiebreaking noise hashes it), and the per-event buffers are flushed every w mini-batches within it and
@@ -38,6 +41,8 @@ struct EventsCtx {
   float2* dOvNorm = nullptr; size_t ov_norm_cap = 0;      //   their normalisers
   int* dOvItems = nullptr; size_t ov_items_cap = 0;       //   their lists
   float* dOvScores = nullptr; size_t ov_scores_cap = 0;
+  int* dOvExOff = nullptr; size_t ov_ex_off_cap = 0;      //   their exclusions (exclude_seen)
+  int* dOvEx = nullptr; size_t ov_ex_cap = 0;
 };
 
 // one g4r_eval_events call
@@ -56,13 +61,20 @@ struct EventsRun {
   int64_t win_ev = 0;                                     // events of the window so far
   std::vector<int64_t> off;                               // window event of lane 0 of every mini-batch of the window
   std::vector<int> survn;                                 // host copy of dSurvN
+  const g4r_schedule* sched = nullptr;
+  int64_t done = 0;                                       // schedule step of the staging window's first mini-batch
+  bool seen = false;                                      // exclude_seen: the lists exclude ex_off / ex (k_seen_csr's output)
+  const int* ex_off = nullptr; const int* ex = nullptr;
 };
+static bool events_lists(const EventsRun* ev) { return ev->k > 0; }
+static void events_window(EventsRun* ev, int64_t done) { ev->done = done; }
 
 static void events_release(EvalCtx& e) {
   if (!e.events) return;
   EventsCtx& x = *static_cast<EventsCtx*>(e.events);
   for (void* p : {(void*)x.dYk, (void*)x.dMk, (void*)x.dIdent, (void*)x.dYw, (void*)x.dSurvN, (void*)x.dNorm, (void*)x.dCnt,
-                  (void*)x.dItems, (void*)x.dScores, (void*)x.dOvSrc, (void*)x.dOvEv, (void*)x.dOvNorm, (void*)x.dOvItems, (void*)x.dOvScores})
+                  (void*)x.dItems, (void*)x.dScores, (void*)x.dOvSrc, (void*)x.dOvEv, (void*)x.dOvNorm, (void*)x.dOvItems, (void*)x.dOvScores,
+                  (void*)x.dOvExOff, (void*)x.dOvEx})
     if (p) cudaFree(p);
   slot_free(x.slot);
   delete static_cast<EventsCtx*>(e.events);
@@ -82,11 +94,12 @@ __global__ void __launch_bounds__(256) k_ev_stage(int slot, int s, float* __rest
   }
 }
 
-// the (#greater, #equal) pairs of the M lanes of step s
-__global__ void __launch_bounds__(256) k_ev_counts(int slot, int s, const int* __restrict__ cnt, int* __restrict__ out) {
+// the (#greater, #equal) pairs of the M lanes of step s; SEEN: (-1, -1) for a lane flagged in miss
+template <bool SEEN = false>
+__global__ void __launch_bounds__(256) k_ev_counts(int slot, int s, const int* __restrict__ cnt, int* __restrict__ out, const int* __restrict__ miss = nullptr) {
   const ModelDev& md = MD;
   const int n = 2 * md.wM[s];
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = cnt[i];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = (SEEN && miss[i >> 1]) ? -1 : cnt[i];
 }
 
 // softmax normaliser (max, sum) of every lane whose survivors overflowed, reduced from the tile partials exactly as k_topk_final
@@ -140,6 +153,25 @@ __global__ void __launch_bounds__(256) k_ev_scatter(const int* __restrict__ item
   }
 }
 
+// appends to ex the seen set of lane b at schedule step g (its session's inputs up to and including that step: the lane's slot is
+// followed back through the steps until its zero-before flag or the schedule's start), sorted and distinct
+static void seen_rebuild(const g4r_schedule* s, int64_t g, int b, std::vector<int>& ex) {
+  const int B = s->B, sl = s->slots[(size_t)(g * B + b)];
+  const size_t e0 = ex.size();
+  for (int64_t t = g; t >= 0; t--) {
+    if (t < g) {                 // the lane that held the slot at step t (tail compaction moves lanes, never slots)
+      int lb = -1;
+      for (int c = 0; c < s->M[(size_t)t]; c++) if (s->slots[(size_t)(t * B + c)] == sl) { lb = c; break; }
+      if (lb < 0) break;
+      b = lb;
+    }
+    ex.push_back(s->X[(size_t)(t * B + b)]);
+    if (s->F[(size_t)(t * B + b)] & 2) break;
+  }
+  std::sort(ex.begin() + e0, ex.end());
+  ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
+}
+
 static int events_ctx(g4r_handle* h, EvalCtx* e, EventsCtx** out) {
   if (!e->events) {
     const int slot = slot_alloc();
@@ -166,8 +198,11 @@ static int events_ctx(g4r_handle* h, EvalCtx* e, EventsCtx** out) {
 }
 
 // checks k, sizes the per-event window and its buffers, prepares the top-k operands
-static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev) {
+static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev, const SeenDev* sd) {
   const int I = h->md.n_items, Be = e->Be, Bs = s->B, ldL = h->md.ldL, k = ev->k;
+  ev->sched = s;
+  ev->seen = sd != nullptr;
+  ev->ex_off = sd ? e->dSeenOff : nullptr; ev->ex = sd ? e->dSeenEx : nullptr;
   if (k > 0) {
     int rc = topk_filter(h, k, e->n_cand > 0 ? e->hCand.data() : nullptr, e->n_cand, &ev->f);
     if (rc) return rc;
@@ -182,11 +217,12 @@ static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, Events
   ev->off.assign((size_t)w, 0);
   CK(dev_grow(&x->dCnt, &x->cnt_cap, (size_t)w * Be * 2));
   if (k == 0) return G4R_OK;
-  // the top-k constants of topk_rank for a call without exclusions; only the tile kind depends on the mini-batch's lanes
+  // the top-k constants of topk_rank (exclude_seen: with exclusions of at most cap items per lane); only the tile kind depends
+  // on the mini-batch's lanes
   const bool use_cand = ev->f.use_cand;
   ev->n_comp = use_cand ? ev->f.n_distinct : I;
-  ev->P = std::min(ev->n_comp, std::max(k, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
-  ev->no_tile = use_cand && ev->P == ev->n_comp;
+  ev->P = std::min(ev->n_comp, std::max(k + (sd ? sd->cap : 0), std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
+  ev->no_tile = (use_cand || ev->seen) && ev->P == ev->n_comp;
   ev->C = std::min(ev->n_comp, 16 * k + TOPK_SURV_BASE);
   const int tc_tiles = (I + TC_N - 1) / TC_N;
   const int n_part = ev->no_tile ? 0 : std::max(2 * tc_tiles, (ev->n_comp + EV_IT - 1) / EV_IT);
@@ -242,7 +278,8 @@ static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStre
   EventsCtx* x = ev->x;
   const int Be = e->Be, M = e->hM[i], k = ev->k, j = i - ev->base;
   const int64_t o = ev->off[(size_t)j];
-  k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(e->slot, i, h->dRankCnt, x->dCnt + 2 * o);
+  if (ev->seen) k_ev_counts<true><<<(2 * Be + 255) / 256, 256, 0, rk>>>(e->slot, i, h->dRankCnt, x->dCnt + 2 * o, e->dMiss);
+  else k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(e->slot, i, h->dRankCnt, x->dCnt + 2 * o);
   h->launches++;
   if (k > 0) {
     int rc = events_topk(h, e, ev, M, j, o, rk);
@@ -258,8 +295,11 @@ static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, i
   TopkCtx* t = ev->t;
   const int I = h->md.n_items, L = h->md.L, P = ev->P, C = ev->C, n_comp = ev->n_comp;
   const bool filt = ev->f.use_cand, soft = h->md.fact.kind > G4R_ACT_SELU;
+  const bool fx = filt || ev->seen;                      // the filtering instances: candidates and / or exclusions
   const unsigned int* dmask = filt ? t->dMask : nullptr;
   const int* dcand = filt ? t->dCand : nullptr;
+  const int* dexoff = ev->seen ? ev->ex_off : nullptr;
+  const int* dex = ev->seen ? ev->ex : nullptr;
   const bool tc = !ev->no_tile && wgmma_tiles(h->cfg, M, n_comp, I);
   const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
   const int n_part = ev->no_tile ? 0 : tc ? 2 * tc_tiles : (n_comp + EV_IT - 1) / EV_IT;
@@ -267,23 +307,23 @@ static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, i
   k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(x->slot, 0, nullptr, nullptr, t->dPre, dcand, P);
   h->launches++;
   if (!ev->no_tile) {
-    (filt ? k_topk_tau<true> : k_topk_tau<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18), dcand, nullptr, nullptr);
+    (fx ? k_topk_tau<true> : k_topk_tau<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18), dcand, dexoff, dex);
     if (tc) {
       k_tc_split<TC_M><<<dim3((M + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(x->dYk, M, h->md.ldL, L, e->dAsplit, tc_chunks, nullptr, 1.0f);
-      (filt ? k_topk_tc<true> : k_topk_tc<false>)<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part, e->dAsplit, e->dBsplit,
-                                                                                                                dmask, nullptr, nullptr);
+      (fx ? k_topk_tc<true> : k_topk_tc<false>)<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part, e->dAsplit, e->dBsplit,
+                                                                                                              dmask, dexoff, dex);
       h->launches += 2;
     } else {
-      (filt ? k_topk_fp32<true> : k_topk_fp32<false>)<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part,
-                                                                                                                             dcand, n_comp, nullptr, nullptr);
+      (fx ? k_topk_fp32<true> : k_topk_fp32<false>)<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part,
+                                                                                                                           dcand, n_comp, dexoff, dex);
       h->launches++;
     }
     h->launches++;
     if (soft) { k_ev_norm<<<M, TOPK_THREADS, 0, rk>>>(cnt, C, t->dPart, n_part, x->dNorm + (size_t)j * Be); h->launches++; }
   }
   // an overflowed lane selects from its truncated list here; its list is replaced at the end of the window
-  (filt ? k_topk_final<true> : k_topk_final<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, k, ev->no_tile ? nullptr : cnt, t->dSurv, t->dSurvPre, C, nullptr, nullptr,
-                                                                                t->dPart, n_part, x->dItems + o * k, x->dScores + o * k, dcand, t->dPre, P, dmask, nullptr, nullptr);
+  (fx ? k_topk_final<true> : k_topk_final<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, k, ev->no_tile ? nullptr : cnt, t->dSurv, t->dSurvPre, C, nullptr, nullptr,
+                                                                              t->dPart, n_part, x->dItems + o * k, x->dScores + o * k, dcand, t->dPre, P, dmask, dexoff, dex);
   h->launches++;
   CK(cudaGetLastError());
   return G4R_OK;
@@ -306,7 +346,7 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
         for (int b = 0; b < e->hM[ev->base + i]; b++)
           if (ev->survn[(size_t)(i * Be + b)] > ev->C) { src.push_back((int)(i * Be + b)); evw.push_back((int)(ev->off[(size_t)i] + b)); }
       const int chunk = (int)std::min<int64_t>(Be, std::max<int64_t>(1, (int64_t)(EVENTS_ROWS_BYTES / ((size_t)I * sizeof(float)))));
-      const bool filt = ev->f.use_cand;
+      const bool filt = ev->f.use_cand, fx = filt || ev->seen;
       TopkCtx* t = ev->t;
       for (size_t j0 = 0; j0 < src.size(); j0 += (size_t)chunk) {
         const int n = (int)std::min<size_t>((size_t)chunk, src.size() - j0);
@@ -318,11 +358,23 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
         CK(dev_grow(&x->dOvScores, &x->ov_scores_cap, (size_t)chunk * k));
         CK(cudaMemcpyAsync(x->dOvSrc, src.data() + j0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rk));
         CK(cudaMemcpyAsync(x->dOvEv, evw.data() + j0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rk));
+        if (ev->seen) {                        // the chunk's seen sets at their own mini-batches, rebuilt from the schedule
+          std::vector<int> eo(1, 0), ex;
+          for (int j = 0; j < n; j++) {
+            const int r = src[j0 + (size_t)j];
+            seen_rebuild(ev->sched, ev->done + ev->base + r / Be, r % Be, ex);
+            eo.push_back((int)ex.size());
+          }
+          CK(dev_grow(&x->dOvExOff, &x->ov_ex_off_cap, eo.size()));
+          CK(dev_grow(&x->dOvEx, &x->ov_ex_cap, std::max<size_t>(1, ex.size())));
+          CK(cudaMemcpyAsync(x->dOvExOff, eo.data(), eo.size() * sizeof(int), cudaMemcpyHostToDevice, rk));
+          if (!ex.empty()) CK(cudaMemcpyAsync(x->dOvEx, ex.data(), ex.size() * sizeof(int), cudaMemcpyHostToDevice, rk));
+        }
         k_ev_gather<<<std::min(2 * h->n_sm, (n * h->md.ldL / 4 + 255) / 256 + 1), 256, 0, rk>>>(x->dYw, x->dOvSrc, n, h->md.ldL, x->dYk, x->dMk, x->dNorm, x->dOvNorm);
         k_topk_rows<<<dim3((I + 127) / 128, n), 128, 0, rk>>>(x->slot, x->dIdent, e->dOut);
-        (filt ? k_topk_final<true> : k_topk_final<false>)<<<n, TOPK_THREADS, 0, rk>>>(x->slot, k, x->dIdent, t->dSurv, t->dSurvPre, ev->C, x->dIdent, e->dOut,
-                                                                                      x->dOvNorm, 1, x->dOvItems, x->dOvScores, filt ? t->dCand : nullptr, t->dPre, ev->P,
-                                                                                      filt ? t->dMask : nullptr, nullptr, nullptr);
+        (fx ? k_topk_final<true> : k_topk_final<false>)<<<n, TOPK_THREADS, 0, rk>>>(x->slot, k, x->dIdent, t->dSurv, t->dSurvPre, ev->C, x->dIdent, e->dOut,
+                                                                                    x->dOvNorm, 1, x->dOvItems, x->dOvScores, filt ? t->dCand : nullptr, t->dPre, ev->P,
+                                                                                    filt ? t->dMask : nullptr, ev->seen ? x->dOvExOff : nullptr, ev->seen ? x->dOvEx : nullptr);
         k_ev_scatter<<<std::min(2 * h->n_sm, (n * k + 255) / 256), 256, 0, rk>>>(x->dOvItems, x->dOvScores, x->dOvEv, n, k, x->dItems, x->dScores);
         h->launches += 4;
         CK(cudaGetLastError());

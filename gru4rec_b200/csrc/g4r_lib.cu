@@ -40,6 +40,7 @@ struct g4r_schedule {
   std::vector<uint8_t> F;
   std::vector<int64_t> P;       // recorded on request (mode | 2): index in data_items of every input X (target at P + 1), -1 on unused lanes
   bool has_pos = false;
+  int64_t max_len = 1;          // events of the longest session walked (its inputs bound a lane's seen list, g4r_seen.cuh)
 };
 
 struct g4r_handle {
@@ -467,6 +468,7 @@ static cudaError_t raise_smem_limit(const void* func, size_t bytes) {
 
 static int tiles2(int cols, int rows) { return ((cols + GB - 1) / GB) * ((rows + GB - 1) / GB); }
 
+#include "g4r_seen.cuh"
 #include "g4r_eval_tc.cuh"
 #include "g4r_tcstep.cuh"
 // The shapes the tensor-core step takes: constrained embedding, one layer, batch <= 256, SGD / Adagrad (+momentum); chosen
@@ -1083,6 +1085,7 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
       if (len > 1) pairs += len - 1;
       max_len = std::max(max_len, len);
     }
+    s->max_len = max_len;
     const size_t guess = (size_t)(pairs / B + max_len + 2);
     s->X.reserve(guess * B); s->Y.reserve(guess * B); s->slots.reserve(guess * B); s->F.reserve(guess * B); s->M.reserve(guess);
     if (want_pos) s->P.reserve(guess * B);

@@ -61,12 +61,6 @@ __device__ __forceinline__ uint64_t topk_key(float kf, int item) {
 }
 __device__ __forceinline__ float topk_keyval(const ActSpec a, float pre) { return a.kind <= G4R_ACT_SELU ? act_fwd(a, pre) : pre; }
 
-// item in the sorted list l[0 .. n)
-__device__ __forceinline__ bool topk_in(const int* __restrict__ l, int n, int item) {
-  int lo = 0, hi = n;
-  while (lo < hi) { const int m = (lo + hi) >> 1; if (l[m] < item) lo = m + 1; else hi = m; }
-  return lo < n && l[lo] == item;
-}
 // item in the candidate bitmap (nullptr: every item)
 __device__ __forceinline__ bool topk_is_cand(const unsigned int* __restrict__ mask, int item) {
   return !mask || ((mask[item >> 5] >> (item & 31)) & 1u);
@@ -75,7 +69,7 @@ __device__ __forceinline__ bool topk_is_cand(const unsigned int* __restrict__ ma
 __device__ __forceinline__ bool topk_excluded(const int* __restrict__ ex_off, const int* __restrict__ ex, int b, int item) {
   if (!ex_off) return false;
   const int e0 = ex_off[b];
-  return topk_in(ex + e0, ex_off[b + 1] - e0, item);
+  return sorted_has(ex + e0, ex_off[b + 1] - e0, item);
 }
 
 // candidates of one lane: position j is item idx[j] (idx == nullptr: item j) with fp32 pre-activation pre[j]; an item outside
@@ -87,7 +81,7 @@ __device__ __forceinline__ uint64_t topk_src_key(const ActSpec a, const TopkSrc&
 __device__ __forceinline__ bool topk_src_live(const TopkSrc& s, int j) {
   if (!s.cand && s.n_ex == 0) return true;
   const int item = s.idx ? s.idx[j] : j;
-  return topk_is_cand(s.cand, item) && !topk_in(s.ex, s.n_ex, item);
+  return topk_is_cand(s.cand, item) && !sorted_has(s.ex, s.n_ex, item);
 }
 __device__ __forceinline__ void topk_set_excl(TopkSrc& s, const int* ex_off, const int* ex, int b) {
   if (ex_off) { s.ex = ex + ex_off[b]; s.n_ex = ex_off[b + 1] - ex_off[b]; }

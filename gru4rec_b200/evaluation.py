@@ -19,12 +19,42 @@ def _prepare(gru, test_data, session_key, item_key, time_key):
     return test_data, test_data.ItemIdx.values, offset_sessions
 
 
+class _ExcludeSeen(object):
+    """exclude_seen on the engine for the duration of one evaluation (reset whatever happens, like the candidate items).  The
+    library refuses seen lists over its budget (lanes x (longest session - 1) int32); the same test on the whole test set is made
+    here first, so that every rank of a torch.distributed job refuses together (a rank's shard never needs more) with a
+    ValueError that names the longest session"""
+
+    def __init__(self, eng, on, test_data, session_key, offset_sessions, lanes):
+        self.eng, self.on = eng, on
+        if on:
+            lens = np.diff(offset_sessions)
+            j = int(np.argmax(lens)) if len(lens) else 0
+            need = int(lanes) * max(1, int(lens[j]) - 1 if len(lens) else 1) * 4
+            if need > _lib.seen_budget():
+                sid = test_data[session_key].values[offset_sessions[j]]
+                sid = sid.item() if isinstance(sid, np.generic) else sid
+                raise ValueError('exclude_seen: session %r has %d events; its seen lists for %d lanes take %d bytes, over the %d-byte '
+                                 'budget' % (sid, int(lens[j]), int(lanes), need, _lib.seen_budget()))
+
+    def __enter__(self):
+        if self.on:
+            self.eng.set_eval_exclude_seen(True)
+        return self
+
+    def __exit__(self, typ, err, tb):
+        if self.on:
+            self.eng.set_eval_exclude_seen(False)
+        return False
+
+
 def _cuts(cut_off):
     multi_cut_off = (type(cut_off) == list) or (type(cut_off) == tuple)
     return list(cut_off) if multi_cut_off else [cut_off]
 
 
-def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard'):
+def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard',
+                 exclude_seen=False):
     '''
     Recall@N and MRR@N of next-item prediction, session-parallel (evaluation.py:15-147).
     Returns (recall_list, mrr_list), one entry per cut-off.  `mode` as in the reference; 'tiebreaking' adds U(0,1)*1e-10 to
@@ -33,6 +63,11 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     reference the target's own score competes only if the target is listed, so 'conservative' can give rank 0 (MRR = inf).
     Under a torch.distributed job (torchrun, one process per GPU) every rank calls this with the same test data and scores
     every world-th session; all ranks return the same (summed) result.  G4R_EVAL_SHARD=0 switches the sharding off.
+    `exclude_seen` (an addition to the reference's signature): evaluate what recommend_next_batch(exclude_seen=True) serves.
+    Each event is ranked without the items its session has input so far, the current input included (with `items`, every
+    occurrence of such an item leaves the list); an event whose target is among them is a miss (rank inf: it adds nothing to
+    Recall or MRR but still counts as an event).  The seen lists live on the device, (batch_size x longest session - 1) int32
+    within 256 MiB: a longer longest session raises ValueError naming it (on every rank of a torch.distributed job).
     '''
     if gru.error_during_train: raise Exception
     if mode not in _MODES:
@@ -51,21 +86,22 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     if items is not None:
         eng.set_eval_items(gru.itemidmap[items].values)       # KeyError for unknown ids, as the reference's gru.itemidmap[items]
     try:
-        if world == 1:
-            sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1)
-            rec, mrr, n = eng.eval_schedule(sched, cuts, _MODES[mode])
-        else:
-            # one process per GPU: rank r scores every world-th session on its full replica of the model; the hit and
-            # reciprocal-rank sums (double) and the event count are summed over the ranks -- no exchange on the data path
-            from .parallel import shard_eval_sessions, allreduce_sum
-            import torch.distributed as dist
-            mine = shard_eval_sessions(n_sessions, rank, world)
-            rec, mrr, n = np.zeros(len(cuts)), np.zeros(len(cuts)), 0
-            if len(mine):
-                sched = _lib.Schedule(test_data_items, offset_sessions, mine, min(batch_size, len(mine)), 0, mode=1)
+        with _ExcludeSeen(eng, exclude_seen, test_data, session_key, offset_sessions, batch_size):
+            if world == 1:
+                sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1)
                 rec, mrr, n = eng.eval_schedule(sched, cuts, _MODES[mode])
-            tot = allreduce_sum(np.concatenate([rec, mrr, [float(n)]]), dist)
-            rec, mrr, n = tot[:len(cuts)], tot[len(cuts):2 * len(cuts)], int(round(tot[-1]))
+            else:
+                # one process per GPU: rank r scores every world-th session on its full replica of the model; the hit and
+                # reciprocal-rank sums (double) and the event count are summed over the ranks -- no exchange on the data path
+                from .parallel import shard_eval_sessions, allreduce_sum
+                import torch.distributed as dist
+                mine = shard_eval_sessions(n_sessions, rank, world)
+                rec, mrr, n = np.zeros(len(cuts)), np.zeros(len(cuts)), 0
+                if len(mine):
+                    sched = _lib.Schedule(test_data_items, offset_sessions, mine, min(batch_size, len(mine)), 0, mode=1)
+                    rec, mrr, n = eng.eval_schedule(sched, cuts, _MODES[mode])
+                tot = allreduce_sum(np.concatenate([rec, mrr, [float(n)]]), dist)
+                rec, mrr, n = tot[:len(cuts)], tot[len(cuts):2 * len(cuts)], int(round(tot[-1]))
     finally:
         if items is not None:
             eng.set_eval_items(None)
@@ -77,16 +113,23 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
 
 
 def _ranks(counts, mode):
-    """rank of every event from its (#greater, #equal) counts, by the formula of `mode` (evaluation.py:60-63)"""
+    """rank of every event from its (#greater, #equal) counts, by the formula of `mode` (evaluation.py:60-63); the counts
+    (-1, -1) of an exclude_seen miss give inf"""
     gt, eq = counts[:, 0].astype(np.float64), counts[:, 1].astype(np.float64)
     if mode == 'conservative':
-        return gt + eq
-    if mode == 'median':
-        return gt + 0.5 * (eq - 1.0) + 1.0
-    return gt + 1.0
+        r = gt + eq
+    elif mode == 'median':
+        r = gt + 0.5 * (eq - 1.0) + 1.0
+    else:
+        r = gt + 1.0
+    miss = counts[:, 0] < 0
+    if miss.any():
+        r[miss] = np.inf
+    return r
 
 
-def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard', k=0):
+def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard', k=0,
+                    exclude_seen=False):
     '''
     evaluate_gpu with per-event outputs, from one evaluation pass on the device.  The test data is prepared, batched and ranked
     exactly as evaluate_gpu does it (same arguments, modes and `items` semantics).  Returns a dict:
@@ -104,6 +147,11 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
       compete and the softmax normaliser runs over them).  The lists do not tie-break like 'rank' does: the rank of a target
       that ties other items depends on `mode`, its place in the list on the item index.
 
+    `exclude_seen` as in evaluate_gpu: every rank, sum and list leaves out the items the session has input so far, the current
+    input included.  'rank' is inf exactly for the events whose target is among them (NDCG 0), and each list is what
+    recommend_next_batch(..., exclude_seen=True) returns after that input; a list with fewer than k eligible items is padded
+    with item None (the item array is then of object dtype) and score NaN, and 'coverage' ignores the padding.
+
     Single process only: under a torch.distributed job it raises NotImplementedError.
     '''
     if gru.error_during_train: raise Exception
@@ -119,8 +167,9 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
     if items is not None:
         eng.set_eval_items(gru.itemidmap[items].values)
     try:
-        sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS)
-        rec, mrr, n, counts, top_i, top_s = eng.eval_events(sched, cuts, _MODES[mode], k)
+        with _ExcludeSeen(eng, exclude_seen, test_data, session_key, offset_sessions, batch_size):
+            sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS)
+            rec, mrr, n, counts, top_i, top_s = eng.eval_events(sched, cuts, _MODES[mode], k)
         pos = sched.positions()
     finally:
         if items is not None:
@@ -141,7 +190,12 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
     if k:
         top_i = top_i[order]
         ids = gru.itemidmap.index.values
-        out['topk_items'] = ids[top_i]
+        pad = top_i < 0                                    # exclude_seen: fewer than k eligible items
+        if pad.any():
+            out['topk_items'] = ids[np.where(pad, 0, top_i)].astype(object)
+            out['topk_items'][pad] = None
+        else:
+            out['topk_items'] = ids[top_i]
         out['topk_scores'] = top_s[order]
-        out['coverage'] = len(np.unique(top_i)) / gru.n_items
+        out['coverage'] = len(np.unique(top_i[~pad])) / gru.n_items
     return out

@@ -209,6 +209,14 @@ int g4r_eval_counts(g4r_handle* h, int32_t* out, int64_t n_lanes);
  * the whole catalogue for subsequent g4r_eval_schedule calls (the target's own score competes only if the target is listed,
  * as in the reference); n = 0 restores the full-catalogue ranking.  G4R_ERR_INDEX on an out-of-range index. */
 int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n);
+/* evaluate_gpu(exclude_seen=True) (DESIGN §3g): on != 0 makes subsequent g4r_eval_schedule / g4r_eval_events calls rank each
+ * event without the items its session has input so far, the current input included (recommend_next_batch's exclude_seen rule);
+ * with g4r_set_eval_items every occurrence of such an item in the candidate list goes.  An event whose target is among them is a
+ * miss: rank +inf, nothing added to the sums, (-1, -1) in g4r_eval_events' out_counts; its lists hold only eligible items, the
+ * slots past them item -1 and score NaN.  The seen lists take eval batch size x (longest session of the schedule - 1) int32 on
+ * the device; a schedule for which that exceeds 256 MiB is refused with G4R_ERR_INVALID before any device work.  on = 0
+ * restores the plain ranking. */
+int g4r_set_eval_exclude_seen(g4r_handle* h, int32_t on);
 /* g4r_eval_schedule with per-event outputs (DESIGN §3f).  Events are numbered in the order the schedule consumes them: mini-batch
  * by mini-batch, lanes 0 .. M-1 of each (g4r_schedule_positions maps them to the test data).  recall_sum / mrr_sum / n_events
  * are bit for bit those of g4r_eval_schedule with the same arguments.  out_counts [n_events x 2]: (#items scoring above the

@@ -24,6 +24,7 @@ _OPTIONS = [
     (('-t', '--test'), dict(metavar='TEST_PATH', type=str, nargs='+', help='Test data set(s).')),
     (('-m', '--measure'), dict(metavar='AT', type=int, nargs='+', default=[20], help='Recommendation list length(s) for recall & MRR (default: 20).')),
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
+    (('--exclude_seen',), dict(action='store_true', help='Rank each test event without the items its session has already input, as recommend_next_batch(exclude_seen=True) serves (see evaluate_gpu).')),
     (('-ss', '--sample_store_size'), dict(metavar='SS', type=int, default=10000000, help='Size of the negative-sample buffer in ids (default: 10000000).')),
     (('--sample_store_on_cpu',), dict(action='store_true', help='Legacy: draw the negative samples on the host.')),
     (('-g', '--gru4rec_model'), dict(metavar='GRFILE', type=str, default='gru4rec', help='Module that provides the GRU4Rec class (default: gru4rec).')),
@@ -112,10 +113,12 @@ def _evaluate(gru, evaluation, args):
     for test_file in args.test:
         print('Loading test data...')
         frame = load_data(test_file, args)
-        print('Starting evaluation (cut-off={}, using {} mode for tiebreaking)'.format(args.measure, args.eval_type))
+        print('Starting evaluation (cut-off={}, using {} mode for tiebreaking{})'.format(args.measure, args.eval_type,
+                                                                                      ', seen items excluded' if args.exclude_seen else ''))
         started = time.time()
+        extra = dict(exclude_seen=True) if args.exclude_seen else {}
         result = evaluation.evaluate_gpu(gru, frame, batch_size=512, cut_off=args.measure, mode=args.eval_type,
-                                         item_key=args.item_key, session_key=args.session_key, time_key=args.time_key)
+                                         item_key=args.item_key, session_key=args.session_key, time_key=args.time_key, **extra)
         print('Evaluation took {:.2f}s'.format(time.time() - started))
         for position, cut in enumerate(args.measure):
             print('Recall@{}: {:.6f} MRR@{}: {:.6f}'.format(cut, result[0][position], cut, result[1][position]))

@@ -5,7 +5,10 @@ GRU(512)), 100 and 512 lanes.  Before timing, the loop's lists must equal eval_e
 the public functions: the pandas preparation of evaluate_gpu / evaluate_events, the events frame and recommend_next_batch's item
 id mapping are left out.
 
-  python scripts/eval_events_bench.py [--rounds R]
+  python scripts/eval_events_bench.py [--rounds R] [--exclude_seen]
+
+--exclude_seen: instead, the cost of exclude_seen (DESIGN §3g): eval_schedule against the same call with the seen lists, and
+eval_events with them at k = 0 and 20, timed in alternating rounds; the lists are checked to hold no seen item.
 
 Env: EE_EVENTS (test events per shape, default 100,000, at least twice the items), EE_SHAPES (e.g. 'rsc15,rees46'), EE_LANES (e.g. '100,512')."""
 import argparse, os, sys, time
@@ -24,6 +27,7 @@ SHAPES = {'rsc15': (37483, 100), 'rees46': (172000, 512)}
 
 ap = argparse.ArgumentParser()
 ap.add_argument('--rounds', type=int, default=3)
+ap.add_argument('--exclude_seen', action='store_true')
 a = ap.parse_args()
 print('card: %s | nvidia-smi name, power.limit, clocks.max.sm: %s' % card(), flush=True)
 n_ev = int(os.environ.get('EE_EVENTS', 100000))
@@ -37,6 +41,46 @@ def timed(f):
         f()
         torch.cuda.synchronize(); ts.append(time.time() - t0)
     return float(np.median(ts))
+
+
+def seen_calls(eng, on, f):
+    eng.set_eval_exclude_seen(on)
+    try:
+        return f()
+    finally:
+        eng.set_eval_exclude_seen(False)
+
+
+def seen_leg(eng, sched, e, shape, I, L, lanes):
+    """eval_schedule with and without exclude_seen, and eval_events with it, in alternating rounds (median of --rounds)"""
+    got = seen_calls(eng, True, lambda: eng.eval_events(sched, CUTS, 0, k=20))
+    cur, j = {}, 0                                             # no list holds an item its session has input so far
+    for s in range(sched.n_steps):
+        for b in range(int(e['M'][s])):
+            sl = int(e['slots'][s, b])
+            if e['F'][s, b] & 2 or sl not in cur:
+                cur[sl] = set()
+            cur[sl].add(int(e['X'][s, b]))
+            if cur[sl] & set(got[4][j].tolist()):
+                raise SystemExit('MISMATCH: a seen item in an exclude_seen list (%s, %d lanes)' % (shape, lanes))
+            j += 1
+    calls = {'eval_schedule': lambda: eng.eval_schedule(sched, CUTS, 0),
+             'eval_schedule exclude_seen': lambda: seen_calls(eng, True, lambda: eng.eval_schedule(sched, CUTS, 0)),
+             'eval_events k=0 exclude_seen': lambda: seen_calls(eng, True, lambda: eng.eval_events(sched, CUTS, 0, k=0)),
+             'eval_events k=20 exclude_seen': lambda: seen_calls(eng, True, lambda: eng.eval_events(sched, CUTS, 0, k=20))}
+    for f in calls.values():
+        f()
+    ts = {n: [] for n in calls}
+    for _ in range(a.rounds):
+        for n, f in calls.items():
+            torch.cuda.synchronize(); t0 = time.time()
+            f()
+            torch.cuda.synchronize(); ts[n].append(time.time() - t0)
+    base = float(np.median(ts['eval_schedule']))
+    for n, v in ts.items():
+        dt = float(np.median(v))
+        print('%-7s I=%d GRU(%d) lanes=%3d %-30s %8.3f s (min-max %.3f-%.3f)  %8.1f us / mini-batch  %+6.1f %%  (%d mini-batches, %d events)'
+              % (shape, I, L, lanes, n, dt, min(v), max(v), dt / sched.n_steps * 1e6, 100.0 * (dt / base - 1.0), sched.n_steps, sched.n_events), flush=True)
 
 
 def loop_topk(eng, sched, e, k):
@@ -62,6 +106,10 @@ for shape in os.environ.get('EE_SHAPES', 'rsc15,rees46').split(','):
         eng = make_engine(I, mk, lanes, w)
         sched = _lib.Schedule(items, offset, None, lanes, 0, mode=1)
         e = sched.export()
+        if a.exclude_seen:
+            seen_leg(eng, sched, e, shape, I, L, lanes)
+            eng.close()
+            continue
         ref = loop_topk(eng, sched, e, 20)
         got = eng.eval_events(sched, CUTS, 0, k=20)
         if not np.array_equal(ref, got[4]):
