@@ -39,7 +39,7 @@ EXPORTS = [
     'g4r_set_sampling_cdf', 'g4r_set_logq_support', 'g4r_generate_samples', 'g4r_generate_samples_from_uniform',
     'g4r_set_sample_store', 'g4r_get_sample_store', 'g4r_sample_store_rows', 'g4r_set_sample_pointer', 'g4r_get_sample_pointer',
     'g4r_mrg_uniform', 'g4r_searchsorted', 'g4r_gather_rows',
-    'g4r_schedule_build', 'g4r_schedule_free', 'g4r_schedule_steps', 'g4r_schedule_events', 'g4r_schedule_export', 'g4r_schedule_positions',
+    'g4r_schedule_build', 'g4r_schedule_build_history', 'g4r_schedule_free', 'g4r_schedule_steps', 'g4r_schedule_events', 'g4r_schedule_export', 'g4r_schedule_positions',
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
@@ -85,6 +85,7 @@ def load():
     lib.g4r_searchsorted.argtypes = [vp, vp, i64, vp, i64, vp]
     lib.g4r_gather_rows.argtypes = [vp, vp, i64, i64, vp, i64, vp]
     lib.g4r_schedule_build.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, C.POINTER(vp)]
+    lib.g4r_schedule_build_history.argtypes = [vp, i64, vp, i64, vp, vp, i32, i32, C.POINTER(vp)]
     lib.g4r_schedule_free.argtypes = [vp]
     lib.g4r_schedule_steps.argtypes = [vp]; lib.g4r_schedule_steps.restype = i64
     lib.g4r_schedule_events.argtypes = [vp]; lib.g4r_schedule_events.restype = i64
@@ -221,9 +222,11 @@ def make_config(n_items, mk, sample_store=0, eval_lanes=0, max_resident_steps=0,
 
 
 class Schedule(object):
-    """Host-side schedule of one epoch (gru4rec.py:594-651 / evaluation.py:90-139), built in C++."""
+    """Host-side schedule of one epoch (gru4rec.py:594-651 / evaluation.py:90-139), built in C++.  n_history (evaluation
+    schedules only): per session id, the number of its leading events that are history; only events whose target lies past
+    them are counted (n_events, flag bit 4 of export()['F'], the outputs of eval_schedule / eval_events)."""
 
-    def __init__(self, data_items, offset_sessions, session_order, batch_size, n_sample, mode=0):
+    def __init__(self, data_items, offset_sessions, session_order, batch_size, n_sample, mode=0, n_history=None):
         lib = load()
         self._lib = lib
         di = np.ascontiguousarray(data_items, dtype=np.int64)
@@ -234,13 +237,20 @@ class Schedule(object):
         n_sess = len(off) - 1 if order is None else len(order)
         if order is not None and len(order) and (order.min() < 0 or order.max() >= len(off) - 1):
             raise IndexError('session_order refers to a session that does not exist')
-        rc = lib.g4r_schedule_build(_ptr(di), len(di), _ptr(off), n_sess, _ptr(order), batch_size, n_sample, mode, C.byref(h))
+        if n_history is None:
+            rc = lib.g4r_schedule_build(_ptr(di), len(di), _ptr(off), n_sess, _ptr(order), batch_size, n_sample, mode, C.byref(h))
+        else:
+            nh = np.ascontiguousarray(n_history, dtype=np.int32)
+            if len(nh) != len(off) - 1 or n_sample != 0:
+                raise ValueError('n_history needs one entry per session and an evaluation schedule')
+            rc = lib.g4r_schedule_build_history(_ptr(di), len(di), _ptr(off), n_sess, _ptr(order), _ptr(nh), batch_size, mode, C.byref(h))
         if rc == G4R_ERR_INDEX:
             raise IndexError(lib.g4r_last_error(None).decode())
         if rc != 0:
             raise RuntimeError(lib.g4r_last_error(None).decode())
         self.h = h
         self.batch_size = batch_size
+        self.history = n_history is not None
         self.n_steps = lib.g4r_schedule_steps(h)
         self.n_events = lib.g4r_schedule_events(h)
 
@@ -259,6 +269,13 @@ class Schedule(object):
         if rc != 0:
             raise RuntimeError(self._lib.g4r_last_error(None).decode())
         return P
+
+    def counted(self):
+        """[n_steps, batch_size] bool: the lanes whose event is counted (every used lane unless built with n_history), in the
+        (step, lane) order eval_events numbers the events in."""
+        e = self.export()
+        used = np.arange(self.batch_size)[None, :] < e['M'][:, None]
+        return used & ((e['F'] & 4) != 0) if self.history else used
 
     def batch_sizes(self):
         """M of every mini-batch (the weights of the epoch loss, gru4rec.py:654) without copying the index arrays."""

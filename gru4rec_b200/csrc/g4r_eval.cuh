@@ -97,10 +97,11 @@ __device__ __forceinline__ void ev_tiles(const ModelDev& md, float* smem, int M,
 }
 
 // target score of every lane, computed with the same sequential k order as the tile kernel (bitwise equal); SEEN: also adds the
-// lane's input to its seen list (seen_insert) and flags the lanes whose target is in it (sd.miss)
-template <bool SEEN = false>
+// lane's input to its seen list (seen_insert) and flags the lanes whose target is in it (sd.miss).  KEY (ranking blocks of
+// g4r_history.cuh): row b's tiebreaking noise is keyed by the (step, lane) pair key[2b], key[2b + 1] it was enqueued from
+template <bool SEEN = false, bool KEY = false>
 __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, int* cnt, unsigned int tie, int subset_mode, int lohi_stride,
-                                                  SeenDev sd = SeenDev{}) {
+                                                  SeenDev sd = SeenDev{}, const int* __restrict__ key = nullptr) {
   const ModelDev& md = MD;
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int M = md.wM[s];
@@ -114,7 +115,10 @@ __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, i
     tc_thresholds(md.fact, md.fact.kind <= G4R_ACT_SELU, sc, pre, lo, hi);
     tgt[lohi_stride + b] = lo; tgt[2 * lohi_stride + b] = hi;
   }
-  if (tie) sc += tie_noise(tie, s, b, subset_mode ? 0x40000000U + (unsigned int)b : (unsigned int)item);
+  if (tie) {
+    const int ks = KEY ? key[2 * b] : s, kb = KEY ? key[2 * b + 1] : b;
+    sc += tie_noise(tie, ks, kb, subset_mode ? 0x40000000U + (unsigned int)kb : (unsigned int)item);
+  }
   tgt[b] = sc;
   cnt[b * 2 + 0] = 0; cnt[b * 2 + 1] = 0;
   if (SEEN) sd.miss[b] = seen_insert(md, sd, s, b, item) ? 1 : 0;
@@ -124,11 +128,11 @@ __global__ void __launch_bounds__(128) k_eval_tgt(int slot, int s, float* tgt, i
 // without a subset, n_cand > 0 scores the leading items 0 .. n_cand - 1 and 0 the catalogue.  WRITE: out[b * n_comp + pos] = score.
 // SEEN (counting only): an item on the lane's seen list is never compared -- a bit per held position, set from the list (a walk
 // of the list's items inside the tile for the catalogue, a binary search per position for a subset, whose every occurrence of a
-// seen item goes)
-template <bool WRITE, bool SEEN = false>
+// seen item goes).  KEY: tiebreaking noise keyed per row as in k_eval_tgt<SEEN, true>
+template <bool WRITE, bool SEEN = false, bool KEY = false>
 __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, const float* __restrict__ tgt, int* cnt, float* out,
                                                            const int* __restrict__ subset, int n_cand, unsigned int tie = 0u,
-                                                           SeenDev sd = SeenDev{}) {
+                                                           SeenDev sd = SeenDev{}, const int* __restrict__ key = nullptr) {
   const ModelDev& md = MD;
   extern __shared__ __align__(16) float smem[];
   int* sCnt = reinterpret_cast<int*>(smem + EV_TILE_FLOATS);   // [EV_TB][2]
@@ -158,6 +162,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
         }
       }
       float* orow = WRITE ? out + (size_t)b * I + i0 + warp : nullptr;   // one row pointer keeps the kernel free of spills
+      const int ks = (KEY && tie) ? key[2 * b] : s, kb = (KEY && tie) ? key[2 * b + 1] : b;
 #pragma unroll
       for (int q = 0; q < 8; q++) {
         const int it = i0 + warp + 8 * q;
@@ -166,7 +171,7 @@ __global__ void __launch_bounds__(EV_THREADS) k_eval_score(int slot, int s, cons
           if (WRITE) orow[8 * q] = sc;
           else {
             if (md.fact.kind <= G4R_ACT_SELU) sc = act_fwd(md.fact, sc);
-            if (tie) sc += tie_noise(tie, s, b, (unsigned int)it);
+            if (tie) sc += tie_noise(tie, ks, kb, (unsigned int)it);
             gt += sc > t; eq += sc == t;
           }
         }
@@ -263,6 +268,7 @@ struct EvalCtx {
   uint64_t split_version = ~0ull;
   void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
   void* events = nullptr;                                         // EventsCtx* of g4r_eval_events (g4r_events.cuh)
+  void* hist = nullptr;                                           // HistCtx* of history schedules (g4r_history.cuh)
   // exclude_seen (g4r_set_eval_exclude_seen, g4r_seen.cuh): per state slot the seen list, its length, the lanes' miss flags, and
   // the per-mini-batch CSR copy the top-k kernels of g4r_eval_events read as their exclusions
   bool seen_on = false;
@@ -272,6 +278,7 @@ struct EvalCtx {
 };
 static void topk_release(EvalCtx& e);
 static void events_release(EvalCtx& e);
+static void hist_release(EvalCtx& e);
 
 // device buffer of at least n elements (contents not kept)
 template <class T>
@@ -310,6 +317,7 @@ static void eval_release(g4r_handle* h) {
   EvalCtx& e = *static_cast<EvalCtx*>(h->eval_ctx);
   topk_release(e);
   events_release(e);
+  hist_release(e);
   cudaFreeHost(e.hX); cudaFreeHost(e.hY); cudaFreeHost(e.hSlot); cudaFreeHost(e.hF); cudaFreeHost(e.hM); cudaFreeHost(e.hSti); cudaFreeHost(e.hG);
   cudaFree(e.dX); cudaFree(e.dY); cudaFree(e.dSlot); cudaFree(e.dF); cudaFree(e.dM); cudaFree(e.dSti); cudaFree(e.dG);
   cudaFree(e.dCut); cudaFree(e.dSums); if (e.dOut) cudaFree(e.dOut); if (e.dCand) cudaFree(e.dCand);
@@ -340,6 +348,8 @@ static int eval_ctx(g4r_handle* h, EvalCtx** out) {
   cudaFuncSetAttribute(k_eval_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
   cudaFuncSetAttribute(k_eval_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
   cudaFuncSetAttribute(k_eval_score<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
+  cudaFuncSetAttribute(k_eval_score<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
+  cudaFuncSetAttribute(k_eval_score<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eval_smem_bytes());
   if (cudaFuncSetAttribute(k_eval_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
   if (cudaFuncSetAttribute(k_eval_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem)) != cudaSuccess) cudaGetLastError();
   h->eval_ctx = new EvalCtx(e);
@@ -370,6 +380,13 @@ static void events_window(EventsRun* ev, int64_t done);
 static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
 static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
 static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t rk);
+static void events_block(EventsRun* ev, int slot, int M, const int* miss, const int64_t* step, const int* lane);
+
+// history schedules (g4r_history.cuh): only the lanes flagged 4 are ranked, in blocks
+struct HistCtx;
+static int hist_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, const SeenDev* sd, HistCtx** out);
+static int hist_run(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const SeenDev* sd, unsigned int tie,
+                    bool tc_possible, int n_cut, int mode, EventsRun* ev);
 
 // exclude_seen: lists of capacity cap = the schedule's longest session - 1 for every scoring slot (eval_run empties them);
 // refused before any device work when B x cap x 4 bytes (B: the schedule's lanes) exceed SEEN_BYTES, the 256 MiB budget of g4r_eval_events' window
@@ -433,6 +450,11 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
     rc = tc_operands(h, e);
     if (rc) return rc;
   }
+  HistCtx* hc = nullptr;
+  if (s->hist) {
+    rc = hist_begin(h, e, s, seen ? &sd : nullptr, &hc);
+    if (rc) return rc;
+  }
   int64_t done = 0;
   while (done < s->n_steps) {
     const int64_t w = std::min<int64_t>(e->cap, s->n_steps - done);
@@ -465,7 +487,11 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
     // sums) is ordered by the ranking stream itself, so the sums accumulate in mini-batch order as before.
     cudaStream_t rk = h->side;
     if (ev) events_window(ev, done);
-    for (int64_t i = 0; i < w; i++) {
+    if (hc) {
+      rc = hist_run(h, e, hc, s, w, done, seen ? &sd : nullptr, tie, tc_possible, n_cut, mode, ev);
+      if (rc) return rc;
+    }
+    for (int64_t i = 0; i < (hc ? 0 : w); i++) {
       eval_forward(h, e, (int)i, h->He);
       CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
       if (seen) {       // inserts this mini-batch's inputs on the ranking stream: after i-1's ranking has read the lists, while
@@ -628,3 +654,4 @@ extern "C" int g4r_reset_eval_hidden(g4r_handle* h) {
 #include "g4r_topk.cuh"
 #include "g4r_sessions.cuh"
 #include "g4r_events.cuh"
+#include "g4r_history.cuh"

@@ -19,6 +19,9 @@
 // stages the schedule in windows of e->cap mini-batches exactly as g4r_eval_schedule does, so every kernel of the evaluation sees
 // the same step index (the tiebreaking noise hashes it), and the per-event buffers are flushed every w mini-batches within it and
 // at its end.
+// On a history schedule (g4r_history.cuh) the unit of this work is a ranking block instead of a mini-batch: events_block names
+// the block's descriptor, rows and miss flags, and the schedule step and lane of every row (an overflowed row's seen set is
+// rebuilt at that step).
 #pragma once
 
 constexpr size_t EVENTS_WINDOW_BYTES = (size_t)256 << 20;   // per-window buffers (y rows, counters, lists): shorter windows, not more
@@ -65,9 +68,16 @@ struct EventsRun {
   int64_t done = 0;                                       // schedule step of the staging window's first mini-batch
   bool seen = false;                                      // exclude_seen: the lists exclude ex_off / ex (k_seen_csr's output)
   const int* ex_off = nullptr; const int* ex = nullptr;
+  std::vector<int> m;                                     // rows of every unit of the window
+  // history schedules: the ranking block of the next events_stage / events_step (src_slot < 0: the staging step's mini-batch)
+  int src_slot = -1, src_M = 0; const int* src_miss = nullptr; const int64_t* src_step = nullptr; const int* src_lane = nullptr;
+  std::vector<int64_t> rstep; std::vector<int> rlane;     // [w x Be] schedule step and lane of every row of the window's blocks
 };
 static bool events_lists(const EventsRun* ev) { return ev->k > 0; }
 static void events_window(EventsRun* ev, int64_t done) { ev->done = done; }
+static void events_block(EventsRun* ev, int slot, int M, const int* miss, const int64_t* step, const int* lane) {
+  ev->src_slot = slot; ev->src_M = M; ev->src_miss = miss; ev->src_step = step; ev->src_lane = lane;
+}
 
 static void events_release(EvalCtx& e) {
   if (!e.events) return;
@@ -215,6 +225,8 @@ static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, Events
   if (x->max_window > 0) w = std::min<int64_t>(w, x->max_window);
   ev->w = (int)w;
   ev->off.assign((size_t)w, 0);
+  ev->m.assign((size_t)w, 0);
+  if (s->hist) { ev->rstep.assign((size_t)w * Be, 0); ev->rlane.assign((size_t)w * Be, 0); }
   CK(dev_grow(&x->dCnt, &x->cnt_cap, (size_t)w * Be * 2));
   if (k == 0) return G4R_OK;
   // the top-k constants of topk_rank (exclude_seen: with exclusions of at most cap items per lane); only the tile kind depends
@@ -250,21 +262,25 @@ static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, Events
   return G4R_OK;
 }
 
-// staging step i, right after its target scores: its events' place in the per-event window (mini-batch j of it), and its y rows
-// saved for the top-k
+// staging step i (a history schedule: ranking block i of the staging window), right after its target scores: its events' place in
+// the per-event window (unit j of it), and its y rows saved for the top-k
 static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk) {
   EventsCtx* x = ev->x;
   if (ev->n == 0) {
     ev->base = i; ev->win_ev = 0;
     if (ev->k > 0 && !ev->no_tile) CK(cudaMemsetAsync(x->dSurvN, 0, ev->survn.size() * sizeof(int), rk));
   }
-  const int j = i - ev->base;
+  const bool blk = ev->src_slot >= 0;
+  const int j = i - ev->base, M = blk ? ev->src_M : e->hM[i];
   ev->off[(size_t)j] = ev->win_ev;
-  ev->win_ev += e->hM[i];
+  ev->m[(size_t)j] = M;
+  ev->win_ev += M;
   ev->n = j + 1;
+  if (blk)
+    for (int b = 0; b < M; b++) { ev->rstep[(size_t)j * e->Be + b] = ev->src_step[b]; ev->rlane[(size_t)j * e->Be + b] = ev->src_lane[b]; }
   if (ev->k > 0) {
     const size_t rows = (size_t)e->Be * h->md.ldL;
-    k_ev_stage<<<std::min<int>((int)((rows / 4 + 255) / 256), 2 * h->n_sm), 256, 0, rk>>>(e->slot, i, x->dYk, x->dYw + (size_t)j * rows, x->dMk);
+    k_ev_stage<<<std::min<int>((int)((rows / 4 + 255) / 256), 2 * h->n_sm), 256, 0, rk>>>(blk ? ev->src_slot : e->slot, blk ? 0 : i, x->dYk, x->dYw + (size_t)j * rows, x->dMk);
     h->launches++;
   }
   return G4R_OK;
@@ -276,10 +292,12 @@ static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, i
 // window is flushed
 static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk) {
   EventsCtx* x = ev->x;
-  const int Be = e->Be, M = e->hM[i], k = ev->k, j = i - ev->base;
+  const bool blk = ev->src_slot >= 0;
+  const int Be = e->Be, j = i - ev->base, M = ev->m[(size_t)j], k = ev->k;
+  const int slot = blk ? ev->src_slot : e->slot, si = blk ? 0 : i;
   const int64_t o = ev->off[(size_t)j];
-  if (ev->seen) k_ev_counts<true><<<(2 * Be + 255) / 256, 256, 0, rk>>>(e->slot, i, h->dRankCnt, x->dCnt + 2 * o, e->dMiss);
-  else k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(e->slot, i, h->dRankCnt, x->dCnt + 2 * o);
+  if (ev->seen) k_ev_counts<true><<<(2 * Be + 255) / 256, 256, 0, rk>>>(slot, si, h->dRankCnt, x->dCnt + 2 * o, blk ? ev->src_miss : e->dMiss);
+  else k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(slot, si, h->dRankCnt, x->dCnt + 2 * o);
   h->launches++;
   if (k > 0) {
     int rc = events_topk(h, e, ev, M, j, o, rk);
@@ -343,7 +361,7 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
       CK(cudaStreamSynchronize(rk));
       std::vector<int> src, evw;
       for (int64_t i = 0; i < w; i++)
-        for (int b = 0; b < e->hM[ev->base + i]; b++)
+        for (int b = 0; b < ev->m[(size_t)i]; b++)
           if (ev->survn[(size_t)(i * Be + b)] > ev->C) { src.push_back((int)(i * Be + b)); evw.push_back((int)(ev->off[(size_t)i] + b)); }
       const int chunk = (int)std::min<int64_t>(Be, std::max<int64_t>(1, (int64_t)(EVENTS_ROWS_BYTES / ((size_t)I * sizeof(float)))));
       const bool filt = ev->f.use_cand, fx = filt || ev->seen;
@@ -362,7 +380,8 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
           std::vector<int> eo(1, 0), ex;
           for (int j = 0; j < n; j++) {
             const int r = src[j0 + (size_t)j];
-            seen_rebuild(ev->sched, ev->done + ev->base + r / Be, r % Be, ex);
+            if (ev->sched->hist) seen_rebuild(ev->sched, ev->rstep[(size_t)r], ev->rlane[(size_t)r], ex);
+            else seen_rebuild(ev->sched, ev->done + ev->base + r / Be, r % Be, ex);
             eo.push_back((int)ex.size());
           }
           CK(dev_grow(&x->dOvExOff, &x->ov_ex_off_cap, eo.size()));

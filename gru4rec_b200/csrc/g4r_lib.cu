@@ -41,6 +41,7 @@ struct g4r_schedule {
   std::vector<int64_t> P;       // recorded on request (mode | 2): index in data_items of every input X (target at P + 1), -1 on unused lanes
   bool has_pos = false;
   int64_t max_len = 1;          // events of the longest session walked (its inputs bound a lane's seen list, g4r_seen.cuh)
+  bool hist = false;            // g4r_schedule_build_history: only lanes flagged 4 are counted events (g4r_history.cuh)
 };
 
 struct g4r_handle {
@@ -1061,19 +1062,22 @@ extern "C" int g4r_gather_rows(g4r_handle* h, const float* table, int64_t rows, 
 // ------------------------------------------------------------------------------------------------
 // schedule builder (gru4rec.py:594-651; evaluation.py:90-139), host C++
 // ------------------------------------------------------------------------------------------------
-extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, const int32_t* offs, int64_t n_sessions,
-                                  const int64_t* order, int32_t B, int32_t n_sample, int32_t mode, g4r_schedule** out) {
+// n_hist (evaluation only, g4r_schedule_build_history): per session id, its leading events that are history -- a lane's target
+// is counted (flag bit 2) only past them, and n_events counts only those lanes
+static int schedule_build(const int64_t* data_items, int64_t n_events, const int32_t* offs, int64_t n_sessions,
+                          const int64_t* order, int32_t B, int32_t n_sample, int32_t mode, const int32_t* n_hist, g4r_schedule** out) {
   if (!data_items || !offs || !out || B <= 0 || n_sessions < 0) return G4R_ERR_INVALID;
   if (n_sessions < B) { g_create_error = "index out of bounds: fewer sessions than batch_size (reference: IndexError at gru4rec.py:596)"; return G4R_ERR_INDEX; }
   const bool want_pos = mode == (1 | G4R_SCHED_POSITIONS);   // evaluation schedule that also records input positions
   if (want_pos) mode = 1;
   g4r_schedule* s = new g4r_schedule();
-  s->B = B; s->mode = mode; s->has_pos = want_pos;
+  s->B = B; s->mode = mode; s->has_pos = want_pos; s->hist = n_hist != nullptr;
   auto sess_of = [&](int64_t it) -> int64_t { return order ? order[it] : it; };
-  std::vector<int64_t> iters(B), start(B), end(B);
+  std::vector<int64_t> iters(B), start(B), end(B), hend(B);   // hend: first counted target position of the lane's session
   std::vector<int32_t> slots(B);
   std::vector<uint8_t> zero_next(B, 0), fin(B), valid(B);
-  for (int b = 0; b < B; b++) { iters[b] = b; start[b] = offs[sess_of(b)]; end[b] = offs[sess_of(b) + 1]; slots[b] = b; }
+  auto hist_end = [&](int64_t ss) -> int64_t { return n_hist ? (int64_t)offs[ss] + n_hist[ss] : 0; };
+  for (int b = 0; b < B; b++) { iters[b] = b; start[b] = offs[sess_of(b)]; end[b] = offs[sess_of(b) + 1]; slots[b] = b; hend[b] = hist_end(sess_of(b)); }
   {
     // capacity up front.  While sessions are left every step runs all B lanes and consumes B (input, target) pairs; once the
     // supply is exhausted the remaining lanes finish their sessions within max_len steps.  A session of length l holds l - 1
@@ -1121,7 +1125,12 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
         for (int b = 0; b < M; b++) if (zero_next[b]) { F[b] = 2; zero_next[b] = 0; }
       }
       s->M.insert(s->M.end(), (size_t)nst, M);
-      s->n_events += nst * M;
+      if (n_hist) {          // bit 2: the lane's target (position start + i + 1) is past its session's history
+        for (int64_t i = 0; i < nst; i++)
+          for (int b = 0; b < M; b++) if (start[b] + i + 1 >= hend[b]) { F[i * B + b] |= 4; s->n_events++; }
+      } else {
+        s->n_events += nst * M;
+      }
     }
     int n_finished = 0;
     for (int b = 0; b < M; b++) { start[b] += minlen - 1; fin[b] = (end[b] - start[b] <= 1); }
@@ -1132,13 +1141,13 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
     if (n_valid == 0 || (mode == 0 && n_valid < 2 && n_sample == 0)) break;
     for (int b = 0; b < M; b++) if (fin[b] && valid[b]) {
       const int64_t ss = sess_of(iters[b]);
-      start[b] = offs[ss]; end[b] = offs[ss + 1];
+      start[b] = offs[ss]; end[b] = offs[ss + 1]; hend[b] = hist_end(ss);
       if (mode == 1) zero_next[b] = 1;
     }
     if (n_valid < M) {
       int w = 0;
       for (int b = 0; b < M; b++) if (valid[b]) {
-        iters[w] = iters[b]; start[w] = start[b]; end[w] = end[b]; slots[w] = slots[b]; zero_next[w] = zero_next[b]; w++;
+        iters[w] = iters[b]; start[w] = start[b]; end[w] = end[b]; slots[w] = slots[b]; zero_next[w] = zero_next[b]; hend[w] = hend[b]; w++;
       }
       M = w;
     }
@@ -1146,6 +1155,28 @@ extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, c
   s->n_steps = (int64_t)s->M.size();
   *out = s;
   return G4R_OK;
+}
+extern "C" int g4r_schedule_build(const int64_t* data_items, int64_t n_events, const int32_t* offs, int64_t n_sessions,
+                                  const int64_t* order, int32_t B, int32_t n_sample, int32_t mode, g4r_schedule** out) {
+  return schedule_build(data_items, n_events, offs, n_sessions, order, B, n_sample, mode, nullptr, out);
+}
+extern "C" int g4r_schedule_build_history(const int64_t* data_items, int64_t n_events, const int32_t* offs, int64_t n_sessions,
+                                          const int64_t* order, const int32_t* n_history, int32_t B, int32_t mode, g4r_schedule** out) {
+  if (!n_history) { g_create_error = "g4r_schedule_build_history: n_history is NULL"; return G4R_ERR_INVALID; }
+  if (mode != 1 && mode != (1 | G4R_SCHED_POSITIONS)) {
+    g_create_error = "g4r_schedule_build_history: mode must be 1 or 1 | G4R_SCHED_POSITIONS (an evaluation schedule)";
+    return G4R_ERR_INVALID;
+  }
+  if (offs && n_sessions > 0) {
+    for (int64_t i = 0; i < n_sessions; i++) {
+      const int64_t ss = order ? order[i] : i;
+      if (n_history[ss] < 0 || n_history[ss] > offs[ss + 1] - offs[ss]) {
+        g_create_error = "g4r_schedule_build_history: n_history of a session is negative or longer than the session";
+        return G4R_ERR_INVALID;
+      }
+    }
+  }
+  return schedule_build(data_items, n_events, offs, n_sessions, order, B, 0, mode, n_history, out);
 }
 extern "C" int g4r_schedule_free(g4r_schedule* s) { delete s; return G4R_OK; }
 extern "C" int64_t g4r_schedule_steps(const g4r_schedule* s) { return s ? s->n_steps : 0; }

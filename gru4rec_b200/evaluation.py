@@ -19,6 +19,27 @@ def _prepare(gru, test_data, session_key, item_key, time_key):
     return test_data, test_data.ItemIdx.values, offset_sessions
 
 
+def _prepare_history(gru, test_data, history, session_key, item_key, time_key):
+    """the test data prepared by _prepare; with a history frame (prepared by the same rules, restricted to the test sessions),
+    each test session becomes its history rows followed by its test rows, whatever their times.  Returns (frame, item indices,
+    session offsets, n_history): n_history (per session, its leading history events) is None when no history row is left, and
+    the evaluation is then exactly the plain one"""
+    test_data, items, offs = _prepare(gru, test_data, session_key, item_key, time_key)
+    if history is None or len(history) == 0:
+        return test_data, items, offs, None
+    hist = _prepare(gru, history, session_key, item_key, time_key)[0]
+    hist = hist[hist[session_key].isin(pd.unique(test_data[session_key]))]
+    if len(hist) == 0:
+        return test_data, items, offs, None
+    sids = test_data[session_key].values[offs[:-1]]
+    n_hist = hist.groupby(session_key).size().reindex(sids, fill_value=0).values.astype(np.int32)
+    both = pd.concat([hist.assign(_g4r_part=0), test_data.assign(_g4r_part=1)], ignore_index=True)
+    both = both.sort_values([session_key, '_g4r_part'], kind='stable').drop(columns='_g4r_part')
+    offs = np.zeros(len(sids) + 1, dtype=np.int32)
+    offs[1:] = both.groupby(session_key).size().reindex(sids).values.cumsum()
+    return both, both.ItemIdx.values, offs, n_hist
+
+
 class _ExcludeSeen(object):
     """exclude_seen on the engine for the duration of one evaluation (reset whatever happens, like the candidate items).  The
     library refuses seen lists over its budget (lanes x (longest session - 1) int32); the same test on the whole test set is made
@@ -54,7 +75,7 @@ def _cuts(cut_off):
 
 
 def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard',
-                 exclude_seen=False):
+                 exclude_seen=False, history=None):
     '''
     Recall@N and MRR@N of next-item prediction, session-parallel (evaluation.py:15-147).
     Returns (recall_list, mrr_list), one entry per cut-off.  `mode` as in the reference; 'tiebreaking' adds U(0,1)*1e-10 to
@@ -68,13 +89,21 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     occurrence of such an item leaves the list); an event whose target is among them is a miss (rank inf: it adds nothing to
     Recall or MRR but still counts as an event).  The seen lists live on the device, (batch_size x longest session - 1) int32
     within 256 MiB: a longer longest session raises ValueError naming it (on every rank of a torch.distributed job).
+    `history` (an addition to the reference's signature): a DataFrame with the test data's key columns, each session's events
+    before its test events.  It is prepared like the test data (unknown items dropped, sorted by session, time and item) and
+    only its sessions that are also in the test data are used.  The evaluation is then that of the concatenated data (every
+    test session's history followed by its test events, whatever their times), counting only the events whose target is a test
+    event: a session with h >= 1 history events and t test events contributes t events, the first one with the last history
+    item as input and the state after the history before it; a session without history contributes t - 1 as before.  With
+    exclude_seen the history's items count as seen, and the seen-list budget applies to the longest concatenated session.
+    Only the counted events are ranked on the device.  history=None or an empty frame: exactly the evaluation without it.
     '''
     if gru.error_during_train: raise Exception
     if mode not in _MODES:
         raise NotImplementedError
     cuts = _cuts(cut_off)
     print('Measuring Recall@{} and MRR@{}'.format(','.join([str(c) for c in cuts]), ','.join([str(c) for c in cuts])))
-    test_data, test_data_items, offset_sessions = _prepare(gru, test_data, session_key, item_key, time_key)
+    test_data, test_data_items, offset_sessions, n_hist = _prepare_history(gru, test_data, history, session_key, item_key, time_key)
     n_sessions = len(offset_sessions) - 1
     world, rank = gru._world()
     if world > 1 and os.environ.get('G4R_EVAL_SHARD', '1') == '0':
@@ -88,7 +117,7 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     try:
         with _ExcludeSeen(eng, exclude_seen, test_data, session_key, offset_sessions, batch_size):
             if world == 1:
-                sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1)
+                sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1, n_history=n_hist)
                 rec, mrr, n = eng.eval_schedule(sched, cuts, _MODES[mode])
             else:
                 # one process per GPU: rank r scores every world-th session on its full replica of the model; the hit and
@@ -98,7 +127,7 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
                 mine = shard_eval_sessions(n_sessions, rank, world)
                 rec, mrr, n = np.zeros(len(cuts)), np.zeros(len(cuts)), 0
                 if len(mine):
-                    sched = _lib.Schedule(test_data_items, offset_sessions, mine, min(batch_size, len(mine)), 0, mode=1)
+                    sched = _lib.Schedule(test_data_items, offset_sessions, mine, min(batch_size, len(mine)), 0, mode=1, n_history=n_hist)
                     rec, mrr, n = eng.eval_schedule(sched, cuts, _MODES[mode])
                 tot = allreduce_sum(np.concatenate([rec, mrr, [float(n)]]), dist)
                 rec, mrr, n = tot[:len(cuts)], tot[len(cuts):2 * len(cuts)], int(round(tot[-1]))
@@ -129,7 +158,7 @@ def _ranks(counts, mode):
 
 
 def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100, mode='standard', k=0,
-                    exclude_seen=False):
+                    exclude_seen=False, history=None):
     '''
     evaluate_gpu with per-event outputs, from one evaluation pass on the device.  The test data is prepared, batched and ranked
     exactly as evaluate_gpu does it (same arguments, modes and `items` semantics).  Returns a dict:
@@ -152,6 +181,10 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
     recommend_next_batch(..., exclude_seen=True) returns after that input; a list with fewer than k eligible items is padded
     with item None (the item array is then of object dtype) and score NaN, and 'coverage' ignores the padding.
 
+    `history` as in evaluate_gpu: 'events' has one row per counted event, in the order of the concatenated data (sessions
+    sorted, each session's history before its test events); the first row of a warm-started session has the session's last
+    history item as 'input_item'.
+
     Single process only: under a torch.distributed job it raises NotImplementedError.
     '''
     if gru.error_during_train: raise Exception
@@ -162,13 +195,13 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
     if gru._world()[0] > 1:
         raise NotImplementedError('evaluate_events runs in a single process (evaluate_gpu shards sessions over the ranks)')
     cuts = _cuts(cut_off)
-    test_data, test_data_items, offset_sessions = _prepare(gru, test_data, session_key, item_key, time_key)
+    test_data, test_data_items, offset_sessions, n_hist = _prepare_history(gru, test_data, history, session_key, item_key, time_key)
     eng = gru._ensure_engine(batch_size)
     if items is not None:
         eng.set_eval_items(gru.itemidmap[items].values)
     try:
         with _ExcludeSeen(eng, exclude_seen, test_data, session_key, offset_sessions, batch_size):
-            sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS)
+            sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS, n_history=n_hist)
             rec, mrr, n, counts, top_i, top_s = eng.eval_events(sched, cuts, _MODES[mode], k)
         pos = sched.positions()
     finally:
@@ -176,8 +209,11 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
             eng.set_eval_items(None)
     gru.predict = None                                     # the scoring hidden state is shared with predict_next_batch
     # events in schedule order -> rows of the sorted frame (the target's row), then frame order
-    M = sched.batch_sizes()
-    row = (pos[np.arange(pos.shape[1])[None, :] < M[:, None]] + 1).astype(np.int64)
+    if n_hist is None:
+        M = sched.batch_sizes()
+        row = (pos[np.arange(pos.shape[1])[None, :] < M[:, None]] + 1).astype(np.int64)
+    else:
+        row = (pos[sched.counted()] + 1).astype(np.int64)
     order = np.argsort(row, kind='stable')
     row = row[order]
     rank = _ranks(counts[order], mode)

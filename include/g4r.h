@@ -130,7 +130,7 @@ int g4r_schedule_build(const int64_t* data_items, int64_t n_events, const int32_
                        const int64_t* session_order, int32_t batch_size, int32_t n_sample, int32_t mode, g4r_schedule** out);
 int g4r_schedule_free(g4r_schedule* s);
 int64_t g4r_schedule_steps(const g4r_schedule* s);
-int64_t g4r_schedule_events(const g4r_schedule* s);       /* sum of batch sizes */
+int64_t g4r_schedule_events(const g4r_schedule* s);       /* sum of batch sizes (history schedules: counted events) */
 /* Copies out step arrays (each step padded to batch_size entries; unused lanes = -1 / 0). Any pointer may be NULL. */
 int g4r_schedule_export(const g4r_schedule* s, int32_t* X, int32_t* Y, uint8_t* flags, int32_t* M, int32_t* slots);
 /* Evaluation schedules built with mode 1 | G4R_SCHED_POSITIONS: pos[step * batch_size + b] = index in data_items of the input X
@@ -138,6 +138,15 @@ int g4r_schedule_export(const g4r_schedule* s, int32_t* X, int32_t* Y, uint8_t* 
  * G4R_ERR_STATE for a schedule built without the flag (other schedules do not spend the memory). */
 #define G4R_SCHED_POSITIONS 2
 int g4r_schedule_positions(const g4r_schedule* s, int64_t* pos);
+/* Evaluation from each session's history (DESIGN §3h): the evaluation schedule (mode 1 or 1 | G4R_SCHED_POSITIONS) of the
+ * sessions as g4r_schedule_build walks them, where session id j's first n_history[j] events are history (0 <= n_history[j] <=
+ * its length).  A lane's event is counted only if its target is past the history: flag bit 2 (value 4) in g4r_schedule_export,
+ * and g4r_schedule_events returns the number of counted events.  g4r_eval_schedule / g4r_eval_events on such a schedule run the
+ * forward over every event but rank only the counted ones: their sums, counts and lists are those of the same call on the plain
+ * schedule of the same data restricted to the counted events, which g4r_eval_events numbers in (step, lane) order -- mini-batch
+ * by mini-batch, the counted lanes of each in lane order.  G4R_ERR_INVALID on a bad mode or n_history entry. */
+int g4r_schedule_build_history(const int64_t* data_items, int64_t n_events, const int32_t* offset_sessions, int64_t n_sessions,
+                               const int64_t* session_order, const int32_t* n_history, int32_t batch_size, int32_t mode, g4r_schedule** out);
 
 /* ---- the compiled step: train_function(X, Y, M, R) -> cost (gru4rec.py:584,623) ------------------- */
 /* One mini-batch from host arrays; returns the cost (D2H) like the reference call. */

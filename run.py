@@ -25,6 +25,7 @@ _OPTIONS = [
     (('-m', '--measure'), dict(metavar='AT', type=int, nargs='+', default=[20], help='Recommendation list length(s) for recall & MRR (default: 20).')),
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
     (('--exclude_seen',), dict(action='store_true', help='Rank each test event without the items its session has already input, as recommend_next_batch(exclude_seen=True) serves (see evaluate_gpu).')),
+    (('--history',), dict(metavar='HISTORY_PATH', type=str, help='Events before the test events of each test session, loaded like -t files: every test file is evaluated from its sessions\' history (see evaluate_gpu).')),
     (('-ss', '--sample_store_size'), dict(metavar='SS', type=int, default=10000000, help='Size of the negative-sample buffer in ids (default: 10000000).')),
     (('--sample_store_on_cpu',), dict(action='store_true', help='Legacy: draw the negative samples on the host.')),
     (('-g', '--gru4rec_model'), dict(metavar='GRFILE', type=str, default='gru4rec', help='Module that provides the GRU4Rec class (default: gru4rec).')),
@@ -110,6 +111,10 @@ def _train(model_class, args):
 
 def _evaluate(gru, evaluation, args):
     primary = ('recall', 'mrr').index(args.primary_metric.lower())
+    history = None
+    if args.history:
+        print('Loading history data...')
+        history = load_data(args.history, args)
     for test_file in args.test:
         print('Loading test data...')
         frame = load_data(test_file, args)
@@ -117,6 +122,8 @@ def _evaluate(gru, evaluation, args):
                                                                                       ', seen items excluded' if args.exclude_seen else ''))
         started = time.time()
         extra = dict(exclude_seen=True) if args.exclude_seen else {}
+        if history is not None:
+            extra['history'] = history
         result = evaluation.evaluate_gpu(gru, frame, batch_size=512, cut_off=args.measure, mode=args.eval_type,
                                          item_key=args.item_key, session_key=args.session_key, time_key=args.time_key, **extra)
         print('Evaluation took {:.2f}s'.format(time.time() - started))
