@@ -372,21 +372,113 @@ static int eval_forward(g4r_handle* h, EvalCtx* e, int s, float* const* Hst) {
   return G4R_OK;
 }
 
+// the staged window (w steps of e->hX .. hG, strided by the engine's scoring lanes) to the device, on the forward stream
+static int eval_upload(g4r_handle* h, EvalCtx* e, int64_t w) {
+  cudaStream_t st = h->stream;
+  const size_t nb = (size_t)w * e->Be;
+  CK(cudaMemcpyAsync(e->dX, e->hX, nb * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dY, e->hY, nb * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dSlot, e->hSlot, nb * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dF, e->hF, nb, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dM, e->hM, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dSti, e->hSti, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->dG, e->hG, (size_t)w * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  return G4R_OK;
+}
+
+// What one ranking (eval_rank) ranks: the M rows of scoring descriptor `slot` at its step s -- a mini-batch of the staging window,
+// or a ranking block of a history schedule (g4r_history.cuh)
+struct RankUnit {
+  int slot = -1, s = 0, M = 0;
+  const float* y = nullptr;             // the rows' final-layer y, as the wgmma split reads them
+  const int* key = nullptr;             // per-row tiebreaking keys, (step, lane) pairs (nullptr: keyed by (s, row))
+  SeenDev sd;                           // exclude_seen: the lists ranked against and the rows' miss flags (list == nullptr: off)
+  bool insert = false;                  // k_eval_tgt adds each row's input to sd (a mini-batch) or only reads it (a block's snapshot)
+  int64_t step = 0;                     // schedule step of every row (steps == nullptr; row b is lane b) ...
+  const int64_t* steps = nullptr; const int* lanes = nullptr;   // ... or of each row, and its lane (host arrays)
+};
+
+// the constants of one eval_run call, shared by every unit it ranks
+struct RankConsts {
+  unsigned int tie = 0u;
+  bool tc_possible = false;             // the wgmma tiles are ready; a unit takes them if wgmma_tiles holds for its rows
+  int n_cut = 0, mode = 0;
+  bool seen = false; SeenDev sd;        // exclude_seen: the live lists of the scoring slots
+};
+
 // g4r_eval_events' per-event outputs (g4r_events.cuh); nullptr on g4r_eval_schedule's path
 struct EventsRun;
 static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev, const SeenDev* sd);
 static bool events_lists(const EventsRun* ev);      // k > 0
-static void events_window(EventsRun* ev, int64_t done);
-static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
-static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk);
+static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, const RankUnit& u, cudaStream_t rk);
+static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, const RankUnit& u, cudaStream_t rk);
 static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t rk);
-static void events_block(EventsRun* ev, int slot, int M, const int* miss, const int64_t* step, const int* lane);
 
 // history schedules (g4r_history.cuh): only the lanes flagged 4 are ranked, in blocks
 struct HistCtx;
 static int hist_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, const SeenDev* sd, HistCtx** out);
-static int hist_run(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const SeenDev* sd, unsigned int tie,
-                    bool tc_possible, int n_cut, int mode, EventsRun* ev);
+static int hist_window(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const RankConsts& cs, EventsRun* ev);
+
+// One ranking of unit u on the ranking stream rk: the target scores (with exclude_seen, a mini-batch's seen insert, and the CSR
+// exclusions of g4r_eval_events' lists), the fp32 or wgmma tiles, the per-cutoff sums, then g4r_eval_events' per-event work
+// (ev != nullptr).  released (nullptr: none) is recorded once the rows' y has been read, and the forward stream waits on it.
+// Everything the ranking kernels share (target scores, counters, operand blocks, metric sums) is ordered by rk itself, so the
+// sums accumulate in unit order.
+static int eval_rank(g4r_handle* h, EvalCtx* e, const RankUnit& u, const RankConsts& cs, EventsRun* ev, cudaStream_t rk, cudaEvent_t released) {
+  const int Be = e->Be, I = h->md.n_items, M = u.M;
+  const bool seen = u.sd.list != nullptr;
+  const int subset_mode = e->n_cand > 0 ? 1 : 0, lohi = cs.tc_possible ? Be : 0;
+  if (seen && u.insert) k_eval_tgt<true><<<(Be + 31) / 32, 32, 0, rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, cs.tie, subset_mode, lohi, u.sd);
+  else if (u.key) k_eval_tgt<false, true><<<(Be + 31) / 32, 32, 0, rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, cs.tie, subset_mode, lohi, SeenDev{}, u.key);
+  else k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, cs.tie, subset_mode, lohi);
+  h->launches++;
+  if (ev) {
+    if (seen && events_lists(ev)) {
+      k_seen_csr<<<1, SEEN_CSR_THREADS, 0, rk>>>(u.slot, u.s, u.sd, e->dSeenOff, e->dSeenEx);
+      h->launches++;
+    }
+    int rc = events_stage(h, e, ev, u, rk);     // saves the rows' y before the forward may move on
+    if (rc) return rc;
+  }
+  if (cs.tc_possible && wgmma_tiles(h->cfg, M, I, I)) {
+    const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;   // + the bias column
+    k_tc_split<TC_M><<<dim3((M + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(u.y, M, h->md.ldL, h->md.L, e->dAsplit, tc_chunks, nullptr, 1.0f);
+    if (released) CK(cudaEventRecord(released, rk));
+    (seen ? k_eval_tc<true> : k_eval_tc<false>)<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(u.slot, u.s, h->dTgt, Be, h->dRankCnt,
+                                                                                                                 e->dAsplit, e->dBsplit, u.sd);
+    h->launches += 2;
+  } else {
+    const int n_comp = e->n_cand > 0 ? e->n_cand : I;
+    auto kern = u.key ? (seen ? k_eval_score<false, true, true> : k_eval_score<false, false, true>) : (seen ? k_eval_score<false, true> : k_eval_score<false>);
+    kern<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr,
+                                                                              e->n_cand, cs.tie, u.sd, u.key);
+    if (released) CK(cudaEventRecord(released, rk));
+    h->launches++;
+  }
+  if (released) CK(cudaStreamWaitEvent(h->stream, released, 0));
+  (seen ? k_eval_rank<true> : k_eval_rank<false>)<<<1, 256, 0, rk>>>(u.slot, u.s, h->dRankCnt, e->dCut, cs.n_cut, cs.mode, e->dSums, u.sd.miss);
+  h->launches++;
+  return ev ? events_step(h, e, ev, u, rk) : G4R_OK;
+}
+
+// the w staged mini-batches of a plain schedule (first schedule step `done`).  Two streams: the GRU forward of mini-batch i+1
+// (forward stream) overlaps the ranking of mini-batch i (ranking stream), which reads the hidden output only in its first kernels
+// (target scores, operand split -- or the fp32 tile kernel itself), after which the forward stream may overwrite it
+static int eval_window(g4r_handle* h, EvalCtx* e, int64_t w, int64_t done, const RankConsts& cs, EventsRun* ev) {
+  cudaStream_t st = h->stream, rk = h->side;
+  for (int64_t i = 0; i < w; i++) {
+    eval_forward(h, e, (int)i, h->He);
+    CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
+    RankUnit u;
+    u.slot = e->slot; u.s = (int)i; u.M = e->hM[i]; u.y = h->md.layer[h->md.n_layers - 1].y;
+    u.sd = cs.sd; u.insert = true;     // inserts this mini-batch's inputs on the ranking stream: after i-1's ranking has read the
+                                       // lists, while i+1's forward runs
+    u.step = done + i;
+    int rc = eval_rank(h, e, u, cs, ev, rk, h->ts_ev[1]);
+    if (rc) return rc;
+  }
+  return G4R_OK;
+}
 
 // exclude_seen: lists of capacity cap = the schedule's longest session - 1 for every scoring slot (eval_run empties them);
 // refused before any device work when B x cap x 4 bytes (B: the schedule's lanes) exceed SEEN_BYTES, the 256 MiB budget of g4r_eval_events' window
@@ -420,20 +512,20 @@ static int seen_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, bool csr
 static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
                     double* recall_sum, double* mrr_sum, int64_t* n_events, EventsRun* ev) {
   if (mode < 0 || mode > 3) FAIL(G4R_ERR_INVALID, "eval mode must be 0 (standard), 1 (conservative), 2 (median) or 3 (tiebreaking)");
-  const unsigned int tie = mode == 3 ? 0x5bd1e995u : 0u;
   cudaSetDevice(h->cfg.device);
   EvalCtx* e = nullptr;
   int rc = eval_ctx(h, &e);
   if (rc) return rc;
   if (s->B > e->Be) FAIL(G4R_ERR_INVALID, "schedule batch size exceeds eval_batch_size");
-  const bool seen = e->seen_on;
-  SeenDev sd;
-  if (seen) {
-    rc = seen_begin(h, e, s, ev && events_lists(ev), &sd);
+  RankConsts cs;
+  cs.tie = mode == 3 ? 0x5bd1e995u : 0u; cs.n_cut = n_cut; cs.mode = mode; cs.seen = e->seen_on;
+  const SeenDev* sd = cs.seen ? &cs.sd : nullptr;
+  if (sd) {
+    rc = seen_begin(h, e, s, ev && events_lists(ev), &cs.sd);
     if (rc) return rc;
   }
   if (ev) {
-    rc = events_begin(h, e, s, ev, seen ? &sd : nullptr);
+    rc = events_begin(h, e, s, ev, sd);
     if (rc) return rc;
   }
   const int Be = e->Be, Bs = s->B, I = h->md.n_items;
@@ -441,18 +533,17 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
   for (int i = 0; i < h->md.n_layers; i++) CK(cudaMemsetAsync(h->He[i], 0, (size_t)Be * h->md.layer[i].ldL * sizeof(float), st));   // gru4rec.py:731-733
   CK(cudaMemcpyAsync(e->dCut, cut_off, n_cut * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(e->dSums, 0, 128 * sizeof(double), st));
-  if (seen) CK(cudaMemsetAsync(sd.n, 0, (size_t)Be * sizeof(int), st));   // every lane starts a session with the schedule
+  if (sd) CK(cudaMemsetAsync(sd->n, 0, (size_t)Be * sizeof(int), st));   // every lane starts a session with the schedule
   // wgmma tiles (full-catalogue ranking of a wide batch; candidate subsets and tiebreaking take the fp32 tiles): decided once
-  // with the schedule's batch, then per mini-batch with its lanes
-  const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;   // + the bias column
-  const bool tc_possible = e->n_cand == 0 && mode != 3 && wgmma_tiles(h->cfg, Bs, I, I);
-  if (tc_possible) {
+  // with the schedule's batch, then per unit with its rows
+  cs.tc_possible = e->n_cand == 0 && mode != 3 && wgmma_tiles(h->cfg, Bs, I, I);
+  if (cs.tc_possible) {
     rc = tc_operands(h, e);
     if (rc) return rc;
   }
   HistCtx* hc = nullptr;
   if (s->hist) {
-    rc = hist_begin(h, e, s, seen ? &sd : nullptr, &hc);
+    rc = hist_begin(h, e, s, sd, &hc);
     if (rc) return rc;
   }
   int64_t done = 0;
@@ -474,68 +565,15 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
         if (x < 0 || x >= I || y < 0 || y >= I) FAIL(G4R_ERR_INDEX, "Index out of bounds");
       }
     }
-    CK(cudaMemcpyAsync(e->dX, e->hX, (size_t)w * Be * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dY, e->hY, (size_t)w * Be * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dSlot, e->hSlot, (size_t)w * Be * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dF, e->hF, (size_t)w * Be, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dM, e->hM, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dSti, e->hSti, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->dG, e->hG, (size_t)w * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    // two streams: the GRU forward of mini-batch i+1 (st) overlaps the ranking of mini-batch i (rk).  The ranking reads the
-    // hidden output only in its first kernels (target scores, operand split -- or the fp32 tile kernel itself), after which the
-    // forward stream may overwrite it; everything the ranking kernels share (target scores, counters, operand blocks, metric
-    // sums) is ordered by the ranking stream itself, so the sums accumulate in mini-batch order as before.
-    cudaStream_t rk = h->side;
-    if (ev) events_window(ev, done);
-    if (hc) {
-      rc = hist_run(h, e, hc, s, w, done, seen ? &sd : nullptr, tie, tc_possible, n_cut, mode, ev);
-      if (rc) return rc;
-    }
-    for (int64_t i = 0; i < (hc ? 0 : w); i++) {
-      eval_forward(h, e, (int)i, h->He);
-      CK(cudaEventRecord(h->ts_ev[0], st)); CK(cudaStreamWaitEvent(rk, h->ts_ev[0], 0));
-      if (seen) {       // inserts this mini-batch's inputs on the ranking stream: after i-1's ranking has read the lists, while
-                        // i+1's forward runs
-        k_eval_tgt<true><<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0, sd);
-        if (ev && events_lists(ev)) {
-          k_seen_csr<<<1, SEEN_CSR_THREADS, 0, rk>>>(e->slot, (int)i, sd, e->dSeenOff, e->dSeenEx);
-          h->launches++;
-        }
-      } else {
-        k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, tie, e->n_cand > 0 ? 1 : 0, tc_possible ? Be : 0);
-      }
-      if (ev) {
-        rc = events_stage(h, e, ev, (int)i, rk);     // saves this mini-batch's y before the forward may move on
-        if (rc) return rc;
-      }
-      const int n_comp = e->n_cand > 0 ? e->n_cand : I;
-      const int M_i = e->hM[i];
-      const bool tc = tc_possible && wgmma_tiles(h->cfg, M_i, I, I);
-      if (tc) {
-        k_tc_split<TC_M><<<dim3((M_i + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(h->md.layer[h->md.n_layers - 1].y, M_i, h->md.ldL, h->md.L, e->dAsplit, tc_chunks, nullptr, 1.0f);
-        CK(cudaEventRecord(h->ts_ev[1], rk));
-        if (seen) k_eval_tc<true><<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(e->slot, (int)i, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit, sd);
-        else k_eval_tc<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(e->slot, (int)i, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit);
-        h->launches++;
-      } else {
-        if (seen) k_eval_score<false, true><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, tie, sd);
-        else k_eval_score<false><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(e->slot, (int)i, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, tie);
-        CK(cudaEventRecord(h->ts_ev[1], rk));
-      }
-      CK(cudaStreamWaitEvent(st, h->ts_ev[1], 0));        // the hidden output of this mini-batch has been consumed
-      if (seen) k_eval_rank<true><<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums, sd.miss);
-      else k_eval_rank<<<1, 256, 0, rk>>>(e->slot, (int)i, h->dRankCnt, e->dCut, n_cut, mode, e->dSums);
-      h->launches += 3;
-      if (ev) {
-        rc = events_step(h, e, ev, (int)i, rk);
-        if (rc) return rc;
-      }
-    }
+    rc = eval_upload(h, e, w);
+    if (rc) return rc;
+    rc = hc ? hist_window(h, e, hc, s, w, done, cs, ev) : eval_window(h, e, w, done, cs, ev);
+    if (rc) return rc;
     if (ev) {
-      rc = events_flush(h, e, ev, rk);         // the rest of the per-event window before the staging is reused
+      rc = events_flush(h, e, ev, h->side);    // the rest of the per-event window before the staging is reused
       if (rc) return rc;
     }
-    CK(cudaEventRecord(h->ts_ev[2], rk)); CK(cudaStreamWaitEvent(st, h->ts_ev[2], 0));   // window complete before its staging is reused
+    CK(cudaEventRecord(h->ts_ev[2], h->side)); CK(cudaStreamWaitEvent(st, h->ts_ev[2], 0));   // window complete before its staging is reused
     CK(cudaGetLastError());
     done += w;
   }
@@ -603,21 +641,13 @@ extern "C" int g4r_set_eval_items(g4r_handle* h, const int64_t* items, int64_t n
 static int predict_stage(g4r_handle* h, EvalCtx* e, const int32_t* X, int32_t batch, const uint8_t* reset_mask) {
   const int Be = e->Be, I = h->md.n_items;
   if (batch <= 0 || batch > Be) FAIL(G4R_ERR_INVALID, "predict batch exceeds eval_batch_size");
-  cudaStream_t st = h->stream;
   for (int b = 0; b < Be; b++) {
     e->hX[b] = b < batch ? X[b] : -1; e->hY[b] = 0; e->hSlot[b] = b;
     e->hF[b] = (b < batch && reset_mask && reset_mask[b]) ? 2 : 0;
     if (b < batch && (X[b] < 0 || X[b] >= I)) FAIL(G4R_ERR_INDEX, "Index out of bounds");
   }
   e->hM[0] = batch; e->hSti[0] = -1; e->hG[0] = 0;
-  CK(cudaMemcpyAsync(e->dX, e->hX, (size_t)Be * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dY, e->hY, (size_t)Be * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dSlot, e->hSlot, (size_t)Be * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dF, e->hF, (size_t)Be, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dM, e->hM, sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dSti, e->hSti, sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dG, e->hG, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  return G4R_OK;
+  return eval_upload(h, e, 1);
 }
 
 extern "C" int g4r_predict(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, float* out) {

@@ -2,26 +2,24 @@
 // (#greater, #equal) counts of every event and optionally its top-k list.  Included at the end of g4r_eval.cuh (uses eval_run,
 // the top-k context and kernels of g4r_topk.cuh).
 //
-// Everything runs on the ranking stream of eval_run, after the kernels g4r_eval_schedule launches for the same mini-batch, so
-// the Recall / MRR sums are those of g4r_eval_schedule and the forward of mini-batch i+1 still overlaps the ranking of i:
-//   stage   right after the target scores: the last layer's y rows of mini-batch i are copied to the top-k descriptor's own
-//           buffer (read by the unchanged top-k kernels through a descriptor slot of their own) and to the window's y buffer
-//   counts  after k_eval_rank: the lanes' counts into the window's per-event buffer
-//   top-k   topk_rank's pipeline (prefix + tau, fp32 or wgmma filter tiles, select) with the window's survivor counters; the
-//           lists go straight into the window's per-event lists.  A lane whose survivors overflowed keeps its softmax
-//           normaliser and is redone at the end of the window
+// The unit of this work is the RankUnit that eval_rank ranks: a mini-batch, or a ranking block of a history schedule
+// (g4r_history.cuh).  Everything runs on the ranking stream inside eval_rank, around the kernels g4r_eval_schedule launches for
+// the same unit, so the Recall / MRR sums are those of g4r_eval_schedule and the forward of mini-batch i+1 still overlaps the
+// ranking of i:
+//   stage   right after the target scores: the unit's y rows are copied to the top-k descriptor's own buffer (read by the
+//           unchanged top-k kernels through a descriptor slot of their own) and to the window's y buffer
+//   counts  after k_eval_rank: the rows' counts into the window's per-event buffer
+//   top-k   topk_rank's pipeline (topk_tiles, topk_select) with the window's survivor counters; the lists go straight into the
+//           window's per-event lists.  A lane whose survivors overflowed keeps its softmax normaliser and is redone at the end
+//           of the window
 //   flush   one read of the window's survivor counters; every overflowed lane is rescored over the whole catalogue in fp32 from
 //           the saved y (k_topk_rows / k_topk_final, in chunks of rows), then the window's outputs go to the host
-// exclude_seen (g4r_seen.cuh): the lanes' seen lists, gathered per mini-batch into the CSR exclusions the top-k kernels read
-// (k_seen_csr), with a prefix of at least k + cap items; an overflowed lane's seen set at its own mini-batch (the lists have moved
-// on by the flush) is rebuilt from the schedule on the host
-// The per-event window (w mini-batches, bounded by the size of its buffers) is separate from eval_run's staging window: eval_run
-// stages the schedule in windows of e->cap mini-batches exactly as g4r_eval_schedule does, so every kernel of the evaluation sees
-// the same step index (the tiebreaking noise hashes it), and the per-event buffers are flushed every w mini-batches within it and
-// at its end.
-// On a history schedule (g4r_history.cuh) the unit of this work is a ranking block instead of a mini-batch: events_block names
-// the block's descriptor, rows and miss flags, and the schedule step and lane of every row (an overflowed row's seen set is
-// rebuilt at that step).
+// exclude_seen (g4r_seen.cuh): the unit's seen lists, gathered into the CSR exclusions the top-k kernels read (k_seen_csr), with a
+// prefix of at least k + cap items; an overflowed row's seen set at its own schedule step and lane, which the unit gives for
+// every row (the lists have moved on by the flush), is rebuilt from the schedule on the host
+// The per-event window (w units, bounded by the size of its buffers) is separate from eval_run's staging window: eval_run stages
+// the schedule in windows of e->cap mini-batches exactly as g4r_eval_schedule does, so every kernel of the evaluation sees the
+// same step index (the tiebreaking noise hashes it), and the per-event buffers are flushed every w units within it and at its end.
 #pragma once
 
 constexpr size_t EVENTS_WINDOW_BYTES = (size_t)256 << 20;   // per-window buffers (y rows, counters, lists): shorter windows, not more
@@ -53,31 +51,20 @@ struct EventsRun {
   int32_t k = 0;
   int32_t* out_counts = nullptr; int32_t* out_items = nullptr; float* out_scores = nullptr;   // host [n_events x 2] / [n_events x k]
   EventsCtx* x = nullptr;
-  TopkCtx* t = nullptr;
-  TopkFilter f;
-  int P = 0, C = 0, n_comp = 0;
-  bool no_tile = false;                                   // every candidate is in the prefix: no filter tiles, no overflow
-  int w = 0;                                              // mini-batches per per-event window
-  int base = 0;                                           // staging step of the window's first mini-batch
-  int n = 0;                                              // mini-batches in the window so far
+  TopkPlan plan;                                          // k > 0: the top-k constants, for units of up to the schedule's lanes
+  int w = 0;                                              // units per per-event window
+  int n = 0;                                              // units in the window so far
   int64_t ev_done = 0;                                    // events of the flushed windows
   int64_t win_ev = 0;                                     // events of the window so far
-  std::vector<int64_t> off;                               // window event of lane 0 of every mini-batch of the window
+  std::vector<int64_t> off;                               // window event of row 0 of every unit of the window
   std::vector<int> survn;                                 // host copy of dSurvN
   const g4r_schedule* sched = nullptr;
-  int64_t done = 0;                                       // schedule step of the staging window's first mini-batch
   bool seen = false;                                      // exclude_seen: the lists exclude ex_off / ex (k_seen_csr's output)
   const int* ex_off = nullptr; const int* ex = nullptr;
   std::vector<int> m;                                     // rows of every unit of the window
-  // history schedules: the ranking block of the next events_stage / events_step (src_slot < 0: the staging step's mini-batch)
-  int src_slot = -1, src_M = 0; const int* src_miss = nullptr; const int64_t* src_step = nullptr; const int* src_lane = nullptr;
-  std::vector<int64_t> rstep; std::vector<int> rlane;     // [w x Be] schedule step and lane of every row of the window's blocks
+  std::vector<int64_t> rstep; std::vector<int> rlane;     // exclude_seen lists: [w x Be] schedule step and lane of every row
 };
 static bool events_lists(const EventsRun* ev) { return ev->k > 0; }
-static void events_window(EventsRun* ev, int64_t done) { ev->done = done; }
-static void events_block(EventsRun* ev, int slot, int M, const int* miss, const int64_t* step, const int* lane) {
-  ev->src_slot = slot; ev->src_M = M; ev->src_miss = miss; ev->src_step = step; ev->src_lane = lane;
-}
 
 static void events_release(EvalCtx& e) {
   if (!e.events) return;
@@ -209,12 +196,13 @@ static int events_ctx(g4r_handle* h, EvalCtx* e, EventsCtx** out) {
 
 // checks k, sizes the per-event window and its buffers, prepares the top-k operands
 static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, EventsRun* ev, const SeenDev* sd) {
-  const int I = h->md.n_items, Be = e->Be, Bs = s->B, ldL = h->md.ldL, k = ev->k;
+  const int Be = e->Be, ldL = h->md.ldL, k = ev->k;
   ev->sched = s;
   ev->seen = sd != nullptr;
   ev->ex_off = sd ? e->dSeenOff : nullptr; ev->ex = sd ? e->dSeenEx : nullptr;
+  TopkFilter f;
   if (k > 0) {
-    int rc = topk_filter(h, k, e->n_cand > 0 ? e->hCand.data() : nullptr, e->n_cand, &ev->f);
+    int rc = topk_filter(h, k, e->n_cand > 0 ? e->hCand.data() : nullptr, e->n_cand, &f);
     if (rc) return rc;
   }
   int rc = events_ctx(h, e, &ev->x);
@@ -226,33 +214,11 @@ static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, Events
   ev->w = (int)w;
   ev->off.assign((size_t)w, 0);
   ev->m.assign((size_t)w, 0);
-  if (s->hist) { ev->rstep.assign((size_t)w * Be, 0); ev->rlane.assign((size_t)w * Be, 0); }
   CK(dev_grow(&x->dCnt, &x->cnt_cap, (size_t)w * Be * 2));
   if (k == 0) return G4R_OK;
-  // the top-k constants of topk_rank (exclude_seen: with exclusions of at most cap items per lane); only the tile kind depends
-  // on the mini-batch's lanes
-  const bool use_cand = ev->f.use_cand;
-  ev->n_comp = use_cand ? ev->f.n_distinct : I;
-  ev->P = std::min(ev->n_comp, std::max(k + (sd ? sd->cap : 0), std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
-  ev->no_tile = (use_cand || ev->seen) && ev->P == ev->n_comp;
-  ev->C = std::min(ev->n_comp, 16 * k + TOPK_SURV_BASE);
-  const int tc_tiles = (I + TC_N - 1) / TC_N;
-  const int n_part = ev->no_tile ? 0 : std::max(2 * tc_tiles, (ev->n_comp + EV_IT - 1) / EV_IT);
-  rc = topk_ctx(h, e, &ev->t);
+  if (sd) { ev->rstep.assign((size_t)w * Be, 0); ev->rlane.assign((size_t)w * Be, 0); }
+  rc = topk_plan(h, e, f, k, sd ? sd->cap : 0, s->B, &ev->plan);   // exclude_seen: at most cap exclusions per lane
   if (rc) return rc;
-  TopkCtx* t = ev->t;
-  rc = topk_upload_cand(h, t, ev->f);
-  if (rc) return rc;
-  CK(dev_grow(&t->dPre, &t->pre_cap, (size_t)Bs * ev->P));
-  if (!ev->no_tile) {
-    CK(dev_grow(&t->dSurv, &t->surv_cap, (size_t)Bs * ev->C));
-    CK(dev_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)Bs * ev->C));
-    CK(dev_grow(&t->dPart, &t->part_cap, (size_t)Bs * n_part));
-    if (wgmma_tiles(h->cfg, Bs, ev->n_comp, I)) {          // some mini-batch may take the wgmma tiles
-      rc = topk_tc_operands(h, e, t);
-      if (rc) return rc;
-    }
-  }
   CK(dev_grow(&x->dYw, &x->yw_cap, (size_t)w * Be * ldL));
   CK(dev_grow(&x->dSurvN, &x->survn_cap, (size_t)w * Be));
   CK(dev_grow(&x->dNorm, &x->norm_cap, (size_t)w * Be));
@@ -262,93 +228,65 @@ static int events_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, Events
   return G4R_OK;
 }
 
-// staging step i (a history schedule: ranking block i of the staging window), right after its target scores: its events' place in
-// the per-event window (unit j of it), and its y rows saved for the top-k
-static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk) {
+// unit u, right after its target scores: its events' place in the per-event window (unit j of it), its rows' schedule step and
+// lane (for the seen sets of the flush), and its y rows saved for the top-k
+static int events_stage(g4r_handle* h, EvalCtx* e, EventsRun* ev, const RankUnit& u, cudaStream_t rk) {
   EventsCtx* x = ev->x;
+  const TopkPlan& p = ev->plan;
   if (ev->n == 0) {
-    ev->base = i; ev->win_ev = 0;
-    if (ev->k > 0 && !ev->no_tile) CK(cudaMemsetAsync(x->dSurvN, 0, ev->survn.size() * sizeof(int), rk));
+    ev->win_ev = 0;
+    if (ev->k > 0 && !p.no_tile) CK(cudaMemsetAsync(x->dSurvN, 0, ev->survn.size() * sizeof(int), rk));
   }
-  const bool blk = ev->src_slot >= 0;
-  const int j = i - ev->base, M = blk ? ev->src_M : e->hM[i];
+  const int j = ev->n++, M = u.M, Be = e->Be;
   ev->off[(size_t)j] = ev->win_ev;
   ev->m[(size_t)j] = M;
   ev->win_ev += M;
-  ev->n = j + 1;
-  if (blk)
-    for (int b = 0; b < M; b++) { ev->rstep[(size_t)j * e->Be + b] = ev->src_step[b]; ev->rlane[(size_t)j * e->Be + b] = ev->src_lane[b]; }
+  if (!ev->rstep.empty())
+    for (int b = 0; b < M; b++) {
+      ev->rstep[(size_t)j * Be + b] = u.steps ? u.steps[b] : u.step;
+      ev->rlane[(size_t)j * Be + b] = u.lanes ? u.lanes[b] : b;
+    }
   if (ev->k > 0) {
-    const size_t rows = (size_t)e->Be * h->md.ldL;
-    k_ev_stage<<<std::min<int>((int)((rows / 4 + 255) / 256), 2 * h->n_sm), 256, 0, rk>>>(blk ? ev->src_slot : e->slot, blk ? 0 : i, x->dYk, x->dYw + (size_t)j * rows, x->dMk);
+    const size_t rows = (size_t)Be * h->md.ldL;
+    k_ev_stage<<<std::min<int>((int)((rows / 4 + 255) / 256), 2 * h->n_sm), 256, 0, rk>>>(u.slot, u.s, x->dYk, x->dYw + (size_t)j * rows, x->dMk);
     h->launches++;
   }
   return G4R_OK;
 }
 
-static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, int64_t o, cudaStream_t rk);
-
-// staging step i after k_eval_rank: its counts, and its lists by topk_rank's pipeline on the staged y rows; a full per-event
-// window is flushed
-static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, int i, cudaStream_t rk) {
+// the lists of unit j of the per-event window (M rows, window events o ..) by topk_rank's pipeline on the staged y rows; a lane
+// whose survivors overflowed keeps its softmax normaliser, selects from its truncated list here and is redone by the flush
+static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, int64_t o, cudaStream_t rk) {
   EventsCtx* x = ev->x;
-  const bool blk = ev->src_slot >= 0;
-  const int Be = e->Be, j = i - ev->base, M = ev->m[(size_t)j], k = ev->k;
-  const int slot = blk ? ev->src_slot : e->slot, si = blk ? 0 : i;
+  const TopkPlan& p = ev->plan;
+  const int Be = e->Be, k = ev->k;
+  int* cnt = x->dSurvN + (size_t)j * Be;
+  const int n_part = topk_tiles(h, e, p, x->slot, x->dYk, M, cnt, ev->ex_off, ev->ex, rk);
+  if (!p.no_tile && h->md.fact.kind > G4R_ACT_SELU) {
+    k_ev_norm<<<M, TOPK_THREADS, 0, rk>>>(cnt, p.C, p.t->dPart, n_part, x->dNorm + (size_t)j * Be);
+    h->launches++;
+  }
+  topk_select(h, p, x->slot, M, p.no_tile ? nullptr : cnt, nullptr, nullptr, p.t->dPart, n_part, x->dItems + o * k, x->dScores + o * k, ev->ex_off, ev->ex, rk);
+  CK(cudaGetLastError());
+  return G4R_OK;
+}
+
+// unit u after k_eval_rank: its counts and lists; a full per-event window is flushed
+static int events_step(g4r_handle* h, EvalCtx* e, EventsRun* ev, const RankUnit& u, cudaStream_t rk) {
+  EventsCtx* x = ev->x;
+  const int Be = e->Be, j = ev->n - 1;
   const int64_t o = ev->off[(size_t)j];
-  if (ev->seen) k_ev_counts<true><<<(2 * Be + 255) / 256, 256, 0, rk>>>(slot, si, h->dRankCnt, x->dCnt + 2 * o, blk ? ev->src_miss : e->dMiss);
-  else k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(slot, si, h->dRankCnt, x->dCnt + 2 * o);
+  if (ev->seen) k_ev_counts<true><<<(2 * Be + 255) / 256, 256, 0, rk>>>(u.slot, u.s, h->dRankCnt, x->dCnt + 2 * o, u.sd.miss);
+  else k_ev_counts<<<(2 * Be + 255) / 256, 256, 0, rk>>>(u.slot, u.s, h->dRankCnt, x->dCnt + 2 * o);
   h->launches++;
-  if (k > 0) {
-    int rc = events_topk(h, e, ev, M, j, o, rk);
+  if (ev->k > 0) {
+    int rc = events_topk(h, e, ev, u.M, j, o, rk);
     if (rc) return rc;
   }
   return ev->n == ev->w ? events_flush(h, e, ev, rk) : G4R_OK;
 }
 
-// the lists of mini-batch j of the per-event window (M lanes, window events o ..)
-static int events_topk(g4r_handle* h, EvalCtx* e, EventsRun* ev, int M, int j, int64_t o, cudaStream_t rk) {
-  EventsCtx* x = ev->x;
-  const int Be = e->Be, k = ev->k;
-  TopkCtx* t = ev->t;
-  const int I = h->md.n_items, L = h->md.L, P = ev->P, C = ev->C, n_comp = ev->n_comp;
-  const bool filt = ev->f.use_cand, soft = h->md.fact.kind > G4R_ACT_SELU;
-  const bool fx = filt || ev->seen;                      // the filtering instances: candidates and / or exclusions
-  const unsigned int* dmask = filt ? t->dMask : nullptr;
-  const int* dcand = filt ? t->dCand : nullptr;
-  const int* dexoff = ev->seen ? ev->ex_off : nullptr;
-  const int* dex = ev->seen ? ev->ex : nullptr;
-  const bool tc = !ev->no_tile && wgmma_tiles(h->cfg, M, n_comp, I);
-  const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
-  const int n_part = ev->no_tile ? 0 : tc ? 2 * tc_tiles : (n_comp + EV_IT - 1) / EV_IT;
-  int* cnt = x->dSurvN + (size_t)j * Be;
-  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(x->slot, 0, nullptr, nullptr, t->dPre, dcand, P);
-  h->launches++;
-  if (!ev->no_tile) {
-    (fx ? k_topk_tau<true> : k_topk_tau<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18), dcand, dexoff, dex);
-    if (tc) {
-      k_tc_split<TC_M><<<dim3((M + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(x->dYk, M, h->md.ldL, L, e->dAsplit, tc_chunks, nullptr, 1.0f);
-      (fx ? k_topk_tc<true> : k_topk_tc<false>)<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part, e->dAsplit, e->dBsplit,
-                                                                                                              dmask, dexoff, dex);
-      h->launches += 2;
-    } else {
-      (fx ? k_topk_fp32<true> : k_topk_fp32<false>)<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), rk>>>(x->slot, t->dTau, cnt, t->dSurv, C, t->dPart, n_part,
-                                                                                                                           dcand, n_comp, dexoff, dex);
-      h->launches++;
-    }
-    h->launches++;
-    if (soft) { k_ev_norm<<<M, TOPK_THREADS, 0, rk>>>(cnt, C, t->dPart, n_part, x->dNorm + (size_t)j * Be); h->launches++; }
-  }
-  // an overflowed lane selects from its truncated list here; its list is replaced at the end of the window
-  (fx ? k_topk_final<true> : k_topk_final<false>)<<<M, TOPK_THREADS, 0, rk>>>(x->slot, k, ev->no_tile ? nullptr : cnt, t->dSurv, t->dSurvPre, C, nullptr, nullptr,
-                                                                              t->dPart, n_part, x->dItems + o * k, x->dScores + o * k, dcand, t->dPre, P, dmask, dexoff, dex);
-  h->launches++;
-  CK(cudaGetLastError());
-  return G4R_OK;
-}
-
-// end of a per-event window (its ev->n mini-batches from staging step ev->base): the overflowed lanes rescored exactly, then the
-// window's outputs to the host
+// end of a per-event window (its ev->n units): the overflowed lanes rescored exactly, then the window's outputs to the host
 static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t rk) {
   EventsCtx* x = ev->x;
   const int Be = e->Be, k = ev->k, I = h->md.n_items, w = ev->n;
@@ -356,16 +294,15 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
   if (w == 0) return G4R_OK;
   CK(cudaMemcpyAsync(ev->out_counts + 2 * ev->ev_done, x->dCnt, (size_t)E * 2 * sizeof(int), cudaMemcpyDeviceToHost, rk));
   if (k > 0) {
-    if (!ev->no_tile) {
+    const TopkPlan& p = ev->plan;
+    if (!p.no_tile) {
       CK(cudaMemcpyAsync(ev->survn.data(), x->dSurvN, (size_t)w * Be * sizeof(int), cudaMemcpyDeviceToHost, rk));
       CK(cudaStreamSynchronize(rk));
       std::vector<int> src, evw;
       for (int64_t i = 0; i < w; i++)
         for (int b = 0; b < ev->m[(size_t)i]; b++)
-          if (ev->survn[(size_t)(i * Be + b)] > ev->C) { src.push_back((int)(i * Be + b)); evw.push_back((int)(ev->off[(size_t)i] + b)); }
+          if (ev->survn[(size_t)(i * Be + b)] > p.C) { src.push_back((int)(i * Be + b)); evw.push_back((int)(ev->off[(size_t)i] + b)); }
       const int chunk = (int)std::min<int64_t>(Be, std::max<int64_t>(1, (int64_t)(EVENTS_ROWS_BYTES / ((size_t)I * sizeof(float)))));
-      const bool filt = ev->f.use_cand, fx = filt || ev->seen;
-      TopkCtx* t = ev->t;
       for (size_t j0 = 0; j0 < src.size(); j0 += (size_t)chunk) {
         const int n = (int)std::min<size_t>((size_t)chunk, src.size() - j0);
         CK(dev_grow(&e->dOut, &e->out_cap, (size_t)n * I));
@@ -376,12 +313,11 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
         CK(dev_grow(&x->dOvScores, &x->ov_scores_cap, (size_t)chunk * k));
         CK(cudaMemcpyAsync(x->dOvSrc, src.data() + j0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rk));
         CK(cudaMemcpyAsync(x->dOvEv, evw.data() + j0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rk));
-        if (ev->seen) {                        // the chunk's seen sets at their own mini-batches, rebuilt from the schedule
+        if (ev->seen) {                        // the chunk's seen sets at their own steps, rebuilt from the schedule
           std::vector<int> eo(1, 0), ex;
           for (int j = 0; j < n; j++) {
-            const int r = src[j0 + (size_t)j];
-            if (ev->sched->hist) seen_rebuild(ev->sched, ev->rstep[(size_t)r], ev->rlane[(size_t)r], ex);
-            else seen_rebuild(ev->sched, ev->done + ev->base + r / Be, r % Be, ex);
+            const size_t r = (size_t)src[j0 + (size_t)j];
+            seen_rebuild(ev->sched, ev->rstep[r], ev->rlane[r], ex);
             eo.push_back((int)ex.size());
           }
           CK(dev_grow(&x->dOvExOff, &x->ov_ex_off_cap, eo.size()));
@@ -391,11 +327,10 @@ static int events_flush(g4r_handle* h, EvalCtx* e, EventsRun* ev, cudaStream_t r
         }
         k_ev_gather<<<std::min(2 * h->n_sm, (n * h->md.ldL / 4 + 255) / 256 + 1), 256, 0, rk>>>(x->dYw, x->dOvSrc, n, h->md.ldL, x->dYk, x->dMk, x->dNorm, x->dOvNorm);
         k_topk_rows<<<dim3((I + 127) / 128, n), 128, 0, rk>>>(x->slot, x->dIdent, e->dOut);
-        (fx ? k_topk_final<true> : k_topk_final<false>)<<<n, TOPK_THREADS, 0, rk>>>(x->slot, k, x->dIdent, t->dSurv, t->dSurvPre, ev->C, x->dIdent, e->dOut,
-                                                                                    x->dOvNorm, 1, x->dOvItems, x->dOvScores, filt ? t->dCand : nullptr, t->dPre, ev->P,
-                                                                                    filt ? t->dMask : nullptr, ev->seen ? x->dOvExOff : nullptr, ev->seen ? x->dOvEx : nullptr);
+        topk_select(h, p, x->slot, n, x->dIdent, x->dIdent, e->dOut, x->dOvNorm, 1, x->dOvItems, x->dOvScores,
+                    ev->seen ? x->dOvExOff : nullptr, ev->seen ? x->dOvEx : nullptr, rk);
         k_ev_scatter<<<std::min(2 * h->n_sm, (n * k + 255) / 256), 256, 0, rk>>>(x->dOvItems, x->dOvScores, x->dOvEv, n, k, x->dItems, x->dScores);
-        h->launches += 4;
+        h->launches += 3;
         CK(cudaGetLastError());
       }
     }

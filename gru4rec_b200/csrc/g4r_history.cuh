@@ -11,8 +11,9 @@
 //            positions come from the schedule on the host: no atomics, a deterministic order
 //   rank     a block is ranked on the ranking stream when it holds the schedule's batch size of rows, and at the end of each
 //            staging window, through a scoring descriptor of its own (y = the block's rows, wY = its targets, wSlot = identity,
-//            so the block's row r reads snapshot r): k_eval_tgt<.., KEY>, the fp32 tiles (k_eval_score<.., KEY>) or the wgmma tiles,
-//            k_eval_rank, and g4r_eval_events' per-event work.  A step with no counted lane ranks nothing.
+//            so the block's row r reads snapshot r).  It is a RankUnit of eval_rank, the sequence that ranks a plain mini-batch,
+//            with per-row noise keys (the KEY instances), its snapshots as the seen lists, and each row's schedule step and lane
+//            for g4r_eval_events' per-event work.  A step with no counted lane ranks nothing.
 // Two blocks alternate: the forward stream fills one while the ranking stream ranks the other, and waits only when it comes back to
 // a block whose ranking has not finished.
 #pragma once
@@ -152,65 +153,29 @@ static int hist_stage(g4r_handle* h, EvalCtx* e, HistCtx* c, int64_t w) {
   return G4R_OK;
 }
 
-// one ranking: the constants eval_run decided for the whole call
-struct HistRank {
-  unsigned int tie = 0u;
-  bool tc_possible = false, seen = false;
-  int n_cut = 0, mode = 0, cap = 0;
-  EventsRun* ev = nullptr;
-};
-
-// block qi (its M rows enqueued on the forward stream) ranked on the ranking stream as block `blk` of the staging window
-static int hist_rank(g4r_handle* h, EvalCtx* e, HistCtx* c, int qi, int M, int blk, const HistRank& r) {
-  HistBlock& q = c->q[qi];
-  const int Be = e->Be, I = h->md.n_items;
-  cudaStream_t st = h->stream, rk = h->side;
-  CK(cudaEventRecord(q.filled, st)); CK(cudaStreamWaitEvent(rk, q.filled, 0));
-  const SeenDev qsd = r.seen ? SeenDev{q.dSeen, q.dSeenN, r.cap, q.dMiss} : SeenDev{};
-  k_eval_tgt<false, true><<<(Be + 31) / 32, 32, 0, rk>>>(q.slot, 0, h->dTgt, h->dRankCnt, r.tie, e->n_cand > 0 ? 1 : 0, r.tc_possible ? Be : 0, SeenDev{}, q.dKey);
-  h->launches++;
-  if (r.ev) {
-    if (r.seen && events_lists(r.ev)) {
-      k_seen_csr<<<1, SEEN_CSR_THREADS, 0, rk>>>(q.slot, 0, qsd, e->dSeenOff, e->dSeenEx);
-      h->launches++;
-    }
-    events_block(r.ev, q.slot, M, q.dMiss, q.step.data(), q.lane.data());
-    int rc = events_stage(h, e, r.ev, blk, rk);
-    if (rc) return rc;
-  }
-  const int n_comp = e->n_cand > 0 ? e->n_cand : I;
-  if (r.tc_possible && wgmma_tiles(h->cfg, M, I, I)) {
-    const int tc_chunks = (h->md.L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
-    k_tc_split<TC_M><<<dim3((M + TC_M - 1) / TC_M, tc_chunks), 256, 0, rk>>>(q.dY, M, h->md.ldL, h->md.L, e->dAsplit, tc_chunks, nullptr, 1.0f);
-    if (r.seen) k_eval_tc<true><<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(q.slot, 0, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit, qsd);
-    else k_eval_tc<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), rk>>>(q.slot, 0, h->dTgt, Be, h->dRankCnt, e->dAsplit, e->dBsplit);
-    h->launches += 2;
-  } else {
-    if (r.seen) k_eval_score<false, true, true><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(q.slot, 0, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, r.tie, qsd, q.dKey);
-    else k_eval_score<false, false, true><<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), rk>>>(q.slot, 0, h->dTgt, h->dRankCnt, nullptr, e->n_cand > 0 ? e->dCand : nullptr, e->n_cand, r.tie, SeenDev{}, q.dKey);
-    h->launches++;
-  }
-  if (r.seen) k_eval_rank<true><<<1, 256, 0, rk>>>(q.slot, 0, h->dRankCnt, e->dCut, r.n_cut, r.mode, e->dSums, q.dMiss);
-  else k_eval_rank<<<1, 256, 0, rk>>>(q.slot, 0, h->dRankCnt, e->dCut, r.n_cut, r.mode, e->dSums);
-  h->launches++;
-  if (r.ev) {
-    int rc = events_step(h, e, r.ev, blk, rk);
-    if (rc) return rc;
-  }
-  CK(cudaEventRecord(q.done, rk));
-  CK(cudaGetLastError());
-  q.step.clear(); q.lane.clear();
-  return G4R_OK;
-}
-
 // the w staged steps of a history schedule (first schedule step `done`): forward, seen insert and enqueue on the forward stream,
 // every full block and the window's last partial block ranked on the ranking stream
-static int hist_window(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const SeenDev* sd, const HistRank& r) {
+static int hist_window(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const RankConsts& cs, EventsRun* ev) {
   const int Bs = s->B;
-  cudaStream_t st = h->stream;
+  cudaStream_t st = h->stream, rk = h->side;
+  const SeenDev* sd = cs.seen ? &cs.sd : nullptr;
   int rc = hist_stage(h, e, c, w);
   if (rc) return rc;
-  int qi = 0, qn = 0, blk = 0;
+  // block q, its M rows enqueued on the forward stream, ranked against its snapshots on the ranking stream
+  auto rank = [&](HistBlock& q, int M) -> int {
+    CK(cudaEventRecord(q.filled, st)); CK(cudaStreamWaitEvent(rk, q.filled, 0));
+    RankUnit u;
+    u.slot = q.slot; u.M = M; u.y = q.dY; u.key = q.dKey;
+    if (sd) u.sd = SeenDev{q.dSeen, q.dSeenN, sd->cap, q.dMiss};
+    u.steps = q.step.data(); u.lanes = q.lane.data();
+    int r = eval_rank(h, e, u, cs, ev, rk, nullptr);
+    if (r) return r;
+    CK(cudaEventRecord(q.done, rk));
+    CK(cudaGetLastError());
+    q.step.clear(); q.lane.clear();
+    return G4R_OK;
+  };
+  int qi = 0, qn = 0;
   for (int64_t i = 0; i < w; i++) {
     eval_forward(h, e, (int)i, h->He);
     if (sd) {
@@ -229,23 +194,16 @@ static int hist_window(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule
       for (int j = 0; j < take; j++) { q.step.push_back(done + i); q.lane.push_back(c->hLanes[l0 + j]); }
       qn += take; p += take;
       if (qn == Bs) {
-        rc = hist_rank(h, e, c, qi, qn, blk++, r);
+        rc = rank(q, qn);
         if (rc) return rc;
         qi ^= 1; qn = 0;
       }
     }
   }
   if (qn > 0) {
-    rc = hist_rank(h, e, c, qi, qn, blk, r);
+    rc = rank(c->q[qi], qn);
     if (rc) return rc;
   }
   CK(cudaGetLastError());
   return G4R_OK;
-}
-
-static int hist_run(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const SeenDev* sd, unsigned int tie,
-                    bool tc_possible, int n_cut, int mode, EventsRun* ev) {
-  HistRank r;
-  r.tie = tie; r.tc_possible = tc_possible; r.seen = sd != nullptr; r.n_cut = n_cut; r.mode = mode; r.cap = sd ? sd->cap : 0; r.ev = ev;
-  return hist_window(h, e, c, s, w, done, sd, r);
 }

@@ -106,19 +106,6 @@ static int sess_check_items(g4r_handle* h, const int32_t* X, int64_t n) {
   return G4R_OK;
 }
 
-// steps 0 .. w-1 staged on the host go to the device window (the staging buffers may be reused once the stream has passed them)
-static int sess_upload(g4r_handle* h, EvalCtx* e, int w) {
-  cudaStream_t st = h->stream;
-  const size_t nb = (size_t)w * e->Be;
-  CK(cudaMemcpyAsync(e->dX, e->hX, nb * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dY, e->hY, nb * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dSlot, e->hSlot, nb * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dF, e->hF, nb, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dM, e->hM, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dSti, e->hSti, (size_t)w * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(e->dG, e->hG, (size_t)w * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  return G4R_OK;
-}
 // step s of the window: lanes b < M take item X[ev[b]], slot slots[ev[b]], flag 2 if fresh[ev[b]]
 static void sess_stage(EvalCtx* e, int s, const int32_t* X, const int* slots, const uint8_t* fresh, const int64_t* ev, int M) {
   const size_t o = (size_t)s * e->Be;
@@ -208,7 +195,7 @@ extern "C" int g4r_sessions_feed(g4r_handle* h, const int64_t* keys, const int32
       sess_stage(e, w++, X, slots.data(), fresh.data(), order.data() + c0, M);
       const bool last = r == n_rounds - 1 && c0 + M == start[(size_t)r + 1];
       if (w == e->cap || last) {                           // a full window (or the call's last step): upload and run it
-        rc = sess_upload(h, e, w);
+        rc = eval_upload(h, e, w);
         if (rc) return rc;
         for (int i = 0; i < w; i++) eval_forward(h, e, i, s->H);
         CK(cudaGetLastError());
@@ -261,7 +248,7 @@ extern "C" int g4r_sessions_topk(g4r_handle* h, const int64_t* keys, const int32
     const int M = (int)std::min<int64_t>(Be, n - c0);
     for (int b = 0; b < M; b++) ev[(size_t)b] = c0 + b;
     sess_stage(e, 0, X, slots.data(), fresh.data(), ev.data(), M);
-    rc = sess_upload(h, e, 1);
+    rc = eval_upload(h, e, 1);
     if (rc) return rc;
     ex_off.clear(); ex.clear();
     if (excl_off || exclude_seen) {

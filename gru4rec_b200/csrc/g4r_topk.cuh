@@ -497,6 +497,88 @@ static int topk_upload_cand(g4r_handle* h, TopkCtx* t, const TopkFilter& f) {
   return G4R_OK;
 }
 
+// The constants of a top-k ranking of units of at most `lanes` lanes under the filter f, with at most max_ex exclusions per lane
+struct TopkPlan {
+  TopkCtx* t = nullptr;
+  int k = 0, n_comp = 0, P = 0, C = 0;
+  int n_part_fp32 = 0, n_part_tc = 0;                     // softmax partials per lane of each tile kind
+  bool no_tile = false;                                   // every candidate is in the prefix: no filter tiles, no overflow
+  bool filt = false;                                      // the filtering instances: candidates and / or exclusions
+  bool tc_any = false;                                    // some unit may take the wgmma tiles (their operands are ready)
+  const unsigned int* dmask = nullptr; const int* dcand = nullptr;   // the candidate set (nullptr: the catalogue)
+};
+
+// the plan, the top-k buffers sized for `lanes` lanes, and the candidate set and wgmma operands on the device.  The prefix is the
+// first P candidates; P covers k eligible items of every lane, or every candidate (then it is the survivor set and no tile runs)
+static int topk_plan(g4r_handle* h, EvalCtx* e, const TopkFilter& f, int k, int max_ex, int lanes, TopkPlan* p) {
+  const int I = h->md.n_items;
+  int rc = topk_ctx(h, e, &p->t);
+  if (rc) return rc;
+  TopkCtx* t = p->t;
+  rc = topk_upload_cand(h, t, f);
+  if (rc) return rc;
+  p->k = k;
+  p->filt = f.use_cand || max_ex > 0;
+  p->n_comp = f.use_cand ? f.n_distinct : I;
+  p->P = std::min(p->n_comp, std::max(k + max_ex, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
+  p->no_tile = p->filt && p->P == p->n_comp;
+  p->C = std::min(p->n_comp, 16 * k + TOPK_SURV_BASE);
+  p->n_part_fp32 = (p->n_comp + EV_IT - 1) / EV_IT;
+  p->n_part_tc = 2 * ((I + TC_N - 1) / TC_N);
+  p->tc_any = !p->no_tile && wgmma_tiles(h->cfg, lanes, p->n_comp, I);
+  p->dmask = f.use_cand ? t->dMask : nullptr;
+  p->dcand = f.use_cand ? t->dCand : nullptr;
+  CK(dev_grow(&t->dPre, &t->pre_cap, (size_t)lanes * p->P));
+  if (!p->no_tile) {
+    CK(dev_grow(&t->dSurv, &t->surv_cap, (size_t)lanes * p->C));
+    CK(dev_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)lanes * p->C));
+    CK(dev_grow(&t->dPart, &t->part_cap, (size_t)lanes * std::max(p->n_part_fp32, p->n_part_tc)));
+  }
+  if (p->tc_any) {
+    rc = topk_tc_operands(h, e, t);
+    if (rc) return rc;
+  }
+  return G4R_OK;
+}
+
+// Steps 1 and 2 for the M lanes of scoring descriptor `slot` (their final-layer y at y) on stream st, under the exclusions
+// ex_off / ex (nullptr: none): the exact prefix scores and tau_b, then, unless no_tile, the filter tiles, which append to the
+// survivor counters cnt (zeroed by the caller) and write the softmax partials.  Returns the partials per lane (0: no tile ran)
+static int topk_tiles(g4r_handle* h, EvalCtx* e, const TopkPlan& p, int slot, const float* y, int M, int* cnt, const int* ex_off, const int* ex,
+                      cudaStream_t st) {
+  TopkCtx* t = p.t;
+  const int I = h->md.n_items, L = h->md.L;
+  k_eval_score<true><<<(p.P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(slot, 0, nullptr, nullptr, t->dPre, p.dcand, p.P);
+  h->launches++;
+  if (p.no_tile) return 0;
+  const bool tc = p.tc_any && wgmma_tiles(h->cfg, M, p.n_comp, I);
+  // delta_b = (||y_b||_1 max|Wy| + max|By|) (L + 3) 2^-18: four times the worst case of |3xTF32 - fp32| (DESIGN §3d)
+  (p.filt ? k_topk_tau<true> : k_topk_tau<false>)<<<M, TOPK_THREADS, 0, st>>>(slot, t->dPre, p.P, p.k, t->dTau, tc ? t->dAbsMax : nullptr,
+                                                                              ldexpf((float)(L + 3), -18), p.dcand, ex_off, ex);
+  if (tc) {
+    const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
+    k_tc_split<TC_M><<<dim3((M + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(y, M, h->md.ldL, L, e->dAsplit, tc_chunks, nullptr, 1.0f);
+    (p.filt ? k_topk_tc<true> : k_topk_tc<false>)<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(
+        slot, t->dTau, cnt, t->dSurv, p.C, t->dPart, p.n_part_tc, e->dAsplit, e->dBsplit, p.dmask, ex_off, ex);
+    h->launches += 3;
+    return p.n_part_tc;
+  }
+  (p.filt ? k_topk_fp32<true> : k_topk_fp32<false>)<<<p.n_part_fp32, EV_THREADS, topk_fp32_smem_bytes(), st>>>(
+      slot, t->dTau, cnt, t->dSurv, p.C, t->dPart, p.n_part_fp32, p.dcand, p.n_comp, ex_off, ex);
+  h->launches += 2;
+  return p.n_part_fp32;
+}
+
+// Step 3 for the M lanes of descriptor `slot`: each lane selects from its survivors (cnt; nullptr: from the prefix) or from its
+// fallback row rows[ov_row[b]] (ov_row nullptr: none), with the softmax partials part [M x n_part], into items / scores [M x k]
+static void topk_select(g4r_handle* h, const TopkPlan& p, int slot, int M, const int* cnt, const int* ov_row, const float* rows, const float2* part,
+                        int n_part, int* items, float* scores, const int* ex_off, const int* ex, cudaStream_t st) {
+  TopkCtx* t = p.t;
+  (p.filt ? k_topk_final<true> : k_topk_final<false>)<<<M, TOPK_THREADS, 0, st>>>(slot, p.k, cnt, t->dSurv, t->dSurvPre, p.C, ov_row, rows, part, n_part,
+                                                                                  items, scores, p.dcand, t->dPre, p.P, p.dmask, ex_off, ex);
+  h->launches++;
+}
+
 extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_t batch, const uint8_t* reset_mask, int32_t k,
                                          const int32_t* cand, int64_t n_cand, const int64_t* excl_off, const int32_t* excl_items,
                                          int32_t* out_items, float* out_scores) {
@@ -534,78 +616,35 @@ extern "C" int g4r_predict_topk_filtered(g4r_handle* h, const int32_t* X, int32_
 static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, int32_t k, const TopkFilter& f,
                      const std::vector<int>& ex_off, const std::vector<int>& ex, int32_t* out_items, float* out_scores) {
   const int I = h->md.n_items;
-  const bool use_cand = f.use_cand;
-  const int n_distinct = f.n_distinct;
   const bool use_ex = !ex.empty();
   int max_ex = 0;
   for (size_t b = 1; b < ex_off.size(); b++) max_ex = std::max(max_ex, ex_off[b] - ex_off[b - 1]);
-  TopkCtx* t = nullptr;
-  int rc = topk_ctx(h, e, &t);
+  TopkPlan p;
+  int rc = topk_plan(h, e, f, k, max_ex, batch, &p);
   if (rc) return rc;
+  TopkCtx* t = p.t;
   cudaStream_t st = h->stream;
-  const int L = h->md.L;
-  rc = topk_upload_cand(h, t, f);
-  if (rc) return rc;
   if (use_ex) {
     CK(dev_grow(&t->dExOff, &t->ex_off_cap, ex_off.size()));
     CK(dev_grow(&t->dEx, &t->ex_cap, ex.size()));
     CK(cudaMemcpyAsync(t->dExOff, ex_off.data(), ex_off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(t->dEx, ex.data(), ex.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   }
-  const unsigned int* dmask = use_cand ? t->dMask : nullptr;
-  const int* dcand = use_cand ? t->dCand : nullptr;
   const int* dexoff = use_ex ? t->dExOff : nullptr;
   const int* dex = use_ex ? t->dEx : nullptr;
-  // the prefix is the first P candidates; P covers k eligible items of every lane, or every candidate (then it is the survivor
-  // set and no tile runs)
-  const int n_comp = use_cand ? n_distinct : I;
-  const int P = std::min(n_comp, std::max(k + max_ex, std::max(TOPK_PREFIX_MIN, (I / 16 + 63) & ~63)));
-  const bool no_tile = (use_cand || use_ex) && P == n_comp;
-  const int C = std::min(n_comp, 16 * k + TOPK_SURV_BASE);
-  const bool tc = !no_tile && wgmma_tiles(h->cfg, batch, n_comp, I);
-  const int tc_chunks = (L + 1 + TC_KC - 1) / TC_KC, tc_tiles = (I + TC_N - 1) / TC_N;
-  const int n_part = no_tile ? 0 : tc ? 2 * tc_tiles : (n_comp + EV_IT - 1) / EV_IT;
-  CK(dev_grow(&t->dPre, &t->pre_cap, (size_t)batch * P));
-  if (!no_tile) {
-    CK(dev_grow(&t->dSurv, &t->surv_cap, (size_t)batch * C));
-    CK(dev_grow(&t->dSurvPre, &t->surv_pre_cap, (size_t)batch * C));
-    CK(dev_grow(&t->dPart, &t->part_cap, (size_t)batch * n_part));
-  }
   CK(dev_grow(&t->dItems, &t->items_cap, (size_t)batch * k));
   CK(dev_grow(&t->dScores, &t->scores_cap, (size_t)batch * k));
-  if (tc) {
-    rc = topk_tc_operands(h, e, t);
-    if (rc) return rc;
-  }
   eval_forward(h, e, 0, Hst);
-  // 1. exact fp32 scores of the prefix (the predict kernel over the first P candidates, or the items 0 .. P-1) and tau_b
-  k_eval_score<true><<<(P + EV_IT - 1) / EV_IT, EV_THREADS, eval_smem_bytes(), st>>>(e->slot, 0, nullptr, nullptr, t->dPre, dcand, P);
-  h->launches++;
+  if (!p.no_tile) CK(cudaMemsetAsync(t->dCnt, 0, (size_t)batch * sizeof(int), st));
+  const int n_part = topk_tiles(h, e, p, e->slot, h->md.layer[h->md.n_layers - 1].y, batch, t->dCnt, dexoff, dex, st);
   int n_ov = 0;
-  if (!no_tile) {
-    // delta_b = (||y_b||_1 max|Wy| + max|By|) (L + 3) 2^-18: four times the worst case of |3xTF32 - fp32| (DESIGN §3d)
-    (use_cand || use_ex ? k_topk_tau<true> : k_topk_tau<false>)<<<batch, TOPK_THREADS, 0, st>>>(e->slot, t->dPre, P, k, t->dTau, tc ? t->dAbsMax : nullptr, ldexpf((float)(L + 3), -18), dcand, dexoff, dex);
-    CK(cudaMemsetAsync(t->dCnt, 0, (size_t)batch * sizeof(int), st));
-    // 2. the candidates in tiles: survivors and softmax partials
-    if (tc) {
-      k_tc_split<TC_M><<<dim3((batch + TC_M - 1) / TC_M, tc_chunks), 256, 0, st>>>(h->md.layer[h->md.n_layers - 1].y, batch, h->md.ldL, L, e->dAsplit, tc_chunks, nullptr, 1.0f);
-      auto kern = (use_cand || use_ex) ? k_topk_tc<true> : k_topk_tc<false>;
-      kern<<<std::min(tc_tiles, h->n_sm), TC_THREADS, sizeof(TcSmem), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part, e->dAsplit, e->dBsplit,
-                                                                            dmask, dexoff, dex);
-      h->launches += 2;
-    } else {
-      auto kern = (use_cand || use_ex) ? k_topk_fp32<true> : k_topk_fp32<false>;
-      kern<<<(n_comp + EV_IT - 1) / EV_IT, EV_THREADS, topk_fp32_smem_bytes(), st>>>(e->slot, t->dTau, t->dCnt, t->dSurv, C, t->dPart, n_part,
-                                                                                    dcand, n_comp, dexoff, dex);
-      h->launches++;
-    }
-    h->launches++;
+  if (!p.no_tile) {
     CK(cudaGetLastError());
-    // 3. overflowed lanes (more survivors than their list holds) take their whole fp32 row, in g4r_predict's score buffer
+    // overflowed lanes (more survivors than their list holds) take their whole fp32 row, in g4r_predict's score buffer
     std::vector<int> cnt((size_t)batch), ov_row((size_t)batch, -1), ov_list;
     CK(cudaMemcpyAsync(cnt.data(), t->dCnt, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    for (int b = 0; b < batch; b++) if (cnt[(size_t)b] > C) { ov_row[(size_t)b] = (int)ov_list.size(); ov_list.push_back(b); }
+    for (int b = 0; b < batch; b++) if (cnt[(size_t)b] > p.C) { ov_row[(size_t)b] = (int)ov_list.size(); ov_list.push_back(b); }
     n_ov = (int)ov_list.size();
     if (n_ov > 0) {
       const size_t need = (size_t)n_ov * I;
@@ -616,10 +655,8 @@ static int topk_rank(g4r_handle* h, EvalCtx* e, float* const* Hst, int batch, in
       h->launches++;
     }
   }
-  // select: from the survivors (or a fallback row), or from the prefix when it holds every candidate
-  (use_cand || use_ex ? k_topk_final<true> : k_topk_final<false>)<<<batch, TOPK_THREADS, 0, st>>>(e->slot, k, no_tile ? nullptr : t->dCnt, t->dSurv, t->dSurvPre, C, n_ov > 0 ? t->dOvRow : nullptr, e->dOut,
-                                               t->dPart, n_part, t->dItems, t->dScores, dcand, t->dPre, P, dmask, dexoff, dex);
-  h->launches++;
+  topk_select(h, p, e->slot, batch, p.no_tile ? nullptr : t->dCnt, n_ov > 0 ? t->dOvRow : nullptr, e->dOut, t->dPart, n_part, t->dItems, t->dScores,
+              dexoff, dex, st);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out_items, t->dItems, (size_t)batch * k * sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(out_scores, t->dScores, (size_t)batch * k * sizeof(float), cudaMemcpyDeviceToHost, st));

@@ -5,10 +5,13 @@ GRU(512)), 100 and 512 lanes.  Before timing, the loop's lists must equal eval_e
 the public functions: the pandas preparation of evaluate_gpu / evaluate_events, the events frame and recommend_next_batch's item
 id mapping are left out.
 
-  python scripts/eval_events_bench.py [--rounds R] [--exclude_seen]
+  python scripts/eval_events_bench.py [--rounds R] [--exclude_seen] [--parent-lib PATH]
 
 --exclude_seen: instead, the cost of exclude_seen (DESIGN §3g): eval_schedule against the same call with the seen lists, and
 eval_events with them at k = 0 and 20, timed in alternating rounds; the lists are checked to hold no seen item.
+--parent-lib: instead, a libg4r.so built from the parent commit runs eval_schedule and eval_events at k = 0 and 20 (with
+--exclude_seen: all with the seen lists) on the same schedule and weights; every output must equal this build's bit for bit, and
+the two builds are timed in alternating rounds (median and min-max of --rounds).
 
 Env: EE_EVENTS (test events per shape, default 100,000, at least twice the items), EE_SHAPES (e.g. 'rsc15,rees46'), EE_LANES (e.g. '100,512')."""
 import argparse, os, sys, time
@@ -21,14 +24,16 @@ from gru4rec_b200 import _lib
 from gru4rec_b200.synth import make_session_arrays
 import gru4rec as g4
 from serve_bench import card
-from serve_filter_bench import make_engine
+from serve_filter_bench import make_engine, parent_lib
 
 SHAPES = {'rsc15': (37483, 100), 'rees46': (172000, 512)}
 
 ap = argparse.ArgumentParser()
 ap.add_argument('--rounds', type=int, default=3)
 ap.add_argument('--exclude_seen', action='store_true')
+ap.add_argument('--parent-lib', default=None)
 a = ap.parse_args()
+plib = parent_lib(a.parent_lib) if a.parent_lib else None
 print('card: %s | nvidia-smi name, power.limit, clocks.max.sm: %s' % card(), flush=True)
 n_ev = int(os.environ.get('EE_EVENTS', 100000))
 CUTS = [1, 5, 20]
@@ -83,6 +88,40 @@ def seen_leg(eng, sched, e, shape, I, L, lanes):
               % (shape, I, L, lanes, n, dt, min(v), max(v), dt / sched.n_steps * 1e6, 100.0 * (dt / base - 1.0), sched.n_steps, sched.n_events), flush=True)
 
 
+def bitwise_equal(x, y):
+    """two results (tuples of arrays, numbers or None) hold the same bytes"""
+    if isinstance(x, tuple):
+        return len(x) == len(y) and all(bitwise_equal(p, q) for p, q in zip(x, y))
+    if x is None or y is None:
+        return x is y
+    x, y = np.asarray(x), np.asarray(y)
+    return x.dtype == y.dtype and x.shape == y.shape and x.tobytes() == y.tobytes()
+
+
+def parent_leg(eng, par, sched, shape, I, L, lanes):
+    """eval_schedule and eval_events of this build and the parent build: bitwise-equal outputs, then alternating rounds"""
+    calls = {'eval_schedule': lambda g: g.eval_schedule(sched, CUTS, 0)}
+    for k in (0, 20):
+        calls['eval_events k=%d' % k] = lambda g, k=k: g.eval_events(sched, CUTS, 0, k=k)
+    tag = ' exclude_seen' if a.exclude_seen else ''
+    for g in (eng, par):
+        g.set_eval_exclude_seen(a.exclude_seen)
+    for n, f in calls.items():
+        if not bitwise_equal(f(eng), f(par)):
+            raise SystemExit('MISMATCH: %s%s differs from the parent build (%s, %d lanes)' % (n, tag, shape, lanes))
+    ts = {(n, b): [] for n in calls for b in ('parent', 'pr')}
+    for r in range(a.rounds):
+        for n, f in calls.items():
+            for b, g in (('parent', par), ('pr', eng))[::1 if r % 2 == 0 else -1]:    # either build first in turn
+                torch.cuda.synchronize(); t0 = time.time()
+                f(g)
+                torch.cuda.synchronize(); ts[(n, b)].append(time.time() - t0)
+    for n in calls:
+        p, q = ts[(n, 'parent')], ts[(n, 'pr')]
+        print('%-7s I=%d GRU(%d) lanes=%3d %-30s parent median %.4f s (min-max %.4f-%.4f)  this build median %.4f s (min-max %.4f-%.4f)  '
+              'same result: True' % (shape, I, L, lanes, n + tag, np.median(p), min(p), max(p), np.median(q), min(q), max(q)), flush=True)
+
+
 def loop_topk(eng, sched, e, k):
     """the per-event lists by predict_topk, one call per mini-batch of the schedule (lanes = state slots)"""
     B = sched.batch_size
@@ -106,6 +145,11 @@ for shape in os.environ.get('EE_SHAPES', 'rsc15,rees46').split(','):
         eng = make_engine(I, mk, lanes, w)
         sched = _lib.Schedule(items, offset, None, lanes, 0, mode=1)
         e = sched.export()
+        if plib is not None:
+            par = make_engine(I, mk, lanes, w, plib)
+            parent_leg(eng, par, sched, shape, I, L, lanes)
+            eng.close(); par.close()
+            continue
         if a.exclude_seen:
             seen_leg(eng, sched, e, shape, I, L, lanes)
             eng.close()

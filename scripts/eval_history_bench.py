@@ -7,7 +7,11 @@ GRU(100)), Rees46 (172,000 items, GRU(512)) and ml20m (27,000 items, GRU(100): w
 both rank a block / mini-batch with the same tile kind (all of them with EH_TC=fp32).  The engine calls are timed, not the
 public functions (their pandas preparation is the same for both).
 
-  python scripts/eval_history_bench.py [--rounds R]
+  python scripts/eval_history_bench.py [--rounds R] [--parent-lib PATH]
+
+--parent-lib: instead of the workaround, a libg4r.so built from the parent commit runs the history schedule (eval_schedule, and
+eval_events at k = 0 and 20, with and without exclude_seen) with the same weights; every output must equal this build's bit for
+bit, and the two builds are timed in alternating rounds (median and min-max of --rounds).
 
 Env: EH_USERS (users per shape, default 20,000), EH_SCALE (history length multiplier, default 4), EH_SHAPES (e.g. 'rsc15,rees46'),
 EH_LANES (default 512), EH_TC ('auto' or 'fp32')."""
@@ -21,12 +25,15 @@ from gru4rec_b200 import _lib
 from gru4rec_b200.synth import make_session_arrays
 import gru4rec as g4
 from serve_bench import card
+from serve_filter_bench import make_engine, parent_lib
 
 SHAPES = {'rsc15': (37483, 100), 'rees46': (172000, 512), 'ml20m': (27000, 100)}
 
 ap = argparse.ArgumentParser()
 ap.add_argument('--rounds', type=int, default=3)
+ap.add_argument('--parent-lib', default=None)
 a = ap.parse_args()
+plib = parent_lib(a.parent_lib) if a.parent_lib else None
 print('card: %s | nvidia-smi name, power.limit, clocks.max.sm: %s' % card(), flush=True)
 n_users = int(os.environ.get('EH_USERS', 20000))
 scale = int(os.environ.get('EH_SCALE', 4))
@@ -62,17 +69,64 @@ def timed(calls):
     return ts
 
 
+def bitwise_equal(x, y):
+    """two results (tuples of arrays, numbers or None) hold the same bytes"""
+    if isinstance(x, tuple):
+        return len(x) == len(y) and all(bitwise_equal(p, q) for p, q in zip(x, y))
+    if x is None or y is None:
+        return x is y
+    x, y = np.asarray(x), np.asarray(y)
+    return x.dtype == y.dtype and x.shape == y.shape and x.tobytes() == y.tobytes()
+
+
+def seen(g, on, f):
+    g.set_eval_exclude_seen(on)
+    try:
+        return f()
+    finally:
+        g.set_eval_exclude_seen(False)
+
+
+def parent_leg(eng, par, hist, shape, I, L):
+    """the history schedule on this build and the parent build: bitwise-equal outputs, then alternating rounds"""
+    calls = {}
+    for on in (False, True):
+        tag = ' exclude_seen' if on else ''
+        calls['eval_schedule' + tag] = lambda g, on=on: seen(g, on, lambda: g.eval_schedule(hist, CUTS, 0))
+        for k in (0, 20):
+            calls['eval_events k=%d%s' % (k, tag)] = lambda g, on=on, k=k: seen(g, on, lambda: g.eval_events(hist, CUTS, 0, k=k))
+    for n, f in calls.items():
+        if not bitwise_equal(f(eng), f(par)):
+            raise SystemExit('MISMATCH: history %s differs from the parent build (%s)' % (n, shape))
+    ts = {(n, b): [] for n in calls for b in ('parent', 'pr')}
+    for r in range(a.rounds):
+        for n, f in calls.items():
+            for b, g in (('parent', par), ('pr', eng))[::1 if r % 2 == 0 else -1]:    # either build first in turn
+                torch.cuda.synchronize(); t0 = time.time()
+                f(g)
+                torch.cuda.synchronize(); ts[(n, b)].append(time.time() - t0)
+    for n in calls:
+        p, q = ts[(n, 'parent')], ts[(n, 'pr')]
+        print('%-7s I=%d GRU(%d) lanes=%d history %-28s parent median %.4f s (min-max %.4f-%.4f)  this build median %.4f s (min-max %.4f-%.4f)  '
+              'same result: True' % (shape, I, L, lanes, n, np.median(p), min(p), max(p), np.median(q), min(q), max(q)), flush=True)
+
+
 for shape in os.environ.get('EH_SHAPES', 'rsc15,rees46').split(','):
     I, L = SHAPES[shape]
     mk = dict(layers=[L], loss='bpr-max', final_act='elu-0.5', batch_size=32, n_sample=0)
     gru = g4.GRU4Rec(**mk); gru.n_items = I
     w = gru._init_host_weights()
-    eng = _lib.Engine(_lib.make_config(I, mk, sample_store=0, eval_lanes=lanes, step_mode=1, eval_tc=tc))
-    for name, arr in w.items():
-        eng.set(name, arr)
+    eng = make_engine(I, mk, lanes, w, eval_tc=tc)
     data, off, nh = leave_one_out(I, seed=1)
     plain = _lib.Schedule(data, off, None, lanes, 0, mode=1)
     hist = _lib.Schedule(data, off, None, lanes, 0, mode=1, n_history=nh)
+    if plib is not None:
+        par = make_engine(I, mk, lanes, w, plib, eval_tc=tc)
+        print('%-7s I=%d GRU(%d) lanes=%d: %d users, %d events, %d mini-batches, %d counted events'
+              % (shape, I, L, lanes, len(nh), int(off[-1]), hist.n_steps, hist.n_events), flush=True)
+        parent_leg(eng, par, hist, shape, I, L)
+        eng.close(); par.close()
+        continue
     used = np.arange(lanes)[None, :] < plain.batch_sizes()[:, None]
     keep = hist.counted()[used]
     got, ref = eng.eval_events(hist, CUTS, 0), eng.eval_events(plain, CUTS, 0)
