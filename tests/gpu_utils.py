@@ -142,20 +142,27 @@ def opt_slots(m):
     return OPT_SLOTS[m.adapt] + (('vel',) if m.momentum > 0 else ())
 
 
-def oracle_f64(eng, mk, n_items, step_count, P0=None):
+def oracle_f64(eng, mk, n_items, step_count, P0=None, dtype=np.float64):
     """A float64 oracle holding the device's current float32 weights, hidden state and optimizer state, at dropout step
-    `step_count`: the reference for one step of the device, free of the float32 rounding of a second implementation."""
-    m = orc.OracleGRU4Rec(dtype=np.float64, **mk)
-    m.init(n_items)
+    `step_count`: the reference for one step of the device, free of the float32 rounding of a second implementation.  With
+    dtype=np.float32, the same oracle in float32: what a second float32 implementation reaches on the same inputs.  The tables
+    are taken from the device as they are (no random initialisation first: at 172,000 x 512 that alone takes seconds)."""
+    m = orc.OracleGRU4Rec(dtype=dtype, **mk)
+    nl = len(m.layers)
+    m.n_items = n_items
+    m.Wx, m.Wh, m.Wrz = ([eng.get('%s%d' % (kind, i)).astype(dtype) for i in range(nl)] for kind in ('Wx', 'Wh', 'Wrz'))
+    m.Bh = [eng.get('Bh%d' % i).astype(dtype).reshape(-1) for i in range(nl)]
+    m.H = [eng.get('H%d' % i).astype(dtype) for i in range(nl)]
+    m.Wy = eng.get('Wy').astype(dtype)
+    m.By = eng.get('By').astype(dtype).reshape(-1, 1)
+    m.E = eng.get('E').astype(dtype) if (m.embedding and not m.constrained_embedding) else None
+    m.init_opt_state()
     for name in param_names(m):
         p = oracle_param(m, name)
-        p[...] = eng.get(name).reshape(p.shape)
         for slot in opt_slots(m):
-            m.opt[(name, slot)] = eng.get('%s.%s' % (name, slot)).reshape(p.shape).astype(np.float64)
-    for i in range(len(m.layers)):
-        m.H[i][...] = eng.get('H%d' % i)
+            m.opt[(name, slot)] = eng.get('%s.%s' % (name, slot)).reshape(p.shape).astype(dtype)
     m.step_count = step_count
-    m.P0 = None if P0 is None else np.asarray(P0, np.float64)
+    m.P0 = None if P0 is None else np.asarray(P0, dtype)
     return m
 
 
@@ -306,7 +313,37 @@ def _assert_path(path, before, after, step_mode, tag):
         tag, path, launches, fast, fallback)
 
 
-def f64_run_steps(eng, mk, n_items, store, steps, P0, path, run=None):
+def _f32_oracle_checks(m, ref_cost, m32, X, Y, R, store_row, lanes, tag, sgd):
+    """The products and the gradients (plain SGD) or updates (any other optimizer) of a float32 oracle `m32`, which holds the
+    state the float64 oracle `m` held before it took the step, against `m`'s on the same inputs -- the comparisons f64_run_steps
+    makes for the device, so the two worst errors measure the same things.  Updates: at the touched rows of the row tables, with
+    one fp32 rounding of the result per applied update."""
+    names, slots = param_names(m32), opt_slots(m32)
+    W0 = {n: np.array(oracle_param(m32, n)) for n in names}
+    S0 = {(n, s): np.array(m32.opt[(n, s)]) for n in names for s in slots}
+    cost = m32.train_step(X, Y, R, samples=store_row, slots=lanes)
+    C, G, C32, G32 = m.last_cache, m.last_grads, m32.last_cache, m32.last_grads
+    out = [(tag + 'cost', np.float64(cost), ref_cost, 0.0)]
+    for i in range(len(m.layers)):
+        out += [(tag + 'H%d' % i, C32['H_new'][i], C['H_new'][i], 0.0), (tag + 'dvec%d' % i, G32['dvec'][i], G['dvec'][i], 0.0)]
+    out += [(tag + 'y%d' % i, a, b, 0.0) for i, (a, b) in enumerate(zip([lc['inp'] for lc in C32['layers'][1:]] + [C32['y_last']],
+                                                                        [lc['inp'] for lc in C['layers'][1:]] + [C['y_last']]))]
+    out += [(tag + 'dSx', G32['dSx'], G['dSx'], 0.0), (tag + 'dSy', G32['dSy'], G['dSy'], 0.0)]
+    if sgd:
+        out += [(tag + 'd' + n, g32, g, 0.0) for (n, g32), (_, g) in zip(dense_grads(m32, G32), dense_grads(m, G))]
+        return out + [(tag + 'd' + n + ' rows', g32, g, 0.0) for (n, _, g32), (_, _, g) in zip(sparse_grads(C32, G32), sparse_grads(C, G))]
+    touched = {n: np.unique(idx, return_counts=True) for n, idx, _ in sparse_grads(C, G)}
+    for n in names:
+        rows, mult = (touched[n][0], touched[n][1][:, None]) if n in touched else (slice(None), 1)
+        pairs = [(n, W0[n], oracle_param(m32, n), oracle_param(m, n))] + [
+            ('%s.%s' % (n, s), S0[(n, s)], m32.opt[(n, s)], m.opt[(n, s)]) for s in slots]
+        for what, a0, a1, r1 in pairs:
+            a0, a1, r1 = (np.asarray(a, np.float64) for a in (a0[rows], a1[rows], r1[rows]))
+            out.append((tag + what + ' update', a1 - a0, r1 - a0, mult * 2.0 ** -23 * (np.abs(a0) + np.abs(a1))))
+    return out
+
+
+def f64_run_steps(eng, mk, n_items, store, steps, P0, path, run=None, keep_weights=True, f32_checks=None, require_dsy=True):
     """Runs `steps` through Engine.train_step on the kernel `path` (one of STEP_PATHS, or one per step; None: no counters are
     checked).  A step is (X, Y, R), or a step of orc.build_train_schedule (a dict that also holds `slots`, the H row of each
     lane: H is compared at those rows and the oracle runs with them); `run(k, X, Y, R)`, if given, runs step k on the device
@@ -317,20 +354,29 @@ def f64_run_steps(eng, mk, n_items, store, steps, P0, path, run=None):
     lr * g (* the grad_cap scale): the dense ones, and the rows of Wx0 / E / Wy / By (one fp32 rounding per duplicate).  Any
     other optimizer: the updates W1 - W0 of every weight and every state tensor against the oracle's, with one fp32 rounding
     of the result per applied update.  Rows of the row tables that no position touched stay bit-identical (weights and state).
+    The row tables are held as the device's float32 arrays and taken to float64 only at the touched rows, so a step costs a
+    few float32 copies of each table besides the oracle's own float64 tables (at 172,000 x 512: 352 MB per copy).
+    `keep_weights=False` leaves the parameters after each step out of the returned outputs (a long run on a large catalogue
+    would hold one copy of every table per step).  `f32_checks`, if a list, receives the same comparisons for a float32 oracle
+    run from the same state on the same inputs (_f32_oracle_checks).  `require_dsy`: a generic step after the first must have
+    written some DSY row (true of f64_step_inputs' second step; the steps of a real schedule need not have a chunk wider than
+    a sub tile, and then their dSy rows are checked through the Wy rows they update).
     Returns ([(what, dev, ref, extra_atol)], {output name: device array} for bitwise comparisons, [grad_cap scale per step])."""
     paths = [path] * len(steps) if path is None or isinstance(path, str) else list(path)
     assert eng.uses_tensor_cores() == (paths[0] == 'tc')
-    lr = mk['learning_rate']
+    lr = mk.get('learning_rate', 0.1)          # the default of make_config and of the oracle
     sgd = mk.get('adapt', 'adagrad') is None and not mk.get('momentum', 0) and not mk.get('lmbd', 0)
     ulp = lambda a, b: 2.0 ** -23 * (np.abs(a) + np.abs(b))        # rounding of one fp32 update
+    f64 = lambda a: np.asarray(a, np.float64)
     checks, outs, scales = [], {}, []
     for k, st in enumerate(steps):
         X, Y, R, lanes = (st['X'], st['Y'], st['R'], st['slots']) if isinstance(st, dict) else tuple(st) + (None,)
         m = oracle_f64(eng, mk, n_items, k, P0)
+        m32 = oracle_f64(eng, mk, n_items, k, None if P0 is None else np.asarray(P0, np.float32), np.float32) if f32_checks is not None else None
         names, slots = param_names(m), opt_slots(m)
         nl = len(m.layers)
-        W0 = {n: eng.get(n).astype(np.float64) for n in names}
-        S0 = {(n, s): eng.get('%s.%s' % (n, s)).astype(np.float64) for n in names for s in slots}
+        W0 = {n: eng.get(n) for n in names}
+        S0 = {(n, s): eng.get('%s.%s' % (n, s)) for n in names for s in slots}
         dsy_all = paths[k] == 'tc' or (paths[k] == 'phases' and m.grad_cap > 0)
         if paths[k] != 'fast' and not dsy_all:
             eng.set('DSY', np.full(eng.shape('DSY'), np.nan, np.float32))
@@ -357,42 +403,53 @@ def f64_run_steps(eng, mk, n_items, store, steps, P0, path, run=None):
             wide = np.bincount(C['Y'])[C['Y'][order]] > SC_CT
             assert wrote.all() or not dsy_all, tag + 'DSY: %d of %d rows not written' % ((~wrote).sum(), N)
             assert wrote[wide].all(), tag + 'DSY: %d rows of duplicate groups wider than a sub tile not written' % (~wrote[wide]).sum()
-            # step 2 has heavy duplicates: some chunk is wider than a sub tile
-            assert wrote.any() or k == 0, tag + 'DSY: no row written'
+            # step 2 of f64_step_inputs has heavy duplicates: some chunk is wider than a sub tile
+            assert wrote.any() or k == 0 or not require_dsy, tag + 'DSY: no row written'
             if wrote.any():
                 dev['DSY'], ref['DSY'] = dsy[wrote], G['dSy'][order][wrote]
-        W1 = {n: eng.get(n).astype(np.float64) for n in names}
+        W1 = {n: eng.get(n) for n in names}
         checks += [(tag + n, dev[n], ref[n], 0.0) for n in dev]
         outs.update({'%d_%s' % (k, n): v for n, v in dev.items()})
-        outs.update({'%d_%s' % (k, n): v for n, v in W1.items()})
+        if keep_weights:
+            outs.update({'%d_%s' % (k, n): v for n, v in W1.items()})
         sc = float(m.last_gscale)
         scales.append(sc)
         sparse = sparse_grads(C, G)
-        counts = {n: np.bincount(idx, minlength=W0[n].shape[0]) for n, idx, _ in sparse}
-        for n, cnt in counts.items():
-            assert np.array_equal(W0[n][cnt == 0], W1[n][cnt == 0]), tag + n + ': an untouched row changed'
+        # the rows each row table's positions touched (ascending) and how many positions touched each
+        touched = {n: np.unique(idx, return_inverse=True, return_counts=True) for n, idx, _ in sparse}
+
+        def untouched_same(n, a0, a1, what):
+            changed = (a0.view(np.uint32) != a1.view(np.uint32)).any(axis=1)
+            changed[touched[n][0]] = False
+            assert not changed.any(), tag + what + ': an untouched row changed'
+        for n in touched:
+            untouched_same(n, W0[n], W1[n], n)
         if sgd:
             for n, g in dense_grads(m, G):
-                checks.append((tag + 'd' + n + ' recovered', (W0[n] - W1[n]) / lr, g * sc, ulp(W0[n], W1[n]) / lr))
+                w0, w1 = f64(W0[n]), f64(W1[n])
+                checks.append((tag + 'd' + n + ' recovered', (w0 - w1) / lr, g * sc, ulp(w0, w1) / lr))
             for n, idx, g in sparse:
-                cnt, rows = counts[n], counts[n] > 0
-                gref = np.zeros(W0[n].shape)
-                np.add.at(gref, idx, g * sc)
-                checks.append((tag + 'd' + n + ' rows recovered', ((W0[n] - W1[n]) / lr)[rows], gref[rows],
-                               cnt[rows, None] * (ulp(W0[n], W1[n]) / lr)[rows]))
+                rows, inv, cnt = touched[n]
+                w0, w1 = f64(W0[n][rows]), f64(W1[n][rows])
+                gref = np.zeros((len(rows),) + W0[n].shape[1:])
+                np.add.at(gref, inv.reshape(-1), g * sc)
+                checks.append((tag + 'd' + n + ' rows recovered', (w0 - w1) / lr, gref, cnt[:, None] * (ulp(w0, w1) / lr)))
         else:
             for n in names:
-                rows = counts[n] > 0 if n in counts else slice(None)
-                mult = counts[n][rows, None] if n in counts else 1
+                rows = touched[n][0] if n in touched else slice(None)
+                mult = touched[n][2][:, None] if n in touched else 1
                 pairs = [(n, W0[n], W1[n], oracle_param(m, n))]
                 for s in slots:
-                    S1 = eng.get('%s.%s' % (n, s)).astype(np.float64)
-                    if n in counts:
-                        assert np.array_equal(S0[(n, s)][counts[n] == 0], S1[counts[n] == 0]), tag + '%s.%s: an untouched row changed' % (n, s)
+                    S1 = eng.get('%s.%s' % (n, s))
+                    if n in touched:
+                        untouched_same(n, S0[(n, s)], S1, '%s.%s' % (n, s))
                     pairs.append(('%s.%s' % (n, s), S0[(n, s)], S1, m.opt[(n, s)]))
                 for what, a0, a1, r1 in pairs:
-                    r1 = np.asarray(r1).reshape(a0.shape)
-                    checks.append((tag + what + ' update', (a1 - a0)[rows], (r1 - a0)[rows], mult * ulp(a0, a1)[rows]))
+                    r1 = np.asarray(r1).reshape(a0.shape)[rows]
+                    a0, a1 = f64(a0[rows]), f64(a1[rows])
+                    checks.append((tag + what + ' update', a1 - a0, r1 - a0, mult * ulp(a0, a1)))
+        if m32 is not None:
+            f32_checks += _f32_oracle_checks(m, ref_cost, m32, X, Y, R, store[k], lanes, tag, sgd)
     return checks, outs, scales
 
 
