@@ -47,6 +47,7 @@ EXPORTS = [
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
     'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
     'g4r_sessions_export', 'g4r_sessions_import',
+    'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
 ]
 
 _lib = None
@@ -127,6 +128,10 @@ def load():
     lib.g4r_sessions_end.argtypes = [vp, vp, i64]
     lib.g4r_sessions_export.argtypes = [vp, vp, vp, vp, vp]
     lib.g4r_sessions_import.argtypes = [vp, vp, vp, vp, vp, i64]
+    lib.g4r_train_state_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
+    lib.g4r_train_state_export.argtypes = [vp, vp, C.c_size_t]
+    lib.g4r_train_state_import.argtypes = [vp, vp, C.c_size_t]
+    lib.g4r_copy_item_tables.argtypes = [vp, vp, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -519,6 +524,34 @@ class Engine(object):
 
     def stream(self):
         return self.lib.g4r_stream(self.h)
+
+    # ---- training state (g4r_train_state_*, g4r_copy_item_tables; DESIGN §3i) ----
+    def train_state_export(self):
+        """uint8 array: the global step, sample pointer and MRG stream states of the handle -- with the named tensors and the
+        sample store, everything a new handle needs to continue this one's run bit for bit"""
+        n = C.c_size_t()
+        self._check(self.lib.g4r_train_state_bytes(self.h, C.byref(n)))
+        blob = np.zeros(n.value, dtype=np.uint8)
+        self._check(self.lib.g4r_train_state_export(self.h, _ptr(blob), n.value))
+        return blob
+
+    def train_state_import(self, blob):
+        """Takes over a train_state_export() blob (after set_sample_store, which rewinds the pointer).  A blob that is truncated,
+        of another version, or exported with another n_sample / store size / seed raises NotImplementedError and changes nothing."""
+        blob = np.ascontiguousarray(blob, dtype=np.uint8)
+        self._check(self.lib.g4r_train_state_import(self.h, _ptr(blob), blob.size))
+
+    def copy_item_tables(self, src, new_Wy=None, new_By=None, new_in=None):
+        """Device-to-device copy of every parameter, optimizer-state tensor and training hidden state of Engine `src`, whose
+        catalogue is a prefix of this one's: the item tables keep src's rows and take new_Wy / new_By / new_in (E, or Wx0 of a
+        model without embedding) in the added rows, zero where None; added rows of the optimizer state are zero."""
+        n_add = int(self.cfg.n_items) - int(src.cfg.n_items)
+
+        def block(name, a):
+            return None if a is None or n_add <= 0 else np.ascontiguousarray(np.asarray(a, dtype=np.float32).reshape(n_add, self.shape(name)[1]))
+        wy, by = block('Wy', new_Wy), block('By', new_By)
+        nin = None if self.cfg.constrained_embedding else block('E' if self.cfg.embedding else 'Wx0', new_in)
+        self._check(self.lib.g4r_copy_item_tables(self.h, src.h, _ptr(wy), _ptr(by), _ptr(nin)))
 
     # ---- scoring ----
     def eval_schedule(self, sched, cut_off, mode=0):

@@ -1000,10 +1000,14 @@ static void matvec_mod(const int64_t A[3][3], const int64_t* v, int64_t m, int64
 static void mrg_ff(const int64_t* s, const int64_t A1[3][3], const int64_t A2[3][3], int64_t* o) {
   matvec_mod(A1, s, MRG_M1, o); matvec_mod(A2, s + 3, MRG_M2, o + 3);
 }
-static void mrg_host_init(g4r_handle* h) {
+// substreams a handle's uniform() draws from: fixed by the size of its sample store
+static int mrg_stream_count(const g4r_handle* h) {
   const int64_t n = (int64_t)h->gen_len * h->cfg.n_sample;
   int64_t r = n; if (r > 6) r = r / 6;
-  h->n_streams = (int)std::min<int64_t>(r, 15360);
+  return (int)std::min<int64_t>(r, 15360);
+}
+static void mrg_host_init(g4r_handle* h) {
+  h->n_streams = mrg_stream_count(h);
   for (int i = 0; i < 6; i++) h->mrg_rstate[i] = h->cfg.mrg_seed ? h->cfg.mrg_seed : 12345;
   // multi-GPU: every rank draws its own negatives -- rank r takes the r-th block of substreams (the block a further
   // uniform() call of the same generator would have taken: the base state advances by 2^134 per call, SURVEY appendix B)
@@ -1470,6 +1474,142 @@ extern "C" int g4r_train_step(g4r_handle* h, const int32_t* X, const int32_t* Y,
   CK(cudaStreamSynchronize(h->stream));
   if (cost) *cost = h->hCost[0];
   if (h->hCost[0] != h->hCost[0]) FAIL(G4R_ERR_NAN, "NaN error!");
+  return G4R_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// training state: checkpoint / resume and catalogue growth (DESIGN §3i)
+// ------------------------------------------------------------------------------------------------
+// Everything a training handle holds besides its named tensors and the sample store, in one flat blob: the header below, then
+// n_streams x 6 int32 MRG31k3p stream states (zero until the first uniform() call seeds them).
+#define G4R_STATE_MAGIC 0x53523447u      /* "G4RS" */
+#define G4R_STATE_VERSION 1u
+struct TrainStateHdr {
+  uint32_t magic, version;
+  uint64_t bytes;
+  // the configuration the state is valid for
+  int32_t n_sample, store_rows; uint32_t mrg_seed, dropout_seed; int32_t world_size, rank;
+  // the state
+  uint32_t global_step; int32_t mrg_init, n_streams, reserved;
+  int64_t sample_ptr, mrg_rstate[6];
+};
+static TrainStateHdr train_state_header(const g4r_handle* h) {
+  TrainStateHdr d; memset(&d, 0, sizeof(d));
+  d.magic = G4R_STATE_MAGIC; d.version = G4R_STATE_VERSION;
+  d.n_streams = mrg_stream_count(h);
+  d.bytes = sizeof(TrainStateHdr) + (size_t)d.n_streams * 6 * sizeof(int32_t);
+  d.n_sample = h->cfg.n_sample; d.store_rows = h->gen_len; d.mrg_seed = h->cfg.mrg_seed; d.dropout_seed = h->cfg.dropout_seed;
+  d.world_size = h->cfg.world_size; d.rank = h->cfg.rank;
+  return d;
+}
+extern "C" int g4r_train_state_bytes(g4r_handle* h, size_t* bytes) {
+  if (!h || !bytes) return G4R_ERR_INVALID;
+  if (h->cfg.world_size > 1) FAIL(G4R_ERR_STATE, "training state export / import is single-GPU only");
+  *bytes = (size_t)train_state_header(h).bytes;
+  return G4R_OK;
+}
+extern "C" int g4r_train_state_export(g4r_handle* h, void* host, size_t bytes) {
+  if (!h || !host) return G4R_ERR_INVALID;
+  if (h->cfg.world_size > 1) FAIL(G4R_ERR_STATE, "training state export / import is single-GPU only");
+  TrainStateHdr d = train_state_header(h);
+  if (bytes != d.bytes) FAIL(G4R_ERR_INVALID, "g4r_train_state_export: buffer size != g4r_train_state_bytes");
+  d.global_step = h->global_step; d.mrg_init = h->mrg_init ? 1 : 0; d.sample_ptr = h->sample_ptr;
+  if (h->mrg_init) memcpy(d.mrg_rstate, h->mrg_rstate, sizeof(d.mrg_rstate));
+  char* out = static_cast<char*>(host);
+  memcpy(out, &d, sizeof(d));
+  const size_t sb = (size_t)d.n_streams * 6 * sizeof(int32_t);
+  cudaSetDevice(h->cfg.device);
+  if (h->mrg_init && sb) {
+    CK(cudaMemcpyAsync(out + sizeof(d), h->dMrgState, sb, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  } else memset(out + sizeof(d), 0, sb);
+  return G4R_OK;
+}
+extern "C" int g4r_train_state_import(g4r_handle* h, const void* host, size_t bytes) {
+  if (!h || !host) return G4R_ERR_INVALID;
+  if (h->cfg.world_size > 1) FAIL(G4R_ERR_STATE, "training state export / import is single-GPU only");
+  // every check comes before the first write: a refused blob leaves the handle as it was
+  const TrainStateHdr want = train_state_header(h);
+  if (bytes < sizeof(TrainStateHdr)) FAIL(G4R_ERR_INVALID, "g4r_train_state_import: truncated blob");
+  TrainStateHdr d; memcpy(&d, host, sizeof(d));
+  if (d.magic != G4R_STATE_MAGIC) FAIL(G4R_ERR_INVALID, "g4r_train_state_import: not a training-state blob");
+  if (d.version != G4R_STATE_VERSION) FAIL(G4R_ERR_INVALID, "g4r_train_state_import: unknown blob version");
+  if (d.bytes != bytes || bytes != want.bytes) FAIL(G4R_ERR_INVALID, "g4r_train_state_import: truncated blob or a blob of another sample-store size");
+  if (d.n_sample != want.n_sample || d.store_rows != want.store_rows || d.n_streams != want.n_streams)
+    FAIL(G4R_ERR_INVALID, "g4r_train_state_import: the blob was exported with another n_sample / sample-store size");
+  if (d.mrg_seed != want.mrg_seed || d.dropout_seed != want.dropout_seed || d.world_size != want.world_size || d.rank != want.rank)
+    FAIL(G4R_ERR_INVALID, "g4r_train_state_import: the blob was exported with other seeds");
+  if (d.sample_ptr < 0 || d.sample_ptr > std::max(want.store_rows, 0) || (d.mrg_init != 0 && d.mrg_init != 1))
+    FAIL(G4R_ERR_INVALID, "g4r_train_state_import: sample pointer / flags out of range");
+  const size_t sb = (size_t)d.n_streams * 6 * sizeof(int32_t);
+  cudaSetDevice(h->cfg.device);
+  if (d.mrg_init && sb) {
+    CK(cudaMemcpyAsync(h->dMrgState, static_cast<const char*>(host) + sizeof(d), sb, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  h->global_step = d.global_step; h->sample_ptr = d.sample_ptr; h->mrg_init = d.mrg_init != 0; h->n_streams = d.mrg_init ? d.n_streams : 0;
+  memcpy(h->mrg_rstate, d.mrg_rstate, sizeof(d.mrg_rstate));
+  return G4R_OK;
+}
+
+// The tensors a trained model consists of: parameters, their optimizer state ("<name>.<slot>") and the training hidden state.
+// *item_table: rows are catalogue items (Wy, By, E; Wx0 without an embedding).
+static bool model_tensor(const g4r_handle* h, const std::string& name, bool* item_table) {
+  const std::string base = name.substr(0, name.find('.'));
+  const std::string kind = base.substr(0, base.find_first_of("0123456789"));
+  *item_table = base == "Wy" || base == "By" || base == "E" || (base == "Wx0" && h->md.mode == 0);
+  return *item_table || kind == "Wx" || kind == "Wh" || kind == "Wrz" || kind == "Bh" || (kind == "H" && name == base);
+}
+extern "C" int g4r_copy_item_tables(g4r_handle* h, g4r_handle* src, const float* new_Wy, const float* new_By, const float* new_in) {
+  if (!h || !src) return G4R_ERR_INVALID;
+  if (h == src) FAIL(G4R_ERR_INVALID, "g4r_copy_item_tables: source and destination are the same handle");
+  const g4r_config &a = h->cfg, &b = src->cfg;
+  if (a.world_size > 1 || b.world_size > 1) FAIL(G4R_ERR_STATE, "g4r_copy_item_tables is single-GPU only");
+  bool same = a.device == b.device && a.n_layers == b.n_layers && a.batch_size == b.batch_size && a.embedding == b.embedding &&
+              a.constrained_embedding == b.constrained_embedding && a.adapt == b.adapt && (a.momentum > 0.f) == (b.momentum > 0.f);
+  for (int i = 0; same && i < a.n_layers; i++) same = a.layers[i] == b.layers[i];
+  if (!same) FAIL(G4R_ERR_INVALID, "g4r_copy_item_tables: the handles differ in more than n_items (layers, batch size, embedding mode, optimizer state)");
+  if (a.n_items < b.n_items) FAIL(G4R_ERR_INVALID, "g4r_copy_item_tables: the destination has fewer items than the source");
+  const int64_t n_old = b.n_items, n_new = a.n_items;
+  // the same names with matching shapes on both sides, before anything is written
+  for (const auto& kv : src->tensors) {
+    bool item = false;
+    if (!model_tensor(src, kv.first, &item)) continue;
+    const TensorInfo* t = find_tensor(h, kv.first.c_str());
+    if (!t || t->cols != kv.second.cols || t->ld != kv.second.ld || t->rows != (item ? n_new : kv.second.rows) || kv.second.rows != (item ? n_old : t->rows))
+      FAIL(G4R_ERR_INVALID, "g4r_copy_item_tables: tensor " + kv.first + " does not match between the handles");
+  }
+  cudaSetDevice(a.device);
+  CK(cudaStreamSynchronize(src->stream));
+  // new rows of the weights: one device block per table, freed after the copy
+  struct Fill { const char* name; const float* host; float* dev; };
+  Fill fills[3] = {{"Wy", new_Wy, nullptr}, {"By", new_By, nullptr}, {h->md.mode == 1 ? "E" : "Wx0", h->md.mode == 2 ? nullptr : new_in, nullptr}};
+  int rc = G4R_OK;
+  auto release = [&]() { for (Fill& f : fills) if (f.dev) { cudaFree(f.dev); f.dev = nullptr; } };
+  if (n_new > n_old) for (Fill& f : fills) {
+    if (!f.host) continue;
+    const size_t nb = (size_t)(n_new - n_old) * find_tensor(h, f.name)->cols * sizeof(float);
+    if (cudaMalloc(&f.dev, nb) != cudaSuccess || cudaMemcpyAsync(f.dev, f.host, nb, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { rc = G4R_ERR_CUDA; break; }
+  }
+  if (rc) { release(); FAIL(rc, "g4r_copy_item_tables: staging the new rows failed"); }
+  for (const auto& kv : src->tensors) {
+    bool item = false;
+    if (!model_tensor(src, kv.first, &item)) continue;
+    const TensorInfo& s = kv.second; const TensorInfo& d = *find_tensor(h, kv.first.c_str());
+    if (!item) {
+      if (cudaMemcpyAsync(d.ptr, s.ptr, (size_t)s.rows * s.ld * sizeof(float), cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = G4R_ERR_CUDA; break; }
+      continue;
+    }
+    const float* fill = nullptr;
+    for (const Fill& f : fills) if (kv.first == f.name) fill = f.dev;
+    const int64_t n = n_new * d.ld;
+    k_rows_extend<<<(unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)h->n_sm * 16), 256, 0, h->stream>>>(d.ptr, s.ptr, n_old, n_new, d.ld, d.cols, fill);
+    h->launches++;
+  }
+  if (!rc && (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(h->stream) != cudaSuccess)) rc = G4R_ERR_CUDA;
+  release();
+  h->wy_version++;
+  if (rc) FAIL(rc, "g4r_copy_item_tables: device copy failed");
   return G4R_OK;
 }
 

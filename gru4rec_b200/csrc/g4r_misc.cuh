@@ -68,6 +68,20 @@ __global__ void __launch_bounds__(128) k_mrg_uniform(int32_t* __restrict__ state
   state[i * 6 + 0] = x11; state[i * 6 + 1] = x12; state[i * 6 + 2] = x13; state[i * 6 + 3] = x21; state[i * 6 + 4] = x22; state[i * 6 + 5] = x23;
 }
 
+// Catalogue growth (g4r_copy_item_tables): dst [n_new x ld] takes rows 0 .. n_old-1 of src [n_old x ld] as they are, padding
+// columns included; rows n_old .. n_new-1 take `fill` ([n_new - n_old x cols], dense) in their first `cols` columns, or zero
+// when fill == nullptr (optimizer state), and zero in the padding columns.
+__global__ void __launch_bounds__(256) k_rows_extend(float* __restrict__ dst, const float* __restrict__ src, int64_t n_old, int64_t n_new,
+                                                      int64_t ld, int64_t cols, const float* __restrict__ fill) {
+  const int64_t n = n_new * ld, n_copy = n_old * ld;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float v = 0.f;
+    if (i < n_copy) v = src[i];
+    else if (fill) { const int64_t r = i / ld, c = i - r * ld; if (c < cols) v = fill[(r - n_old) * cols + c]; }
+    dst[i] = v;
+  }
+}
+
 // Column plan of one step: score columns [Y | samples] sorted by (item, position); chunk boundaries that never
 // split a duplicate group; target column of each lane; duplicate chains of X.  One CTA per step.
 __global__ void __launch_bounds__(256) k_plan(ModelDev md, int* xnext, uint8_t* xflag, int npow2) {

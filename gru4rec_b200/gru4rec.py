@@ -14,9 +14,13 @@ exception types and the NumPy random-stream consumption order are the interface,
 tests/golden/set_params_cases.json + the golden fixtures pin them against the reference class.  Everything below that
 surface (schedule, step, optimizers, evaluation, persistence plumbing, multi-GPU) is this repository's own design.
 """
+import hashlib
+import json
+import os
 import pickle
 import time
 import weakref
+from types import SimpleNamespace
 from collections import OrderedDict  # noqa: F401  (param files use it)
 
 import numpy as np
@@ -301,6 +305,7 @@ class GRU4Rec:
             eng.sessions_import(*sessions[1])
         self._engine = eng
         self._engine_eval_lanes = eval_lanes
+        self._engine_training = bool(training)     # it holds optimizer state: fit_more() / save_checkpoint() keep it
         self._host = None
         self._bind_params()
         return eng
@@ -355,8 +360,16 @@ class GRU4Rec:
         Trains the network.  Same arguments, data-frame side effects ('ItemIdx' column, in-place sort) and
         printed lines as the reference (gru4rec.py:515-664).
         '''
+        offset_sessions = self._index_items(data)
+        plan = self._plan_training(data, offset_sessions, sample_store, store_type)
+        for _ in self._epochs(plan):
+            pass
+
+    def _index_items(self, data):
+        '''fit()'s preamble: the id map in order of first appearance, the item index column, fresh weights; returns the session offsets'''
         self.predict = None
         self.error_during_train = False
+        self._host_state = None
         # id map in order of first appearance, item index column, supports -- one factorize + one bincount (same values as the
         # reference's unique() / Series lookup / groupby().size() chain, gru4rec.py:534-545)
         codes, itemids = pd.factorize(data[self.item_key].values)
@@ -365,11 +378,20 @@ class GRU4Rec:
         self.n_items = len(itemids)
         self.itemidmap = pd.Series(data=np.arange(self.n_items), index=itemids, name='ItemIdx')
         data['ItemIdx'] = codes.astype(np.int64)
-        offset_sessions = self.init(data)
+        return self.init(data)
+
+    def _plan_training(self, data, offset_sessions, sample_store, store_type, build=None, restore=None, absent_logq=None):
+        '''Everything between the item index and the epoch loop (gru4rec.py:539-585): sampling CDF and logQ support from `data`,
+        the sample-store decision and its printed lines, the training engine -- from build(store size in ids), by default a new
+        engine with the host weights -- and its first sample store.  `restore`: a checkpoint whose tensors, sample store and
+        training state the engine takes over instead of drawing a store.  `absent_logq`: logQ support given to items that do
+        not occur in `data` (fit_more; in fit() every item occurs).'''
         pop = pd.Series(np.bincount(data['ItemIdx'].values, minlength=self.n_items), index=self.itemidmap.index.values)
         P0 = None
         if self.logq:
             P0 = pop[self.itemidmap.index.values].values.astype(np.float32)
+            if absent_logq is not None:
+                P0[P0 == 0] = absent_logq
         generate_length = 0
         use_store = False
         if self.n_sample:
@@ -414,49 +436,72 @@ class GRU4Rec:
             raise NotImplementedError("store_type='cpu' is not available for multi-GPU training; use the device sample store")
         # the training engine carries no scoring lanes: the step scratch keeps the leading dimension of the mini-batch
         # (the scoring engine with `eval_lanes` lanes is created on the first evaluate_gpu / predict_next_batch call)
-        eng = self._build_engine(sample_store=(sample_store if use_store else (2 * self.n_sample if per_step_sampling else 0)), eval_lanes=0,
-                                 keep_sessions=False)
+        n_store = sample_store if use_store else (2 * self.n_sample if per_step_sampling else 0)
+        eng = self._build_engine(sample_store=n_store, eval_lanes=0, keep_sessions=False) if build is None else build(n_store)
         if P0 is not None:
             eng.set_logq_support(P0)
         if use_store:
             eng.set_sampling_cdf(pop.astype(np.float32))
+        if restore is not None:
+            self._push_train_state(eng, restore)
+        if use_store:
             if store_type == 'gpu':
-                eng.generate_samples()
+                if restore is None:
+                    eng.generate_samples()
                 print('Created sample store with {} batches of samples (type=GPU)'.format(generate_length))
-            else:
+            elif restore is None:
                 eng.set_sample_store(self.generate_neg_samples(pop, generate_length))
         # first event time of every session = the time at its offset (the frame is sorted by session, time) -- gru4rec.py:585
         base_order = np.argsort(data[self.time_key].values[offset_sessions[:-1]]) if self.time_sort else np.arange(len(offset_sessions) - 1)
-        data_items = data.ItemIdx.values
+        return SimpleNamespace(eng=eng, pop=pop, generate_length=generate_length, use_store=use_store, per_step_sampling=per_step_sampling,
+                               store_type=store_type, offset_sessions=offset_sessions, base_order=base_order,
+                               data_items=data.ItemIdx.values, world=world, rank=rank)
+
+    def _epochs(self, plan, epochs=None, every=None, resume=None):
+        '''The epoch loop of fit() (gru4rec.py:586-664) as a generator: it yields a progress record wherever a checkpoint may be
+        taken -- after every `every` mini-batches of an epoch (never, if None) and after each epoch's printed line.  A run
+        continued from such a record (`resume`, on an engine restored to that moment) goes on bit for bit.  A record holds the
+        epoch, the next step of its schedule, the costs of its steps so far (the epoch loss is one sum over all of them, so a
+        resumed run adds them up exactly as the uninterrupted one does) and its session order.'''
+        eng, world, rank = plan.eng, plan.world, plan.rank
+        offset_sessions = plan.offset_sessions
         # under torchrun: synchronous data parallelism, every rank trains a shard of the sessions
         sched = None
         n_sample_eff = self.n_sample
-        for epoch in range(self.n_epochs):
+        for epoch in (range(self.n_epochs) if epochs is None else epochs):
             t0 = time.time()
-            eng.reset_hidden()
-            session_idx_arr = np.random.permutation(len(offset_sessions) - 1) if self.train_random_order else base_order
+            if resume is not None and resume['step'] > 0:        # inside an epoch: hidden state and session order are the checkpoint's
+                session_idx_arr = resume['order'] if self.train_random_order else plan.base_order
+                done, costs = int(resume['step']), [np.asarray(resume['costs'], dtype=np.float32)]
+            else:
+                eng.reset_hidden()
+                session_idx_arr = np.random.permutation(len(offset_sessions) - 1) if self.train_random_order else plan.base_order
+                done, costs = 0, []
+            resume = None
             if sched is None or self.train_random_order:
                 n_steps = None
                 if world > 1:
                     import torch.distributed as dist
                     from .parallel import shard_sessions, common_steps
                     session_idx_arr = shard_sessions(session_idx_arr, rank, world)
-                sched = _lib.Schedule(data_items, offset_sessions, session_idx_arr, self.batch_size, n_sample_eff, mode=0)
+                sched = _lib.Schedule(plan.data_items, offset_sessions, session_idx_arr, self.batch_size, n_sample_eff, mode=0)
                 n_steps = sched.n_steps if world == 1 else common_steps(sched.n_steps, dist)
                 cc = sched.batch_sizes()[:n_steps].astype(np.float64)
             try:
-                if per_step_sampling:
-                    c = self._train_epoch_per_step_samples(eng, sched, pop)
-                elif use_store and store_type == 'cpu':
-                    c = self._train_epoch_cpu_store(eng, sched, pop, generate_length)
-                else:
-                    c = eng.train_steps(sched, 0, n_steps)
+                while True:
+                    n = n_steps - done if every is None else min(every, n_steps - done)
+                    costs.append(self._train_range(plan, sched, done, n))
+                    done += n
+                    if done >= n_steps:
+                        break
+                    yield dict(epoch=epoch, step=done, costs=np.concatenate(costs), order=session_idx_arr)
             except _lib.NaNError:
                 print(str(epoch) + ': NaN error!')
                 self.error_during_train = True
                 if world > 1:      # the peers find out at their next exchange (time-out -> RuntimeError); nothing collective here
                     self._engine.close(); self._engine = None; self._host = None
                 return
+            c = costs[0] if len(costs) == 1 else np.concatenate(costs)
             sum_c, sum_e, n_mb = np.sum(c * cc), np.sum(cc), len(c)
             if world > 1:
                 # one epoch line for the whole job: event-weighted loss, mini-batches and events of all ranks
@@ -470,8 +515,253 @@ class GRU4Rec:
             t1 = time.time()
             dt = t1 - t0
             print('Epoch{} --> loss: {:.6f} \t({:.2f}s) \t[{:.2f} mb/s | {:.0f} e/s]'.format(epoch + 1, avgc, dt, n_mb / dt, sum_e / dt))
+            yield dict(epoch=epoch + 1, step=0, costs=np.zeros(0, np.float32), order=None)
         if world > 1:
             self._release_multi_gpu_engine()
+
+    def _train_range(self, plan, sched, first, n):
+        '''costs of mini-batches [first, first + n) of the epoch's schedule, with the plan's sampler'''
+        if plan.per_step_sampling:
+            return self._train_epoch_per_step_samples(plan.eng, sched, plan.pop, first, n)
+        if plan.use_store and plan.store_type == 'cpu':
+            return self._train_epoch_cpu_store(plan.eng, sched, plan.pop, plan.generate_length, first, n)
+        return plan.eng.train_steps(sched, first, n)
+
+    # ---- continuing a trained model (additions to the reference surface; DESIGN §3i) ----
+    _CKPT_VERSION = 1
+
+    def _ctor_params(self):
+        keys = ('loss', 'final_act', 'hidden_act', 'layers', 'n_epochs', 'batch_size', 'dropout_p_hidden', 'dropout_p_embed', 'learning_rate',
+                'momentum', 'lmbd', 'embedding', 'n_sample', 'sample_alpha', 'smoothing', 'constrained_embedding', 'adapt', 'adapt_params',
+                'grad_cap', 'bpreg', 'logq', 'sigma', 'init_as_normal', 'train_random_order', 'time_sort', 'session_key', 'item_key', 'time_key')
+        as_json = lambda v: v.item() if isinstance(v, np.generic) else ([as_json(x) for x in v] if isinstance(v, (list, tuple)) else v)
+        return {k: as_json(getattr(self, k)) for k in keys}
+
+    def _state_names(self):
+        '''optimizer-state tensors and training hidden states, as the engine names them'''
+        slots = {None: (), 'adagrad': ('acc',), 'rmsprop': ('acc',), 'adadelta': ('acc', 'upd'), 'adam': ('acc', 'meang', 'countt')}[self.adapt]
+        slots = slots + (('vel',) if self.momentum > 0 else ())
+        return ['%s.%s' % (n, s) for n in self._param_names() for s in slots] + ['H%d' % i for i in range(len(self.layers))]
+
+    def _has_train_state(self):
+        return (self._engine is not None and getattr(self, '_engine_training', False)) or getattr(self, '_host_state', None) is not None
+
+    def _pull_train_state(self):
+        '''the training state of the live training engine as host arrays, or the one load_checkpoint() left; None if there is none'''
+        eng = self._engine
+        if eng is None or not getattr(self, '_engine_training', False):
+            return getattr(self, '_host_state', None)
+        rows = eng.sample_store_rows()
+        return dict(tensors={n: eng.get(n) for n in self._state_names()}, blob=eng.train_state_export(),
+                    store=eng.get_sample_store().astype(np.int32) if rows > 0 else None,
+                    sample_store=int(eng.cfg.sample_store))
+
+    def _push_train_state(self, eng, st):
+        for name in self._param_names():
+            if name in st.get('params', {}):
+                eng.set(name, st['params'][name])
+        for name, a in st['tensors'].items():
+            eng.set(name, a)
+        if st['store'] is not None:
+            eng.set_sample_store(st['store'])
+        eng.train_state_import(st['blob'])
+
+    def save_checkpoint(self, path, _progress=None, _fingerprint=None):
+        '''
+        Writes everything needed to continue training this model to one .npz file (arrays and one JSON string; no pickle): the
+        constructor parameters, the item id map, all parameters and -- when the model holds a training engine (after fit(),
+        fit_more(), inside fit_resumable()) or came from load_checkpoint() -- all optimizer state, the training hidden state, the
+        sample store and the engine's training state.  The file is written under a temporary name and moved into place.
+        savemodel() pickles are unaffected (weights only, reference-compatible).
+        '''
+        st = self._pull_train_state()
+        ids = np.asarray(self.itemidmap.index.values)
+        ids_are_objects = ids.dtype.kind not in 'iufUS'          # item ids read as str: stored as a fixed-width string array
+        meta = dict(version=self._CKPT_VERSION, params=self._ctor_params(), n_items=int(self.n_items), ids_are_objects=bool(ids_are_objects),
+                    engine=dict(dropout_seed=int(self.dropout_seed), step_mode=int(self.step_mode)),
+                    has_state=st is not None, sample_store=None if st is None else st['sample_store'], has_store=st is not None and st['store'] is not None,
+                    fingerprint=_fingerprint, progress=None)
+        arrays = {'itemids': ids.astype(str) if ids_are_objects else ids}
+        host = self._host if self._engine is None else self._pull_host()
+        arrays.update({'param/' + n: host[n] for n in self._param_names()})
+        if st is not None:
+            arrays.update({'state/' + n: a for n, a in st['tensors'].items()})
+            arrays['blob'] = st['blob']
+            if st['store'] is not None:
+                arrays['sample_store'] = st['store']
+        if _progress is not None:
+            meta['progress'] = dict(epoch=int(_progress['epoch']), step=int(_progress['step']), has_order=_progress['order'] is not None)
+            arrays['epoch_costs'] = _progress['costs']
+            if _progress['order'] is not None:
+                arrays['epoch_order'] = np.asarray(_progress['order'], dtype=np.int64)
+            rng = np.random.get_state()
+            meta['rng'] = [rng[0], int(rng[2]), int(rng[3]), float(rng[4])]
+            arrays['rng_keys'] = rng[1]
+        arrays['meta'] = np.array(json.dumps(meta))
+        tmp = '%s.tmp.%d' % (path, os.getpid())
+        try:
+            with open(tmp, 'wb') as f:
+                np.savez(f, **arrays)
+                f.flush()
+                os.fsync(f.fileno())
+            os.replace(tmp, path)
+        finally:
+            if os.path.exists(tmp):
+                os.remove(tmp)
+
+    @staticmethod
+    def _read_checkpoint(path):
+        with np.load(path, allow_pickle=False) as z:
+            meta = json.loads(str(z['meta']))
+            if meta.get('version') != GRU4Rec._CKPT_VERSION:
+                raise ValueError('%s: checkpoint version %r, this build reads version %d' % (path, meta.get('version'), GRU4Rec._CKPT_VERSION))
+            ck = dict(meta=meta, itemids=z['itemids'], params={k[6:]: z[k] for k in z.files if k.startswith('param/')},
+                      tensors={k[6:]: z[k] for k in z.files if k.startswith('state/')},
+                      blob=z['blob'] if 'blob' in z.files else None, store=z['sample_store'] if 'sample_store' in z.files else None,
+                      sample_store=meta['sample_store'])
+            if meta['progress'] is not None:
+                ck['progress'] = dict(epoch=meta['progress']['epoch'], step=meta['progress']['step'], costs=z['epoch_costs'],
+                                      order=z['epoch_order'] if meta['progress']['has_order'] else None)
+                r = meta['rng']
+                ck['rng'] = (r[0], z['rng_keys'], r[1], r[2], r[3])
+        return ck
+
+    @classmethod
+    def load_checkpoint(cls, path):
+        '''The model save_checkpoint() wrote: parameters for scoring at once, and -- if the file holds them -- optimizer state,
+        hidden state, sample store and training state, which fit_more() continues from.'''
+        ck = cls._read_checkpoint(path)
+        meta = ck['meta']
+        gru = cls(**meta['params'])
+        gru.dropout_seed, gru.step_mode = meta['engine']['dropout_seed'], meta['engine']['step_mode']
+        ids = ck['itemids'].astype(object) if meta['ids_are_objects'] else ck['itemids']
+        gru.predict = None
+        gru.error_during_train = False
+        gru._host_state = dict(tensors=ck['tensors'], blob=ck['blob'], store=ck['store'], sample_store=ck['sample_store']) if meta['has_state'] else None
+        gru.n_items = int(meta['n_items'])
+        gru.itemidmap = pd.Series(data=np.arange(gru.n_items), index=ids, name='ItemIdx')
+        gru._host = {n: (a.reshape(-1) if n.startswith('Bh') else a) for n, a in ck['params'].items()}
+        gru._bind_params()
+        return gru
+
+    def _data_fingerprint(self, data, sample_store, store_type, params):
+        '''what a checkpoint of fit_resumable() must agree with to be continued: the data (events, items, a hash of the item index
+        column of the sorted frame), the sample-store arguments and the constructor parameters the run started with'''
+        return dict(n_events=int(len(data)), n_items=int(self.n_items), items_sha256=hashlib.sha256(np.ascontiguousarray(data['ItemIdx'].values, dtype=np.int64).tobytes()).hexdigest(),
+                    sample_store=int(sample_store), store_type=store_type, params=params)
+
+    def fit_resumable(self, data, path, every_steps, sample_store=10000000, store_type='gpu', on_checkpoint=None):
+        '''
+        fit() that survives an interruption: the same loop, with a checkpoint (save_checkpoint's format, plus the progress of the
+        run and NumPy's random state) written to `path` after every `every_steps` mini-batches of an epoch and after every epoch.
+        If `path` exists and was written for the same data, sample-store arguments and constructor parameters, training continues
+        from it, and the finished run equals an uninterrupted fit() bit for bit -- weights, optimizer state and the epoch loss
+        lines; otherwise a warning is printed and training starts anew.  `on_checkpoint(epoch, step)`, if given, is called after
+        each checkpoint is in place.  Single GPU only.
+        '''
+        if self._world()[0] > 1:
+            raise NotImplementedError('fit_resumable() runs on one GPU; checkpoints of a multi-GPU run are not implemented')
+        every_steps = int(every_steps)
+        if every_steps < 1:
+            raise ValueError('every_steps must be at least 1, got %d' % every_steps)
+        params = self._ctor_params()
+        ck = self._read_checkpoint(path) if os.path.exists(path) else None
+        offset_sessions = self._index_items(data)
+        fingerprint = self._data_fingerprint(data, sample_store, store_type, params)
+        if ck is not None and (ck['meta']['fingerprint'] != fingerprint or ck.get('progress') is None or not ck['meta']['has_state']):
+            print('WARNING: checkpoint {} was written for other data or parameters; starting a new run'.format(path))
+            ck = None
+        plan = self._plan_training(data, offset_sessions, sample_store, store_type, restore=ck)
+        resume = None
+        if ck is not None:
+            resume = ck['progress']
+            np.random.set_state(ck['rng'])
+            print('Resuming from checkpoint {} (epoch {}, mini-batch {})'.format(path, resume['epoch'] + 1, resume['step']))
+        for prog in self._epochs(plan, epochs=range(resume['epoch'] if resume else 0, self.n_epochs), every=every_steps, resume=resume):
+            self.save_checkpoint(path, _progress=prog, _fingerprint=fingerprint)
+            if on_checkpoint is not None:
+                on_checkpoint(prog['epoch'], prog['step'])
+
+    def _init_rows(self, rs, shape):
+        '''init_matrix's rule (sigma, init_as_normal) for a matrix of `shape`, drawn from the RandomState `rs`'''
+        sigma = self.sigma if self.sigma != 0 else np.sqrt(6.0 / (shape[0] + shape[1]))
+        if self.init_as_normal:
+            return np.asarray(rs.randn(*shape) * sigma, dtype=np.float32)
+        return np.asarray(rs.rand(*shape) * sigma * 2 - sigma, dtype=np.float32)
+
+    def fit_more(self, data, n_epochs=None, sample_store=10000000, store_type='gpu'):
+        '''
+        Continues training the current model (after fit(), fit_resumable(), load_checkpoint() or loadmodel()) on `data` for
+        n_epochs epochs (default: self.n_epochs), through fit()'s loop and with its printed lines.
+
+        Items of `data` that the model does not know are appended to the item id map in order of first appearance; existing
+        indices never move, so session histories, candidate lists and saved models stay valid.  Their rows of Wy and of E / Wx0
+        are drawn by init_matrix's rule for a matrix of the new rows' shape from RandomState(42 + number of items before); their
+        By and all their optimizer state are zero.  All other optimizer state is kept if the model has any (a live training
+        engine, or load_checkpoint()) and starts from zero if not (loadmodel(), or a scoring engine has replaced the training
+        engine); one printed line says which.  The sampling distribution is recomputed from `data` over the grown catalogue: an
+        item absent from `data` is never a target or a sample (its logQ support is set to 1, so that its correction is zero).
+        The sample store is drawn anew from the continuing random streams, the dropout step counter continues, and the session
+        store of recommend_sessions survives.  Single GPU only.
+        '''
+        if self._world()[0] > 1:
+            raise NotImplementedError('fit_more() runs on one GPU; growing a row-sharded model is not implemented')
+        if getattr(self, 'itemidmap', None) is None or (self._engine is None and self._host is None):
+            raise RuntimeError('fit_more() continues a trained model: call fit(), load_checkpoint() or loadmodel() first')
+        self.predict = None
+        self.error_during_train = False
+        ids = data[self.item_key].values
+        known = self.itemidmap.index.get_indexer(ids) >= 0
+        new_ids = pd.unique(ids[~known])
+        n_old, n_add = int(self.n_items), len(new_ids)
+        # the model as a training engine of its present size: the live one, or one built from the host copy (+ checkpoint state)
+        kept = self._has_train_state()
+        if self._engine is None or not getattr(self, '_engine_training', False):
+            st = getattr(self, '_host_state', None)
+            eng = self._build_engine(sample_store=st['sample_store'] if st else 0, eval_lanes=0, single=True)
+            if st is not None:
+                self._push_train_state(eng, st)
+            self._host_state = None
+        print('Optimizer state kept' if kept else 'No optimizer state to keep: it starts from zero')
+        rows = {}
+        if n_add:
+            rs = np.random.RandomState(42 + n_old)
+            if self.embedding and not self.constrained_embedding:
+                rows['new_in'] = self._init_rows(rs, (n_add, self.embedding))
+            elif not self.constrained_embedding:
+                rows['new_in'] = np.hstack([self._init_rows(rs, (n_add, self.layers[0])) for _ in range(3)])
+            rows['new_Wy'] = self._init_rows(rs, (n_add, self.layers[-1]))
+            self.itemidmap = pd.Series(data=np.arange(n_old + n_add), index=np.concatenate([self.itemidmap.index.values, new_ids]), name='ItemIdx')
+            self.n_items = n_old + n_add
+            print('Added {} new items to the catalogue ({} items)'.format(n_add, self.n_items))
+        data['ItemIdx'] = self.itemidmap.index.get_indexer(ids).astype(np.int64)
+        datatools.sort_if_needed(data, [self.session_key, self.time_key])
+        offset_sessions = datatools.compute_offset(data, self.session_key)
+        plan = self._plan_training(data, offset_sessions, sample_store, store_type, build=lambda n_store: self._grow_engine(n_store, rows),
+                                   absent_logq=1.0)
+        for _ in self._epochs(plan, epochs=range(self.n_epochs if n_epochs is None else int(n_epochs))):
+            pass
+
+    def _grow_engine(self, n_store, rows):
+        '''the training engine for the catalogue as it is now, holding everything the present engine holds (fit_more)'''
+        old = self._engine
+        if int(old.cfg.n_items) == self.n_items and int(old.cfg.sample_store) == int(n_store):
+            return old
+        sessions = (old.session_capacity, old.sessions_export()) if getattr(old, 'session_capacity', None) is not None else None
+        eng = _lib.Engine(self._make_config(n_store, 0, True, single=True), device=self.device)
+        eng.copy_item_tables(old, **rows)
+        if int(old.cfg.sample_store):      # (an engine built only to hold a loaded model has no streams to continue)
+            try:
+                eng.train_state_import(old.train_state_export())
+            except NotImplementedError:
+                print('The sample store changes size: the sample streams and the dropout step counter start anew')
+        old.close()
+        if sessions is not None:
+            eng.sessions_open(sessions[0])
+            eng.sessions_import(*sessions[1])
+        self._engine, self._engine_eval_lanes, self._engine_training, self._host = eng, 0, True, None
+        self._bind_params()
+        return eng
 
     def _release_multi_gpu_engine(self):
         """End of a multi-GPU fit(): every rank assembles the full parameter set on the host (the item tables are row-sharded
@@ -487,22 +777,22 @@ class GRU4Rec:
         self._engine = None
         self._host = host
 
-    def _train_epoch_cpu_store(self, eng, sched, pop, generate_length):
+    def _train_epoch_cpu_store(self, eng, sched, pop, generate_length, first=0, n=None):
         """store_type='cpu' (legacy, gru4rec.py:605-614): samples are drawn by NumPy on the host, one store at a time."""
-        costs = []
-        done = 0
-        while done < sched.n_steps:
+        costs = [np.zeros(0, np.float32)]
+        done, end = first, sched.n_steps if n is None else first + n
+        while done < end:
             if eng.get_sample_pointer() >= generate_length:
                 eng.set_sample_store(self.generate_neg_samples(pop, generate_length))
-            n = min(sched.n_steps - done, generate_length - eng.get_sample_pointer())
+            n = min(end - done, generate_length - eng.get_sample_pointer())
             costs.append(eng.train_steps(sched, done, n))
             done += n
         return np.concatenate(costs)
 
-    def _train_epoch_per_step_samples(self, eng, sched, pop):
+    def _train_epoch_per_step_samples(self, eng, sched, pop, first=0, n=None):
         """store_type='cpu' without a store (gru4rec.py:612-613): one host draw of n_sample items per mini-batch."""
-        costs = []
-        for k in range(sched.n_steps):
+        costs = [np.zeros(0, np.float32)]
+        for k in range(first, sched.n_steps if n is None else first + n):
             row = np.asarray(self.generate_neg_samples(pop, 1)).reshape(1, self.n_sample)
             eng.set_sample_store(np.vstack([row, row]))
             eng.set_sample_pointer(0)
@@ -749,7 +1039,7 @@ class GRU4Rec:
         st['final_activation'] = self._act_object(self.final_act)
         st['hidden_activation'] = self._act_object(self.hidden_act)
         for k in ('device', 'dropout_seed', 'eval_lanes', 'step_mode', 'session_capacity', '_engine_eval_lanes', 'predict', 'predict_batch',
-                  'current_session', '_seen', '_seen_n'):
+                  'current_session', '_seen', '_seen_n', '_engine_training', '_host_state'):
             st.pop(k, None)
         st['predict'] = None
         return st

@@ -92,7 +92,8 @@ const char* g4r_last_error(const g4r_handle* h);   /* h may be NULL: last creati
 void* g4r_stream(g4r_handle* h);
 
 /* ---- parameters: shared-variable get_value/set_value (gru4rec.py:745-767, 590, 649-651) ----------- */
-/* names: "Wx0".."Wx7","Wh*","Wrz*","Bh*","H*","Wy","By","E", and optimizer state "<name>.acc", "<name>.vel". */
+/* names: "Wx0".."Wx7","Wh*","Wrz*","Bh*","H*","Wy","By","E", and optimizer state "<name>.acc" (adagrad / rmsprop / adadelta /
+ * adam), "<name>.upd" (adadelta), "<name>.meang" and "<name>.countt" (adam), "<name>.vel" (momentum > 0). */
 int g4r_tensor_shape(g4r_handle* h, const char* name, int64_t* rows, int64_t* cols);
 int g4r_set_tensor(g4r_handle* h, const char* name, const float* host, int64_t rows, int64_t cols);
 int g4r_get_tensor(g4r_handle* h, const char* name, float* host, int64_t rows, int64_t cols);
@@ -176,6 +177,29 @@ int g4r_persistent_stamps(g4r_handle* h, int32_t enable, unsigned long long* out
 int g4r_phase_count(void);
 /* Counters for bench.py: kernels launched by this handle so far. */
 int64_t g4r_kernel_launches(const g4r_handle* h);
+
+/* ---- training state: checkpoint / resume and catalogue growth (DESIGN §3i; no reference counterpart) -----------------------
+ * A training handle consists of its named tensors (parameters, optimizer state "<name>.acc" / ".upd" / ".meang" / ".countt" /
+ * ".vel", the hidden state "H<l>": g4r_get_tensor / g4r_set_tensor), the sample store (g4r_get_sample_store /
+ * g4r_set_sample_store) and the state these three functions move as one versioned blob: the global step that keys the dropout
+ * masks, the sample pointer, and the MRG31k3p base and stream states.  A handle that receives all of them continues the run of
+ * the handle they came from bit for bit.  The blob names the n_sample, sample-store rows, seeds and world / rank it is valid
+ * for.  g4r_train_state_import checks magic, version, size and those fields before it changes anything: G4R_ERR_INVALID leaves
+ * the handle as it was.  Call it after g4r_set_sample_store (which rewinds the sample pointer).  G4R_ERR_STATE on a multi-GPU
+ * handle. */
+int g4r_train_state_bytes(g4r_handle* h, size_t* bytes);
+int g4r_train_state_export(g4r_handle* h, void* host, size_t bytes);
+int g4r_train_state_import(g4r_handle* h, const void* host, size_t bytes);
+/* Catalogue growth: a handle keeps its n_items, so a model takes in new items by moving to a new handle.  Copies, device to
+ * device, every parameter, optimizer-state tensor and training hidden state of `src` into `dst`, whose n_items is >= src's.
+ * Item tables (Wy, By, E, and Wx0 of a model without embedding) and each of their state tensors keep rows 0 .. n_old-1 as
+ * they are; rows n_old .. n_new-1 of the weights come from new_Wy [n_new - n_old x L_last], new_By [n_new - n_old] and new_in
+ * (the new rows of E, or of Wx0 without embedding: [n_new - n_old x embedding | 3 L_0]; ignored with constrained_embedding),
+ * row-major host blocks, NULL = zero; the new rows of every state tensor are zero.  The handles must be single-GPU, on one
+ * device, and agree in layers, batch size, embedding mode, optimizer and whether momentum is on (everything that shapes a
+ * copied tensor), else G4R_ERR_INVALID before anything is written.  Nothing else moves: sampling tables, sample store and the
+ * training-state blob are the caller's to set. */
+int g4r_copy_item_tables(g4r_handle* dst, g4r_handle* src, const float* new_Wy, const float* new_By, const float* new_in);
 
 /* ---- multi-GPU (one process per GPU; SURVEY section 8e) -------------------------------------------------------
  * Handles created with world_size > 1 compute gradients only; g4r_train_steps then exchanges them over NCCL

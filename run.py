@@ -21,6 +21,9 @@ _OPTIONS = [
                                        help='Python file defining an OrderedDict named `gru4rec_params`. Exclusive with -ps and -l.')),
     (('-l', '--load_model'), dict(action='store_true', help='Load a trained model from PATH instead of training. Exclusive with -ps and -pf.')),
     (('-s', '--save_model'), dict(metavar='MODEL_PATH', type=str, help='Save the trained model to MODEL_PATH.')),
+    (('--load_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Load the model, with its optimizer and training state, from a checkpoint written by --save_checkpoint. Exclusive with -ps, -pf and -l.')),
+    (('--save_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Save the model with its optimizer and training state to CKPT_PATH (.npz), so that a later run can train it further.')),
+    (('--fit_more',), dict(action='store_true', help='With --load_checkpoint: continue training the loaded model on the training data PATH (new items are added to the catalogue) instead of building a new model.')),
     (('-t', '--test'), dict(metavar='TEST_PATH', type=str, nargs='+', help='Test data set(s).')),
     (('-m', '--measure'), dict(metavar='AT', type=int, nargs='+', default=[20], help='Recommendation list length(s) for recall & MRR (default: 20).')),
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
@@ -103,10 +106,29 @@ def _train(model_class, args):
     started = time.time()
     gru.fit(frame, sample_store=args.sample_store_size, store_type=store_type)
     print('Total training time: {:.2f}s'.format(time.time() - started))
-    if args.save_model is not None and getattr(args, 'rank', 0) == 0:
+    _save(gru, args)
+    return gru
+
+
+def _save(gru, args):
+    if getattr(args, 'rank', 0) != 0:
+        return
+    if args.save_model is not None:
         print('Saving trained model to: {}'.format(args.save_model))
         gru.savemodel(args.save_model)
-    return gru
+    if args.save_checkpoint is not None:
+        print('Saving checkpoint to: {}'.format(args.save_checkpoint))
+        gru.save_checkpoint(args.save_checkpoint)
+
+
+def _train_more(gru, args):
+    print('Loading training data...')
+    frame = load_data(args.path, args)
+    print('Started training')
+    started = time.time()
+    gru.fit_more(frame, sample_store=args.sample_store_size, store_type='cpu' if args.sample_store_on_cpu else 'gpu')
+    print('Total training time: {:.2f}s'.format(time.time() - started))
+    _save(gru, args)
 
 
 def _evaluate(gru, evaluation, args):
@@ -155,10 +177,18 @@ def main(argv=None):
     args.rank = rank
     model_class = importlib.import_module(args.gru4rec_model).GRU4Rec
     import evaluation
-    chosen = [args.parameter_string is not None, args.parameter_file is not None, bool(args.load_model)]
+    chosen = [args.parameter_string is not None, args.parameter_file is not None, bool(args.load_model), args.load_checkpoint is not None]
     if sum(chosen) != 1:
-        _abort('ERROR. Exactly one of the following parameters must be provided: --parameter_string, --parameter_file, --load_model')
-    if args.load_model:
+        _abort('ERROR. Exactly one of the following parameters must be provided: --parameter_string, --parameter_file, --load_model'
+               + (', --load_checkpoint' if args.load_checkpoint is not None or args.fit_more else ''))
+    if args.fit_more and args.load_checkpoint is None:
+        _abort('ERROR. --fit_more continues the model of --load_checkpoint')
+    if args.load_checkpoint is not None:
+        print('Loading checkpoint from file: {}'.format(args.load_checkpoint))
+        gru = model_class.load_checkpoint(args.load_checkpoint)
+        if args.fit_more:
+            _train_more(gru, args)
+    elif args.load_model:
         print('Loading trained model from file: {}'.format(args.path))
         gru = model_class.loadmodel(args.path)
     else:
