@@ -48,6 +48,8 @@ EXPORTS = [
     'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
     'g4r_sessions_export', 'g4r_sessions_import',
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
+    'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
+    'g4r_bl_rows_import', 'g4r_bl_evaluate',
 ]
 
 _lib = None
@@ -132,6 +134,14 @@ def load():
     lib.g4r_train_state_export.argtypes = [vp, vp, C.c_size_t]
     lib.g4r_train_state_import.argtypes = [vp, vp, C.c_size_t]
     lib.g4r_copy_item_tables.argtypes = [vp, vp, vp, vp, vp]
+    lib.g4r_bl_create.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
+    lib.g4r_bl_destroy.argtypes = [vp]
+    lib.g4r_bl_last_error.argtypes = [vp]; lib.g4r_bl_last_error.restype = C.c_char_p
+    lib.g4r_bl_knn_fit.argtypes = [vp, vp, i64, vp, i64, vp, vp, C.POINTER(i64), C.POINTER(C.c_size_t), C.POINTER(C.c_float)]
+    lib.g4r_bl_set_pop.argtypes = [vp, vp, i64]
+    lib.g4r_bl_rows_export.argtypes = [vp, vp, vp, vp]
+    lib.g4r_bl_rows_import.argtypes = [vp, vp, vp, vp]
+    lib.g4r_bl_evaluate.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, i32, i32, vp, vp, C.POINTER(i64), vp, vp, vp]
     _lib = lib
     return lib
 
@@ -722,3 +732,91 @@ class Engine(object):
         if off is not None and off.size != keys.size + 1:
             raise ValueError('hist_off must have %d entries' % (keys.size + 1))
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
+
+
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2}
+
+
+class Baselines(object):
+    """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
+    a baseline.  kind: 'pop', 'sessionpop' or 'itemknn'; n_keep: top_n or n_sims."""
+
+    def __init__(self, kind, n_items, n_keep, device=0):
+        lib = load()
+        self.lib = lib
+        self.kind, self.n_items, self.n_keep = kind, int(n_items), int(n_keep)
+        h = C.c_void_p()
+        rc = lib.g4r_bl_create(BASELINE_KINDS[kind], self.n_items, self.n_keep, device, C.byref(h))
+        if rc != 0:
+            msg = lib.g4r_bl_last_error(None).decode()
+            raise (ValueError if rc == G4R_ERR_INVALID else RuntimeError)('g4r_bl_create: ' + msg)
+        self.h = h
+
+    def close(self):
+        if getattr(self, 'h', None):
+            self.lib.g4r_bl_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, rc):
+        if rc == 0:
+            return
+        msg = self.lib.g4r_bl_last_error(self.h).decode()
+        if rc == G4R_ERR_INDEX:
+            raise IndexError(msg)
+        if rc == G4R_ERR_INVALID:
+            raise ValueError(msg)
+        raise RuntimeError('libg4r: %s (status %d)' % (msg, rc))
+
+    def knn_fit(self, session_offsets, items, a, b):
+        """ItemKNN rows from the training events (session CSR of item indices) and the norm factors; returns
+        (pair work, scratch bytes, fit kernel ms)"""
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        a = np.ascontiguousarray(a, dtype=np.float64); b = np.ascontiguousarray(b, dtype=np.float64)
+        if a.size != self.n_items or b.size != self.n_items:
+            raise ValueError('a and b need n_items entries')
+        pw, sb, ms = C.c_int64(), C.c_size_t(), C.c_float()
+        self._check(self.lib.g4r_bl_knn_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(a), _ptr(b), C.byref(pw), C.byref(sb), C.byref(ms)))
+        return pw.value, sb.value, ms.value
+
+    def set_pop(self, scores):
+        sc = np.ascontiguousarray(scores, dtype=np.float64)
+        self._check(self.lib.g4r_bl_set_pop(self.h, _ptr(sc), sc.size))
+
+    def rows_export(self):
+        """(idx int32 [n_items, n_keep], sim float64 [n_items, n_keep], len int32 [n_items])"""
+        idx = np.empty((self.n_items, self.n_keep), np.int32); sim = np.empty((self.n_items, self.n_keep), np.float64)
+        ln = np.empty(self.n_items, np.int32)
+        self._check(self.lib.g4r_bl_rows_export(self.h, _ptr(idx), _ptr(sim), _ptr(ln)))
+        return idx, sim, ln
+
+    def rows_import(self, idx, sim, ln):
+        idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int32).reshape(self.n_items, self.n_keep))
+        sim = np.ascontiguousarray(np.asarray(sim, dtype=np.float64).reshape(self.n_items, self.n_keep))
+        ln = np.ascontiguousarray(ln, dtype=np.int32)
+        if ln.size != self.n_items:
+            raise ValueError('len needs n_items entries')
+        self._check(self.lib.g4r_bl_rows_import(self.h, _ptr(idx), _ptr(sim), _ptr(ln)))
+
+    def evaluate(self, items, session_offsets, n_history, cut_off, mode, cand=None, exclude_seen=False, k=0, counts=True):
+        """(recall sums, mrr sums, n_counted, counts int32 [n, 2] or None, items int32 [n, k] or None, scores float64 [n, k] or
+        None), events in data order (g4r_bl_evaluate)"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        cut = np.ascontiguousarray(cut_off, dtype=np.int32)
+        cd = None if cand is None else np.ascontiguousarray(cand, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        rec = np.zeros(len(cut)); mrr = np.zeros(len(cut)); nc = C.c_int64()
+        cnt = np.empty((n, 2), np.int32) if counts else None
+        ti = np.empty((n, k), np.int32) if k else None
+        ts = np.empty((n, k), np.float64) if k else None
+        self._check(self.lib.g4r_bl_evaluate(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), int(mode), _ptr(cut), cut.size,
+                                             _ptr(cd), 0 if cd is None else cd.size, 1 if exclude_seen else 0, int(k),
+                                             _ptr(rec), _ptr(mrr), C.byref(nc), _ptr(cnt), _ptr(ti), _ptr(ts)))
+        return rec, mrr, nc.value, cnt, ti, ts

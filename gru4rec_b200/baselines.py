@@ -1,0 +1,174 @@
+"""Session baselines of the reference (baselines.py:52-301): Pop, SessionPop and ItemKNN, with its constructor signatures,
+fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids).  ItemKNN's fit runs on the device (the co-occurrence
+counts, the normalisation and the top n_sims per row, DESIGN §3j); evaluate_gpu / evaluate_events rank every test event of a
+baseline on the device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted rows.
+RandomPred and BPR are not provided: the first has nothing to accelerate, the second is sequential SGD on global random draws."""
+import numpy as np
+import pandas as pd
+
+from . import _lib
+from .gru4rec import GRU4Rec as _GRU4Rec
+
+
+class Baseline(object):
+    """What the baselines share: the item index (ids in unique() order, as GRU4Rec builds it), the device handle (created on
+    first use, never pickled) and the evaluation hooks of evaluation.py."""
+    error_during_train = False
+    _kind = None
+    _world = staticmethod(_GRU4Rec._world)
+
+    def _index(self, data):
+        """itemidmap / n_items from the training data; returns the item index of every row"""
+        ids = data[self.item_key].values
+        itemids = pd.unique(ids)
+        self.n_items = len(itemids)
+        self.itemidmap = pd.Series(data=np.arange(self.n_items), index=itemids)
+        return pd.Index(itemids).get_indexer(ids)
+
+    def _n_keep(self):
+        raise NotImplementedError
+
+    def _upload(self, dev):
+        raise NotImplementedError
+
+    def _device(self):
+        dev = self.__dict__.get('_dev')
+        if dev is None:
+            dev = _lib.Baselines(self._kind, self.n_items, self._n_keep())
+            self._upload(dev)
+            self._dev = dev
+        return dev
+
+    def __getstate__(self):
+        state = self.__dict__.copy()
+        state.pop('_dev', None)
+        return state
+
+
+def _pop_scores(model, data):
+    """(dense scores [n_items] float64, 0 past top_n) of Pop / SessionPop: supp / (supp + 1) of the top_n items by (score desc,
+    index asc); supp counts the events of an item, or with support_by_key the distinct values of that column"""
+    model._index(data)
+    grp = data.groupby(model.item_key)
+    supp = grp.size() if model.support_by_key is None else grp[model.support_by_key].nunique()
+    supp = supp.reindex(model.itemidmap.index).values.astype(np.int64)
+    score = supp / (supp + 1)
+    keep = np.lexsort((np.arange(model.n_items), -score))[:model.top_n]
+    dense = np.zeros(model.n_items)
+    dense[keep] = score[keep]
+    model.pop_list = pd.Series(data=score[keep], index=model.itemidmap.index.values[keep])
+    return dense
+
+
+class Pop(Baseline):
+    '''
+    Pop(top_n=100, item_key='ItemId', support_by_key=None)
+
+    Popularity predictor (baselines.py:52-118): the score of an item is supp / (supp + 1) for the top_n items by support and 0
+    for the rest.  supp counts the events of the item, or with support_by_key the distinct values of that column.
+    '''
+    _kind = 'pop'
+
+    def __init__(self, top_n=100, item_key='ItemId', support_by_key=None):
+        self.top_n = top_n
+        self.item_key = item_key
+        self.support_by_key = support_by_key
+
+    def fit(self, data):
+        self.pop_scores = _pop_scores(self, data)
+        self.__dict__.pop('_dev', None)
+
+    def _n_keep(self):
+        return self.top_n
+
+    def _upload(self, dev):
+        dev.set_pop(self.pop_scores)
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        preds = np.zeros(len(predict_for_item_ids))
+        mask = np.isin(predict_for_item_ids, self.pop_list.index)
+        preds[mask] = self.pop_list[predict_for_item_ids[mask]]
+        return pd.Series(data=preds, index=predict_for_item_ids)
+
+
+class SessionPop(Pop):
+    '''
+    SessionPop(top_n=100, item_key='ItemId', support_by_key=None)
+
+    Session popularity predictor (baselines.py:120-197): the Pop score plus the number of times the item occurs among the
+    session's inputs so far, the current input included.
+    '''
+    _kind = 'sessionpop'
+
+    def fit(self, data):
+        Pop.fit(self, data)
+        self.prev_session_id = -1
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        if self.prev_session_id != session_id:
+            self.prev_session_id = session_id
+            self.pers = dict()
+        self.pers[input_item_id] = self.pers.get(input_item_id, 0) + 1
+        preds = np.array(Pop.predict_next(self, session_id, input_item_id, predict_for_item_ids).values)
+        ser = pd.Series(self.pers)
+        mask = np.isin(predict_for_item_ids, ser.index)
+        preds[mask] += ser[predict_for_item_ids[mask]].values
+        return pd.Series(data=preds, index=predict_for_item_ids)
+
+
+class ItemKNN(Baseline):
+    '''
+    ItemKNN(n_sims=100, lmbd=20, alpha=0.5, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Item-to-item predictor (baselines.py:199-301).  For every occurrence of item i in a session, each distinct item j of the
+    session gains 1: cnt(i, j) = sum over sessions of (occurrences of i) * [j in session], cnt(i, i) = 0.  The similarity is
+    cnt / ((supp_i + lmbd)^alpha * (supp_j + lmbd)^(1 - alpha)) in float64 (supp: events of the item); each item keeps its n_sims
+    largest positive similarities (ties by the smaller item index), every other item scores 0.
+    '''
+    _kind = 'itemknn'
+
+    def __init__(self, n_sims=100, lmbd=20, alpha=0.5, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.n_sims = n_sims
+        self.lmbd = lmbd
+        self.alpha = alpha
+        self.item_key = item_key
+        self.session_key = session_key
+        self.time_key = time_key
+
+    def _n_keep(self):
+        return self.n_sims
+
+    def norm_factors(self, supp):
+        """(a, b): a[i] = (supp_i + lmbd)^alpha, b[j] = (supp_j + lmbd)^(1 - alpha), computed as the reference computes them
+        (baselines.py:272: a per row with numpy's scalar power, b over the support array), so that the device's sims are
+        bitwise the reference's"""
+        a = np.array([np.power((s + self.lmbd), self.alpha) for s in supp], dtype=np.float64)
+        b = np.power((supp + self.lmbd), (1.0 - self.alpha)).astype(np.float64)
+        return a, b
+
+    def fit(self, data):
+        idx = self._index(data)
+        sess = data[self.session_key].values
+        codes = pd.Index(pd.unique(sess)).get_indexer(sess)
+        order = np.argsort(codes, kind='stable')                   # session CSR of the item indices
+        offsets = np.zeros(codes.max() + 2 if len(codes) else 1, dtype=np.int64)
+        offsets[1:] = np.cumsum(np.bincount(codes, minlength=len(offsets) - 1))
+        supp = np.bincount(idx, minlength=self.n_items).astype(np.int64)
+        a, b = self.norm_factors(supp)
+        self.__dict__.pop('_dev', None)
+        dev = _lib.Baselines(self._kind, self.n_items, self.n_sims)
+        self.fit_stats = dev.knn_fit(offsets, idx[order], a, b)
+        self.rows = dev.rows_export()
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.rows_import(*self.rows)
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        i = self.itemidmap[input_item_id]
+        idx, sim, ln = self.rows
+        kept = pd.Series(data=sim[i, :ln[i]], index=self.itemidmap.index.values[idx[i, :ln[i]]])
+        preds = np.zeros(len(predict_for_item_ids))
+        mask = np.isin(predict_for_item_ids, kept.index)
+        preds[mask] = kept[predict_for_item_ids[mask]].values
+        return pd.Series(data=preds, index=predict_for_item_ids)

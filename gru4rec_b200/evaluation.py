@@ -5,6 +5,7 @@ import numpy as np
 import pandas as pd
 
 from . import _lib
+from .baselines import Baseline
 
 _MODES = {'standard': 0, 'conservative': 1, 'median': 2, 'tiebreaking': 3}
 
@@ -98,6 +99,8 @@ def evaluate_gpu(gru, test_data, items=None, session_key='SessionId', item_key='
     exclude_seen the history's items count as seen, and the seen-list budget applies to the longest concatenated session.
     Only the counted events are ranked on the device.  history=None or an empty frame: exactly the evaluation without it.
     '''
+    if isinstance(gru, Baseline):
+        return _evaluate_baseline(gru, test_data, items, session_key, item_key, time_key, cut_off, mode, 0, exclude_seen, history, True)
     if gru.error_during_train: raise Exception
     if mode not in _MODES:
         raise NotImplementedError
@@ -187,6 +190,8 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
 
     Single process only: under a torch.distributed job it raises NotImplementedError.
     '''
+    if isinstance(gru, Baseline):
+        return _evaluate_baseline(gru, test_data, items, session_key, item_key, time_key, cut_off, mode, k, exclude_seen, history, False)
     if gru.error_during_train: raise Exception
     if mode not in _MODES:
         raise NotImplementedError
@@ -215,8 +220,14 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
     else:
         row = (pos[sched.counted()] + 1).astype(np.int64)
     order = np.argsort(row, kind='stable')
-    row = row[order]
-    rank = _ranks(counts[order], mode)
+    return _events_result(gru, test_data, row[order], counts[order], rec, mrr, n, cuts, mode, k, top_i[order] if k else None,
+                          top_s[order] if k else None, session_key, item_key, time_key)
+
+
+def _events_result(gru, test_data, row, counts, rec, mrr, n, cuts, mode, k, top_i, top_s, session_key, item_key, time_key):
+    """evaluate_events' result from the counted events in frame order: `row` the frame rows of their targets, their counts,
+    the device sums and (k > 0) their lists of item indices"""
+    rank = _ranks(counts, mode)
     tgt, inp = test_data.iloc[row], test_data.iloc[row - 1]
     events = pd.DataFrame({session_key: tgt[session_key].values, time_key: tgt[time_key].values, 'input_item': inp[item_key].values,
                            item_key: tgt[item_key].values, 'rank': rank})
@@ -224,7 +235,6 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
         ndcg = [float(np.where(rank <= c, 1.0 / np.log2(rank + 1.0), 0.0).mean()) if n else float('nan') for c in cuts]
     out = {'events': events, 'recall': [float(r) / n for r in rec], 'mrr': [float(m) / n for m in mrr], 'ndcg': ndcg}
     if k:
-        top_i = top_i[order]
         ids = gru.itemidmap.index.values
         pad = top_i < 0                                    # exclude_seen: fewer than k eligible items
         if pad.any():
@@ -232,6 +242,32 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
             out['topk_items'][pad] = None
         else:
             out['topk_items'] = ids[top_i]
-        out['topk_scores'] = top_s[order]
+        out['topk_scores'] = top_s
         out['coverage'] = len(np.unique(top_i[~pad])) / gru.n_items
     return out
+
+
+def _evaluate_baseline(model, test_data, items, session_key, item_key, time_key, cut_off, mode, k, exclude_seen, history, sums_only):
+    """evaluate_gpu (sums_only) / evaluate_events of a baseline (DESIGN §3j): the same preparation, `items` lookup, rank rules
+    and result layout as for a GRU4Rec model; every counted event is ranked on the device on its own (a baseline has no
+    recurrent state), so batch_size has no effect.  Single process only."""
+    if mode not in _MODES:
+        raise NotImplementedError
+    if model._world()[0] > 1:
+        raise NotImplementedError('the baselines are evaluated in a single process')
+    cand = None if items is None else model.itemidmap[items].values      # KeyError for unknown ids
+    if k != 0:
+        k = _lib.check_topk(k, model.n_items if cand is None else len(set(cand)))
+    cuts = _cuts(cut_off)
+    if sums_only:
+        print('Measuring Recall@{} and MRR@{}'.format(','.join([str(c) for c in cuts]), ','.join([str(c) for c in cuts])))
+    test_data, test_data_items, offset_sessions, n_hist = _prepare_history(model, test_data, history, session_key, item_key, time_key)
+    rec, mrr, n, counts, top_i, top_s = model._device().evaluate(test_data_items, offset_sessions, n_hist, cuts, _MODES[mode], cand,
+                                                                 exclude_seen, k, counts=not sums_only)
+    if sums_only:
+        return [float(r) / n for r in rec], [float(m) / n for m in mrr]
+    # the counted events' targets: every row past the first max(n_history, 1) of its session, in frame order
+    lens = np.diff(offset_sessions)
+    first = np.repeat(np.maximum(n_hist if n_hist is not None else np.zeros(len(lens), np.int32), 1), lens)
+    row = np.flatnonzero(np.arange(len(test_data)) - np.repeat(offset_sessions[:-1], lens) >= first)
+    return _events_result(model, test_data, row, counts, rec, mrr, n, cuts, mode, k, top_i, top_s, session_key, item_key, time_key)

@@ -319,6 +319,47 @@ int g4r_sessions_export(g4r_handle* h, int64_t* keys, float* states, int64_t* hi
 int g4r_sessions_import(g4r_handle* h, const int64_t* keys, const float* states, const int64_t* hist_off,
                         const int32_t* hist_items, int64_t n);
 
+/* ---- session baselines: ItemKNN, Pop and SessionPop of the reference's baselines.py (baselines.py:52-301; DESIGN §3j) -------
+ * A separate handle: a baseline has no training config.  Item indices are 0 .. n_items - 1.  Every argument is checked before any
+ * device work; G4R_ERR_STATE for a call the handle's kind does not have or before the model is fitted. */
+typedef struct g4r_baselines g4r_baselines;
+#define G4R_BL_POP 0
+#define G4R_BL_SESSIONPOP 1
+#define G4R_BL_ITEMKNN 2
+/* n_keep: n_sims of ItemKNN (1 .. 1024), top_n of Pop / SessionPop.  Device memory is allocated by the library. */
+int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out);
+int g4r_bl_destroy(g4r_baselines* b);
+const char* g4r_bl_last_error(const g4r_baselines* b);   /* b may be NULL: last creation error */
+/* ItemKNN fit (baselines.py:235-276) from the training events as session CSR (items[session_offsets[s] .. session_offsets[s+1]),
+ * any order within a session) and the caller's norm factors a[i] = (supp_i + lmbd)^alpha, b[j] = (supp_j + lmbd)^(1 - alpha)
+ * (finite, >= 0).  cnt(i, j) = sum over sessions s of (occurrences of i in s) * [j in s], cnt(i, i) = 0; sim = cnt / (a_i * b_j)
+ * (a zero norm counts as 1), each product and quotient correctly rounded in float64; each row keeps its n_keep largest positive
+ * sims by (sim desc, index asc).  Out (may be NULL): the pair work sum_s n_s d_s (events x distinct items per session), the
+ * scratch bytes of the accumulators, the device time (CUDA events) from the first kernel that derives the per-session and per-item
+ * lists from the uploaded events to the last kernel of the fit.  After the upload everything runs on the device. */
+int g4r_bl_knn_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_events,
+                   const double* a, const double* bf, int64_t* pair_work, size_t* scratch_bytes, float* device_ms);
+/* Pop / SessionPop scores (baselines.py:79-118,146-161): n = n_items float64, 0 past the top_n (at most top_n positive). */
+int g4r_bl_set_pop(g4r_baselines* b, const double* scores, int64_t n);
+/* ItemKNN rows: idx [n_items x n_keep] (-1 past len), sim [n_items x n_keep] float64 (0 past len), len [n_items].  Import checks
+ * every row (indices, positive finite sims, (sim desc, index asc) order) before it changes anything. */
+int g4r_bl_rows_export(g4r_baselines* b, int32_t* idx, double* sim, int32_t* len);
+int g4r_bl_rows_import(g4r_baselines* b, const int32_t* idx, const double* sim, const int32_t* len);
+/* evaluate_gpu / evaluate_events of a baseline.  Sessions as CSR of item indices; n_history (NULL: none) as in
+ * g4r_schedule_build_history: an event is counted when its target lies past the session's first max(n_history, 1) events.  Each
+ * counted event (input items[p], target items[p + 1], session items so far items[start .. p]) is ranked against the competitors:
+ * the catalogue, or the multiset cand[0 .. n_cand) (the target competes only if listed).  exclude_seen: the session's items so
+ * far leave the competitors and a target among them is a miss, (-1, -1).  mode 0 .. 3 as g4r_eval_schedule; 'tiebreaking' adds
+ * U(0,1) * 1e-10 to every float64 score, a counter hash of (counted event, item).  recall_sum / mrr_sum: n_cut sums (a hit when
+ * rank <= N); *n_counted: counted events.  out_counts (may be NULL): [n_counted x 2] (#greater, #equal incl. the target), in data
+ * order.  k > 0: the k best eligible distinct competitors of each event by (score desc, index asc), zero scores included, into
+ * out_items / out_scores [n_counted x k] (item -1, score NaN past the eligible ones).  G4R_ERR_INVALID unless
+ * 0 <= k <= min(distinct competitors, 1024). */
+int g4r_bl_evaluate(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                    const int32_t* n_history, int32_t mode, const int32_t* cut_off, int32_t n_cut, const int32_t* cand, int64_t n_cand,
+                    int32_t exclude_seen, int32_t k, double* recall_sum, double* mrr_sum, int64_t* n_counted,
+                    int32_t* out_counts, int32_t* out_items, double* out_scores);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,6 +24,7 @@ _OPTIONS = [
     (('--load_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Load the model, with its optimizer and training state, from a checkpoint written by --save_checkpoint. Exclusive with -ps, -pf and -l.')),
     (('--save_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Save the model with its optimizer and training state to CKPT_PATH (.npz), so that a later run can train it further.')),
     (('--fit_more',), dict(action='store_true', help='With --load_checkpoint: continue training the loaded model on the training data PATH (new items are added to the catalogue) instead of building a new model.')),
+    (('--baseline',), dict(metavar='NAME', choices=['pop', 'sessionpop', 'itemknn'], help='Fit a session baseline of the reference (Pop, SessionPop or ItemKNN) instead of GRU4Rec; -ps gives its constructor parameters (e.g. n_sims=200,lmbd=20,alpha=0.5), each converted to the type of its default. Exclusive with -pf, -l, -s and the checkpoint options.')),
     (('-t', '--test'), dict(metavar='TEST_PATH', type=str, nargs='+', help='Test data set(s).')),
     (('-m', '--measure'), dict(metavar='AT', type=int, nargs='+', default=[20], help='Recommendation list length(s) for recall & MRR (default: 20).')),
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
@@ -131,6 +132,28 @@ def _train_more(gru, args):
     _save(gru, args)
 
 
+def _train_baseline(args):
+    """a baselines.Pop / SessionPop / ItemKNN from -ps (values converted to the type of the constructor's default), fitted on PATH"""
+    import inspect
+    import baselines
+    model_class = {'pop': baselines.Pop, 'sessionpop': baselines.SessionPop, 'itemknn': baselines.ItemKNN}[args.baseline]
+    defaults = {n: p.default for n, p in inspect.signature(model_class.__init__).parameters.items() if n != 'self'}
+    params = {}
+    for name, value in (_training_parameters(args).items() if args.parameter_string else []):
+        if name not in defaults:
+            _abort('ERROR. {} has no parameter "{}" (it takes: {})'.format(model_class.__name__, name, ', '.join(defaults)))
+        params[name] = value if defaults[name] is None else type(defaults[name])(value)
+    print('Creating {} model'.format(model_class.__name__))
+    model = model_class(**params)
+    print('Loading training data...')
+    frame = load_data(args.path, args)
+    print('Started training')
+    started = time.time()
+    model.fit(frame)
+    print('Total training time: {:.2f}s'.format(time.time() - started))
+    return model
+
+
 def _evaluate(gru, evaluation, args):
     primary = ('recall', 'mrr').index(args.primary_metric.lower())
     history = None
@@ -175,8 +198,17 @@ def main(argv=None):
         sys.path.insert(0, here)
     world, rank = _join_distributed_job()
     args.rank = rank
-    model_class = importlib.import_module(args.gru4rec_model).GRU4Rec
     import evaluation
+    if args.baseline is not None:
+        conflicts = [flag for flag, on in (('-pf', args.parameter_file), ('-l', args.load_model), ('--load_checkpoint', args.load_checkpoint),
+                                           ('--fit_more', args.fit_more), ('-s', args.save_model), ('--save_checkpoint', args.save_checkpoint)) if on]
+        if conflicts:
+            _abort('ERROR. --baseline cannot be combined with {}'.format(', '.join(conflicts)))
+        model = _train_baseline(args)
+        if args.test is not None:
+            _evaluate(model, evaluation, args)
+        return
+    model_class = importlib.import_module(args.gru4rec_model).GRU4Rec
     chosen = [args.parameter_string is not None, args.parameter_file is not None, bool(args.load_model), args.load_checkpoint is not None]
     if sum(chosen) != 1:
         _abort('ERROR. Exactly one of the following parameters must be provided: --parameter_string, --parameter_file, --load_model'
