@@ -49,7 +49,7 @@ EXPORTS = [
     'g4r_sessions_export', 'g4r_sessions_import',
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
-    'g4r_bl_rows_import', 'g4r_bl_evaluate',
+    'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
 ]
 
 _lib = None
@@ -142,6 +142,11 @@ def load():
     lib.g4r_bl_rows_export.argtypes = [vp, vp, vp, vp]
     lib.g4r_bl_rows_import.argtypes = [vp, vp, vp, vp]
     lib.g4r_bl_evaluate.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, i32, i32, vp, vp, C.POINTER(i64), vp, vp, vp]
+    lib.g4r_bl_bpr_begin.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp]
+    f64 = C.c_double
+    lib.g4r_bl_bpr_iterate.argtypes = [vp, vp, vp, f64, f64, f64, i32, C.POINTER(f64), C.POINTER(i64), C.POINTER(C.c_float)]
+    lib.g4r_bl_bpr_export.argtypes = [vp, vp, vp]
+    lib.g4r_bl_bpr_import.argtypes = [vp, vp, vp]
     _lib = lib
     return lib
 
@@ -734,12 +739,13 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3}
 
 
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
-    a baseline.  kind: 'pop', 'sessionpop' or 'itemknn'; n_keep: top_n or n_sims."""
+    a baseline, and the BPR-MF fit and factors (DESIGN §3k).  kind: 'pop', 'sessionpop', 'itemknn' or 'bpr'; n_keep: top_n,
+    n_sims or n_factors."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -820,3 +826,42 @@ class Baselines(object):
                                              _ptr(cd), 0 if cd is None else cd.size, 1 if exclude_seen else 0, int(k),
                                              _ptr(rec), _ptr(mrr), C.byref(nc), _ptr(cnt), _ptr(ti), _ptr(ts)))
         return rec, mrr, nc.value, cnt, ti, ts
+
+    def bpr_begin(self, row_session, row_item, n_sessions, U, I, bI):
+        """starts a BPR fit: the merged training rows' session and item indices and the initial U [n_sessions, F], I, bI"""
+        rs = np.ascontiguousarray(row_session, dtype=np.int32); ri = np.ascontiguousarray(row_item, dtype=np.int32)
+        U = np.ascontiguousarray(U, dtype=np.float64); I = np.ascontiguousarray(I, dtype=np.float64)
+        bI = np.ascontiguousarray(bI, dtype=np.float64)
+        if rs.size != ri.size or U.shape != (int(n_sessions), self.n_keep) or I.shape != (self.n_items, self.n_keep) or bI.size != self.n_items:
+            raise ValueError('bpr_begin: need rows of equal length, U [n_sessions, n_factors], I [n_items, n_factors], bI [n_items]')
+        if rs.size < self.n_items:
+            raise ValueError('bpr_begin: need n_rows >= n_items (the negative draws index rows below n_items)')
+        self._check(self.lib.g4r_bl_bpr_begin(self.h, _ptr(rs), _ptr(ri), rs.size, int(n_sessions), _ptr(U), _ptr(I), _ptr(bI)))
+        self.bpr_rows, self.bpr_sessions = rs.size, int(n_sessions)
+
+    def bpr_iterate(self, perm, negrow, learning_rate, lambda_session, lambda_item, max_warps=1 << 30):
+        """one SGD pass in perm order with negative rows negrow; returns (mean log sigm, largest level, device ms)"""
+        pm = np.asarray(perm)
+        ng = np.asarray(negrow)
+        if pm.shape != (self.bpr_rows,) or ng.shape != (self.bpr_rows,):
+            raise ValueError('bpr_iterate: perm and negrow need one entry per training row')
+        if pm.size and (pm.min() < 0 or pm.max() >= self.bpr_rows or ng.min() < 0 or ng.max() >= min(self.n_items, self.bpr_rows)):
+            raise IndexError('bpr_iterate: perm must index the rows and negrow must be below min(n_items, n_rows)')
+        pm = np.ascontiguousarray(pm, dtype=np.int32); ng = np.ascontiguousarray(ng, dtype=np.int32)
+        mean, lv, ms = C.c_double(), C.c_int64(), C.c_float()
+        self._check(self.lib.g4r_bl_bpr_iterate(self.h, _ptr(pm), _ptr(ng), float(learning_rate), float(lambda_session), float(lambda_item),
+                                                int(min(max_warps, 1 << 30)), C.byref(mean), C.byref(lv), C.byref(ms)))
+        return mean.value, lv.value, ms.value
+
+    def bpr_export(self):
+        """(U [n_sessions, F], I [n_items, F]) of the fit"""
+        U = np.empty((self.bpr_sessions, self.n_keep)); I = np.empty((self.n_items, self.n_keep))
+        self._check(self.lib.g4r_bl_bpr_export(self.h, _ptr(U), _ptr(I)))
+        return U, I
+
+    def bpr_import(self, I, bI):
+        """the item factors and biases a BPR is evaluated with (a model loaded from a pickle)"""
+        I = np.ascontiguousarray(I, dtype=np.float64); bI = np.ascontiguousarray(bI, dtype=np.float64)
+        if I.shape != (self.n_items, self.n_keep) or bI.size != self.n_items:
+            raise ValueError('bpr_import: need I [n_items, n_factors] and bI [n_items]')
+        self._check(self.lib.g4r_bl_bpr_import(self.h, _ptr(I), _ptr(bI)))

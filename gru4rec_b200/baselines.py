@@ -1,8 +1,9 @@
-"""Session baselines of the reference (baselines.py:52-301): Pop, SessionPop and ItemKNN, with its constructor signatures,
-fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids).  ItemKNN's fit runs on the device (the co-occurrence
-counts, the normalisation and the top n_sims per row, DESIGN §3j); evaluate_gpu / evaluate_events rank every test event of a
-baseline on the device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted rows.
-RandomPred and BPR are not provided: the first has nothing to accelerate, the second is sequential SGD on global random draws."""
+"""Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
+signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids).  ItemKNN's fit runs on the device (the
+co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
+sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
+device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
+provided: it has nothing to fit, and its scores are unseeded noise."""
 import numpy as np
 import pandas as pd
 
@@ -172,3 +173,84 @@ class ItemKNN(Baseline):
         mask = np.isin(predict_for_item_ids, kept.index)
         preds[mask] = kept[predict_for_item_ids[mask]].values
         return pd.Series(data=preds, index=predict_for_item_ids)
+
+
+class BPR(Baseline):
+    '''
+    BPR(n_factors=100, n_iterations=10, learning_rate=0.01, lambda_session=0.0, lambda_item=0.0, sigma=0.05, init_normal=False,
+        session_key='SessionId', item_key='ItemId')
+
+    Bayesian Personalized Ranking matrix factorisation (baselines.py:303-418) with sessions as users.  fit draws from the global
+    np.random state exactly as the reference does (U, then I, then per iteration a permutation of the training rows and one
+    randint(n_items) per event, which indexes a training *row* whose item is the negative) and runs each iteration's SGD on the
+    device in the reference's order, bit for bit a sequential run (DESIGN §3k).  It prints `it, mean(log sigm)` per iteration.
+    predict_next scores I[j] . mean(I[session inputs so far]) + bI[j].  After fit, `fit_stats` holds per iteration (mean log
+    sigm, largest level = the longest chain of dependent updates, device ms).
+    '''
+    _kind = 'bpr'
+
+    def __init__(self, n_factors=100, n_iterations=10, learning_rate=0.01, lambda_session=0.0, lambda_item=0.0, sigma=0.05, init_normal=False,
+                 session_key='SessionId', item_key='ItemId'):
+        self.n_factors = n_factors
+        self.n_iterations = n_iterations
+        self.learning_rate = learning_rate
+        self.lambda_session = lambda_session
+        self.lambda_item = lambda_item
+        self.sigma = sigma
+        self.init_normal = init_normal
+        self.session_key = session_key
+        self.item_key = item_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.n_factors
+
+    def init(self, data):
+        """the reference's init (baselines.py:343-347): U, then I, from the global np.random state"""
+        if not self.init_normal:
+            self.U = np.random.rand(self.n_sessions, self.n_factors) * 2 * self.sigma - self.sigma
+            self.I = np.random.rand(self.n_items, self.n_factors) * 2 * self.sigma - self.sigma
+        else:
+            self.U = np.random.randn(self.n_sessions, self.n_factors) * self.sigma
+            self.I = np.random.randn(self.n_items, self.n_factors) * self.sigma
+        self.bU = np.zeros(self.n_sessions)
+        self.bI = np.zeros(self.n_items)
+
+    def fit(self, data):
+        itemids = data[self.item_key].unique()
+        self.n_items = len(itemids)
+        self.itemidmap = pd.Series(data=np.arange(self.n_items), index=itemids)
+        sessionids = data[self.session_key].unique()
+        self.n_sessions = len(sessionids)
+        # the reference's two merges: the random draws index rows of the merged frame, so its row order is kept
+        data = pd.merge(data, pd.DataFrame({self.item_key: itemids, 'ItemIdx': np.arange(self.n_items)}), on=self.item_key, how='inner')
+        data = pd.merge(data, pd.DataFrame({self.session_key: sessionids, 'SessionIdx': np.arange(self.n_sessions)}), on=self.session_key, how='inner')
+        self.init(data)
+        self.__dict__.pop('_dev', None)
+        dev = _lib.Baselines(self._kind, self.n_items, self.n_factors)
+        dev.bpr_begin(data.SessionIdx.values, data.ItemIdx.values, self.n_sessions, self.U, self.I, self.bI)
+        self.fit_stats = []
+        N = len(data)
+        for it in range(self.n_iterations):
+            perm = np.random.permutation(N)
+            negrow = np.random.randint(self.n_items, size=N)   # consumes the stream as N scalar randint(n_items) calls do
+            stats = dev.bpr_iterate(perm, negrow, self.learning_rate, self.lambda_session, self.lambda_item)
+            self.fit_stats.append(stats)
+            print(it, np.float64(stats[0]))
+        self.U, self.I = dev.bpr_export()
+        dev.bpr_import(self.I, self.bI)                        # ends the fit: U and the per-row buffers leave the device
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.bpr_import(self.I, self.bI)
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        iidx = self.itemidmap[input_item_id]
+        if self.current_session is None or self.current_session != session_id:
+            self.current_session = session_id
+            self.session = [iidx]
+        else:
+            self.session.append(iidx)
+        uF = self.I[self.session].mean(axis=0)
+        iIdxs = self.itemidmap[predict_for_item_ids]
+        return pd.Series(data=self.I[iIdxs].dot(uF) + self.bI[iIdxs], index=predict_for_item_ids)

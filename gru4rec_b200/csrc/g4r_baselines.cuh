@@ -4,7 +4,8 @@
 // nothing here touches a g4r_handle.
 #pragma once
 
-constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2;
+constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3;
+constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
 constexpr size_t KF_SCRATCH = (size_t)512 << 20;        // dense accumulators of the fit's resident CTAs
@@ -24,6 +25,18 @@ struct g4r_baselines {
   int* dTop = nullptr;
   std::vector<int> hTop;
   std::vector<double> hPop;
+  // BPR: item factors [n_items x n_keep] and biases float64; the fit's session factors and per-iteration buffers (bpr_mem, from
+  // g4r_bl_bpr_begin until an import or the destroy)
+  double *dI = nullptr, *dBI = nullptr, *dU = nullptr, *dLsig = nullptr;
+  int *dRowS = nullptr, *dRowI = nullptr, *dPerm = nullptr, *dNeg = nullptr, *dPred = nullptr, *dLevel = nullptr, *dCtr = nullptr;
+  unsigned long long *dKeys = nullptr, *dKeys2 = nullptr;
+  unsigned* dFlag = nullptr;
+  unsigned char* dCub = nullptr;
+  std::vector<void*> bpr_mem;
+  int64_t bpr_rows = 0, bpr_sessions = 0;
+  size_t bpr_cub_bytes = 0;
+  int bpr_end_bit = 64;
+  unsigned bpr_tag = 0;                                 // the iteration's done-flag value (flags are never cleared)
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -555,8 +568,10 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
   if (!h) return G4R_OK;
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* p : {(void*)h->dIdx, (void*)h->dIdxI, (void*)h->dLen, (void*)h->dSim, (void*)h->dSimI, (void*)h->dPop, (void*)h->dTopS, (void*)h->dTop})
+  for (void* p : {(void*)h->dIdx, (void*)h->dIdxI, (void*)h->dLen, (void*)h->dSim, (void*)h->dSimI, (void*)h->dPop, (void*)h->dTopS, (void*)h->dTop,
+                  (void*)h->dI, (void*)h->dBI})
     if (p) cudaFree(p);
+  for (void* p : h->bpr_mem) cudaFree(p);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -566,9 +581,10 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if (kind < BL_POP || kind > BL_ITEMKNN) { g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop) or 2 (ItemKNN)"; return G4R_ERR_INVALID; }
-  if (n_items < 1 || n_keep < 1 || (kind == BL_ITEMKNN && n_keep > KF_KEEP_MAX)) {
-    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN)";
+  if (kind < BL_POP || kind > BL_BPR) { g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN) or 3 (BPR)"; return G4R_ERR_INVALID; }
+  if (n_items < 1 || n_keep < 1 || (kind == BL_ITEMKNN && n_keep > KF_KEEP_MAX) || (kind == BL_BPR && n_keep > BPR_F_MAX)) {
+    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, <= " +
+                        std::to_string(BPR_F_MAX) + " n_factors for BPR)";
     return G4R_ERR_INVALID;
   }
   int dev_count = 0;
@@ -577,7 +593,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
     return G4R_ERR_CUDA;
   }
   g4r_baselines* h = new g4r_baselines();
-  h->kind = kind; h->n_items = n_items; h->n_keep = kind == BL_ITEMKNN ? n_keep : std::min(n_keep, n_items); h->device = device;
+  h->kind = kind; h->n_items = n_items; h->n_keep = (kind == BL_ITEMKNN || kind == BL_BPR) ? n_keep : std::min(n_keep, n_items); h->device = device;
   auto bail = [&](const char* m) { g_bl_create_error = m; g4r_bl_destroy(h); return G4R_ERR_CUDA; };
   if (cudaSetDevice(device) != cudaSuccess) return bail("cudaSetDevice failed");
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
@@ -585,7 +601,9 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1);
   const size_t rows = (size_t)n_items * h->n_keep;
   bool ok = true;
-  if (kind == BL_ITEMKNN) {
+  if (kind == BL_BPR) {
+    ok &= bl_alloc(&h->dI, rows) == cudaSuccess && bl_alloc(&h->dBI, n_items) == cudaSuccess;
+  } else if (kind == BL_ITEMKNN) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
   } else {
@@ -715,7 +733,7 @@ extern "C" int g4r_bl_knn_fit(g4r_baselines* h, const int64_t* session_offsets, 
 
 extern "C" int g4r_bl_set_pop(g4r_baselines* h, const double* scores, int64_t n) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind == BL_ITEMKNN) FAIL(G4R_ERR_STATE, "g4r_bl_set_pop: the handle is an ItemKNN");
+  if (h->kind == BL_ITEMKNN || h->kind == BL_BPR) FAIL(G4R_ERR_STATE, "g4r_bl_set_pop: the handle is not a Pop / SessionPop");
   if (!scores || n != h->n_items) FAIL(G4R_ERR_INVALID, "g4r_bl_set_pop: need n_items scores");
   std::vector<int> top;
   for (int64_t i = 0; i < n; i++) {
@@ -783,6 +801,11 @@ extern "C" int g4r_bl_rows_import(g4r_baselines* h, const int32_t* idx, const do
   return G4R_OK;
 }
 
+static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                        const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
+                        const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
+                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_bpr.cuh
+
 extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                                const int32_t* n_history, int32_t mode, const int32_t* cut_off, int32_t n_cut, const int32_t* cand,
                                int64_t n_cand, int32_t exclude_seen, int32_t k, double* recall_sum, double* mrr_sum, int64_t* n_counted,
@@ -819,6 +842,13 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   }
   const int64_t n_ev = ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
+  if (h->kind == BL_BPR) {
+    cudaSetDevice(h->device);
+    const int rc = bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult, cdist,
+                                exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores);
+    if (rc == G4R_OK && n_counted) *n_counted = n_ev;
+    return rc;
+  }
   // competitor weights of the Pop list: prefix sums along (score desc, index asc)
   std::vector<long long> topW(h->hTop.size() + 1, 0);
   for (size_t r = 0; r < h->hTop.size(); r++) topW[r + 1] = topW[r] + (n_cand > 0 ? mult[h->hTop[r]] : 1);

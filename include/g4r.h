@@ -360,6 +360,31 @@ int g4r_bl_evaluate(g4r_baselines* b, const int32_t* items, int64_t n_events, co
                     int32_t exclude_seen, int32_t k, double* recall_sum, double* mrr_sum, int64_t* n_counted,
                     int32_t* out_counts, int32_t* out_items, double* out_scores);
 
+/* ---- BPR-MF of the reference's baselines.py (BPR, baselines.py:303-418; DESIGN §3k) ---------------------------------------------
+ * g4r_bl_create(G4R_BL_BPR, n_items, n_factors (1 .. 1024), ...).  The fit replays the caller's random draws and applies the
+ * reference's SGD updates in its order, in float64; the result equals a strictly sequential run bit for bit. */
+#define G4R_BL_BPR 3
+/* Begins a fit: the training rows (the reference's merged frame, in its order) as session and item indices, and the initial
+ * factors U [n_sessions x n_factors], I [n_items x n_factors] and biases bI [n_items] (bI is never updated, but scores add it).
+ * n_items <= n_rows <= (2^31 - 1) / 3 (the negative draws index rows below n_items; a merged frame has a row per item at least)
+ * and n_sessions + n_items < 2^32 - 1.  The device must hold U, I and 92 bytes per row; the call refuses with G4R_ERR_CUDA and a
+ * message naming the sizes otherwise. */
+int g4r_bl_bpr_begin(g4r_baselines* b, const int32_t* row_session, const int32_t* row_item, int64_t n_rows, int64_t n_sessions,
+                     const double* U, const double* I, const double* bI);
+/* One iteration: for t = 0 .. n_rows - 1, row e = perm[t] (a permutation of the rows), u, p its session and item, n the item of
+ * row negrow[t] (0 <= negrow[t] < n_items <= n_rows), the update of baselines.py:349-358 with uF, I[p], I[n] read before it.  max_warps >= 1
+ * bounds the warps that apply updates at once (1: one warp in order; the result is the same).  Out (may be NULL): the mean of
+ * log(sigm) over the events (summed in a fixed order), the largest level (1 + the largest level of the event's predecessors on
+ * its rows: the longest chain of dependent updates) and the device time (CUDA events) from the predecessor sort to the mean. */
+int g4r_bl_bpr_iterate(g4r_baselines* b, const int32_t* perm, const int32_t* negrow, double learning_rate, double lambda_session,
+                       double lambda_item, int32_t max_warps, double* mean_log_sigm, int64_t* max_level, float* device_ms);
+/* The fit's U [n_sessions x n_factors] (NULL: skipped; G4R_ERR_STATE unless a fit has begun) and I [n_items x n_factors]. */
+int g4r_bl_bpr_export(g4r_baselines* b, double* U, double* I);
+/* The item factors and biases of a fitted model (a model loaded from a pickle); ends any fit in progress.  g4r_bl_evaluate of a
+ * BPR handle scores item j after input p as (sum over f = 0 .. n_factors - 1 in order of I[j,f] * uF[f]) + bI[j], every product
+ * and sum correctly rounded in float64, uF the mean of I over the session's items[start .. p]. */
+int g4r_bl_bpr_import(g4r_baselines* b, const double* I, const double* bI);
+
 #ifdef __cplusplus
 }
 #endif
