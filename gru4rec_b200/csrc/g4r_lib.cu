@@ -1,6 +1,7 @@
 // g4r_lib.cu -- host side of libg4r.so: handle, workspace carving, the session-parallel schedule builder,
 // the per-step launch sequence, negative sampling, and the C ABI declared in include/g4r.h.
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -12,7 +13,7 @@
 #include "g4r_kernels.cuh"
 #include "g4r_misc.cuh"
 
-#define G4R_VERSION 100
+#define G4R_VERSION 101
 
 static thread_local std::string g_create_error;
 struct g4r_handle;
@@ -42,6 +43,21 @@ struct g4r_schedule {
   bool has_pos = false;
   int64_t max_len = 1;          // events of the longest session walked (its inputs bound a lane's seen list, g4r_seen.cuh)
   bool hist = false;            // g4r_schedule_build_history: only lanes flagged 4 are counted events (g4r_history.cuh)
+};
+
+// window buffers of truncated BPTT (g4r_bptt.cuh): per-step slices [T][B][ld] of the forward saves and gradients, per-layer
+// scratch of the backward, and the merged row list of the window
+struct BpttDev {
+  float *Hold[G4R_MAX_LAYERS], *R[G4R_MAX_LAYERS], *Z[G4R_MAX_LAYERS], *Ah[G4R_MAX_LAYERS], *Ht[G4R_MAX_LAYERS];   // forward saves
+  float *In[G4R_MAX_LAYERS];       // layer inputs (layers with an input product)
+  float *Dvec[G4R_MAX_LAYERS];     // [T][B][ld3] gate gradients (rows past a step's M stay zero)
+  float *Carry[G4R_MAX_LAYERS];    // [B][ldL] gradient wrt the hidden state a step leaves, by physical slot
+  float *Dyl[G4R_MAX_LAYERS], *Dh[G4R_MAX_LAYERS], *DHr[G4R_MAX_LAYERS];   // [B][ldL] scratch of the step being differentiated
+  float *Dy;                       // [T][B][ldL] dL/dy of the top layer (chunk partials summed)
+  float *DSY, *DBY; int* Item;     // [T][NP][ldL], [T][NP], [T][NP]: score-column gradients and their items in plan order
+  float *DSx;                      // [T][B][ld_in0] gradients of the gathered input rows (embedding modes)
+  int *M, *N, *X, *Slot; uint8_t* F; uint32_t* G;   // per step: lanes, columns, inputs, slots, flags, dropout step
+  unsigned long long *keys, *keys2;                  // [T][B + NP] merged row list, unsorted / sorted
 };
 
 struct g4r_handle {
@@ -92,6 +108,7 @@ struct g4r_handle {
   float* dGscale = nullptr;
   bool tc_ok = false; void* ts_buf = nullptr; unsigned long long* ts_dbg = nullptr; cudaStream_t side = nullptr, side2 = nullptr; cudaEvent_t ts_ev[12] = {};      // tensor-core training step (g4r_tcstep.cuh): TsBuf*
   std::vector<cudaEvent_t> prof_ev; std::vector<int> prof_phase;
+  BpttDev bw = {}; void* bptt_cub = nullptr; size_t bptt_cub_bytes = 0; int64_t bptt_windows = 0;   // bptt > 1 (g4r_bptt.cuh)
 };
 
 enum { PH_GATHER = 0, PH_F1, PH_F2, PH_SCORE, PH_STATS, PH_LOSSGRAD, PH_B1, PH_B2, PH_B3, PH_DENSE, PH_SPARSE_IN, PH_STATS2, PH_GRADCAP, PH_COUNT };
@@ -149,6 +166,8 @@ static int validate_config(const g4r_config& c, std::string& err) {
   if (c.smoothing < 0.f) { err = "smoothing < 0"; return G4R_ERR_INVALID; }
   if (c.constrained_embedding && c.embedding) { /* reference: constrained wins (gru4rec.py:272) */ }
   if (c.n_sample < 0) { err = "n_sample < 0"; return G4R_ERR_INVALID; }
+  if (c.bptt < 0 || c.bptt > 64) { err = "bptt must be in [1, 64]"; return G4R_ERR_INVALID; }
+  if (c.bptt > 1 && c.world_size > 1) { err = "bptt > 1 is a single-GPU option"; return G4R_ERR_INVALID; }
   return G4R_OK;
 }
 
@@ -258,7 +277,7 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
   // multi-GPU: dense-gradient twins (one flat all-reduce buffer) and the gathered / merged per-window state
   MgDev mgd; memset(&mgd, 0, sizeof(mgd));
   std::vector<MgTensor> mgt;
-  const bool twins = R > 1 || c.grad_cap > 0.f;      // dense gradients are exported (all-reduced / norm-capped) before they are applied
+  const bool twins = R > 1 || c.grad_cap > 0.f || c.bptt > 1;      // dense gradients are exported (all-reduced / norm-capped / summed over a window) before they are applied
   if (twins) {
     size_t cnt = 0;
     for (int i = 0; i < nl; i++) {
@@ -318,6 +337,26 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     tsb.Pb = cv.take<float>(ts_shape(3 * L, L, tsb.Bk / 32, n_sm, 0).p_floats);
     tsb.O = cv.take<float>((size_t)tsb.Mpad * tsb.ldO); tsb.bias = cv.take<float>(tsb.Nk);
   }
+  // truncated BPTT: window slices
+  BpttDev bw; memset(&bw, 0, sizeof(bw));
+  if (c.bptt > 1) {
+    const size_t TB = (size_t)c.bptt * B;
+    for (int i = 0; i < nl; i++) {
+      const LayerDev& ly = md.layer[i];
+      bw.Hold[i] = cv.take<float>(TB * ly.ldL); bw.R[i] = cv.take<float>(TB * ly.ldL); bw.Z[i] = cv.take<float>(TB * ly.ldL);
+      bw.Ah[i] = cv.take<float>(TB * ly.ldL); bw.Ht[i] = cv.take<float>(TB * ly.ldL);
+      bw.In[i] = ly.in_dim > 0 ? cv.take<float>(TB * ly.ld_in) : nullptr;
+      bw.Dvec[i] = cv.take<float>(TB * ly.ld3);
+      bw.Carry[i] = cv.take<float>((size_t)B * ly.ldL); bw.Dyl[i] = cv.take<float>((size_t)B * ly.ldL);
+      bw.Dh[i] = cv.take<float>((size_t)B * ly.ldL); bw.DHr[i] = cv.take<float>((size_t)B * ly.ldL);
+    }
+    bw.Dy = cv.take<float>(TB * ldL);
+    bw.DSY = cv.take<float>((size_t)c.bptt * NP * ldL); bw.DBY = cv.take<float>((size_t)c.bptt * NP); bw.Item = cv.take<int>((size_t)c.bptt * NP);
+    bw.DSx = mode != 0 ? cv.take<float>(TB * md.ld_in0) : nullptr;
+    bw.M = cv.take<int>(c.bptt); bw.N = cv.take<int>(c.bptt); bw.X = cv.take<int>(TB); bw.Slot = cv.take<int>(TB);
+    bw.F = cv.take<uint8_t>(TB); bw.G = cv.take<uint32_t>(c.bptt);
+    bw.keys = cv.take<unsigned long long>((size_t)c.bptt * (B + NP)); bw.keys2 = cv.take<unsigned long long>((size_t)c.bptt * (B + NP));
+  }
   // evaluation
   int* dRank = cv.take<int>((size_t)Be * 4); float* dTgt = cv.take<float>((size_t)Be * 3);   // target scores | lower | upper pre-activation thresholds (tensor-core ranking)
   if (!cv.dry) {
@@ -332,6 +371,7 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     h->shard_ws = shard_ws; h->shard_ws_bytes = shard_ws_bytes;
     h->tc_ok = tc;
     if (tc) { if (!h->ts_buf) h->ts_buf = new TsBuf(); *static_cast<TsBuf*>(h->ts_buf) = tsb; }
+    h->bw = bw;
     h->dGscale = gsc; h->two_pass = c.grad_cap > 0.f; h->phase_only = c.grad_cap > 0.f || md.smoothing > 0.f;
   }
 }
@@ -414,7 +454,7 @@ __global__ void k_advance(int* base, int n) { if (threadIdx.x == 0 && blockIdx.x
 static bool fast_shape(const g4r_config& c, int n_sm) {
   const int L = c.layers[0], ldL = round4(L);
   const bool smoothing = (c.loss == G4R_LOSS_XE || c.loss == G4R_LOSS_XE_LOGIT) && c.smoothing > 0.f;
-  return c.step_mode == 2 && c.adapt <= G4R_ADAPT_ADAGRAD && !(c.grad_cap > 0.f) && !smoothing && model_mode(c) == 0 && c.n_layers == 1 &&
+  return c.step_mode == 2 && c.bptt <= 1 && c.adapt <= G4R_ADAPT_ADAGRAD && !(c.grad_cap > 0.f) && !smoothing && model_mode(c) == 0 && c.n_layers == 1 &&
          ldL <= 128 && c.batch_size <= FK_B && 2 * L <= FK_W1 * FK_G && L <= FK_W2 * FK_G && n_sm >= FK_G + 1 &&
          n_sm - ldL / 4 >= c.batch_size && !tc_eligible(c) && !shard_eligible(c, n_sm);
 }
@@ -476,7 +516,7 @@ static int tiles2(int cols, int rows) { return ((cols + GB - 1) / GB) * ((rows +
 // automatically for wide layers (L >= 160), or for any such model with step_mode 4.
 static bool tc_eligible(const g4r_config& c) {
   if (!c.constrained_embedding || c.n_layers != 1 || c.batch_size > 256 || (c.layers[0] & 3)) return false;
-  if (c.adapt > G4R_ADAPT_ADAGRAD || c.grad_cap > 0.f || c.smoothing != 0.f || c.world_size > 1) return false;
+  if (c.adapt > G4R_ADAPT_ADAGRAD || c.grad_cap > 0.f || c.smoothing != 0.f || c.world_size > 1 || c.bptt > 1) return false;
   return c.step_mode == 4 || (c.step_mode >= 1 && c.step_mode <= 3 && c.layers[0] >= 160);
 }
 // G4R_TS_STAMP=1: per-product phase timeline of the last step (median / max over the CTAs, microseconds after the first CTA's entry)
@@ -634,9 +674,8 @@ static int enqueue_tc_step(g4r_handle* h, const int* base, int off) {
   return G4R_OK;
 }
 
-// enqueue the kernels of one training step (window-relative index = *base + off when base != nullptr)
-static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
-  if (h->tc_ok) return enqueue_tc_step(h, base, off);
+// the forward and score phases of one step, through the loss gradient (window-relative index = *base + off when base != nullptr)
+static void enqueue_forward_scores(g4r_handle* h, const int* base, int off) {
   const ModelDev& md = h->md;
   cudaStream_t st = h->stream;
   const int B = md.B;
@@ -653,6 +692,15 @@ static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
     LAUNCH(PH_STATS2, k_stats2b<<<B, 256, 0, st>>>(h->slot, base, off));
   }
   LAUNCH(PH_LOSSGRAD, k_lossgrad<<<md.NCH, SC_THREADS, lossgrad_smem_bytes(md.Bld, md.ldL), st>>>(h->slot, base, off));
+}
+
+// enqueue the kernels of one training step (window-relative index = *base + off when base != nullptr)
+static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
+  if (h->tc_ok) return enqueue_tc_step(h, base, off);
+  const ModelDev& md = h->md;
+  cudaStream_t st = h->stream;
+  const int B = md.B;
+  enqueue_forward_scores(h, base, off);
   for (int li = md.n_layers - 1; li >= 0; li--) {
     const LayerDev& ly = md.layer[li];
     LAUNCH(PH_B1, k_b1<<<std::max(1, std::min(h->n_sm, (B * ly.L * 8 + 255) / 256)), 256, 0, st>>>(h->slot, base, off, li, 0));
@@ -720,6 +768,7 @@ extern "C" int g4r_destroy(g4r_handle* h) {
   if (h->hCost) cudaFreeHost(h->hCost);
   if (h->hFlags) cudaFreeHost(h->hFlags);
   if (h->own_ws && h->ws) cudaFree(h->ws);
+  if (h->bptt_cub) cudaFree(h->bptt_cub);
   if (h->ts_dbg) { ts_print_stamps(h); cudaFree(h->ts_dbg); }
   if (h->side) cudaStreamDestroy(h->side);
   if (h->side2) cudaStreamDestroy(h->side2);
@@ -776,7 +825,13 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
   layout(*cfg, cv, h, chunk_cap);
   h->slot = slot_alloc();
   if (h->slot < 0) return bail(G4R_ERR_STATE, "too many live g4r handles in this process");
-  if (h->two_pass) h->md.export_only = 1;       // grad_cap: every update waits for the global gradient norm
+  if (h->two_pass || cfg->bptt > 1) h->md.export_only = 1;       // grad_cap: every update waits for the global gradient norm; bptt: for the window
+  if (cfg->bptt > 1) {
+    const int nk = cfg->bptt * (h->md.B + h->md.NP);
+    if (cub::DeviceRadixSort::SortKeys(nullptr, h->bptt_cub_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, nk, 0, 64, h->stream) != cudaSuccess ||
+        cudaMalloc(&h->bptt_cub, std::max<size_t>(h->bptt_cub_bytes, 256)) != cudaSuccess)
+      return bail(G4R_ERR_CUDA, "bptt: sort scratch allocation failed");
+  }
   if (slot_upload(h->slot, h->md, h->stream) != cudaSuccess) return bail(G4R_ERR_CUDA, "constant upload failed");
   const int B = cfg->batch_size, CAP = h->CAP;
   bool ok = true;
@@ -1332,6 +1387,7 @@ static int run_window(g4r_handle* h, int64_t n) {
 
 #include "g4r_multi.cuh"
 #include "g4r_shard.cuh"
+#include "g4r_bptt.cuh"
 static bool mg_is_ready(g4r_handle* h) { return h->mg_host && static_cast<MgHost*>(h->mg_host)->ready; }
 
 extern "C" int g4r_upload_steps(g4r_handle* h, const g4r_schedule* s, int64_t first, int64_t n) {
@@ -1340,6 +1396,7 @@ extern "C" int g4r_upload_steps(g4r_handle* h, const g4r_schedule* s, int64_t fi
   if (s->B != h->md.B) FAIL(G4R_ERR_INVALID, "schedule batch size != model batch size");
   if (first < 0 || n <= 0 || first + n > s->n_steps) FAIL(G4R_ERR_INVALID, "step range out of schedule");
   if (n > h->CAP) FAIL(G4R_ERR_INVALID, "n exceeds the resident window capacity");
+  if (h->cfg.bptt > 1 && !bptt_aligned(h, s, first, n)) FAIL(G4R_ERR_INVALID, "bptt: the range must start at a multiple of bptt and hold whole windows unless it runs to the schedule's end");
   cudaSetDevice(h->cfg.device);
   if (h->gen_len > 0 && h->sample_ptr + n > h->gen_len) FAIL(G4R_ERR_STATE, "window would wrap the sample store; regenerate or shorten");
   const int64_t got = stage_window(h, s, first, n);
@@ -1356,7 +1413,7 @@ extern "C" int g4r_run_uploaded(g4r_handle* h, float* cost_out, float* device_ms
   if (h->cfg.world_size > 1 && !mg_is_ready(h)) FAIL(G4R_ERR_STATE, "multi-GPU handle: call g4r_mg_init first");
   if (h->cfg.world_size > 1 && !h->shard) FAIL(G4R_ERR_STATE, "g4r_run_uploaded on a multi-GPU handle needs the row-sharded path");
   CK(cudaEventRecord(h->ev0, h->stream));
-  int rc = h->shard ? mgs_run_window(h, n) : run_window(h, n);
+  int rc = h->shard ? mgs_run_window(h, n) : (h->cfg.bptt > 1 ? bptt_run_uploaded(h, n) : run_window(h, n));
   if (rc) return rc;
   CK(cudaEventRecord(h->ev1, h->stream));
   if (cost_out) CK(cudaMemcpyAsync(h->hCost, h->md.cost, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -1372,6 +1429,7 @@ extern "C" int g4r_run_uploaded(g4r_handle* h, float* cost_out, float* device_ms
 extern "C" int g4r_profile_uploaded(g4r_handle* h, float* phase_ms, int32_t* phase_launches, int32_t n_phases) {
   if (!h || !phase_ms || !phase_launches || n_phases < PH_COUNT) return G4R_ERR_INVALID;
   if (h->shard) FAIL(G4R_ERR_STATE, "per-phase profiling is a single-GPU measurement (row-sharded handle)");
+  if (h->cfg.bptt > 1) FAIL(G4R_ERR_STATE, "per-phase profiling measures one-step updates (bptt > 1 handle)");
   if (h->win_steps <= 0) FAIL(G4R_ERR_STATE, "no uploaded window");
   cudaSetDevice(h->cfg.device);
   h->wy_version++;
@@ -1408,6 +1466,7 @@ extern "C" int64_t g4r_fast_windows(const g4r_handle* h, int64_t* fallback_windo
   if (fallback_windows) *fallback_windows = h->slow_windows;
   return h->fast_windows;
 }
+extern "C" int64_t g4r_bptt_windows(const g4r_handle* h) { return h ? h->bptt_windows : 0; }
 extern "C" const char* g4r_phase_name(int32_t i) { return (i >= 0 && i < PH_COUNT) ? kPhaseNames[i] : ""; }
 extern "C" int g4r_phase_count(void) { return PH_COUNT; }
 
@@ -1415,9 +1474,11 @@ extern "C" int g4r_train_steps(g4r_handle* h, const g4r_schedule* s, int64_t fir
   if (!h || !s) return G4R_ERR_INVALID;
   if (s->B != h->md.B) FAIL(G4R_ERR_INVALID, "schedule batch size != model batch size");
   if (first < 0 || n < 0 || first + n > s->n_steps) FAIL(G4R_ERR_INVALID, "step range out of schedule");
+  if (h->cfg.bptt > 1 && n > 0 && !bptt_aligned(h, s, first, n)) FAIL(G4R_ERR_INVALID, "bptt: the range must start at a multiple of bptt and hold whole windows unless it runs to the schedule's end");
   cudaSetDevice(h->cfg.device);
   h->wy_version++;
   if (nan_step) *nan_step = -1;
+  if (h->cfg.bptt > 1) return bptt_train_steps(h, s, first, n, cost_out, nan_step);
   int64_t done = 0;
   while (done < n) {
     if (h->gen_len > 0 && (!h->have_store || h->sample_ptr >= h->gen_len)) {   // gru4rec.py:618-621
@@ -1455,6 +1516,7 @@ extern "C" int g4r_train_step(g4r_handle* h, const int32_t* X, const int32_t* Y,
   const int B = h->md.B;
   if (M <= 0 || M > B) FAIL(G4R_ERR_INVALID, "M out of range");
   if (h->shard) FAIL(G4R_ERR_STATE, "g4r_train_step: not available on a row-sharded multi-GPU handle (use g4r_train_steps)");
+  if (h->cfg.bptt > 1) FAIL(G4R_ERR_STATE, "g4r_train_step: a bptt > 1 handle trains whole windows (use g4r_train_steps)");
   cudaSetDevice(h->cfg.device);
   h->wy_version++;
   if (h->gen_len > 0 && (!h->have_store || h->sample_ptr >= h->gen_len)) {

@@ -102,6 +102,7 @@ class GRU4Rec:
         self.eval_lanes = 512            # run.py evaluates with batch_size=512 (run.py:127)
         self.step_mode = 2               # role-specialised persistent kernel where the shape allows, else generic persistent
         self.session_capacity = 100000   # sessions kept by recommend_sessions / feed_sessions (least recently used evicted)
+        self.bptt = 1                    # > 1: truncated backpropagation through time, one update per window of bptt mini-batches (DESIGN §3l)
         self._engine = None
         self._host = None                # numpy copies of the parameters when no engine is alive
 
@@ -264,6 +265,7 @@ class GRU4Rec:
         cfg.world_size, cfg.rank = (1, 0) if single else self._world()
         cfg.eval_batch_size = eval_lanes
         cfg.step_mode = self.step_mode
+        cfg.bptt = int(self.bptt) if training else 1
         if self.step_mode == 2 and len(self.layers) == 1 and 120 < self.layers[0] <= 128 and not self.constrained_embedding and not self.embedding and self.batch_size <= 32:
             cfg.step_mode = 3        # the 48-CTA GRU group of step_mode 2 covers 120 hidden units; the cluster variant takes up to 128
         return cfg
@@ -414,6 +416,7 @@ class GRU4Rec:
             else:
                 print('No example store was used')
         per_step_sampling = False
+        self._check_bptt(store_type)
         if self.n_sample and not use_store:
             if store_type == 'cpu':
                 # gru4rec.py:612-613: without a store every mini-batch draws its own row on the host (generate_neg_samples(pop, 1))
@@ -456,6 +459,18 @@ class GRU4Rec:
         return SimpleNamespace(eng=eng, pop=pop, generate_length=generate_length, use_store=use_store, per_step_sampling=per_step_sampling,
                                store_type=store_type, offset_sessions=offset_sessions, base_order=base_order,
                                data_items=data.ItemIdx.values, world=world, rank=rank)
+
+    def _check_bptt(self, store_type):
+        '''the training options bptt > 1 does not cover, refused before any engine is built'''
+        bptt = int(self.bptt)
+        if bptt < 1 or bptt > 64:
+            raise ValueError('bptt must be in [1, 64], got %r' % (self.bptt,))
+        if bptt == 1:
+            return
+        if self._world()[0] > 1:
+            raise NotImplementedError('bptt > 1 trains on one GPU; truncated BPTT over several GPUs is not implemented')
+        if self.n_sample and store_type == 'cpu':
+            raise NotImplementedError("bptt > 1 draws its negatives from the device sample store: store_type='cpu' is not implemented")
 
     def _epochs(self, plan, epochs=None, every=None, resume=None):
         '''The epoch loop of fit() (gru4rec.py:586-664) as a generator: it yields a progress record wherever a checkpoint may be
@@ -578,7 +593,7 @@ class GRU4Rec:
         ids = np.asarray(self.itemidmap.index.values)
         ids_are_objects = ids.dtype.kind not in 'iufUS'          # item ids read as str: stored as a fixed-width string array
         meta = dict(version=self._CKPT_VERSION, params=self._ctor_params(), n_items=int(self.n_items), ids_are_objects=bool(ids_are_objects),
-                    engine=dict(dropout_seed=int(self.dropout_seed), step_mode=int(self.step_mode)),
+                    engine=dict(dropout_seed=int(self.dropout_seed), step_mode=int(self.step_mode), bptt=int(self.bptt)),
                     has_state=st is not None, sample_store=None if st is None else st['sample_store'], has_store=st is not None and st['store'] is not None,
                     fingerprint=_fingerprint, progress=None)
         arrays = {'itemids': ids.astype(str) if ids_are_objects else ids}
@@ -634,6 +649,7 @@ class GRU4Rec:
         meta = ck['meta']
         gru = cls(**meta['params'])
         gru.dropout_seed, gru.step_mode = meta['engine']['dropout_seed'], meta['engine']['step_mode']
+        gru.bptt = int(meta['engine'].get('bptt', 1))             # written before bptt existed: one update per mini-batch
         ids = ck['itemids'].astype(object) if meta['ids_are_objects'] else ck['itemids']
         gru.predict = None
         gru.error_during_train = False
@@ -664,6 +680,8 @@ class GRU4Rec:
         every_steps = int(every_steps)
         if every_steps < 1:
             raise ValueError('every_steps must be at least 1, got %d' % every_steps)
+        if every_steps % int(self.bptt) != 0:
+            raise ValueError('every_steps (%d) must be a multiple of bptt (%d): a checkpoint falls between two windows' % (every_steps, int(self.bptt)))
         params = self._ctor_params()
         ck = self._read_checkpoint(path) if os.path.exists(path) else None
         offset_sessions = self._index_items(data)
@@ -745,7 +763,7 @@ class GRU4Rec:
     def _grow_engine(self, n_store, rows):
         '''the training engine for the catalogue as it is now, holding everything the present engine holds (fit_more)'''
         old = self._engine
-        if int(old.cfg.n_items) == self.n_items and int(old.cfg.sample_store) == int(n_store):
+        if int(old.cfg.n_items) == self.n_items and int(old.cfg.sample_store) == int(n_store) and int(old.cfg.bptt) == int(self.bptt):
             return old
         sessions = (old.session_capacity, old.sessions_export()) if getattr(old, 'session_capacity', None) is not None else None
         eng = _lib.Engine(self._make_config(n_store, 0, True, single=True), device=self.device)
@@ -1069,7 +1087,7 @@ class GRU4Rec:
         self._host = host
         self._engine = None
         self.predict = None
-        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2), ('session_capacity', 100000)):
+        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2), ('session_capacity', 100000), ('bptt', 1)):
             if not hasattr(self, k):
                 setattr(self, k, v)
 

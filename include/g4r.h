@@ -74,6 +74,11 @@ typedef struct g4r_config {
   float adapt_p1, adapt_p1c;      /* adapt_params[0] and 1 - adapt_params[0] (rmsprop / adadelta decay; adam beta1), gru4rec.py:301-304,342-343,368-369 */
   float adapt_p2, adapt_p2c;      /* adapt_params[1] and 1 - adapt_params[1] (adam beta2) */
   float grad_cap;                 /* > 0: gradients are scaled to this global L2 norm when they exceed it (gru4rec.py:386-389) */
+  int32_t bptt;                   /* 0 / 1: one update per mini-batch.  2..64: truncated backpropagation through time, one update per
+                                     window of bptt consecutive mini-batches of the schedule (DESIGN §3l).  Single GPU; step_mode
+                                     has no effect.  g4r_train_steps / g4r_upload_steps then take ranges that start at a multiple
+                                     of bptt and hold whole windows unless they run to the schedule's end (else G4R_ERR_INVALID);
+                                     g4r_train_step and g4r_profile_uploaded return G4R_ERR_STATE */
 } g4r_config;
 
 typedef struct g4r_handle g4r_handle;
@@ -167,6 +172,8 @@ const char* g4r_phase_name(int32_t i);
 /* step_mode 2: number of windows run by the role-specialised kernel, and (out) windows that fell back to the
  * generic persistent kernel because a chunk of score columns was wider than 16. */
 int64_t g4r_fast_windows(const g4r_handle* h, int64_t* fallback_windows);
+/* bptt > 1: number of windows trained (each one backward through time and one update) */
+int64_t g4r_bptt_windows(const g4r_handle* h);
 /* 1 if the handle trains with the tensor-core step (wgmma 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh): constrained
  * embedding, one layer, batch <= 256, SGD / Adagrad (+momentum); automatic for layers >= 160 units, forced with step_mode 4. */
 int g4r_uses_tensor_cores(const g4r_handle* h);
