@@ -44,7 +44,7 @@ EXPORTS = [
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
     'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_bptt_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
-    'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_set_eval_exclude_seen', 'g4r_predict', 'g4r_reset_eval_hidden',
+    'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_rest', 'g4r_eval_rest_pairs', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_set_eval_exclude_seen', 'g4r_predict', 'g4r_reset_eval_hidden',
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
     'g4r_sessions_open', 'g4r_sessions_count', 'g4r_sessions_feed', 'g4r_sessions_topk', 'g4r_sessions_end',
     'g4r_sessions_export', 'g4r_sessions_import',
@@ -118,6 +118,8 @@ def load():
     lib.g4r_mg_segment_bytes.argtypes = [C.POINTER(G4RConfig), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.g4r_eval_schedule.argtypes = [vp, vp, vp, i32, i32, vp, vp, C.POINTER(i64)]
     lib.g4r_eval_events.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, C.POINTER(i64), vp, vp, vp]
+    lib.g4r_eval_rest.argtypes = [vp, vp, vp, i32, i32, vp, C.POINTER(i64), C.POINTER(i64), vp, vp]
+    lib.g4r_eval_rest_pairs.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.g4r_eval_counts.argtypes = [vp, vp, i64]
     lib.g4r_set_eval_items.argtypes = [vp, vp, i64]
     lib.g4r_set_eval_exclude_seen.argtypes = [vp, i32]
@@ -600,6 +602,25 @@ class Engine(object):
         self._check(self.lib.g4r_eval_events(self.h, sched.h, _ptr(cut), len(cut), mode, int(k), _ptr(rec), _ptr(mrr), C.byref(n),
                                              _ptr(counts), _ptr(items), _ptr(scores)))
         return rec, mrr, n.value, counts, items, scores
+
+    def eval_rest(self, sched, cut_off, mode=0):
+        """Rest-of-session ranking of the schedule's counted events (schedules built with mode=1 | SCHED_POSITIONS): every
+        distinct later item of an event's session ranked as if it were the target, under set_eval_items / set_eval_exclude_seen
+        (a seen or unlisted item is a miss, counts (-1, -1)).  Returns (sums float64 [6, n_cut]: per cut-off the sums of
+        HitRate, Precision, Recall, MRR, NDCG and MAP over the events; n_events; n_pairs; counts int32 [n_pairs, 2] in the event
+        order of eval_events, each event's items in first-occurrence order; offsets int64 [n_events + 1] of each event's pairs).
+        Over the relevant-list budget (lanes x longest session - 1 int32 within 256 MiB): NotImplementedError."""
+        cut = np.ascontiguousarray(cut_off, dtype=np.int32)
+        ne, npairs = C.c_int64(), C.c_int64()
+        if self.lib.g4r_eval_rest_pairs(sched.h, C.byref(ne), C.byref(npairs)) != 0:
+            raise RuntimeError('libg4r: %s' % self.lib.g4r_last_error(None).decode())
+        counts = np.empty((npairs.value, 2), dtype=np.int32)
+        offsets = np.empty(ne.value + 1, dtype=np.int64)
+        sums = np.zeros(6 * len(cut), dtype=np.float64)
+        n, n_pairs = C.c_int64(), C.c_int64()
+        self._check(self.lib.g4r_eval_rest(self.h, sched.h, _ptr(cut), len(cut), mode, _ptr(sums), C.byref(n), C.byref(n_pairs),
+                                           _ptr(counts), _ptr(offsets)))
+        return sums.reshape(6, len(cut)), n.value, n_pairs.value, counts, offsets
 
     def eval_counts(self, n_lanes):
         """[n_lanes x 2] int32: (#items scoring above the target, #items tied with it incl. the target) of every lane of the last

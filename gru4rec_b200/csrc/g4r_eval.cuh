@@ -269,6 +269,7 @@ struct EvalCtx {
   void* topk = nullptr;                                           // TopkCtx* of g4r_predict_topk (g4r_topk.cuh)
   void* events = nullptr;                                         // EventsCtx* of g4r_eval_events (g4r_events.cuh)
   void* hist = nullptr;                                           // HistCtx* of history schedules (g4r_history.cuh)
+  void* rest = nullptr;                                           // RestCtx* of g4r_eval_rest (g4r_rest.cuh)
   // exclude_seen (g4r_set_eval_exclude_seen, g4r_seen.cuh): per state slot the seen list, its length, the lanes' miss flags, and
   // the per-mini-batch CSR copy the top-k kernels of g4r_eval_events read as their exclusions
   bool seen_on = false;
@@ -279,6 +280,7 @@ struct EvalCtx {
 static void topk_release(EvalCtx& e);
 static void events_release(EvalCtx& e);
 static void hist_release(EvalCtx& e);
+static void rest_release(EvalCtx& e);
 
 // device buffer of at least n elements (contents not kept)
 template <class T>
@@ -318,6 +320,7 @@ static void eval_release(g4r_handle* h) {
   topk_release(e);
   events_release(e);
   hist_release(e);
+  rest_release(e);
   cudaFreeHost(e.hX); cudaFreeHost(e.hY); cudaFreeHost(e.hSlot); cudaFreeHost(e.hF); cudaFreeHost(e.hM); cudaFreeHost(e.hSti); cudaFreeHost(e.hG);
   cudaFree(e.dX); cudaFree(e.dY); cudaFree(e.dSlot); cudaFree(e.dF); cudaFree(e.dM); cudaFree(e.dSti); cudaFree(e.dG);
   cudaFree(e.dCut); cudaFree(e.dSums); if (e.dOut) cudaFree(e.dOut); if (e.dCand) cudaFree(e.dCand);
@@ -398,12 +401,15 @@ struct RankUnit {
   const int64_t* steps = nullptr; const int* lanes = nullptr;   // ... or of each row, and its lane (host arrays)
 };
 
+struct RestRun;
+
 // the constants of one eval_run call, shared by every unit it ranks
 struct RankConsts {
   unsigned int tie = 0u;
   bool tc_possible = false;             // the wgmma tiles are ready; a unit takes them if wgmma_tiles holds for its rows
   int n_cut = 0, mode = 0;
   bool seen = false; SeenDev sd;        // exclude_seen: the live lists of the scoring slots
+  RestRun* rest = nullptr;              // g4r_eval_rest's per-unit work (g4r_rest.cuh); nullptr on the other entry points
 };
 
 // g4r_eval_events' per-event outputs (g4r_events.cuh); nullptr on g4r_eval_schedule's path
@@ -419,6 +425,12 @@ struct HistCtx;
 static int hist_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, const SeenDev* sd, HistCtx** out);
 static int hist_window(g4r_handle* h, EvalCtx* e, HistCtx* c, const g4r_schedule* s, int64_t w, int64_t done, const RankConsts& cs, EventsRun* ev);
 
+// g4r_eval_rest (g4r_rest.cuh): relevant lists and thresholds before the tiles, the multi-threshold passes after k_eval_rank
+static int rest_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, RestRun* rr, int n_cut, bool tc);
+static int rest_stage(g4r_handle* h, EvalCtx* e, RestRun* rr, const RankUnit& u, const RankConsts& cs, cudaStream_t rk);
+static int rest_step(g4r_handle* h, EvalCtx* e, RestRun* rr, const RankUnit& u, const RankConsts& cs, cudaStream_t rk);
+static int rest_flush(g4r_handle* h, RestRun* rr, cudaStream_t rk);
+
 // One ranking of unit u on the ranking stream rk: the target scores (with exclude_seen, a mini-batch's seen insert, and the CSR
 // exclusions of g4r_eval_events' lists), the fp32 or wgmma tiles, the per-cutoff sums, then g4r_eval_events' per-event work
 // (ev != nullptr).  released (nullptr: none) is recorded once the rows' y has been read, and the forward stream waits on it.
@@ -432,6 +444,10 @@ static int eval_rank(g4r_handle* h, EvalCtx* e, const RankUnit& u, const RankCon
   else if (u.key) k_eval_tgt<false, true><<<(Be + 31) / 32, 32, 0, rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, cs.tie, subset_mode, lohi, SeenDev{}, u.key);
   else k_eval_tgt<<<(Be + 31) / 32, 32, 0, rk>>>(u.slot, u.s, h->dTgt, h->dRankCnt, cs.tie, subset_mode, lohi);
   h->launches++;
+  if (cs.rest) {
+    int rc = rest_stage(h, e, cs.rest, u, cs, rk);     // reads the rows' y before the forward may move on
+    if (rc) return rc;
+  }
   if (ev) {
     if (seen && events_lists(ev)) {
       k_seen_csr<<<1, SEEN_CSR_THREADS, 0, rk>>>(u.slot, u.s, u.sd, e->dSeenOff, e->dSeenEx);
@@ -458,6 +474,10 @@ static int eval_rank(g4r_handle* h, EvalCtx* e, const RankUnit& u, const RankCon
   if (released) CK(cudaStreamWaitEvent(h->stream, released, 0));
   (seen ? k_eval_rank<true> : k_eval_rank<false>)<<<1, 256, 0, rk>>>(u.slot, u.s, h->dRankCnt, e->dCut, cs.n_cut, cs.mode, e->dSums, u.sd.miss);
   h->launches++;
+  if (cs.rest) {
+    int rc = rest_step(h, e, cs.rest, u, cs, rk);
+    if (rc) return rc;
+  }
   return ev ? events_step(h, e, ev, u, rk) : G4R_OK;
 }
 
@@ -510,7 +530,7 @@ static int seen_begin(g4r_handle* h, EvalCtx* e, const g4r_schedule* s, bool csr
 // per-event work on the ranking stream, after the kernels of g4r_eval_schedule, which stay as they are and see the same step
 // indices (the tiebreaking noise hashes them) whatever the per-event window
 static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode,
-                    double* recall_sum, double* mrr_sum, int64_t* n_events, EventsRun* ev) {
+                    double* recall_sum, double* mrr_sum, int64_t* n_events, EventsRun* ev, RestRun* rest = nullptr) {
   if (mode < 0 || mode > 3) FAIL(G4R_ERR_INVALID, "eval mode must be 0 (standard), 1 (conservative), 2 (median) or 3 (tiebreaking)");
   cudaSetDevice(h->cfg.device);
   EvalCtx* e = nullptr;
@@ -540,6 +560,11 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
   if (cs.tc_possible) {
     rc = tc_operands(h, e);
     if (rc) return rc;
+  }
+  if (rest) {
+    rc = rest_begin(h, e, s, rest, n_cut, cs.tc_possible);   // its passes take the wgmma tiles where the next-item ranking would
+    if (rc) return rc;
+    cs.rest = rest;
   }
   HistCtx* hc = nullptr;
   if (s->hist) {
@@ -571,6 +596,10 @@ static int eval_run(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off
     if (rc) return rc;
     if (ev) {
       rc = events_flush(h, e, ev, h->side);    // the rest of the per-event window before the staging is reused
+      if (rc) return rc;
+    }
+    if (rest) {
+      rc = rest_flush(h, rest, h->side);
       if (rc) return rc;
     }
     CK(cudaEventRecord(h->ts_ev[2], h->side)); CK(cudaStreamWaitEvent(st, h->ts_ev[2], 0));   // window complete before its staging is reused
@@ -685,3 +714,4 @@ extern "C" int g4r_reset_eval_hidden(g4r_handle* h) {
 #include "g4r_sessions.cuh"
 #include "g4r_events.cuh"
 #include "g4r_history.cuh"
+#include "g4r_rest.cuh"

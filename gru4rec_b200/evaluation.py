@@ -224,6 +224,117 @@ def evaluate_events(gru, test_data, items=None, session_key='SessionId', item_ke
                           top_s[order] if k else None, session_key, item_key, time_key)
 
 
+def _relevant(test_data_items, offset_sessions, n_hist):
+    """the counted events in frame order and their relevant sets: for the input at row p, the distinct items of rows p+1 ..
+    end of its session, first occurrence first.  Returns (input rows, items, offsets (row of first occurrence - p), CSR
+    pointer [n_events + 1])"""
+    rows, items, offs, ptr = [], [], [], [0]
+    for s in range(len(offset_sessions) - 1):
+        a, b = int(offset_sessions[s]), int(offset_sessions[s + 1])
+        for t in range(a + max(int(n_hist[s]) if n_hist is not None else 0, 1), b):
+            seen = set()
+            for q in range(t, b):
+                it = test_data_items[q]
+                if it not in seen:
+                    seen.add(it)
+                    items.append(it)
+                    offs.append(q - t + 1)
+            rows.append(t - 1)
+            ptr.append(len(items))
+    return np.array(rows, np.int64), np.array(items, np.int64), np.array(offs, np.int64), np.array(ptr, np.int64)
+
+
+def _rest_budget(test_data, session_key, offset_sessions, lanes):
+    """the library's limit on the relevant lists (lanes x (longest session - 1) int32 within the seen-list budget), checked
+    here first for a ValueError that names the longest session"""
+    lens = np.diff(offset_sessions)
+    if not len(lens):
+        return
+    j = int(np.argmax(lens))
+    need = int(lanes) * max(1, int(lens[j]) - 1) * 4
+    if need > _lib.seen_budget():
+        sid = test_data[session_key].values[offset_sessions[j]]
+        sid = sid.item() if isinstance(sid, np.generic) else sid
+        raise ValueError('evaluate_rest: session %r has %d events; its relevant lists for %d lanes take %d bytes, over the %d-byte '
+                         'budget' % (sid, int(lens[j]), int(lanes), need, _lib.seen_budget()))
+
+
+_REST_METRICS = ('hitrate', 'precision', 'recall', 'mrr', 'ndcg', 'map')
+
+
+def evaluate_rest(gru, test_data, items=None, session_key='SessionId', item_key='ItemId', time_key='Time', cut_off=[20], batch_size=100,
+                  mode='standard', exclude_seen=False, history=None):
+    '''
+    Rest-of-session evaluation: every event evaluate_gpu counts (same arguments, including `history`) is scored once against
+    the catalogue, and each DISTINCT item of the rest of its session (the items after the input, first occurrence first, the
+    next item first) is ranked as if it were the event's target, among the same competitors and by the formula of `mode`.
+    Two relevant items compete with each other like any other items, so a rank is a list position.  In 'tiebreaking' a
+    relevant item's score carries the noise of its own column, so it never beats itself.
+
+    - `exclude_seen`: competitors leave out the session's inputs so far, as in evaluate_gpu; a relevant item the session has
+      already input is a miss (rank inf) and still counts in |R|.
+    - `items`: only these items compete, as in evaluate_gpu.  A relevant item that is NOT listed can never be recommended: it
+      is a miss (rank inf) and still counts in |R|.  This differs from evaluate_gpu, where an unlisted target still gets a rank.
+
+    Per event, with R the relevant set, r_j the rank of j and hits = |{j in R: r_j <= N}| (misses never hit), averaged over the
+    events: HitRate@N = [hits > 0], Precision@N = hits / N, Recall@N = hits / |R|, MRR@N = 1 / min r_j if that is <= N,
+    NDCG@N = sum_{r_j <= N} 1 / log2(r_j + 1) over sum_{i <= min(|R|, N)} 1 / log2(i + 1), MAP@N = sum_{r_j <= N}
+    (|{i in R: r_i <= r_j}| / r_j) / min(|R|, N).  With |R| = 1 they are evaluate_gpu's Recall (HitRate, Recall) and MRR
+    (MRR, MAP), evaluate_events' NDCG, and Precision = Recall / N.
+
+    Returns a dict: 'hitrate', 'precision', 'recall', 'mrr', 'ndcg', 'map' (lists, one entry per cut-off, from sums kept in
+    double on the device), 'n_events', 'n_pairs' and 'pairs': a DataFrame with one row per (event, relevant item) in frame order:
+    session id, the event's time (that of its next item, as in evaluate_events), 'input_item', the relevant item (`item_key`),
+    'offset' (events after the input where the item first occurs; 1 = the next item) and 'rank' (float64, inf for a miss).
+    The relevant lists take batch_size x (longest session - 1) int32 on the device within 256 MiB; over that it raises
+    ValueError naming the session.  They take the tile kind of the next-item ranking.  Single process only (NotImplementedError
+    under torch.distributed); the baselines are not covered yet (NotImplementedError).
+    '''
+    if isinstance(gru, Baseline):
+        raise NotImplementedError('evaluate_rest does not cover the baselines yet')
+    if gru.error_during_train: raise Exception
+    if mode not in _MODES:
+        raise NotImplementedError
+    if gru._world()[0] > 1:
+        raise NotImplementedError('evaluate_rest runs in a single process')
+    cuts = _cuts(cut_off)
+    test_data, test_data_items, offset_sessions, n_hist = _prepare_history(gru, test_data, history, session_key, item_key, time_key)
+    _rest_budget(test_data, session_key, offset_sessions, batch_size)
+    rows, rel, off, ptr = _relevant(test_data_items, offset_sessions, n_hist)
+    eng = gru._ensure_engine(batch_size)
+    if items is not None:
+        eng.set_eval_items(gru.itemidmap[items].values)
+    try:
+        with _ExcludeSeen(eng, exclude_seen, test_data, session_key, offset_sessions, batch_size):
+            sched = _lib.Schedule(test_data_items, offset_sessions, None, batch_size, 0, mode=1 | _lib.SCHED_POSITIONS, n_history=n_hist)
+            sums, n, n_pairs, counts, offsets = eng.eval_rest(sched, cuts, _MODES[mode])
+        pos = sched.positions()
+    finally:
+        if items is not None:
+            eng.set_eval_items(None)
+    gru.predict = None                                     # the scoring hidden state is shared with predict_next_batch
+    # events in schedule order -> frame order (by input row); each event's pairs keep their first-occurrence order
+    if n_hist is None:
+        M = sched.batch_sizes()
+        inp = pos[np.arange(pos.shape[1])[None, :] < M[:, None]].astype(np.int64)
+    else:
+        inp = pos[sched.counted()].astype(np.int64)
+    order = np.argsort(inp, kind='stable')
+    lens = np.diff(offsets)[order]
+    if n != len(rows) or n_pairs != len(rel) or not np.array_equal(inp[order], rows) or not np.array_equal(lens, np.diff(ptr)):
+        raise RuntimeError('evaluate_rest: the device ranked other events than the test data holds')
+    idx = np.repeat(offsets[:-1][order] - ptr[:-1], lens) + np.arange(len(rel))
+    rank = _ranks(counts[idx], mode) if len(rel) else np.zeros(0)
+    ev = np.repeat(np.arange(len(rows)), lens)
+    inp_rows, tgt_rows = rows[ev], rows[ev] + 1
+    pairs = pd.DataFrame({session_key: test_data[session_key].values[inp_rows], time_key: test_data[time_key].values[tgt_rows],
+                          'input_item': test_data[item_key].values[inp_rows], item_key: gru.itemidmap.index.values[rel],
+                          'offset': off, 'rank': rank})
+    out = {m: [float(v) / n if n else float('nan') for v in sums[i]] for i, m in enumerate(_REST_METRICS)}
+    out.update(n_events=int(n), n_pairs=int(n_pairs), pairs=pairs)
+    return out
+
+
 def _events_result(gru, test_data, row, counts, rec, mrr, n, cuts, mode, k, top_i, top_s, session_key, item_key, time_key):
     """evaluate_events' result from the counted events in frame order: `row` the frame rows of their targets, their counts,
     the device sums and (k > 0) their lists of item indices"""

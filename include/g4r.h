@@ -269,6 +269,21 @@ int g4r_set_eval_exclude_seen(g4r_handle* h, int32_t on);
  * 0 <= k <= min(distinct candidates, G4R_TOPK_MAX). */
 int g4r_eval_events(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode, int32_t k,
                     double* recall_sum, double* mrr_sum, int64_t* n_events, int32_t* out_counts, int32_t* out_items, float* out_scores);
+/* Rest-of-session evaluation (DESIGN §3m) on a schedule built with mode 1 | G4R_SCHED_POSITIONS (plain or history): every event
+ * g4r_eval_schedule counts is ranked against each distinct item of the rest of its session (first occurrence first, the next
+ * item first), each as if it were the event's target, with the same competitors, mode, g4r_set_eval_items and
+ * g4r_set_eval_exclude_seen.  A relevant item the session has already input, or (with candidate items) one that is not listed,
+ * is a miss.  sums_out [6 x n_cut]: per cut-off the sums over the events of HitRate, Precision, Recall, MRR, NDCG and MAP, in
+ * double, accumulated in a fixed order.  out_counts [n_pairs x 2] (NULL: not written): (#greater, #equal) of every pair, (-1, -1)
+ * for a miss, events in the order of g4r_eval_events, each event's items in first-occurrence order; out_offsets [n_events + 1]
+ * (NULL: not written): every event's first pair.  The relevant lists take lanes x (longest session - 1) int32 under the 256 MiB
+ * budget of the seen lists (G4R_SEEN_BUDGET lowers it): over it G4R_ERR_INVALID before any device work.  G4R_ERR_STATE for a
+ * schedule built without positions.  The pairs take the tile kind of the next-item ranking (fp32, or wgmma under
+ * cfg.eval_tc / wgmma_tiles). */
+int g4r_eval_rest(g4r_handle* h, const g4r_schedule* s, const int32_t* cut_off, int32_t n_cut, int32_t mode, double* sums_out,
+                  int64_t* n_events, int64_t* n_pairs, int32_t* out_counts, int64_t* out_offsets);
+/* host only: the counted events and (event, relevant item) pairs g4r_eval_rest will report for schedule s (positions needed) */
+int g4r_eval_rest_pairs(const g4r_schedule* s, int64_t* n_events, int64_t* n_pairs);
 
 /* predict_next_batch's device call: scores of all items for `batch` lanes; reset_mask zeroes lanes first
  * (gru4rec.py:712-717).  out: [batch x n_items] row-major. */

@@ -30,6 +30,7 @@ _OPTIONS = [
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
     (('--exclude_seen',), dict(action='store_true', help='Rank each test event without the items its session has already input, as recommend_next_batch(exclude_seen=True) serves (see evaluate_gpu).')),
     (('--history',), dict(metavar='HISTORY_PATH', type=str, help='Events before the test events of each test session, loaded like -t files: every test file is evaluated from its sessions\' history (see evaluate_gpu).')),
+    (('--rest_of_session',), dict(action='store_true', help='Also rank every test event against all later items of its session (see evaluate_rest): after the Recall / MRR lines, one line per list length with HitRate, Precision, Recall, MAP, NDCG and MRR. Single GPU, GRU4Rec models only.')),
     (('-ss', '--sample_store_size'), dict(metavar='SS', type=int, default=10000000, help='Size of the negative-sample buffer in ids (default: 10000000).')),
     (('--sample_store_on_cpu',), dict(action='store_true', help='Legacy: draw the negative samples on the host.')),
     (('-g', '--gru4rec_model'), dict(metavar='GRFILE', type=str, default='gru4rec', help='Module that provides the GRU4Rec class (default: gru4rec).')),
@@ -180,6 +181,12 @@ def _evaluate(gru, evaluation, args):
         print('Evaluation took {:.2f}s'.format(time.time() - started))
         for position, cut in enumerate(args.measure):
             print('Recall@{}: {:.6f} MRR@{}: {:.6f}'.format(cut, result[0][position], cut, result[1][position]))
+        if args.rest_of_session:
+            rest = evaluation.evaluate_rest(gru, frame, batch_size=512, cut_off=args.measure, mode=args.eval_type,
+                                            item_key=args.item_key, session_key=args.session_key, time_key=args.time_key, **extra)
+            for position, cut in enumerate(args.measure):
+                print('Rest@{}: HitRate {:.6f} Precision {:.6f} Recall {:.6f} MAP {:.6f} NDCG {:.6f} MRR {:.6f}'.format(
+                    cut, *(rest[m][position] for m in ('hitrate', 'precision', 'recall', 'map', 'ndcg', 'mrr'))))
         if args.log_primary_metric:
             print('PRIMARY METRIC: {}'.format(result[primary][0]))
 
@@ -199,6 +206,10 @@ def _join_distributed_job():
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
+    if args.rest_of_session and args.baseline is not None:
+        _abort('ERROR. --rest_of_session does not cover the baselines yet')
+    if args.rest_of_session and int(os.environ.get('WORLD_SIZE', '1') or 1) > 1:
+        _abort('ERROR. --rest_of_session runs in a single process (evaluate_rest is not sharded over a torchrun job)')
     here = os.path.dirname(os.path.abspath(__file__))
     if here not in sys.path:
         sys.path.insert(0, here)
