@@ -8,7 +8,9 @@ prefix followed by j, ranked by eval_events -- is an exact oracle for every pair
 - tiebreaking where the noise decides (a block of items scoring exactly 0, with and without a reordered candidate list):
   deterministic, every ranked item ties itself, the block's ties resolved
 - |R| = 1 reductions against eval_schedule / eval_events; the device sums against a host recomputation from the counts
-- history schedules (leave-one-out included), determinism, and eval_events unchanged after an eval_rest call"""
+- history schedules (leave-one-out included), determinism, and eval_events unchanged after an eval_rest call
+These run at one shape (16 lanes, one K chunk, full item tiles).  test_gpu_eval_rest_f64.py holds every pair's counts and the
+metric sums to a float64 bracket at the shapes users run, on both tile kinds and the automatic choice."""
 import numpy as np
 import pytest
 import gru4rec_oracle as orc
@@ -60,12 +62,11 @@ def _rest(eng, items, off, cuts, mode, n_hist=None):
 
 
 def _relevant(items, off, p):
+    """(the distinct items of rows p+1 .. end of p's session, first occurrence first; the session's first row)"""
     s = np.searchsorted(off, p, side='right') - 1
-    out = []
-    for q in range(p + 1, off[s + 1]):
-        if items[q] not in out:
-            out.append(int(items[q]))
-    return out, off[s]
+    rest = np.asarray(items[p + 1:off[s + 1]])
+    first = np.sort(np.unique(rest, return_index=True)[1])
+    return [int(v) for v in rest[first]], off[s]
 
 
 def _workaround(eng, items, off, inp, mode):

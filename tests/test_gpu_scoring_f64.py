@@ -155,29 +155,50 @@ def _competitors(m, items=None):
     return out
 
 
+def _flat_regions(fact):
+    """Pre-activation ranges over which the device's fp32 final activation (act_fwd) is one constant, so that all scores in one
+    of them tie exactly: [(from, to, value)].  relu: 0 at and below 0.  tanhf: +-1 past |x| = 10 (1 - tanh(10) = 4e-9, far
+    below half an ulp of 1, 3e-8).  elu / selu: expf(x) - 1 rounds to -1 below x = -20 (expf(-20) = 2e-9, against half an ulp
+    of 1 of 6e-8), so the score is -p1 (elu) or p1 * (p2 * -1) (selu) there.  CUDA documents tanhf to 2 ulp and expf to 2 ulp,
+    which alone would allow 1 - 6e-8 past |x| = 10: no threshold makes an exact 1 follow from the documented bounds.  That
+    these functions round to exactly +-1 / -1 there is what the H100's tanhf and expf (and numpy's float32 ones, in
+    test_host_eval_rest_f64.py) do, checked by the tests that use it: a library that did not would count those pairs as
+    greater or smaller, outside the bracket, and fail them rather than pass a wrong count."""
+    kind, p1, p2 = fact
+    return {'relu': [(-np.inf, 0.0, 0.0)], 'tanh': [(-np.inf, -10.0, -1.0), (10.0, np.inf, 1.0)],
+            'elu': [(-np.inf, -20.0, -p1)], 'selu': [(-np.inf, -20.0, -p1 * p2)]}.get(kind, [])
+
+
+def _act_interval(m, x, d):
+    """(lo, hi, flat): the interval of the device's activated score for the float64 pre-activation scores x +- d (softmax ranks
+    by the pre-activation score), widened by 2^-22 relative for the fp32 rounding of the activation itself; flat: index in
+    _flat_regions of the region that holds all of x +- d (-1: none), where the interval is that of the region's one value"""
+    kind = orc.parse_act(m.final_act)
+    lo, hi = (x - d, x + d) if kind[0] in ('softmax', 'softmax_logit') else (orc.act_fwd(kind, x - d), orc.act_fwd(kind, x + d))
+    flat = np.full(np.shape(x), -1, np.int8)
+    for k, (a, b, v) in enumerate(_flat_regions(kind)):
+        inside = (x - d >= a) & (x + d <= b)
+        flat[inside] = k
+        lo, hi = np.where(inside, v, lo), np.where(inside, v, hi)
+    return lo - 2.0 ** -22 * np.abs(lo), hi + 2.0 ** -22 * np.abs(hi), flat
+
+
 def _bounds(m, tab, y, Y, hid_abs=0.0):
     """Per lane: (#competitors surely above the target, #surely tied with it, #ambiguous) from float64 scores of the float64 hidden
     output y.  Competitors (`tab`, _competitors): the whole catalogue (the target itself included, one sure tie), or a candidate
     list with its duplicates (the target ties with each copy of itself).  A pair is decided when the activation intervals of the
-    two scores do not overlap, or when both sit in one flat region of the activation (relu below zero: an exact tie)."""
+    two scores do not overlap, or when both sit in one flat region of the activation (_flat_regions: an exact tie)."""
     Wy, By = m.Wy, m.By.ravel()
-    kind = orc.parse_act(m.final_act)
-    act = (lambda v: v) if kind[0] in ('softmax', 'softmax_logit') else (lambda v: orc.act_fwd(kind, v))
     ay = np.abs(y)
-
-    def interval(x, d):
-        lo, hi = act(x - d), act(x + d)
-        return lo - 2.0 ** -22 * np.abs(lo), hi + 2.0 ** -22 * np.abs(hi)        # fp32 rounding of the activation itself
-
     wt = Wy[Y]
-    lo_t, hi_t = interval((y * wt).sum(1) + By[Y], 2.0 ** -19 * ((ay * np.abs(wt)).sum(1) + np.abs(By[Y])) + hid_abs * np.abs(wt).sum(1))
-    lo_t, hi_t = lo_t[:, None], hi_t[:, None]
+    lo_t, hi_t, f_t = _act_interval(m, (y * wt).sum(1) + By[Y], 2.0 ** -19 * ((ay * np.abs(wt)).sum(1) + np.abs(By[Y])) + hid_abs * np.abs(wt).sum(1))
+    lo_t, hi_t, f_t = lo_t[:, None], hi_t[:, None], f_t[:, None]
     gt = np.zeros(len(Y), np.int64); eq = np.zeros(len(Y), np.int64); amb = np.zeros(len(Y), np.int64)
     for c, W, aWT, l1, b, ab in tab:
-        lo, hi = interval(y @ W.T + b, 2.0 ** -19 * (ay @ aWT + ab) + hid_abs * l1)
+        lo, hi, f = _act_interval(m, y @ W.T + b, 2.0 ** -19 * (ay @ aWT + ab) + hid_abs * l1)
         own = c[None, :] == Y[:, None]
         g = (lo > hi_t) & ~own
-        e = ((lo == hi) & (lo == lo_t) & (lo_t == hi_t)) | own
+        e = ((f == f_t) & (f_t >= 0)) | own
         a = ~(g | e | (hi < lo_t))
         gt += g.sum(1); eq += e.sum(1); amb += a.sum(1)
     return gt, eq, amb
