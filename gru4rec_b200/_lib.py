@@ -30,7 +30,7 @@ class G4RConfig(C.Structure):
         ('max_resident_steps', C.c_int32), ('device', C.c_int32), ('world_size', C.c_int32), ('rank', C.c_int32),
         ('eval_batch_size', C.c_int32), ('step_mode', C.c_int32), ('mg_replicated', C.c_int32), ('eval_tc', C.c_int32),
         ('adapt_p1', C.c_float), ('adapt_p1c', C.c_float), ('adapt_p2', C.c_float), ('adapt_p2c', C.c_float), ('grad_cap', C.c_float),
-        ('bptt', C.c_int32),
+        ('bptt', C.c_int32), ('full_softmax', C.c_int32),
     ]
 
 
@@ -42,7 +42,7 @@ EXPORTS = [
     'g4r_mrg_uniform', 'g4r_searchsorted', 'g4r_gather_rows',
     'g4r_schedule_build', 'g4r_schedule_build_history', 'g4r_schedule_free', 'g4r_schedule_steps', 'g4r_schedule_events', 'g4r_schedule_export', 'g4r_schedule_positions',
     'g4r_train_step', 'g4r_train_steps', 'g4r_upload_steps', 'g4r_run_uploaded', 'g4r_kernel_launches',
-    'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_bptt_windows', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
+    'g4r_profile_uploaded', 'g4r_phase_name', 'g4r_phase_count', 'g4r_persistent_stamps', 'g4r_fast_windows', 'g4r_bptt_windows', 'g4r_full_steps', 'g4r_uses_tensor_cores', 'g4r_mg_unique_id', 'g4r_mg_init',
     'g4r_mg_sharded', 'g4r_mg_ipc_handle', 'g4r_mg_ipc_open', 'g4r_mg_owner', 'g4r_mg_local_row', 'g4r_mg_shard_rows', 'g4r_mg_segment_bytes',
     'g4r_eval_schedule', 'g4r_eval_events', 'g4r_eval_rest', 'g4r_eval_rest_pairs', 'g4r_eval_counts', 'g4r_set_eval_items', 'g4r_set_eval_exclude_seen', 'g4r_predict', 'g4r_reset_eval_hidden',
     'g4r_predict_topk', 'g4r_predict_topk_filtered',
@@ -106,6 +106,7 @@ def load():
     lib.g4r_persistent_stamps.argtypes = [vp, i32, vp, i64]
     lib.g4r_fast_windows.argtypes = [vp, C.POINTER(i64)]; lib.g4r_fast_windows.restype = i64
     lib.g4r_bptt_windows.argtypes = [vp]; lib.g4r_bptt_windows.restype = i64
+    lib.g4r_full_steps.argtypes = [vp]; lib.g4r_full_steps.restype = i64
     lib.g4r_uses_tensor_cores.argtypes = [vp]
     lib.g4r_mg_unique_id.argtypes = [vp]
     lib.g4r_mg_init.argtypes = [vp, vp]
@@ -207,7 +208,7 @@ def set_adapt_params(cfg, adapt, adapt_params, grad_cap):
     cfg.grad_cap = float(grad_cap or 0.0)
 
 
-def make_config(n_items, mk, sample_store=0, eval_lanes=0, max_resident_steps=0, step_mode=0, world_size=1, rank=0, replicated=False, eval_tc=None, bptt=1):
+def make_config(n_items, mk, sample_store=0, eval_lanes=0, max_resident_steps=0, step_mode=0, world_size=1, rank=0, replicated=False, eval_tc=None, bptt=1, full_softmax=False):
     cfg = G4RConfig()
     layers = mk.get('layers', [100])
     cfg.n_items = n_items
@@ -242,6 +243,7 @@ def make_config(n_items, mk, sample_store=0, eval_lanes=0, max_resident_steps=0,
     cfg.eval_tc = 0 if eval_tc is None else (2 if eval_tc else 1)   # scoring path: auto / force tensor-core tiles / force fp32 FFMA tiles
     set_adapt_params(cfg, mk.get('adapt', 'adagrad'), mk.get('adapt_params', []), mk.get('grad_cap', 0.0))
     cfg.bptt = bptt              # truncated backpropagation through time over windows of this many mini-batches (DESIGN §3l)
+    cfg.full_softmax = 1 if full_softmax else 0      # train against the whole catalogue instead of sampled columns (DESIGN §3n)
     return cfg
 
 
@@ -335,6 +337,9 @@ class Engine(object):
             import torch
             if not torch.cuda.is_available():
                 raise RuntimeError('gru4rec_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback')
+            if cfg.full_softmax and torch.cuda.mem_get_info(device)[0] < nbytes.value:
+                raise NotImplementedError('full_softmax: the training workspace needs %d bytes of device memory, %d are free on cuda:%d'
+                                          % (nbytes.value, torch.cuda.mem_get_info(device)[0], device))
             self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device='cuda:%d' % device)
             ws_ptr = C.c_void_p(self._ws.data_ptr())
         h = C.c_void_p()
@@ -542,6 +547,10 @@ class Engine(object):
     def bptt_windows(self):
         """windows trained with truncated backpropagation through time (bptt > 1)"""
         return self.lib.g4r_bptt_windows(self.h)
+
+    def full_steps(self):
+        """training steps run against the whole catalogue (full_softmax)"""
+        return self.lib.g4r_full_steps(self.h)
 
     def kernel_launches(self):
         return self.lib.g4r_kernel_launches(self.h)

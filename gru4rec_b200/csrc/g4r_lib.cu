@@ -13,7 +13,7 @@
 #include "g4r_kernels.cuh"
 #include "g4r_misc.cuh"
 
-#define G4R_VERSION 101
+#define G4R_VERSION 102
 
 static thread_local std::string g_create_error;
 struct g4r_handle;
@@ -29,6 +29,11 @@ static int shard_set_tensor(g4r_handle* h, const TensorInfo& t, const float* hos
 static int shard_get_tensor(g4r_handle* h, const TensorInfo& t, float* host);
 static int mgs_run_window(g4r_handle* h, int64_t n);
 static int mgs_plan_window(g4r_handle* h, int64_t n);
+static int enqueue_full_step(g4r_handle* h, const int* base, int off);
+static int64_t full_launches_per_step(const g4r_handle* h);
+static void full_mark_inputs(g4r_handle* h, int64_t n);
+static int full_opt_in(g4r_handle* h);
+static bool wgmma_tiles(const g4r_config& cfg, int lanes, int n_comp, int n_items);
 
 // sharded: row i of the logical [rows x cols] tensor lives on rank i % R at local row i / R; seg_off = byte offset of element
 // (0, 0) inside every rank's peer-mapped segment (g4r_shard.cuh)
@@ -59,6 +64,32 @@ struct BpttDev {
   int *M, *N, *X, *Slot; uint8_t* F; uint32_t* G;   // per step: lanes, columns, inputs, slots, flags, dropout step
   unsigned long long *keys, *keys2;                  // [T][B + NP] merged row list, unsorted / sorted
 };
+
+// full-softmax training (g4r_full.cuh): every step scores the whole catalogue, on fp32 tiles of FS_IT items or on the wgmma
+// tiles of the evaluation path (FS_TC_M lanes x FS_TC_N items, K chunks of FS_TC_KC), whose statistics come per FS_TC_N / 2 items
+constexpr int FS_IT = 64;          // items per fp32 score tile (== EV_IT of the fp32 evaluation tiles it reuses)
+constexpr int FS_TC_M = 128, FS_TC_N = 256, FS_TC_KC = 32;   // == TC_M, TC_N, TC_KC (g4r_eval_tc.cuh)
+struct FullDev {
+  float* dO;                       // [n_items][Bld] dL/do of the step, item-major (lanes contiguous)
+  float* stat;                     // [tiles][B][4] per-(tile, lane) max, sum-exp, target score, has-target
+  int tiles, ks, kchunk;           // statistics tiles; K splits of dL/dy = dO . Wy and the items per split (a multiple of GK)
+  bool tc;                         // score sweeps on the wgmma 3xTF32 tiles (chosen like the evaluation's, wgmma_tiles)
+  int chunks;                      // wgmma: K chunks of L + 1 (the bias column)
+  unsigned char *Asplit, *Bsplit;  // wgmma: [hi | lo] blocks of y (per step) and of Wy | By (per step: every row changes)
+};
+static FullDev full_shape(const g4r_config& c, int n_sm) {
+  FullDev f; memset(&f, 0, sizeof(f));
+  const int L = c.layers[c.n_layers - 1];
+  f.tc = wgmma_tiles(c, c.batch_size, c.n_items, c.n_items);
+  f.chunks = (L + 1 + FS_TC_KC - 1) / FS_TC_KC;
+  f.tiles = f.tc ? 2 * ((c.n_items + FS_TC_N - 1) / FS_TC_N) : (c.n_items + FS_IT - 1) / FS_IT;
+  const int mn = ((c.batch_size + GB - 1) / GB) * ((L + GB - 1) / GB);
+  const int slabs = (c.n_items + GK - 1) / GK;
+  int ks = std::max(1, std::min(slabs, (2 * n_sm + mn - 1) / mn));
+  f.kchunk = ((slabs + ks - 1) / ks) * GK;
+  f.ks = (c.n_items + f.kchunk - 1) / f.kchunk;          // no empty splits
+  return f;
+}
 
 struct g4r_handle {
   g4r_config cfg;
@@ -109,6 +140,7 @@ struct g4r_handle {
   bool tc_ok = false; void* ts_buf = nullptr; unsigned long long* ts_dbg = nullptr; cudaStream_t side = nullptr, side2 = nullptr; cudaEvent_t ts_ev[12] = {};      // tensor-core training step (g4r_tcstep.cuh): TsBuf*
   std::vector<cudaEvent_t> prof_ev; std::vector<int> prof_phase;
   BpttDev bw = {}; void* bptt_cub = nullptr; size_t bptt_cub_bytes = 0; int64_t bptt_windows = 0;   // bptt > 1 (g4r_bptt.cuh)
+  FullDev fs = {}; int64_t full_steps = 0;                                                            // full_softmax (g4r_full.cuh)
 };
 
 enum { PH_GATHER = 0, PH_F1, PH_F2, PH_SCORE, PH_STATS, PH_LOSSGRAD, PH_B1, PH_B2, PH_B3, PH_DENSE, PH_SPARSE_IN, PH_STATS2, PH_GRADCAP, PH_COUNT };
@@ -168,6 +200,14 @@ static int validate_config(const g4r_config& c, std::string& err) {
   if (c.n_sample < 0) { err = "n_sample < 0"; return G4R_ERR_INVALID; }
   if (c.bptt < 0 || c.bptt > 64) { err = "bptt must be in [1, 64]"; return G4R_ERR_INVALID; }
   if (c.bptt > 1 && c.world_size > 1) { err = "bptt > 1 is a single-GPU option"; return G4R_ERR_INVALID; }
+  if (c.full_softmax != 0 && c.full_softmax != 1) { err = "full_softmax must be 0 or 1"; return G4R_ERR_INVALID; }
+  if (c.full_softmax) {
+    if (c.loss != G4R_LOSS_XE && c.loss != G4R_LOSS_XE_LOGIT) { err = "full_softmax: only loss cross-entropy / softmax and xe_logit / softmax_logit are implemented"; return G4R_ERR_INVALID; }
+    if (c.smoothing > 0.f) { err = "full_softmax: label smoothing is not implemented"; return G4R_ERR_INVALID; }
+    if (c.grad_cap > 0.f) { err = "full_softmax: grad_cap is not implemented"; return G4R_ERR_INVALID; }
+    if (c.bptt > 1) { err = "full_softmax: bptt > 1 is not implemented"; return G4R_ERR_INVALID; }
+    if (c.world_size > 1) { err = "full_softmax is a single-GPU option"; return G4R_ERR_INVALID; }
+  }
   return G4R_OK;
 }
 
@@ -186,7 +226,8 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
   const bool mom = c.momentum > 0.f;
   const bool ada = c.adapt != G4R_ADAPT_NONE;            // at least one adaptive state array ("acc")
   const int nacc = opt_states(c.adapt);                  // acc | acc, upd | acc, meang, countt -- stacked behind `*.acc`
-  const int gen_len = (c.n_sample > 0 && c.sample_store > 0) ? c.sample_store / c.n_sample : 0;
+  const bool full = c.full_softmax != 0;                 // the catalogue is the score column list: no sample store (DESIGN §3n)
+  const int gen_len = (!full && c.n_sample > 0 && c.sample_store > 0) ? c.sample_store / c.n_sample : 0;
   const bool store = gen_len > 1;
   const int S = store ? c.n_sample : 0;
   const int NP = round4(B + S);
@@ -198,7 +239,7 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
   md.NP = NP; md.NCH = NCH; md.CAP = CAP; md.S_cfg = c.n_sample; md.shardR = shard ? R : 0;
   md.loss = c.loss; md.fact = {c.final_act, c.final_act_p1, c.final_act_p2}; md.hact = {c.hidden_act, c.hidden_act_p1, c.hidden_act_p2};
   md.p_drop_h = c.dropout_p_hidden; md.p_drop_e = c.dropout_p_embed; md.lr = c.learning_rate; md.mom = c.momentum; md.lmbd = c.lmbd;
-  md.bpreg = c.bpreg; md.logq = c.logq; md.alpha = c.sample_alpha; md.adapt = c.adapt;
+  md.bpreg = c.bpreg; md.logq = full ? 0.f : c.logq; md.alpha = c.sample_alpha; md.adapt = c.adapt;   // logq corrects a sampled softmax only
   md.ap1 = c.adapt_p1; md.ap1c = c.adapt_p1c; md.ap2 = c.adapt_p2; md.ap2c = c.adapt_p2c; md.grad_cap = c.grad_cap;
   md.smoothing = (c.loss == G4R_LOSS_XE || c.loss == G4R_LOSS_XE_LOGIT) ? c.smoothing : 0.f;    // the other losses ignore it (gru4rec.py:237-248)
   md.drop_seed = c.dropout_seed + (c.world_size > 1 ? (uint32_t)c.rank * 0x9E3779B1u : 0u);   // multi-GPU: independent masks per rank
@@ -248,7 +289,8 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
   // step scratch
   md.O = cv.take<float>((size_t)NP * md.Bld);
   md.DSY = cv.take<float>((size_t)NP * ldL); md.DBY = cv.take<float>((size_t)NP);
-  md.part = cv.take<float>((size_t)NCH * B * ldL);
+  const FullDev fsh = full ? full_shape(c, n_sm) : FullDev{};
+  md.part = cv.take<float>((size_t)std::max(NCH, fsh.ks) * B * ldL);    // full_softmax: the K-split partials of dL/dy
   md.stat = cv.take<float>((size_t)NCH * B * G4R_NSTAT);
   md.RS = cv.take<float>((size_t)Bmax * G4R_NSTAT);
   md.stat2 = md.smoothing > 0.f ? cv.take<float>((size_t)NCH * B * 2) : nullptr;
@@ -357,6 +399,15 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     bw.F = cv.take<uint8_t>(TB); bw.G = cv.take<uint32_t>(c.bptt);
     bw.keys = cv.take<unsigned long long>((size_t)c.bptt * (B + NP)); bw.keys2 = cv.take<unsigned long long>((size_t)c.bptt * (B + NP));
   }
+  // full-softmax training: dL/do of the step over the catalogue, per-tile row statistics
+  FullDev fs = fsh;
+  if (full) {
+    fs.dO = cv.take<float>((size_t)c.n_items * md.Bld); fs.stat = cv.take<float>((size_t)fsh.tiles * B * 4);
+    if (fsh.tc) {
+      fs.Asplit = cv.take<unsigned char>((size_t)((B + FS_TC_M - 1) / FS_TC_M) * fsh.chunks * 2 * FS_TC_M * FS_TC_KC * 4);
+      fs.Bsplit = cv.take<unsigned char>((size_t)((c.n_items + FS_TC_N - 1) / FS_TC_N) * fsh.chunks * 2 * FS_TC_N * FS_TC_KC * 4);
+    }
+  }
   // evaluation
   int* dRank = cv.take<int>((size_t)Be * 4); float* dTgt = cv.take<float>((size_t)Be * 3);   // target scores | lower | upper pre-activation thresholds (tensor-core ranking)
   if (!cv.dry) {
@@ -371,8 +422,8 @@ static void layout(const g4r_config& c, Carver& cv, g4r_handle* h, int n_sm) {
     h->shard_ws = shard_ws; h->shard_ws_bytes = shard_ws_bytes;
     h->tc_ok = tc;
     if (tc) { if (!h->ts_buf) h->ts_buf = new TsBuf(); *static_cast<TsBuf*>(h->ts_buf) = tsb; }
-    h->bw = bw;
-    h->dGscale = gsc; h->two_pass = c.grad_cap > 0.f; h->phase_only = c.grad_cap > 0.f || md.smoothing > 0.f;
+    h->bw = bw; h->fs = fs;
+    h->dGscale = gsc; h->two_pass = c.grad_cap > 0.f; h->phase_only = c.grad_cap > 0.f || md.smoothing > 0.f || full;
   }
 }
 
@@ -516,7 +567,7 @@ static int tiles2(int cols, int rows) { return ((cols + GB - 1) / GB) * ((rows +
 // automatically for wide layers (L >= 160), or for any such model with step_mode 4.
 static bool tc_eligible(const g4r_config& c) {
   if (!c.constrained_embedding || c.n_layers != 1 || c.batch_size > 256 || (c.layers[0] & 3)) return false;
-  if (c.adapt > G4R_ADAPT_ADAGRAD || c.grad_cap > 0.f || c.smoothing != 0.f || c.world_size > 1 || c.bptt > 1) return false;
+  if (c.adapt > G4R_ADAPT_ADAGRAD || c.grad_cap > 0.f || c.smoothing != 0.f || c.world_size > 1 || c.bptt > 1 || c.full_softmax) return false;
   return c.step_mode == 4 || (c.step_mode >= 1 && c.step_mode <= 3 && c.layers[0] >= 160);
 }
 // G4R_TS_STAMP=1: per-product phase timeline of the last step (median / max over the CTAs, microseconds after the first CTA's entry)
@@ -674,8 +725,8 @@ static int enqueue_tc_step(g4r_handle* h, const int* base, int off) {
   return G4R_OK;
 }
 
-// the forward and score phases of one step, through the loss gradient (window-relative index = *base + off when base != nullptr)
-static void enqueue_forward_scores(g4r_handle* h, const int* base, int off) {
+// the input gather and the GRU forward of one training step (window-relative index = *base + off when base != nullptr)
+static void enqueue_forward(g4r_handle* h, const int* base, int off) {
   const ModelDev& md = h->md;
   cudaStream_t st = h->stream;
   const int B = md.B;
@@ -685,6 +736,13 @@ static void enqueue_forward_scores(g4r_handle* h, const int* base, int off) {
     LAUNCH(PH_F1, k_f1<<<tiles2(2 * ly.L, B), GEMM_THREADS, 0, st>>>(h->slot, base, off, li, ly.H));
     LAUNCH(PH_F2, k_f2<<<tiles2(ly.L, B), GEMM_THREADS, 0, st>>>(h->slot, base, off, li, ly.H, 1));
   }
+}
+// the forward and score phases of one step, through the loss gradient
+static void enqueue_forward_scores(g4r_handle* h, const int* base, int off) {
+  const ModelDev& md = h->md;
+  cudaStream_t st = h->stream;
+  const int B = md.B;
+  enqueue_forward(h, base, off);
   LAUNCH(PH_SCORE, k_score<<<md.NCH, SC_THREADS, score_smem_bytes(md.Bld), st>>>(h->slot, base, off));
   LAUNCH(PH_STATS, k_stats<<<B, 256, 256 * sizeof(float), st>>>(h->slot, base, off));
   if (md.smoothing > 0.f) {      // label smoothing: second statistics pass once the row maxima / normalisers are final
@@ -694,16 +752,14 @@ static void enqueue_forward_scores(g4r_handle* h, const int* base, int off) {
   LAUNCH(PH_LOSSGRAD, k_lossgrad<<<md.NCH, SC_THREADS, lossgrad_smem_bytes(md.Bld, md.ldL), st>>>(h->slot, base, off));
 }
 
-// enqueue the kernels of one training step (window-relative index = *base + off when base != nullptr)
-static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
-  if (h->tc_ok) return enqueue_tc_step(h, base, off);
+// the backward phases and updates of one step once dL/dy of the top layer is in md.part (nch partials; 0: one per column chunk)
+static void enqueue_backward(g4r_handle* h, const int* base, int off, int nch) {
   const ModelDev& md = h->md;
   cudaStream_t st = h->stream;
   const int B = md.B;
-  enqueue_forward_scores(h, base, off);
   for (int li = md.n_layers - 1; li >= 0; li--) {
     const LayerDev& ly = md.layer[li];
-    LAUNCH(PH_B1, k_b1<<<std::max(1, std::min(h->n_sm, (B * ly.L * 8 + 255) / 256)), 256, 0, st>>>(h->slot, base, off, li, 0));
+    LAUNCH(PH_B1, k_b1<<<std::max(1, std::min(h->n_sm, (B * ly.L * 8 + 255) / 256)), 256, 0, st>>>(h->slot, base, off, li, nch));
     LAUNCH(PH_B2, k_b2<<<tiles2(ly.L, B), GEMM_THREADS, 0, st>>>(h->slot, base, off, li));
     if (ly.in_dim > 0) LAUNCH(PH_B3, k_b3<<<tiles2(ly.in_dim, B), GEMM_THREADS, 0, st>>>(h->slot, base, off, li));
     const DenseJobs dj = dense_jobs(ly.L, ly.in_dim);
@@ -718,6 +774,14 @@ static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
     for (const MgTensor& t : h->mg_tensors) LAUNCH(PH_GRADCAP, k_apply_dense<<<(t.count + 255) / 256, 256, 0, st>>>(h->slot, t.p, t.acc, t.vel, mg.gradFlat + t.goff, t.count));
     LAUNCH(PH_GRADCAP, k_sparse_in<<<B, 128, 0, st>>>(h->slot, base, off, 1));
   }
+}
+
+// enqueue the kernels of one training step (window-relative index = *base + off when base != nullptr)
+static int enqueue_train_step(g4r_handle* h, const int* base, int off) {
+  if (h->tc_ok) return enqueue_tc_step(h, base, off);
+  if (h->cfg.full_softmax) return enqueue_full_step(h, base, off);
+  enqueue_forward_scores(h, base, off);
+  enqueue_backward(h, base, off, 0);
   return G4R_OK;
 }
 
@@ -810,7 +874,10 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
     if (workspace_bytes < need) return bail(G4R_ERR_INVALID, "workspace too small");
     h->ws = (char*)device_workspace; h->own_ws = false;
   } else {
-    if (cudaMalloc(&h->ws, need) != cudaSuccess) return bail(G4R_ERR_CUDA, "cudaMalloc of workspace failed");
+    if (cudaMalloc(&h->ws, need) != cudaSuccess) {
+      if (cfg->full_softmax) return bail(G4R_ERR_INVALID, "full_softmax: the workspace of " + std::to_string(need) + " bytes does not fit in device memory");
+      return bail(G4R_ERR_CUDA, "cudaMalloc of workspace failed");
+    }
     h->own_ws = true;
   }
   h->ws_bytes = need;
@@ -877,6 +944,7 @@ extern "C" int g4r_create(const g4r_config* cfg, void* device_workspace, size_t 
     if (ts_opt_in(h) != G4R_OK) return bail(G4R_ERR_CUDA, "k_ts_gemm: shared memory / cluster opt-in failed");
     h->fast_ok = false; h->fastc_ok = false;
   }
+  if (cfg->full_softmax && full_opt_in(h) != G4R_OK) return bail(G4R_ERR_INVALID, "full_softmax: this batch size needs more shared memory per block than the device offers");
   if (cfg->step_mode == 1 && h->pk_blocks == 0) return bail(G4R_ERR_INVALID, "persistent mode unavailable (cooperative launch / shared memory)");
   if (h->md.shardR > 0) {
     const int src = shard_create(h);
@@ -1310,6 +1378,7 @@ static int upload_window(g4r_handle* h, int64_t n) {
   CK(cudaMemsetAsync(h->md.nanflag + 2, 0, sizeof(int), st));
   k_plan<<<(unsigned)n, 256, (size_t)h->npow2 * 8 + 1024, st>>>(h->md, h->dXnext, h->dXflag, h->npow2);
   h->launches++;
+  if (h->cfg.full_softmax) full_mark_inputs(h, n);
   CK(cudaGetLastError());
   h->win_steps = (int)n;
   if (h->shard) return mgs_plan_window(h, n);
@@ -1331,6 +1400,7 @@ static int build_graph(g4r_handle* h, int unroll, cudaGraphExec_t* out) {
 static int64_t launches_per_step(const g4r_handle* h) {
   const ModelDev& md = h->md;
   if (h->tc_ok) return 25;
+  if (h->cfg.full_softmax) return full_launches_per_step(h);
   int64_t n = (md.mode != 0 ? 1 : 0) + 4;        // gather + score/stats/lossgrad + sparse_in
   for (int li = 0; li < md.n_layers; li++) n += 2 + 2 + (md.layer[li].in_dim > 0 ? 1 : 0) + 1;
   if (md.smoothing > 0.f) n += 2;
@@ -1382,6 +1452,7 @@ static int run_window(g4r_handle* h, int64_t n) {
   CK(cudaGetLastError());
   if (h->gen_len > 0) h->sample_ptr += n;
   h->global_step += (uint32_t)n;
+  if (h->cfg.full_softmax) h->full_steps += n;
   return G4R_OK;
 }
 
@@ -1467,6 +1538,7 @@ extern "C" int64_t g4r_fast_windows(const g4r_handle* h, int64_t* fallback_windo
   return h->fast_windows;
 }
 extern "C" int64_t g4r_bptt_windows(const g4r_handle* h) { return h ? h->bptt_windows : 0; }
+extern "C" int64_t g4r_full_steps(const g4r_handle* h) { return h ? h->full_steps : 0; }
 extern "C" const char* g4r_phase_name(int32_t i) { return (i >= 0 && i < PH_COUNT) ? kPhaseNames[i] : ""; }
 extern "C" int g4r_phase_count(void) { return PH_COUNT; }
 
@@ -1676,5 +1748,6 @@ extern "C" int g4r_copy_item_tables(g4r_handle* h, g4r_handle* src, const float*
 }
 
 #include "g4r_eval.cuh"
+#include "g4r_full.cuh"
 #include "g4r_baselines.cuh"
 #include "g4r_bpr.cuh"

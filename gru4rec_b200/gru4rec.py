@@ -103,6 +103,7 @@ class GRU4Rec:
         self.step_mode = 2               # role-specialised persistent kernel where the shape allows, else generic persistent
         self.session_capacity = 100000   # sessions kept by recommend_sessions / feed_sessions (least recently used evicted)
         self.bptt = 1                    # > 1: truncated backpropagation through time, one update per window of bptt mini-batches (DESIGN §3l)
+        self.full_softmax = False        # True: every training step scores and updates the whole catalogue, no sampling (DESIGN §3n)
         self._engine = None
         self._host = None                # numpy copies of the parameters when no engine is alive
 
@@ -266,6 +267,7 @@ class GRU4Rec:
         cfg.eval_batch_size = eval_lanes
         cfg.step_mode = self.step_mode
         cfg.bptt = int(self.bptt) if training else 1
+        cfg.full_softmax = 1 if (training and self.full_softmax) else 0
         if self.step_mode == 2 and len(self.layers) == 1 and 120 < self.layers[0] <= 128 and not self.constrained_embedding and not self.embedding and self.batch_size <= 32:
             cfg.step_mode = 3        # the 48-CTA GRU group of step_mode 2 covers 120 hidden units; the cluster variant takes up to 128
         return cfg
@@ -396,7 +398,11 @@ class GRU4Rec:
                 P0[P0 == 0] = absent_logq
         generate_length = 0
         use_store = False
-        if self.n_sample:
+        self._check_full_softmax()
+        if self.full_softmax:
+            P0 = None
+            print('Full softmax: every item is a score column of every mini-batch; n_sample, sample_alpha and logq (the correction of a sampled softmax) are not used')
+        elif self.n_sample:
             pop = pop[self.itemidmap.index.values].values ** self.sample_alpha
             pop = pop.cumsum() / pop.sum()
             pop[-1] = 1
@@ -417,7 +423,7 @@ class GRU4Rec:
                 print('No example store was used')
         per_step_sampling = False
         self._check_bptt(store_type)
-        if self.n_sample and not use_store:
+        if self.n_sample and not use_store and not self.full_softmax:
             if store_type == 'cpu':
                 # gru4rec.py:612-613: without a store every mini-batch draws its own row on the host (generate_neg_samples(pop, 1))
                 per_step_sampling = True
@@ -471,6 +477,22 @@ class GRU4Rec:
             raise NotImplementedError('bptt > 1 trains on one GPU; truncated BPTT over several GPUs is not implemented')
         if self.n_sample and store_type == 'cpu':
             raise NotImplementedError("bptt > 1 draws its negatives from the device sample store: store_type='cpu' is not implemented")
+
+    def _check_full_softmax(self):
+        '''the training options full_softmax does not cover, refused before any engine is built'''
+        if not self.full_softmax:
+            return
+        if (self.loss, self.final_act) not in (('cross-entropy', 'softmax'), ('xe_logit', 'softmax_logit')):
+            raise NotImplementedError("full_softmax trains loss='cross-entropy' with final_act='softmax' or loss='xe_logit' with "
+                                      "final_act='softmax_logit'; got %r / %r" % (self.loss, self.final_act))
+        if self.smoothing > 0:
+            raise NotImplementedError('full_softmax with label smoothing is not implemented')
+        if self.grad_cap > 0:
+            raise NotImplementedError('full_softmax with grad_cap is not implemented')
+        if int(self.bptt) > 1:
+            raise NotImplementedError('full_softmax with bptt > 1 is not implemented')
+        if self._world()[0] > 1:
+            raise NotImplementedError('full_softmax trains on one GPU; the full catalogue over several GPUs is not implemented')
 
     def _epochs(self, plan, epochs=None, every=None, resume=None):
         '''The epoch loop of fit() (gru4rec.py:586-664) as a generator: it yields a progress record wherever a checkpoint may be
@@ -593,7 +615,8 @@ class GRU4Rec:
         ids = np.asarray(self.itemidmap.index.values)
         ids_are_objects = ids.dtype.kind not in 'iufUS'          # item ids read as str: stored as a fixed-width string array
         meta = dict(version=self._CKPT_VERSION, params=self._ctor_params(), n_items=int(self.n_items), ids_are_objects=bool(ids_are_objects),
-                    engine=dict(dropout_seed=int(self.dropout_seed), step_mode=int(self.step_mode), bptt=int(self.bptt)),
+                    engine=dict(dropout_seed=int(self.dropout_seed), step_mode=int(self.step_mode), bptt=int(self.bptt),
+                                full_softmax=bool(self.full_softmax)),
                     has_state=st is not None, sample_store=None if st is None else st['sample_store'], has_store=st is not None and st['store'] is not None,
                     fingerprint=_fingerprint, progress=None)
         arrays = {'itemids': ids.astype(str) if ids_are_objects else ids}
@@ -650,6 +673,7 @@ class GRU4Rec:
         gru = cls(**meta['params'])
         gru.dropout_seed, gru.step_mode = meta['engine']['dropout_seed'], meta['engine']['step_mode']
         gru.bptt = int(meta['engine'].get('bptt', 1))             # written before bptt existed: one update per mini-batch
+        gru.full_softmax = bool(meta['engine'].get('full_softmax', False))    # written before full_softmax existed: sampled columns
         ids = ck['itemids'].astype(object) if meta['ids_are_objects'] else ck['itemids']
         gru.predict = None
         gru.error_during_train = False
@@ -763,12 +787,13 @@ class GRU4Rec:
     def _grow_engine(self, n_store, rows):
         '''the training engine for the catalogue as it is now, holding everything the present engine holds (fit_more)'''
         old = self._engine
-        if int(old.cfg.n_items) == self.n_items and int(old.cfg.sample_store) == int(n_store) and int(old.cfg.bptt) == int(self.bptt):
+        if int(old.cfg.n_items) == self.n_items and int(old.cfg.sample_store) == int(n_store) and int(old.cfg.bptt) == int(self.bptt) and \
+                bool(old.cfg.full_softmax) == bool(self.full_softmax):
             return old
         sessions = (old.session_capacity, old.sessions_export()) if getattr(old, 'session_capacity', None) is not None else None
         eng = _lib.Engine(self._make_config(n_store, 0, True, single=True), device=self.device)
         eng.copy_item_tables(old, **rows)
-        if int(old.cfg.sample_store):      # (an engine built only to hold a loaded model has no streams to continue)
+        if int(old.cfg.sample_store) or int(old.cfg.full_softmax):   # (an engine built only to hold a loaded model has no streams to continue)
             try:
                 eng.train_state_import(old.train_state_export())
             except NotImplementedError:
@@ -1087,7 +1112,7 @@ class GRU4Rec:
         self._host = host
         self._engine = None
         self.predict = None
-        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2), ('session_capacity', 100000), ('bptt', 1)):
+        for k, v in (('device', 0), ('dropout_seed', 0), ('eval_lanes', 512), ('step_mode', 2), ('session_capacity', 100000), ('bptt', 1), ('full_softmax', False)):
             if not hasattr(self, k):
                 setattr(self, k, v)
 

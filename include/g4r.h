@@ -70,7 +70,8 @@ typedef struct g4r_config {
                                      4: tensor-core step (wgmma GEMMs) whenever the model allows it -- modes 1-3 pick it
                                         automatically for constrained-embedding models with a layer of >= 160 units */
   int32_t mg_replicated;          /* 1: multi-GPU with replicated tables + NCCL exchange instead of row sharding */
-  int32_t eval_tc;                /* scoring path: 0 auto, 1 fp32 FFMA tiles only, 2 wgmma (3xTF32) tiles whenever the ranking is full-catalogue */
+  int32_t eval_tc;                /* scoring path: 0 auto, 1 fp32 FFMA tiles only, 2 wgmma (3xTF32) tiles whenever the ranking is full-catalogue;
+                                     also the score tiles of full_softmax training (auto: wgmma from 64 lanes and 2048 items) */
   float adapt_p1, adapt_p1c;      /* adapt_params[0] and 1 - adapt_params[0] (rmsprop / adadelta decay; adam beta1), gru4rec.py:301-304,342-343,368-369 */
   float adapt_p2, adapt_p2c;      /* adapt_params[1] and 1 - adapt_params[1] (adam beta2) */
   float grad_cap;                 /* > 0: gradients are scaled to this global L2 norm when they exceed it (gru4rec.py:386-389) */
@@ -79,6 +80,11 @@ typedef struct g4r_config {
                                      has no effect.  g4r_train_steps / g4r_upload_steps then take ranges that start at a multiple
                                      of bptt and hold whole windows unless they run to the schedule's end (else G4R_ERR_INVALID);
                                      g4r_train_step and g4r_profile_uploaded return G4R_ERR_STATE */
+  int32_t full_softmax;           /* 0: sampled output layer (Y | samples).  1: every training step scores the whole catalogue 0..n_items-1,
+                                     each item once, and updates every Wy / By row (DESIGN §3n).  loss XE / softmax or xe_logit /
+                                     softmax_logit only; logq, n_sample, sample_alpha and sample_store are ignored (no sample store
+                                     is allocated).  Refused (G4R_ERR_INVALID): smoothing > 0, grad_cap > 0, bptt > 1, world_size > 1.
+                                     step_mode has no effect */
 } g4r_config;
 
 typedef struct g4r_handle g4r_handle;
@@ -174,6 +180,8 @@ const char* g4r_phase_name(int32_t i);
 int64_t g4r_fast_windows(const g4r_handle* h, int64_t* fallback_windows);
 /* bptt > 1: number of windows trained (each one backward through time and one update) */
 int64_t g4r_bptt_windows(const g4r_handle* h);
+/* full_softmax = 1: number of training steps run against the whole catalogue */
+int64_t g4r_full_steps(const g4r_handle* h);
 /* 1 if the handle trains with the tensor-core step (wgmma 3xTF32 GEMMs with fused epilogues, csrc/g4r_tcstep.cuh): constrained
  * embedding, one layer, batch <= 256, SGD / Adagrad (+momentum); automatic for layers >= 160 units, forced with step_mode 4. */
 int g4r_uses_tensor_cores(const g4r_handle* h);
