@@ -51,6 +51,7 @@ EXPORTS = [
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
+    'g4r_bl_sknn_fit',
 ]
 
 _lib = None
@@ -152,6 +153,7 @@ def load():
     lib.g4r_bl_bpr_iterate.argtypes = [vp, vp, vp, f64, f64, f64, i32, C.POINTER(f64), C.POINTER(i64), C.POINTER(C.c_float)]
     lib.g4r_bl_bpr_export.argtypes = [vp, vp, vp]
     lib.g4r_bl_bpr_import.argtypes = [vp, vp, vp]
+    lib.g4r_bl_sknn_fit.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32]
     _lib = lib
     return lib
 
@@ -776,13 +778,14 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5}
+SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 
 
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
-    a baseline, and the BPR-MF fit and factors (DESIGN §3k).  kind: 'pop', 'sessionpop', 'itemknn' or 'bpr'; n_keep: top_n,
-    n_sims or n_factors."""
+    a baseline, the BPR-MF fit and factors (DESIGN §3k), and the SessionKNN index (DESIGN §3o).  kind: 'pop', 'sessionpop',
+    'itemknn', 'bpr' or 'sknn'; n_keep: top_n, n_sims, n_factors or k."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -902,3 +905,15 @@ class Baselines(object):
         if I.shape != (self.n_items, self.n_keep) or bI.size != self.n_items:
             raise ValueError('bpr_import: need I [n_items, n_factors] and bI [n_items]')
         self._check(self.lib.g4r_bl_bpr_import(self.h, _ptr(I), _ptr(bI)))
+
+    def sknn_fit(self, session_offsets, items, recency, sample_size, similarity):
+        """the SessionKNN index: the training sessions' distinct items ascending as CSR, each session's recency rank (0: most
+        recent), sample_size and 'cosine' / 'vector'"""
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        rc = np.ascontiguousarray(recency, dtype=np.int32)
+        if rc.size != off.size - 1:
+            raise ValueError('sknn_fit: need one recency rank per session')
+        if similarity not in SKNN_SIMILARITY:
+            raise ValueError('sknn_fit: similarity must be one of %s' % sorted(SKNN_SIMILARITY))
+        self._check(self.lib.g4r_bl_sknn_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(rc), int(sample_size),
+                                             SKNN_SIMILARITY[similarity]))

@@ -1,5 +1,6 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
-signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids).  ItemKNN's fit runs on the device (the
+signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), and session-based kNN (SessionKNN, DESIGN
+§3o) with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -254,3 +255,117 @@ class BPR(Baseline):
         uF = self.I[self.session].mean(axis=0)
         iIdxs = self.itemidmap[predict_for_item_ids]
         return pd.Series(data=self.I[iIdxs].dot(uF) + self.bI[iIdxs], index=predict_for_item_ids)
+
+
+class SessionKNN(Baseline):
+    '''
+    SessionKNN(k=100, sample_size=500, similarity='cosine', session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Session-based kNN: S-KNN (similarity='cosine', Jannach & Ludewig, RecSys 2017) and a position-weighted variant in the style
+    of V-SKNN (similarity='vector', Ludewig & Jannach, UMUAI 2018).  These are this project's definitions of the two methods
+    (DESIGN §3o); they are not claimed to match any other implementation bit for bit.
+
+    A training session s has its distinct items I(s) and time T(s), the largest time_key of its events; the recency order sorts
+    the sessions by T descending, then by first appearance in the training data.  For the session's inputs so far c = (x_1 ..
+    x_t), the current input included, the candidates are the first sample_size sessions in recency order that share an item
+    with c.  Their similarity is |I(c) & I(s)| / sqrt(|I(c)| |I(s)|) ('cosine'), or ('vector') the sum, in order of position,
+    of w(i) = p / t over the shared items, p the position of i's last occurrence in c.  The k most similar candidates (ties: the
+    more recent) are the neighbours; item j scores the sum of the similarities of the neighbours that contain j, in float64 in
+    neighbour order, and every other item scores 0.  Items of the current session are scored like any others.  evaluate_gpu /
+    evaluate_events rank every event on the device; predict_next computes the same scores on the host.
+    '''
+    _kind = 'sknn'
+
+    def __init__(self, k=100, sample_size=500, similarity='cosine', session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.k = k
+        self.sample_size = sample_size
+        self.similarity = similarity
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.k
+
+    def fit(self, data):
+        if self.similarity not in _lib.SKNN_SIMILARITY:
+            raise ValueError('similarity must be one of %s, not %r' % (sorted(_lib.SKNN_SIMILARITY), self.similarity))
+        if not 1 <= self.sample_size <= 8192:
+            raise ValueError('sample_size must be in 1 .. 8192, not %r' % (self.sample_size,))
+        if not 1 <= self.k <= min(self.sample_size, 1024):
+            raise ValueError('k must be in 1 .. min(sample_size, 1024), not %r' % (self.k,))
+        idx = self._index(data).astype(np.int64)
+        sess = data[self.session_key].values
+        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
+        self.n_sessions = S = int(code.max()) + 1 if len(code) else 0
+        T = pd.Series(data[self.time_key].values).groupby(code).max().values
+        order = np.argsort(-T, kind='stable')                    # T descending, ties by first appearance
+        self.recency = np.empty(S, np.int32)
+        self.recency[order] = np.arange(S, dtype=np.int32)
+        pairs = np.unique(code.astype(np.int64) * self.n_items + idx)   # (session, item) distinct, items ascending per session
+        self.session_items = (pairs % self.n_items).astype(np.int32)
+        self.session_offsets = np.zeros(S + 1, np.int64)
+        self.session_offsets[1:] = np.cumsum(np.bincount(pairs // self.n_items, minlength=S))
+        self.current_session = None
+        self.__dict__.pop('_dev', None)
+        self.__dict__.pop('_post', None)
+        self._device()
+
+    def _upload(self, dev):
+        dev.sknn_fit(self.session_offsets, self.session_items, self.recency, self.sample_size, self.similarity)
+
+    def __getstate__(self):
+        state = Baseline.__getstate__(self)
+        state.pop('_post', None)
+        return state
+
+    def _postings(self):
+        """(per item offsets, the ranks of its sessions ascending, the session of each rank), built on first use"""
+        post = self.__dict__.get('_post')
+        if post is None:
+            rank = np.repeat(self.recency, np.diff(self.session_offsets))
+            o = np.lexsort((rank, self.session_items))
+            ioff = np.zeros(self.n_items + 1, np.int64)
+            ioff[1:] = np.cumsum(np.bincount(self.session_items, minlength=self.n_items))
+            post = self._post = (ioff, rank[o], np.argsort(self.recency))
+        return post
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        prefix = np.asarray(prefix, dtype=np.int64)
+        t = len(prefix)
+        u, first_rev = np.unique(prefix[::-1], return_index=True)
+        last = t - first_rev                                      # 1-based position of the last occurrence
+        o = np.argsort(last)
+        ci, pos = u[o], last[o]
+        ioff, ranks, by_rank = self._postings()
+        S = self.sample_size
+        cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
+        sess = by_rank[cand]
+        starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
+        owner = np.repeat(np.arange(len(cand)), lens)
+        flat = self.session_items[np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())]
+        sims, cnt = np.zeros(len(cand)), np.zeros(len(cand), np.int64)
+        for m, i in enumerate(ci):                                # c's items in order of their last position
+            hit = np.zeros(len(cand), bool)
+            hit[owner[flat == i]] = True
+            cnt += hit
+            sims = sims + np.where(hit, pos[m] / t, 0.0)
+        if self.similarity == 'cosine':
+            sims = cnt / np.sqrt((len(ci) * lens).astype(np.float64))
+        score = np.zeros(self.n_items)
+        for q in np.lexsort((cand, -sims))[:self.k]:
+            j = flat[owner == q]
+            score[j] = score[j] + sims[q]
+        return score
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        x = self.itemidmap[input_item_id]
+        if self.current_session is None or self.current_session != session_id:
+            self.current_session = session_id
+            self.session = [x]
+        else:
+            self.session.append(x)
+        score = self.score_prefix(self.session)
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)

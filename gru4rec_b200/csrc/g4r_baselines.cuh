@@ -4,7 +4,7 @@
 // nothing here touches a g4r_handle.
 #pragma once
 
-constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3;
+constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5;   // 4 stays unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
@@ -37,6 +37,12 @@ struct g4r_baselines {
   size_t bpr_cub_bytes = 0;
   int bpr_end_bit = 64;
   unsigned bpr_tag = 0;                                 // the iteration's done-flag value (flags are never cleared)
+  // SessionKNN (g4r_sknn.cuh): training sessions by recency rank (distinct items ascending), every item's sessions by rank
+  int64_t *dSkOff = nullptr, *dSkIoff = nullptr;
+  int *dSkItem = nullptr, *dSkIsess = nullptr;
+  std::vector<void*> sknn_mem;
+  int64_t sk_sessions = 0, sk_zmax = 0;                 // sk_zmax: distinct items of the n_keep longest training sessions
+  int sk_sample = 0, sk_sim = 0;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -388,6 +394,9 @@ __device__ __forceinline__ long long bl_w(const BlEvalDev& d, int j) { return d.
 __device__ __forceinline__ bool bl_eligible(const BlEvalDev& d, const int* pl, const int* pc, int n, int j) {
   return (!d.mult || d.mult[j] > 0) && !(d.exclude && bl_plcount(pl, pc, n, j) > 0);
 }
+// the competitors outside a scored set all score 0: they tie a target that scores 0 (sx: weight of the competitors the caller
+// accounted for itself, the scored ones and the excluded zeros)
+__device__ __forceinline__ long long bl_zero_eq(const BlEvalDev& d, double t, long long sx) { return t == 0.0 ? d.wtot - sx : 0ll; }
 // first r of the descending topS[0 .. n) with topS[r] <= t (STRICT: < t)
 template <bool STRICT>
 __device__ __forceinline__ int bl_top_pos(const double* s, int n, double t) {
@@ -472,7 +481,7 @@ __global__ void __launch_bounds__(256, 1) k_bl_rank(BlEvalDev d, int64_t n_sessi
           }
       }
       for (int o = 16; o > 0; o >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, o);
-      if (lane == 0 && t == 0.0) eq += d.wtot - sx;
+      if (lane == 0) eq += bl_zero_eq(d, t, sx);
     }
     for (int o = 16; o > 0; o >>= 1) { gt += __shfl_xor_sync(0xffffffffu, gt, o); eq += __shfl_xor_sync(0xffffffffu, eq, o); }
     if (lane == 0) {
@@ -572,6 +581,7 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
                   (void*)h->dI, (void*)h->dBI})
     if (p) cudaFree(p);
   for (void* p : h->bpr_mem) cudaFree(p);
+  for (void* p : h->sknn_mem) cudaFree(p);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -581,9 +591,12 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if (kind < BL_POP || kind > BL_BPR) { g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN) or 3 (BPR)"; return G4R_ERR_INVALID; }
-  if (n_items < 1 || n_keep < 1 || (kind == BL_ITEMKNN && n_keep > KF_KEEP_MAX) || (kind == BL_BPR && n_keep > BPR_F_MAX)) {
-    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, <= " +
+  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN) {
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR) or 5 (SessionKNN)";
+    return G4R_ERR_INVALID;
+  }
+  if (n_items < 1 || n_keep < 1 || ((kind == BL_ITEMKNN || kind == BL_SKNN) && n_keep > KF_KEEP_MAX) || (kind == BL_BPR && n_keep > BPR_F_MAX)) {
+    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN and SessionKNN, <= " +
                         std::to_string(BPR_F_MAX) + " n_factors for BPR)";
     return G4R_ERR_INVALID;
   }
@@ -593,7 +606,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
     return G4R_ERR_CUDA;
   }
   g4r_baselines* h = new g4r_baselines();
-  h->kind = kind; h->n_items = n_items; h->n_keep = (kind == BL_ITEMKNN || kind == BL_BPR) ? n_keep : std::min(n_keep, n_items); h->device = device;
+  h->kind = kind; h->n_items = n_items; h->n_keep = (kind >= BL_ITEMKNN) ? n_keep : std::min(n_keep, n_items); h->device = device;
   auto bail = [&](const char* m) { g_bl_create_error = m; g4r_bl_destroy(h); return G4R_ERR_CUDA; };
   if (cudaSetDevice(device) != cudaSuccess) return bail("cudaSetDevice failed");
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
@@ -606,7 +619,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   } else if (kind == BL_ITEMKNN) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
-  } else {
+  } else if (kind != BL_SKNN) {                        // SessionKNN allocates at g4r_bl_sknn_fit
     ok &= bl_alloc(&h->dPop, n_items) == cudaSuccess && bl_alloc(&h->dTopS, h->n_keep) == cudaSuccess && bl_alloc(&h->dTop, h->n_keep) == cudaSuccess;
   }
   if (!ok) return bail("device allocation failed");
@@ -733,7 +746,7 @@ extern "C" int g4r_bl_knn_fit(g4r_baselines* h, const int64_t* session_offsets, 
 
 extern "C" int g4r_bl_set_pop(g4r_baselines* h, const double* scores, int64_t n) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind == BL_ITEMKNN || h->kind == BL_BPR) FAIL(G4R_ERR_STATE, "g4r_bl_set_pop: the handle is not a Pop / SessionPop");
+  if (h->kind != BL_POP && h->kind != BL_SESSIONPOP) FAIL(G4R_ERR_STATE, "g4r_bl_set_pop: the handle is not a Pop / SessionPop");
   if (!scores || n != h->n_items) FAIL(G4R_ERR_INVALID, "g4r_bl_set_pop: need n_items scores");
   std::vector<int> top;
   for (int64_t i = 0; i < n; i++) {
@@ -805,6 +818,10 @@ static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events
                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
                         double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_bpr.cuh
+static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
+                         const std::vector<int>& mult, const std::vector<int>& cdist, long long wtot, int32_t exclude_seen, int32_t k,
+                         double* recall_sum, double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_sknn.cuh
 
 extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                                const int32_t* n_history, int32_t mode, const int32_t* cut_off, int32_t n_cut, const int32_t* cand,
@@ -842,10 +859,12 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   }
   const int64_t n_ev = ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
-  if (h->kind == BL_BPR) {
+  if (h->kind == BL_BPR || h->kind == BL_SKNN) {
     cudaSetDevice(h->device);
-    const int rc = bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult, cdist,
-                                exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores);
+    const int rc = h->kind == BL_BPR ? bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
+                                                    cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)
+                                     : sknn_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
+                                                     cdist, wtot, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores);
     if (rc == G4R_OK && n_counted) *n_counted = n_ev;
     return rc;
   }

@@ -350,6 +350,7 @@ int g4r_sessions_import(g4r_handle* h, const int64_t* keys, const float* states,
                         const int32_t* hist_items, int64_t n);
 
 /* ---- session baselines: ItemKNN, Pop and SessionPop of the reference's baselines.py (baselines.py:52-301; DESIGN §3j) -------
+ * (BPR-MF and SessionKNN below share the handle and g4r_bl_evaluate.)
  * A separate handle: a baseline has no training config.  Item indices are 0 .. n_items - 1.  Every argument is checked before any
  * device work; G4R_ERR_STATE for a call the handle's kind does not have or before the model is fitted. */
 typedef struct g4r_baselines g4r_baselines;
@@ -414,6 +415,19 @@ int g4r_bl_bpr_export(g4r_baselines* b, double* U, double* I);
  * BPR handle scores item j after input p as (sum over f = 0 .. n_factors - 1 in order of I[j,f] * uF[f]) + bI[j], every product
  * and sum correctly rounded in float64, uF the mean of I over the session's items[start .. p]. */
 int g4r_bl_bpr_import(g4r_baselines* b, const double* I, const double* bI);
+
+/* ---- session-based kNN: S-KNN (cosine) and V-SKNN-style position weights (DESIGN §3o) -------------------------------------------
+ * g4r_bl_create(G4R_BL_SKNN, n_items, k (1 .. 1024), ...).  Kind 4 is not used. */
+#define G4R_BL_SKNN 5
+/* The index: the training sessions' distinct items as CSR (items[session_offsets[s] .. session_offsets[s+1]) strictly ascending),
+ * recency[s] the rank of session s in recency order (a permutation of 0 .. n_sessions - 1, 0 the most recent), sample_size
+ * 1 .. 8192 (k <= sample_size), similarity 0 (cosine) or 1 (vector).  The library builds every item's sessions in recency order
+ * and keeps both on the device; a later call replaces the index.  g4r_bl_evaluate of a SessionKNN handle ranks each counted
+ * event by the scores of DESIGN §3o: the candidates are the first sample_size training sessions in recency order that share an
+ * item with the session's items[start .. p]; the k most similar (ties: the more recent) are the neighbours, and item j scores
+ * the sum, in float64 in neighbour order, of the similarities of the neighbours that contain j. */
+int g4r_bl_sknn_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
+                    const int32_t* recency, int32_t sample_size, int32_t similarity);
 
 #ifdef __cplusplus
 }
