@@ -51,7 +51,7 @@ EXPORTS = [
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
-    'g4r_bl_sknn_fit',
+    'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1',
 ]
 
 _lib = None
@@ -154,6 +154,8 @@ def load():
     lib.g4r_bl_bpr_export.argtypes = [vp, vp, vp]
     lib.g4r_bl_bpr_import.argtypes = [vp, vp, vp]
     lib.g4r_bl_sknn_fit.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32]
+    lib.g4r_bl_stan_fit.argtypes = [vp, vp, i64, vp, i64, vp, vp, vp, vp, i64, i32]
+    lib.g4r_bl_stan_set_w1.argtypes = [vp, vp, i64]
     _lib = lib
     return lib
 
@@ -778,14 +780,14 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 
 
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
-    a baseline, the BPR-MF fit and factors (DESIGN §3k), and the SessionKNN index (DESIGN §3o).  kind: 'pop', 'sessionpop',
-    'itemknn', 'bpr' or 'sknn'; n_keep: top_n, n_sims, n_factors or k."""
+    a baseline, the BPR-MF fit and factors (DESIGN §3k), and the SessionKNN and STAN indexes (DESIGN §3o, §3p).  kind: 'pop',
+    'sessionpop', 'itemknn', 'bpr', 'sknn' or 'stan'; n_keep: top_n, n_sims, n_factors or k."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -917,3 +919,26 @@ class Baselines(object):
             raise ValueError('sknn_fit: similarity must be one of %s' % sorted(SKNN_SIMILARITY))
         self._check(self.lib.g4r_bl_sknn_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(rc), int(sample_size),
                                              SKNN_SIMILARITY[similarity]))
+
+    def stan_fit(self, session_offsets, items, positions, recency, w2, w3, sample_size):
+        """the STAN index: sknn_fit's CSR and ranks, each entry's last position in its session, W2 per session (in the order of
+        session_offsets) and the W3 table"""
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        pos = np.ascontiguousarray(positions, dtype=np.int32); rc = np.ascontiguousarray(recency, dtype=np.int32)
+        w2 = np.ascontiguousarray(w2, dtype=np.float64); w3 = np.ascontiguousarray(w3, dtype=np.float64)
+        if off.ndim != 1 or off.size < 2 or it.ndim != 1 or pos.shape != it.shape:
+            raise ValueError('stan_fit: need session offsets and one position per item entry')
+        if rc.shape != (off.size - 1,) or w2.shape != (off.size - 1,):
+            raise ValueError('stan_fit: need one recency rank and one w2 weight per session')
+        if w3.ndim != 1 or w3.size < 1:
+            raise ValueError('stan_fit: w3 must be a non-empty 1-D table')
+        self._check(self.lib.g4r_bl_stan_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(pos), _ptr(rc), _ptr(w2), _ptr(w3),
+                                             w3.size, int(sample_size)))
+
+    def stan_set_w1(self, w1):
+        """the STAN prefix-distance table W1[0 .. n): it must cover every counted event's prefix length"""
+        w1 = np.ascontiguousarray(w1, dtype=np.float64)
+        if w1.ndim != 1 or w1.size < 1:
+            raise ValueError('stan_set_w1: w1 must be a non-empty 1-D table')
+        self._check(self.lib.g4r_bl_stan_set_w1(self.h, _ptr(w1), w1.size))
+        self.n_w1 = w1.size

@@ -1,6 +1,6 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), and session-based kNN (SessionKNN, DESIGN
-§3o) with the same surface.  ItemKNN's fit runs on the device (the
+§3o; STAN, §3p) with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -32,6 +32,9 @@ class Baseline(object):
 
     def _upload(self, dev):
         raise NotImplementedError
+
+    def _cover(self, max_len):
+        """prepares the device model for test sessions of up to max_len events (history included); only STAN needs to"""
 
     def _device(self):
         dev = self.__dict__.get('_dev')
@@ -369,3 +372,118 @@ class SessionKNN(Baseline):
             self.session.append(x)
         score = self.score_prefix(self.session)
         return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+class STAN(SessionKNN):
+    '''
+    STAN(k=100, sample_size=500, lambda_spw=1.02, lambda_snh=432000.0, lambda_inh=2.05, session_key='SessionId', item_key='ItemId',
+         time_key='Time')
+
+    Session kNN with the three decays of STAN (Garg et al., SIGIR 2019): recent items of the current session, recent neighbour
+    sessions and items close to the neighbour's most recent shared item count more.  This is this project's definition in the
+    style of STAN (DESIGN §3p); it is not claimed to match any other implementation bit for bit.
+
+    Everything SessionKNN defines stays: the item index, T(s), the recency order, the prefix c = (x_1 .. x_t), I(c) and the
+    candidates.  A training session's events are ordered by time_key (ties by row order); q_n(j) is the 1-based position of item
+    j's last occurrence in session n, p_i the last position of i in c.  The tables, computed by NumPy: W1[d] = exp(-(d /
+    lambda_spw)), W2[n] = exp(-(float64(T_max - T(n)) / lambda_snh)) with T_max the largest training time, W3[d] = exp(-(d /
+    lambda_inh)).  sim(n) = (sum of W1[t - p_i] over I(c) & I(n) in ascending p_i) / sqrt(|I(c)| |I(n)|) * W2[n]; the k
+    largest (ties: the more recent) are the neighbours; score(j) is the float64 sum, in neighbour order, of sim(n) *
+    W3[|q_n(j) - q_n(r(n))|] over the neighbours containing j, r(n) the shared item with the largest p_i.  A lambda of inf
+    switches its decay off; with all three at inf the scores are SessionKNN(similarity='cosine')'s.  lambda_snh is in time_key
+    units (the default is 5 days in seconds).
+    '''
+    _kind = 'stan'
+
+    def __init__(self, k=100, sample_size=500, lambda_spw=1.02, lambda_snh=432000.0, lambda_inh=2.05, session_key='SessionId', item_key='ItemId',
+                 time_key='Time'):
+        self.k = k
+        self.sample_size = sample_size
+        self.lambda_spw = lambda_spw
+        self.lambda_snh = lambda_snh
+        self.lambda_inh = lambda_inh
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def fit(self, data):
+        if not 1 <= self.sample_size <= 8192:
+            raise ValueError('sample_size must be in 1 .. 8192, not %r' % (self.sample_size,))
+        if not 1 <= self.k <= min(self.sample_size, 1024):
+            raise ValueError('k must be in 1 .. min(sample_size, 1024), not %r' % (self.k,))
+        for name in ('lambda_spw', 'lambda_snh', 'lambda_inh'):
+            if not float(getattr(self, name)) > 0.0:
+                raise ValueError('%s must be in (0, inf], not %r' % (name, getattr(self, name)))
+        col = data[self.time_key]
+        if not pd.api.types.is_numeric_dtype(col) or pd.api.types.is_bool_dtype(col):
+            raise ValueError('STAN needs a numeric time column %r, not %s' % (self.time_key, col.dtype))
+        times = col.values
+        idx = self._index(data).astype(np.int64)
+        sess = data[self.session_key].values
+        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
+        self.n_sessions = S = int(code.max()) + 1 if len(code) else 0
+        T = pd.Series(times).groupby(code).max().values
+        order = np.argsort(-T, kind='stable')                    # T descending, ties by first appearance
+        self.recency = np.empty(S, np.int32)
+        self.recency[order] = np.arange(S, dtype=np.int32)
+        lens = np.bincount(code, minlength=S)
+        o = np.lexsort((times, code))                            # each session's events by time, ties by row order
+        pos = np.arange(len(o)) - np.repeat(np.cumsum(lens) - lens, lens) + 1
+        key = code[o].astype(np.int64) * self.n_items + idx[o]
+        o2 = np.lexsort((pos, key))
+        key, pos = key[o2], pos[o2]
+        last = np.r_[key[1:] != key[:-1], True]                  # (session, item) distinct, items ascending; its last position
+        self.session_items = (key[last] % self.n_items).astype(np.int32)
+        self.positions = pos[last].astype(np.int32)
+        self.session_offsets = np.zeros(S + 1, np.int64)
+        self.session_offsets[1:] = np.cumsum(np.bincount(key[last] // self.n_items, minlength=S))
+        self.w2 = np.exp(-((T.max() - T).astype(np.float64) / float(self.lambda_snh)))
+        self.w3 = np.exp(-(np.arange(int(lens.max())) / float(self.lambda_inh)))
+        self.current_session = None
+        self.__dict__.pop('_dev', None)
+        self.__dict__.pop('_post', None)
+        self._device()
+
+    def _w1(self, n):
+        return np.exp(-(np.arange(n) / float(self.lambda_spw)))
+
+    def _upload(self, dev):
+        dev.stan_fit(self.session_offsets, self.session_items, self.positions, self.recency, self.w2, self.w3, self.sample_size)
+        dev.stan_set_w1(self._w1(len(self.w3)))
+
+    def _cover(self, max_len):
+        dev = self._device()
+        if dev.n_w1 < max_len:
+            dev.stan_set_w1(self._w1(max_len))
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        prefix = np.asarray(prefix, dtype=np.int64)
+        t = len(prefix)
+        u, first_rev = np.unique(prefix[::-1], return_index=True)
+        last = t - first_rev                                      # 1-based position of the last occurrence
+        o = np.argsort(last)
+        ci, pos = u[o], last[o]
+        ioff, ranks, by_rank = self._postings()
+        S = self.sample_size
+        cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
+        sess = by_rank[cand]
+        starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
+        owner = np.repeat(np.arange(len(cand)), lens)
+        at = np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())
+        flat, fpos = self.session_items[at], self.positions[at]
+        w1 = self._w1(t)
+        v, qr = np.zeros(len(cand)), np.zeros(len(cand), np.int64)
+        for m, i in enumerate(ci):                                # c's items in order of their last position
+            sel = flat == i
+            hit = np.zeros(len(cand), bool)
+            hit[owner[sel]] = True
+            v = v + np.where(hit, w1[t - pos[m]], 0.0)
+            qr[owner[sel]] = fpos[sel]                            # ends at the shared item with the largest p_i
+        sims = v / np.sqrt((len(ci) * lens).astype(np.float64)) * self.w2[sess]
+        score = np.zeros(self.n_items)
+        for q in np.lexsort((cand, -sims))[:self.k]:
+            sel = owner == q
+            score[flat[sel]] = score[flat[sel]] + sims[q] * self.w3[np.abs(fpos[sel] - qr[q])]
+        return score

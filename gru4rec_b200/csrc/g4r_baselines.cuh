@@ -4,7 +4,7 @@
 // nothing here touches a g4r_handle.
 #pragma once
 
-constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5;   // 4 stays unused
+constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6;   // 4 stays unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
@@ -43,6 +43,11 @@ struct g4r_baselines {
   std::vector<void*> sknn_mem;
   int64_t sk_sessions = 0, sk_zmax = 0;                 // sk_zmax: distinct items of the n_keep longest training sessions
   int sk_sample = 0, sk_sim = 0;
+  // STAN (the SessionKNN index above plus): each entry's last position in its session, W2 by rank and W3 (freed with the index);
+  // W1 by prefix distance (g4r_bl_stan_set_w1, kept across index replacements)
+  int* dStPos = nullptr;
+  double *dStW2 = nullptr, *dStW3 = nullptr, *dStW1 = nullptr;
+  int64_t st_n_w1 = 0;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -578,7 +583,7 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   for (void* p : {(void*)h->dIdx, (void*)h->dIdxI, (void*)h->dLen, (void*)h->dSim, (void*)h->dSimI, (void*)h->dPop, (void*)h->dTopS, (void*)h->dTop,
-                  (void*)h->dI, (void*)h->dBI})
+                  (void*)h->dI, (void*)h->dBI, (void*)h->dStW1})
     if (p) cudaFree(p);
   for (void* p : h->bpr_mem) cudaFree(p);
   for (void* p : h->sknn_mem) cudaFree(p);
@@ -591,12 +596,13 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN) {
-    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR) or 5 (SessionKNN)";
+  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN) {
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN) or 6 (STAN)";
     return G4R_ERR_INVALID;
   }
-  if (n_items < 1 || n_keep < 1 || ((kind == BL_ITEMKNN || kind == BL_SKNN) && n_keep > KF_KEEP_MAX) || (kind == BL_BPR && n_keep > BPR_F_MAX)) {
-    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN and SessionKNN, <= " +
+  if (n_items < 1 || n_keep < 1 || ((kind == BL_ITEMKNN || kind == BL_SKNN || kind == BL_STAN) && n_keep > KF_KEEP_MAX) ||
+      (kind == BL_BPR && n_keep > BPR_F_MAX)) {
+    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN and STAN, <= " +
                         std::to_string(BPR_F_MAX) + " n_factors for BPR)";
     return G4R_ERR_INVALID;
   }
@@ -619,7 +625,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   } else if (kind == BL_ITEMKNN) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
-  } else if (kind != BL_SKNN) {                        // SessionKNN allocates at g4r_bl_sknn_fit
+  } else if (kind != BL_SKNN && kind != BL_STAN) {     // SessionKNN and STAN allocate at their fit
     ok &= bl_alloc(&h->dPop, n_items) == cudaSuccess && bl_alloc(&h->dTopS, h->n_keep) == cudaSuccess && bl_alloc(&h->dTop, h->n_keep) == cudaSuccess;
   }
   if (!ok) return bail("device allocation failed");
@@ -859,7 +865,7 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   }
   const int64_t n_ev = ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
-  if (h->kind == BL_BPR || h->kind == BL_SKNN) {
+  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN) {
     cudaSetDevice(h->device);
     const int rc = h->kind == BL_BPR ? bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
                                                     cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)

@@ -1,5 +1,6 @@
-// g4r_sknn.cuh -- session-based kNN (S-KNN with cosine similarity, V-SKNN-style position weights) on the device (DESIGN §3o):
-// the index of the training sessions and the event-parallel ranking of evaluate_gpu / evaluate_events, one CTA per counted event.
+// g4r_sknn.cuh -- session-based kNN (S-KNN with cosine similarity, V-SKNN-style position weights, DESIGN §3o; STAN-style time
+// and position decays, §3p) on the device: the index of the training sessions and the event-parallel ranking of evaluate_gpu /
+// evaluate_events, one CTA per counted event.
 // Included at the end of g4r_lib.cu after g4r_baselines.cuh (the handle, BlEvalDev, bl_w, bl_noise, bl_zero_eq, bl_emit,
 // cta_bitonic, k_bl_sums, BlBufs).
 #pragma once
@@ -15,6 +16,9 @@ struct SknnEvalDev {
   const int64_t* s_off; const int* s_item;              // training sessions by recency rank: distinct items ascending
   const int64_t* i_off; const int* i_sess;              // every item's sessions, as ranks ascending (recency order)
   int sample, sim, nbr;                                 // sample_size, 0 cosine / 1 vector, k (neighbours)
+  // STAN (§3p): per entry of s_item the 1-based position of the item's last occurrence in its session; the decay tables W1
+  // (prefix distance), W2 (per session, by rank) and W3 (distance inside a neighbour)
+  const int* s_pos; const double* w1; const double* w2; const double* w3;
   // per-CTA slices of global scratch: the prefix (c_cap entries) and the neighbours' (item, neighbour) pairs (z_cap entries)
   unsigned long long* c_key; int* c_flag; int* c_item; double* c_w; int c_cap;
   unsigned long long* z_key; int* u_item; double* u_sc; double* l_sc; int* l_item; int z_cap;
@@ -73,6 +77,11 @@ __device__ __forceinline__ double sk_score(const int* ui, const double* us, int 
   const int p = sorted_lb(ui, U, j);
   return (p < U && ui[p] == j) ? us[p] : 0.0;
 }
+// j among the U scored items (ascending)
+__device__ __forceinline__ bool sk_scored(const int* ui, int U, int j) {
+  const int p = sorted_lb(ui, U, j);
+  return p < U && ui[p] == j;
+}
 
 // One CTA per counted event (grid-stride over the events):
 //  1. the prefix c = items[start .. p]: its (item, position) keys sorted, the last occurrence of every item flagged, and the
@@ -83,6 +92,10 @@ __device__ __forceinline__ double sk_score(const int* ui, const double* us, int 
 //  4. the candidates sorted by (sim desc, rank asc); the first nbr are the neighbours;
 //  5. (item, neighbour) pairs of the neighbours' items sorted, each item's sims summed in neighbour order;
 //  6. (#greater, #equal) of the target, and with k > 0 its top-k list.
+// STAN (§3p) changes three steps: the weights of step 1 are W1[t - p], step 3 is the W1 sum over sqrt(|I(c)| |I(n)|) times W2[n],
+// and step 5 first finds each neighbour's most recent shared item r(n) and multiplies each summand by W3[|q_n(j) - q_n(r(n))|].
+// Its scored items may score exactly 0 (underflow): they are counted as scored items and listed with the zero-score items.
+template <bool STAN>
 __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
   extern __shared__ __align__(16) unsigned char sk_smem[];
   __shared__ int sW[SK_THREADS / 32];
@@ -119,7 +132,7 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
       const bool f = q < t && cf[q];
       int tot;
       const int r = sk_rank_flag(f, sW, tot);
-      if (f) { ci[D + r] = b.items[st + q]; cw[D + r] = __ddiv_rn((double)(q + 1), (double)t); }
+      if (f) { ci[D + r] = b.items[st + q]; cw[D + r] = STAN ? d.w1[t - 1 - q] : __ddiv_rn((double)(q + 1), (double)t); }
       D += tot;
     }
     __syncthreads();
@@ -167,15 +180,29 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
       for (int m = 0; m < D; m++) {
         const int j = ci[m];
         const int x = sorted_lb(it, ns, j);
-        if (x < ns && it[x] == j) { cnt++; if (d.sim) v = __dadd_rn(v, cw[m]); }
+        if (x < ns && it[x] == j) { cnt++; if (STAN || d.sim) v = __dadd_rn(v, cw[m]); }
       }
-      if (!d.sim) v = __ddiv_rn((double)cnt, __dsqrt_rn((double)((long long)D * ns)));
+      if (STAN) v = __dmul_rn(__ddiv_rn(v, __dsqrt_rn((double)((long long)D * ns))), d.w2[r]);
+      else if (!d.sim) v = __ddiv_rn((double)cnt, __dsqrt_rn((double)((long long)D * ns)));
       sS[q] = v;
     }
     // 4. neighbours
     cta_bitonic<false>(sS, cand, Pn);
     const int nK = min(d.nbr, nB);
-    // 5. scores
+    // 5. scores (STAN: nxt, free since the merge, holds q_n(r(n)) of neighbour n; c's items are searched from the last position)
+    if (STAN) {
+      for (int r = tid; r < nK; r += SK_THREADS) {
+        const int64_t a0 = d.s_off[cand[r]];
+        const int ns = (int)(d.s_off[cand[r] + 1] - a0);
+        const int* it = d.s_item + a0;
+        int qr = 0;
+        for (int m = D - 1; m >= 0; m--) {
+          const int x = sorted_lb(it, ns, ci[m]);
+          if (x < ns && it[x] == ci[m]) { qr = d.s_pos[a0 + x]; break; }
+        }
+        nxt[r] = qr;
+      }
+    }
     if (tid == 0) sZ = 0;
     __syncthreads();
     for (int r = tid >> 5; r < nK; r += SK_THREADS / 32) {
@@ -199,7 +226,14 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
       if (head) {
         const unsigned j = (unsigned)(zk[z] >> 32);
         double acc = 0.0;
-        for (int w = z; w < Z && (unsigned)(zk[w] >> 32) == j; w++) acc = __dadd_rn(acc, sS[(int)(zk[w] & 0xffffffffu)]);
+        for (int w = z; w < Z && (unsigned)(zk[w] >> 32) == j; w++) {
+          const int n = (int)(zk[w] & 0xffffffffu);
+          if (STAN) {
+            const int64_t a0 = d.s_off[cand[n]];
+            const int x = sorted_lb(d.s_item + a0, (int)(d.s_off[cand[n] + 1] - a0), (int)j);
+            acc = __dadd_rn(acc, __dmul_rn(sS[n], d.w3[abs(d.s_pos[a0 + x] - nxt[n])]));
+          } else acc = __dadd_rn(acc, sS[n]);
+        }
         ui[U + r] = (int)j; us[U + r] = acc;
       }
       U += tot;
@@ -224,12 +258,13 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
         const int j = ui[q];
         const double sc = us[q];
         const long long w = bl_w(b, j);
-        sx += w;                                         // scored items are not zeros
+        sx += w;                                         // scored items are compared here, zeros included
         if (b.exclude && sk_seen(ck, t, j)) continue;
         gt += sc > ty ? w : 0; eq += sc == ty ? w : 0;
       }
       if (b.exclude)
-        for (int m = tid; m < D; m += SK_THREADS) if (sk_score(ui, us, U, ci[m]) == 0.0) sx += bl_w(b, ci[m]);
+        for (int m = tid; m < D; m += SK_THREADS)
+          if (STAN ? !sk_scored(ui, U, ci[m]) : sk_score(ui, us, U, ci[m]) == 0.0) sx += bl_w(b, ci[m]);
     }
     gt = sk_sum(gt, sRed); eq = sk_sum(eq, sRed); sx = sk_sum(sx, sRed);
     if (tid == 0) {
@@ -247,10 +282,10 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
         int* o_i = b.out_items + (size_t)e * b.k;
         double* o_s = b.out_scores + (size_t)e * b.k;
         int base = 0;
-        for (int q0 = 0; q0 < U && base < b.k; q0 += 32) {        // the scored items by (score desc, index asc)
+        for (int q0 = 0; q0 < U && base < b.k; q0 += 32) {        // the positive scored items by (score desc, index asc)
           const int q = q0 + lane;
           const int j = q < U ? li[q] : 0;
-          const bool ok = q < U && (!b.mult || b.mult[j] > 0) && !(b.exclude && sk_seen(ck, t, j));
+          const bool ok = q < U && (!STAN || ls[q] > 0.0) && (!b.mult || b.mult[j] > 0) && !(b.exclude && sk_seen(ck, t, j));
           bl_emit(ok, j, q < U ? ls[q] : 0.0, o_i, o_s, b.k, base);
         }
         const int n_comp = b.mult ? b.n_cdist : b.n_items;          // then the zero-score items, by index
@@ -270,36 +305,56 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
 // ---------------------------------------------------------------------------------------------------------------------------
 // C ABI (include/g4r.h)
 // ---------------------------------------------------------------------------------------------------------------------------
-extern "C" int g4r_bl_sknn_fit(g4r_baselines* h, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
-                               const int32_t* recency, int32_t sample_size, int32_t similarity) {
-  if (!h) return G4R_ERR_INVALID;
-  if (h->kind != BL_SKNN) FAIL(G4R_ERR_STATE, "g4r_bl_sknn_fit: the handle is not a SessionKNN");
+// the index of a SessionKNN (similarity; positions, w2 and w3 null) or a STAN handle: every argument checked on the host before any device
+// write, the sessions renumbered by rank and every item's sessions built by a counting sort that visits the ranks in order
+static int sk_index(g4r_baselines* h, const std::string& fn, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items,
+                    int64_t n_entries, const int32_t* recency, int32_t sample_size, int32_t similarity, const int32_t* positions,
+                    const double* w2, const double* w3, int64_t n_w3) {
+  const bool stan = h->kind == BL_STAN;
   if (!session_offsets || !recency || n_sessions < 1 || n_sessions >= INT32_MAX || n_entries < 0 || (n_entries > 0 && !items))
-    FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: null argument, or n_sessions outside 1 .. 2^31 - 2");
-  if (sample_size < 1 || sample_size > SK_SAMPLE_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: sample_size must be in 1 .. 8192");
-  if (h->n_keep > sample_size) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: k (n_keep) must not exceed sample_size");
-  if (similarity != 0 && similarity != 1) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: similarity must be 0 (cosine) or 1 (vector)");
-  if (!bl_offsets_ok(session_offsets, n_sessions, n_entries)) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: session offsets must rise from 0 to n_entries");
+    FAIL(G4R_ERR_INVALID, fn + ": null argument, or n_sessions outside 1 .. 2^31 - 2");
+  if (stan && (!w2 || !w3 || n_w3 < 1 || n_w3 > (1 << 30) || (n_entries > 0 && !positions)))
+    FAIL(G4R_ERR_INVALID, fn + ": null positions, w2 or w3, or n_w3 outside 1 .. 2^30");
+  if (sample_size < 1 || sample_size > SK_SAMPLE_MAX) FAIL(G4R_ERR_INVALID, fn + ": sample_size must be in 1 .. 8192");
+  if (h->n_keep > sample_size) FAIL(G4R_ERR_INVALID, fn + ": k (n_keep) must not exceed sample_size");
+  if (!stan && similarity != 0 && similarity != 1) FAIL(G4R_ERR_INVALID, fn + ": similarity must be 0 (cosine) or 1 (vector)");
+  if (!bl_offsets_ok(session_offsets, n_sessions, n_entries)) FAIL(G4R_ERR_INVALID, fn + ": session offsets must rise from 0 to n_entries");
   const int NI = h->n_items;
   for (int64_t s = 0; s < n_sessions; s++)
     for (int64_t q = session_offsets[s]; q < session_offsets[s + 1]; q++) {
-      if (items[q] < 0 || items[q] >= NI) FAIL(G4R_ERR_INDEX, "g4r_bl_sknn_fit: item index out of range");
-      if (q > session_offsets[s] && items[q] <= items[q - 1]) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: a session's items must be distinct and ascending");
+      if (items[q] < 0 || items[q] >= NI) FAIL(G4R_ERR_INDEX, fn + ": item index out of range");
+      if (q > session_offsets[s] && items[q] <= items[q - 1]) FAIL(G4R_ERR_INVALID, fn + ": a session's items must be distinct and ascending");
     }
+  if (stan) {
+    // a session of L events has its distinct items' last positions distinct in 1 .. L, and L <= n_w3 (W3 covers 0 .. L - 1)
+    std::vector<int64_t> mark(n_w3 + 1, -1);
+    for (int64_t s = 0; s < n_sessions; s++)
+      for (int64_t q = session_offsets[s]; q < session_offsets[s + 1]; q++) {
+        if (positions[q] < 1 || positions[q] > n_w3) FAIL(G4R_ERR_INVALID, fn + ": positions must be in 1 .. n_w3 (the longest session's length)");
+        if (mark[positions[q]] == s) FAIL(G4R_ERR_INVALID, fn + ": two items of a session at one position");
+        mark[positions[q]] = s;
+      }
+    for (int64_t s = 0; s < n_sessions; s++)
+      if (!(w2[s] >= 0.0 && w2[s] <= 1.0)) FAIL(G4R_ERR_INVALID, fn + ": w2 entries must be in [0, 1]");
+    for (int64_t q = 0; q < n_w3; q++)
+      if (!(w3[q] >= 0.0 && w3[q] <= 1.0)) FAIL(G4R_ERR_INVALID, fn + ": w3 entries must be in [0, 1]");
+  }
   const int64_t S = n_sessions;
   std::vector<int64_t> by_rank(S, -1);
   for (int64_t s = 0; s < S; s++) {
-    if (recency[s] < 0 || recency[s] >= S) FAIL(G4R_ERR_INDEX, "g4r_bl_sknn_fit: recency rank out of range");
-    if (by_rank[recency[s]] >= 0) FAIL(G4R_ERR_INVALID, "g4r_bl_sknn_fit: the recency ranks must be a permutation of 0 .. n_sessions - 1");
+    if (recency[s] < 0 || recency[s] >= S) FAIL(G4R_ERR_INDEX, fn + ": recency rank out of range");
+    if (by_rank[recency[s]] >= 0) FAIL(G4R_ERR_INVALID, fn + ": the recency ranks must be a permutation of 0 .. n_sessions - 1");
     by_rank[recency[s]] = s;
   }
   // the sessions renumbered by rank, and every item's sessions: a counting sort that visits the ranks in order
   std::vector<int64_t> off(S + 1, 0), ioff(NI + 1, 0);
-  std::vector<int> sit(n_entries), isess(n_entries);
+  std::vector<int> sit(n_entries), isess(n_entries), spos(stan ? n_entries : 0);
+  std::vector<double> rw2(stan ? S : 0);
   std::vector<int64_t> lens(S);
   for (int64_t r = 0; r < S; r++) {
     const int64_t s = by_rank[r], a = session_offsets[s], n = session_offsets[s + 1] - a;
     std::copy(items + a, items + a + n, sit.begin() + off[r]);
+    if (stan) { std::copy(positions + a, positions + a + n, spos.begin() + off[r]); rw2[r] = w2[s]; }
     off[r + 1] = off[r] + n;
     lens[r] = n;
     for (int64_t q = a; q < a + n; q++) ioff[items[q] + 1]++;
@@ -318,24 +373,62 @@ extern "C" int g4r_bl_sknn_fit(g4r_baselines* h, const int64_t* session_offsets,
   h->ready = false;
   for (void* p : h->sknn_mem) cudaFree(p);
   h->sknn_mem.clear();
-  h->dSkOff = h->dSkIoff = nullptr; h->dSkItem = h->dSkIsess = nullptr;
+  h->dSkOff = h->dSkIoff = nullptr; h->dSkItem = h->dSkIsess = h->dStPos = nullptr; h->dStW2 = h->dStW3 = nullptr;
   auto take = [&](auto** p, size_t n) { cudaError_t e = bl_alloc(p, n); if (e == cudaSuccess) h->sknn_mem.push_back(*p); else *p = nullptr; return e; };
   CK(take(&h->dSkOff, S + 1)); CK(take(&h->dSkIoff, NI + 1));
   CK(take(&h->dSkItem, n_entries)); CK(take(&h->dSkIsess, n_entries));
+  if (stan) { CK(take(&h->dStPos, n_entries)); CK(take(&h->dStW2, S)); CK(take(&h->dStW3, n_w3)); }
   cudaStream_t st = h->stream;
   CK(cudaMemcpyAsync(h->dSkOff, off.data(), (S + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(h->dSkIoff, ioff.data(), (NI + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   if (n_entries) {
     CK(cudaMemcpyAsync(h->dSkItem, sit.data(), n_entries * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(h->dSkIsess, isess.data(), n_entries * sizeof(int), cudaMemcpyHostToDevice, st));
+    if (stan) CK(cudaMemcpyAsync(h->dStPos, spos.data(), n_entries * sizeof(int), cudaMemcpyHostToDevice, st));
+  }
+  if (stan) {
+    CK(cudaMemcpyAsync(h->dStW2, rw2.data(), S * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(h->dStW3, w3, n_w3 * sizeof(double), cudaMemcpyHostToDevice, st));
   }
   CK(cudaStreamSynchronize(st));
-  h->sk_sessions = S; h->sk_zmax = zmax; h->sk_sample = sample_size; h->sk_sim = similarity;
+  h->sk_sessions = S; h->sk_zmax = zmax; h->sk_sample = sample_size; h->sk_sim = stan ? 0 : similarity;
   h->ready = true;
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a SessionKNN, after its argument checks: resident CTAs over the counted events, each with its own slices of
+extern "C" int g4r_bl_sknn_fit(g4r_baselines* h, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
+                               const int32_t* recency, int32_t sample_size, int32_t similarity) {
+  if (!h) return G4R_ERR_INVALID;
+  if (h->kind != BL_SKNN) FAIL(G4R_ERR_STATE, "g4r_bl_sknn_fit: the handle is not a SessionKNN");
+  return sk_index(h, "g4r_bl_sknn_fit", session_offsets, n_sessions, items, n_entries, recency, sample_size, similarity, nullptr, nullptr,
+                  nullptr, 0);
+}
+
+extern "C" int g4r_bl_stan_fit(g4r_baselines* h, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
+                               const int32_t* positions, const int32_t* recency, const double* w2, const double* w3, int64_t n_w3,
+                               int32_t sample_size) {
+  if (!h) return G4R_ERR_INVALID;
+  if (h->kind != BL_STAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_fit: the handle is not a STAN");
+  return sk_index(h, "g4r_bl_stan_fit", session_offsets, n_sessions, items, n_entries, recency, sample_size, 0, positions, w2, w3, n_w3);
+}
+
+extern "C" int g4r_bl_stan_set_w1(g4r_baselines* h, const double* w1, int64_t n_w1) {
+  if (!h) return G4R_ERR_INVALID;
+  if (h->kind != BL_STAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_set_w1: the handle is not a STAN");
+  if (!w1 || n_w1 < 1 || n_w1 > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_stan_set_w1: null w1, or n_w1 outside 1 .. 2^30");
+  for (int64_t q = 0; q < n_w1; q++)
+    if (!(w1[q] >= 0.0 && w1[q] <= 1.0)) FAIL(G4R_ERR_INVALID, "g4r_bl_stan_set_w1: w1 entries must be in [0, 1]");
+  cudaSetDevice(h->device);
+  if (h->dStW1) cudaFree(h->dStW1);
+  h->dStW1 = nullptr; h->st_n_w1 = 0;
+  CK(bl_alloc(&h->dStW1, n_w1));
+  CK(cudaMemcpyAsync(h->dStW1, w1, n_w1 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->st_n_w1 = n_w1;
+  return G4R_OK;
+}
+
+// g4r_bl_evaluate of a SessionKNN or a STAN, after its argument checks: resident CTAs over the counted events, each with its own slices of
 // a global scratch of at most SK_SCRATCH bytes (fewer CTAs when the slices are large; one at least)
 static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                          const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
@@ -345,6 +438,11 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
   int64_t max_len = 1;
   for (int64_t s = 0; s < n_sessions; s++) max_len = std::max(max_len, session_offsets[s + 1] - session_offsets[s]);
   if (max_len > (1 << 30) || h->sk_zmax > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a session or the neighbours' items exceed 2^30 entries");
+  const bool stan = h->kind == BL_STAN;
+  if (stan)                                             // W1 must cover the prefix distances 0 .. t - 1 of every counted event
+    for (int64_t s = 0; s < n_sessions; s++)
+      if (ev0[s + 1] > ev0[s] && session_offsets[s + 1] - session_offsets[s] - 1 > h->st_n_w1)
+        FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a counted event's prefix is longer than the STAN W1 table (g4r_bl_stan_set_w1)");
   cudaStream_t st = h->stream;
   BlBufs bb;
   SknnEvalDev d{};
@@ -364,12 +462,14 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
   d.n_ev = n_ev; d.n_sess = n_sessions;
   d.s_off = h->dSkOff; d.s_item = h->dSkItem; d.i_off = h->dSkIoff; d.i_sess = h->dSkIsess;
   d.sample = h->sk_sample; d.sim = h->sk_sim; d.nbr = h->n_keep;
+  d.s_pos = h->dStPos; d.w1 = h->dStW1; d.w2 = h->dStW2; d.w3 = h->dStW3;
+  const auto kern = stan ? k_sknn_rank<true> : k_sknn_rank<false>;
   int PS = 1;
   while (PS < d.sample) PS <<= 1;
   const size_t smem = (size_t)PS * (sizeof(double) + 2 * sizeof(int)) + SK_CHUNK * sizeof(int);
-  CK(cudaFuncSetAttribute(k_sknn_rank, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_sknn_rank, SK_THREADS, smem));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, SK_THREADS, smem));
   int cc = 1, zc = 1;
   while (cc < max_len) cc <<= 1;
   while (zc < h->sk_zmax) zc <<= 1;
@@ -382,7 +482,7 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
   CK(bb.take(&d.z_key, (size_t)zc * grid)); CK(bb.take(&d.u_item, (size_t)zc * grid)); CK(bb.take(&d.u_sc, (size_t)zc * grid));
   if (k) { CK(bb.take(&d.l_sc, (size_t)zc * grid)); CK(bb.take(&d.l_item, (size_t)zc * grid)); }
   if (n_ev > 0) {
-    k_sknn_rank<<<(unsigned)grid, SK_THREADS, smem, st>>>(d);
+    kern<<<(unsigned)grid, SK_THREADS, smem, st>>>(d);
     CK(cudaGetLastError());
   }
   const int* dCut = nullptr; double* dSums = nullptr;

@@ -373,6 +373,7 @@ def _evaluate_baseline(model, test_data, items, session_key, item_key, time_key,
     if sums_only:
         print('Measuring Recall@{} and MRR@{}'.format(','.join([str(c) for c in cuts]), ','.join([str(c) for c in cuts])))
     test_data, test_data_items, offset_sessions, n_hist = _prepare_history(model, test_data, history, session_key, item_key, time_key)
+    model._cover(int(np.diff(offset_sessions).max(initial=0)))
     rec, mrr, n, counts, top_i, top_s = model._device().evaluate(test_data_items, offset_sessions, n_hist, cuts, _MODES[mode], cand,
                                                                  exclude_seen, k, counts=not sums_only)
     if sums_only:

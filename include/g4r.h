@@ -429,6 +429,25 @@ int g4r_bl_bpr_import(g4r_baselines* b, const double* I, const double* bI);
 int g4r_bl_sknn_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
                     const int32_t* recency, int32_t sample_size, int32_t similarity);
 
+/* ---- STAN-style time- and position-aware session kNN (DESIGN §3p) ---------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_STAN, n_items, k (1 .. 1024), ...).  The SessionKNN index plus three decay tables the caller computes, so
+ * the device only multiplies, adds, divides and takes square roots (correctly rounded). */
+#define G4R_BL_STAN 6
+/* The index as g4r_bl_sknn_fit's, plus: positions[e] the 1-based position of items[e]'s last occurrence in its session (distinct
+ * within a session, 1 .. n_w3), w2[s] session s's recency weight in [0, 1] (sessions in the order of session_offsets), and
+ * w3[0 .. n_w3) the in-neighbour distance weights in [0, 1], n_w3 the longest training session's length in events.  Every
+ * argument is checked before any device write; a later call replaces the index (not W1). */
+int g4r_bl_stan_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_entries,
+                    const int32_t* positions, const int32_t* recency, const double* w2, const double* w3, int64_t n_w3,
+                    int32_t sample_size);
+/* W1[0 .. n_w1): the weight of a prefix item at distance d = t - p from the current input, entries in [0, 1]; replaces any
+ * earlier table.  g4r_bl_evaluate of a STAN handle refuses (G4R_ERR_INVALID, before any device work) a frame with a counted event
+ * whose prefix is longer than n_w1.  It ranks by DESIGN §3p: v(n) the sum of W1[t - p_i] over the shared items in ascending p_i,
+ * sim(n) = v / sqrt(|I(c)| |I(n)|) * w2[n]; the k largest (ties: the more recent) are the neighbours; item j scores the sum, in
+ * neighbour order, of sim(n) * w3[|q_n(j) - q_n(r(n))|], r(n) the shared item with the largest p_i; each product and sum
+ * correctly rounded in float64.  Lists hold the positive scores first, then every zero-score item by index. */
+int g4r_bl_stan_set_w1(g4r_baselines* b, const double* w1, int64_t n_w1);
+
 #ifdef __cplusplus
 }
 #endif
