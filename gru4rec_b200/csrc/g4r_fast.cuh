@@ -766,6 +766,154 @@ __device__ __forceinline__ void fk_dby(SM& sm, int M, int nj) {
     if (lane == 0) sm.sDby[jj] = a;
   }
 }
+// ---------------- scores and row statistics of the column role (k_fast_t and k_fast_mg) ----------------
+// target activations into sT (pairwise losses: a warp per lane), then this thread's column products y_b . Sy_j into acc
+// (lane b = lane, columns jj = warp + FK_NW q)
+template <class SM>
+__device__ __forceinline__ void fk_scores(const ModelDev& md, SM& sm, float (&acc)[FK_Q], int M, int nj, bool pw) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, kw = md.ldL / 4;
+  if (pw) {
+    for (int b = warp; b < FK_B; b += FK_NW) {
+      if (b < M) {
+        float a = 0.f;
+        if (lane < kw) {
+          const float4 y = ld4(sm.sY + b * FK_LDS + lane * 4), w = ld4(sm.sTW + b * FK_LDS + lane * 4);
+          a = fmaf(w.x, y.x, a); a = fmaf(w.y, y.y, a); a = fmaf(w.z, y.z, a); a = fmaf(w.w, y.w, a);
+        }
+        a = warp_sum(a);
+        if (lane == 0) sm.sT[b] = act_fwd(md.fact, a + sm.sTB[b]);
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < FK_Q; q++) acc[q] = 0.f;
+  const float* yr = sm.sY + lane * FK_LDS;
+  for (int c4 = 0; c4 < kw; c4++) {
+    const float4 y = ld4(yr + c4 * 4);
+#pragma unroll
+    for (int q = 0; q < FK_Q; q++) {
+      if (warp + FK_NW * q < nj) {
+        const float4 w = ld4(sm.sS + (warp + FK_NW * q) * FK_LDS + c4 * 4);
+        acc[q] = fmaf(y.x, w.x, acc[q]); acc[q] = fmaf(y.y, w.y, acc[q]); acc[q] = fmaf(y.z, w.z, acc[q]); acc[q] = fmaf(y.w, w.w, acc[q]);
+      }
+    }
+  }
+}
+// scores o = acc + bias into sO, then the chunk statistics of lane b by 16 threads (columns sub, sub + 16) into md.stat: row
+// max first, then plain sums -- one expf per column instead of an exp-rescaling merge per element.  The summands are written
+// out here rather than taken from loss_terms: through loss_terms the compiler contracts fewer products into FMAs in this
+// kernel, and the headline step's results change in the last bit.
+template <class SM>
+__device__ __forceinline__ void fk_chunk_stats(const ModelDev& md, SM& sm, const float (&acc)[FK_Q], int buf, int M, int cb, int nj,
+                                               int chunk, bool has_chunk, bool pw) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int q = 0; q < FK_Q; q++) {
+    const int jj = warp + q * FK_NW;
+    if (jj < nj && lane < M) sm.sO[jj * FK_B + lane] = acc[q] + sm.sBias[jj];
+  }
+  __syncthreads();                          // sT and sO complete
+  const int b = tid >> 4, sub = tid & 15;   // FK_THREADS / 16 == FK_B lanes
+  const bool okb = b < M;
+  const int tc = okb ? sm.sTc[buf][b] : -1;
+  const float t = (pw && okb) ? sm.sT[b] : 0.f;
+  const bool xe = loss_xe(md.loss);
+  float yv[2]; bool use[2], ist[2];
+  float mloc = -INFINITY;                   // max over the columns the loss weights by their softmax
+#pragma unroll
+  for (int q = 0; q < 2; q++) {
+    const int jj = sub + 16 * q;
+    use[q] = okb && jj < nj;
+    ist[q] = use[q] && (tc == cb + jj);
+    const float o = use[q] ? sm.sO[jj * FK_B + b] : 0.f;
+    yv[q] = xe ? o : act_fwd(md.fact, o);
+    if (use[q] && (xe || (loss_softmaxneg(md.loss) && !ist[q]))) mloc = fmaxf(mloc, yv[q]);
+  }
+#pragma unroll
+  for (int o = 1; o < 16; o <<= 1) mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, o));
+  float Z = 0.f, A = 0.f, Q = 0.f, D = 0.f, T = 0.f, has = 0.f;
+#pragma unroll
+  for (int q = 0; q < 2; q++) {
+    if (!use[q]) continue;
+    const float y = yv[q];
+    if (ist[q]) has = 1.f;
+    if (xe) { Z += expf(y - mloc); if (ist[q]) T = y; }
+    else if (md.loss == G4R_LOSS_BPR_MAX) { if (!ist[q]) { const float e = expf(y - mloc), sg = sigmoidf_(t - y); Z += e; A += sg * e; Q += y * y * e; D += sg * (1.f - sg) * e; } }
+    else if (md.loss == G4R_LOSS_TOP1_MAX) { if (!ist[q]) { const float e = expf(y - mloc), a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y); Z += e; A += (a1 + b1) * e; D += a1 * (1.f - a1) * e; } }
+    else if (md.loss == G4R_LOSS_BPR) { const float sg = sigmoidf_(t - y); A += -logf(sg); if (!ist[q]) D += 1.f - sg; }
+    else { const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y); A += a1 + b1; if (!ist[q]) D += a1 * (1.f - a1); }
+  }
+#pragma unroll
+  for (int o = 1; o < 16; o <<= 1) {
+    Z += __shfl_xor_sync(0xffffffffu, Z, o); A += __shfl_xor_sync(0xffffffffu, A, o); Q += __shfl_xor_sync(0xffffffffu, Q, o);
+    D += __shfl_xor_sync(0xffffffffu, D, o); T += __shfl_xor_sync(0xffffffffu, T, o); has += __shfl_xor_sync(0xffffffffu, has, o);
+  }
+  if (has_chunk && okb && sub == 0) {
+    float* st = md.stat + ((size_t)chunk * md.B + b) * G4R_NSTAT;
+    st4(st, make_float4(mloc, Z, A, Q));
+    st4(st + 4, make_float4(D, T, has > 0.f ? 1.f : 0.f, pw ? t : 0.f));
+  }
+}
+// RS[b] of lane b from every chunk's statistics (one CTA per lane): row max over the chunk maxima, one rescale exp per chunk,
+// then plain sums (fixed shuffle / warp order)
+template <class SM>
+__device__ __forceinline__ void fk_row_stats(const ModelDev& md, SM& sm, int b, int M, int N) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float mc = -INFINITY, Z = 0.f, A = 0.f, Q = 0.f, D = 0.f, T = 0.f, has = 0.f, tt = 0.f;
+  if (tid < md.NCH) {
+    const float* st = md.stat + ((size_t)tid * md.B + b) * G4R_NSTAT;
+    const float4 u = ld4(st), v = ld4(st + 4);
+    mc = u.x; Z = u.y; A = u.z; Q = u.w; D = v.x; T = v.y; has = v.z;
+    if (tid == 0) tt = v.w;
+  }
+  float mg = mc;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) mg = fmaxf(mg, __shfl_xor_sync(0xffffffffu, mg, o));
+  if (lane == 0) sm.sPart[warp] = mg;
+  __syncthreads();
+  mg = sm.sPart[0];
+  for (int w = 1; w < FK_NW; w++) mg = fmaxf(mg, sm.sPart[w]);
+  if (loss_softmaxneg(md.loss)) mg = fmaxf(mg, 0.f);          // the zeroed diagonal takes part in the max (gru4rec.py:200-202)
+  if (loss_weighted(md.loss)) {
+    const float sc = (mc == -INFINITY) ? 0.f : expf(mc - mg);
+    Z *= sc; A *= sc; Q *= sc; D *= sc;
+  }
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    Z += __shfl_xor_sync(0xffffffffu, Z, o); A += __shfl_xor_sync(0xffffffffu, A, o); Q += __shfl_xor_sync(0xffffffffu, Q, o);
+    D += __shfl_xor_sync(0xffffffffu, D, o); T += __shfl_xor_sync(0xffffffffu, T, o); has += __shfl_xor_sync(0xffffffffu, has, o);
+  }
+  __syncthreads();
+  if (lane == 0) { float* w = sm.sPart + 32 + warp * 8; w[0] = Z; w[1] = A; w[2] = Q; w[3] = D; w[4] = T; w[5] = has; w[6] = tt; }
+  __syncthreads();
+  if (tid == 0) {
+    tt = sm.sPart[32 + 6];
+    for (int w = 1; w < FK_NW; w++) { const float* q = sm.sPart + 32 + w * 8; Z += q[0]; A += q[1]; Q += q[2]; D += q[3]; T += q[4]; }
+    stats_finalize(md, b, M, N, mg, Z, A, Q, D, T, tt);
+  }
+}
+// every lane's RS into sRS; chunk 0 writes the step's cost (the lanes' losses over batch_size)
+template <class SM>
+__device__ __forceinline__ void fk_cost(const ModelDev& md, SM& sm, int s, int M, int chunk) {
+  const int tid = threadIdx.x;
+  if (tid < M * 2) st4(sm.sRS + tid * 4, ld4(md.RS + tid * 4));
+  __syncthreads();
+  if (chunk == 0 && tid == 0) {
+    float c = 0.f;
+    for (int b = 0; b < M; b++) c += sm.sRS[b * 8 + 6];
+    c = __fdiv_rn(c, (float)md.B);
+    md.cost[s] = c;
+    if (c != c) atomicExch(md.nanflag, 1);
+  }
+}
+// dL/do of the chunk's columns into sG (zero outside the nj x M tile)
+template <class SM>
+__device__ __forceinline__ void fk_grad(const ModelDev& md, SM& sm, int buf, int M, int N, int cb, int nj) {
+  for (int i = threadIdx.x; i < FK_CT * FK_B; i += FK_THREADS) {
+    const int jj = i / FK_B, b = i % FK_B;
+    sm.sG[i] = (jj < nj && b < M) ? loss_grad_elem(md, sm.sRS + (size_t)b * 8, sm.sO[i], sm.sTc[buf][b] == cb + jj, M, N) : 0.f;
+  }
+}
 #include "g4r_fastc.cuh"
 
 // CL = false: GRU phases on a 48-CTA group with global group barriers (step_mode 2).
@@ -778,7 +926,7 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
   const ModelDev& md = MD;
   const LayerDev& ly = md.layer[0];
   const int cta = blockIdx.x, ncta = gridDim.x;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int G = CL ? (int)cl_size() : md.ldL / 4;   // CTAs of the GRU role (step_mode 2: one quad of hidden units each)
   const bool gru = cta < G;
   // column CTAs: step_mode 2 the CTAs after the GRU group (the host sized NCH <= ncta - G), step_mode 3 every CTA.  Column CTA
@@ -892,85 +1040,11 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
     const int cb = sm.sCb[buf][0], ce = sm.sCb[buf][1];
     const int nj = ce - cb;
     // ---- scores + partial statistics ----
-    if (pw) {                                   // target activations: warp per 4 lanes
-      for (int b = warp; b < FK_B; b += FK_NW) {
-        if (b < M) {
-          float a = 0.f;
-          if (lane < kw) {
-            const float4 y = ld4(sm.sY + b * FK_LDS + lane * 4), w = ld4(sm.sTW + b * FK_LDS + lane * 4);
-            a = fmaf(w.x, y.x, a); a = fmaf(w.y, y.y, a); a = fmaf(w.z, y.z, a); a = fmaf(w.w, y.w, a);
-          }
-          a = warp_sum(a);
-          if (lane == 0) sm.sT[b] = act_fwd(md.fact, a + sm.sTB[b]);
-        }
-      }
-    }
     {
-      float accq[FK_Q];
-#pragma unroll
-      for (int q = 0; q < FK_Q; q++) accq[q] = 0.f;
-      const float* yr = sm.sY + lane * FK_LDS;
-      for (int c4 = 0; c4 < kw; c4++) {
-        const float4 y = ld4(yr + c4 * 4);
-#pragma unroll
-        for (int q = 0; q < FK_Q; q++) {
-          if (warp + FK_NW * q < nj) {
-            const float4 w = ld4(sm.sS + (warp + FK_NW * q) * FK_LDS + c4 * 4);
-            accq[q] = fmaf(y.x, w.x, accq[q]); accq[q] = fmaf(y.y, w.y, accq[q]); accq[q] = fmaf(y.z, w.z, accq[q]); accq[q] = fmaf(y.w, w.w, accq[q]);
-          }
-        }
-      }
+      float acc[FK_Q];
+      fk_scores(md, sm, acc, M, nj, pw);
       FK_STAMP(9);
-#pragma unroll
-      for (int q = 0; q < FK_Q; q++) {
-        const int jj = warp + q * FK_NW;
-        if (jj < nj && lane < M) sm.sO[jj * FK_B + lane] = accq[q] + sm.sBias[jj];
-      }
-      __syncthreads();                          // sT and sO complete
-      // chunk statistics of lane b by 16 threads (column jj = sub, sub + 16): row max first, then plain sums -- one expf
-      // per column instead of an exp-rescaling merge per element
-      {
-        const int b = tid >> 4, sub = tid & 15;            // FK_THREADS / 16 == FK_B lanes
-        const bool okb = b < M;
-        const int tc = okb ? sm.sTc[buf][b] : -1;
-        const float t = (pw && okb) ? sm.sT[b] : 0.f;
-        float yv[2]; bool use[2], ist[2];
-        float mloc = -INFINITY;
-        const bool smx = loss_softmaxneg(md.loss), xe = (md.loss == G4R_LOSS_XE || md.loss == G4R_LOSS_XE_LOGIT);
-#pragma unroll
-        for (int q = 0; q < 2; q++) {
-          const int jj = sub + 16 * q;
-          use[q] = okb && jj < nj;
-          ist[q] = use[q] && (tc == cb + jj);
-          const float o = use[q] ? sm.sO[jj * FK_B + b] : 0.f;
-          yv[q] = xe ? o : act_fwd(md.fact, o);
-          if (use[q] && (xe || (smx && !ist[q]))) mloc = fmaxf(mloc, yv[q]);
-        }
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1) mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, o));
-        float Z = 0.f, A = 0.f, Q = 0.f, D = 0.f, T = 0.f, has = 0.f;
-#pragma unroll
-        for (int q = 0; q < 2; q++) {
-          if (!use[q]) continue;
-          const float y = yv[q];
-          if (ist[q]) has = 1.f;
-          if (xe) { Z += expf(y - mloc); if (ist[q]) T = y; }
-          else if (md.loss == G4R_LOSS_BPR_MAX) { if (!ist[q]) { const float e = expf(y - mloc), sg = sigmoidf_(t - y); Z += e; A += sg * e; Q += y * y * e; D += sg * (1.f - sg) * e; } }
-          else if (md.loss == G4R_LOSS_TOP1_MAX) { if (!ist[q]) { const float e = expf(y - mloc), a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y); Z += e; A += (a1 + b1) * e; D += a1 * (1.f - a1) * e; } }
-          else if (md.loss == G4R_LOSS_BPR) { const float sg = sigmoidf_(t - y); A += -logf(sg); if (!ist[q]) D += 1.f - sg; }
-          else { const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y); A += a1 + b1; if (!ist[q]) D += a1 * (1.f - a1); }
-        }
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1) {
-          Z += __shfl_xor_sync(0xffffffffu, Z, o); A += __shfl_xor_sync(0xffffffffu, A, o); Q += __shfl_xor_sync(0xffffffffu, Q, o);
-          D += __shfl_xor_sync(0xffffffffu, D, o); T += __shfl_xor_sync(0xffffffffu, T, o); has += __shfl_xor_sync(0xffffffffu, has, o);
-        }
-        if (has_chunk && okb && sub == 0) {
-          float* st = md.stat + ((size_t)chunk * md.B + b) * G4R_NSTAT;
-          st4(st, make_float4(mloc, Z, A, Q));
-          st4(st + 4, make_float4(D, T, has > 0.f ? 1.f : 0.f, pw ? t : 0.f));
-        }
-      }
+      fk_chunk_stats(md, sm, acc, buf, M, cb, nj, chunk, has_chunk, pw);
     }
     // ---- barrier B2, then lane b's statistics are combined by column CTA b (all lanes in parallel, fixed merge order) ----
     __syncthreads();
@@ -979,72 +1053,17 @@ __global__ void __launch_bounds__(FK_THREADS, 1) k_fast_t(int slot, int n_steps,
     if (tid == 0) { red_release_add(&fs->bar, 1u); wait_ge(&fs->bar, bar_epoch * (unsigned int)ncol); }
     __syncthreads();
     if (chunk < M) {
-      // lane b = chunk: row max over the chunk maxima, one rescale exp per chunk, then plain sums (fixed shuffle / warp order)
-      const int b = chunk;
-      const bool maxed = !(md.loss == G4R_LOSS_BPR || md.loss == G4R_LOSS_TOP1);
-      float mc = -INFINITY, Z = 0.f, A = 0.f, Q = 0.f, D = 0.f, T = 0.f, has = 0.f, tt = 0.f;
-      if (tid < md.NCH) {
-        const float* st = md.stat + ((size_t)tid * md.B + b) * G4R_NSTAT;
-        const float4 u = ld4(st), v = ld4(st + 4);
-        mc = u.x; Z = u.y; A = u.z; Q = u.w; D = v.x; T = v.y; has = v.z;
-        if (tid == 0) tt = v.w;
-      }
-      float mg = mc;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) mg = fmaxf(mg, __shfl_xor_sync(0xffffffffu, mg, o));
-      if (lane == 0) sm.sPart[warp] = mg;
-      __syncthreads();
-      mg = sm.sPart[0];
-      for (int w = 1; w < FK_NW; w++) mg = fmaxf(mg, sm.sPart[w]);
-      if (loss_softmaxneg(md.loss)) mg = fmaxf(mg, 0.f);          // the zeroed diagonal takes part in the max (gru4rec.py:200-202)
-      if (maxed) {
-        const float sc = (mc == -INFINITY) ? 0.f : expf(mc - mg);
-        Z *= sc; A *= sc; Q *= sc; D *= sc;
-      }
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        Z += __shfl_xor_sync(0xffffffffu, Z, o); A += __shfl_xor_sync(0xffffffffu, A, o); Q += __shfl_xor_sync(0xffffffffu, Q, o);
-        D += __shfl_xor_sync(0xffffffffu, D, o); T += __shfl_xor_sync(0xffffffffu, T, o); has += __shfl_xor_sync(0xffffffffu, has, o);
-      }
-      __syncthreads();
-      if (lane == 0) { float* w = sm.sPart + 32 + warp * 8; w[0] = Z; w[1] = A; w[2] = Q; w[3] = D; w[4] = T; w[5] = has; w[6] = tt; }
-      __syncthreads();
-      if (tid == 0) {
-        tt = sm.sPart[32 + 6];
-        for (int w = 1; w < FK_NW; w++) { const float* q = sm.sPart + 32 + w * 8; Z += q[0]; A += q[1]; Q += q[2]; D += q[3]; T += q[4]; }
-        const float m = mg;
-        float* rs = md.RS + (size_t)b * G4R_NSTAT;
-        float loss = 0.f, r0 = m, r1 = Z, r2 = 0.f, r3 = 0.f, r4 = 0.f, r5 = tt;
-        if (md.loss == G4R_LOSS_XE) { const float pt = __fdiv_rn(expf(T - m), Z); loss = -logf(pt + G4R_EPS_LOG); r2 = pt; r5 = T; }
-        else if (md.loss == G4R_LOSS_XE_LOGIT) { loss = logf(Z) - (T - m); r5 = T; }
-        else if (md.loss == G4R_LOSS_BPR_MAX) { r2 = __fdiv_rn(A, Z); r3 = __fdiv_rn(Q, Z); r4 = __fdiv_rn(D, Z); loss = -logf(r2 + G4R_EPS_LOG) + md.bpreg * r3; }
-        else if (md.loss == G4R_LOSS_TOP1_MAX) { r2 = __fdiv_rn(A, Z); r4 = __fdiv_rn(D, Z); loss = r2; }
-        else if (md.loss == G4R_LOSS_BPR) { loss = A; r4 = D; }
-        else { const float c = sigmoidf_(tt * tt); loss = (float)M * (__fdiv_rn(A, (float)N) - __fdiv_rn(c, (float)(M + md.S_cfg))); r4 = D; }
-        st4(rs, make_float4(r0, r1, r2, r3));
-        st4(rs + 4, make_float4(r4, r5, loss, 0.f));
-        red_release_add(&fs->stats, 1u);
-      }
+      fk_row_stats(md, sm, chunk, M, N);
+      if (tid == 0) red_release_add(&fs->stats, 1u);
     }
     stats_target += (unsigned int)M;
     if (tid == 0) wait_ge(&fs->stats, stats_target);
     __syncthreads();
     FK_STAMP(2);
     // ---- loss gradient, dSy, partial dL/dh, sparse update of this chunk's rows ----
-    if (tid < M * 2) st4(sm.sRS + tid * 4, ld4(md.RS + tid * 4));
-    __syncthreads();
-    if (chunk == 0 && tid == 0) {
-      float c = 0.f;
-      for (int b = 0; b < M; b++) c += sm.sRS[b * 8 + 6];
-      c = __fdiv_rn(c, (float)md.B);
-      md.cost[s] = c;
-      if (c != c) atomicExch(md.nanflag, 1);
-    }
+    fk_cost(md, sm, s, M, chunk);
     FK_STAMP(11);
-    for (int i = tid; i < FK_CT * FK_B; i += FK_THREADS) {
-      const int jj = i / FK_B, b = i % FK_B;
-      sm.sG[i] = (jj < nj && b < M) ? loss_grad_elem(md, sm.sRS + (size_t)b * 8, sm.sO[i], sm.sTc[buf][b] == cb + jj, M, N) : 0.f;
-    }
+    fk_grad(md, sm, buf, M, N, cb, nj);
     __syncthreads();
     fk_dby(sm, M, nj);
     FK_STAMP(12);

@@ -544,47 +544,7 @@ constexpr int SC_KT = 128;   // feature slab
 constexpr int SC_LDS = SC_KT + 4;
 constexpr int SC_THREADS = 256;
 
-struct RowStat { float m, Z, A, Q, D, T, aux; };
-
-__device__ __forceinline__ bool loss_pairwise(int loss) { return loss == G4R_LOSS_BPR_MAX || loss == G4R_LOSS_TOP1_MAX || loss == G4R_LOSS_BPR || loss == G4R_LOSS_TOP1; }
-__device__ __forceinline__ bool loss_softmaxneg(int loss) { return loss == G4R_LOSS_BPR_MAX || loss == G4R_LOSS_TOP1_MAX; }
-
-// merge (m,Z,A,Q,D) of two partial softmax-weighted sums
-__device__ __forceinline__ void stat_merge(float& m, float& Z, float& A, float& Q, float& D, float m2, float Z2, float A2, float Q2, float D2) {
-  const float mn = fmaxf(m, m2);
-  const float e1 = (m == -INFINITY) ? 0.f : expf(m - mn), e2 = (m2 == -INFINITY) ? 0.f : expf(m2 - mn);
-  Z = Z * e1 + Z2 * e2; A = A * e1 + A2 * e2; Q = Q * e1 + Q2 * e2; D = D * e1 + D2 * e2; m = mn;
-}
-
-// accumulate one score column into a row's running statistics (online softmax-style merge)
-__device__ __forceinline__ void stat_add_elem(const ModelDev& md, float o, bool is_t, float t, float& m, float& Z, float& A, float& Q, float& D, float& T, float& has) {
-  if (md.loss == G4R_LOSS_XE || md.loss == G4R_LOSS_XE_LOGIT) {
-    stat_merge(m, Z, A, Q, D, o, 1.f, 0.f, 0.f, 0.f);
-    if (is_t) { T = o; has = 1.f; }
-    return;
-  }
-  const float y = act_fwd(md.fact, o);
-  if (is_t) has = 1.f;
-  if (md.loss == G4R_LOSS_BPR_MAX) {
-    if (!is_t) { const float sg = sigmoidf_(t - y); stat_merge(m, Z, A, Q, D, y, 1.f, sg, y * y, sg * (1.f - sg)); }
-  } else if (md.loss == G4R_LOSS_TOP1_MAX) {
-    if (!is_t) { const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y); stat_merge(m, Z, A, Q, D, y, 1.f, a1 + b1, 0.f, a1 * (1.f - a1)); }
-  } else if (md.loss == G4R_LOSS_BPR) {
-    const float sg = sigmoidf_(t - y);
-    A += -logf(sg);
-    if (!is_t) D += 1.f - sg;
-  } else {  // TOP1
-    const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y);
-    A += a1 + b1;
-    if (!is_t) D += a1 * (1.f - a1);
-  }
-}
-__device__ __forceinline__ void stat_combine(const ModelDev& md, float& m, float& Z, float& A, float& Q, float& D, float& T, float& has,
-                                             float m2, float Z2, float A2, float Q2, float D2, float T2, float has2) {
-  if (md.loss == G4R_LOSS_BPR || md.loss == G4R_LOSS_TOP1) { A += A2; D += D2; }
-  else stat_merge(m, Z, A, Q, D, m2, Z2, A2, Q2, D2);
-  if (has2 > 0.f) { T = T2; has = 1.f; }
-}
+#include "g4r_loss.cuh"
 
 __device__ void phase_score(const ModelDev& md, int s, int chunk, float* smem) {
   const int M = md.wM[s];
@@ -723,40 +683,9 @@ __host__ __device__ inline size_t score_smem_bytes(int Bld) {
   return (size_t)(SC_TB * SC_LDS + SC_CT * SC_LDS + Bld + Bld * 8 + 8 * SC_TB * 8 + SC_CT + 2 * SC_CT + 32) * sizeof(float);
 }
 
-// final row statistics RS[b] = {m, Z, A', Q', D', t or target score, loss_b} from the merged sums (gru4rec.py:225-248)
-__device__ __forceinline__ void stats_finalize(const ModelDev& md, int b, int M, int N, float m, float Z, float A, float Q, float D, float T, float tt) {
-  float* rs = md.RS + (size_t)b * G4R_NSTAT;
-  float loss = 0.f;
-  if (md.loss == G4R_LOSS_XE) {
-    const float pt = __fdiv_rn(expf(T - m), Z);
-    loss = -logf(pt + G4R_EPS_LOG);
-    rs[0] = m; rs[1] = Z; rs[5] = T; rs[2] = pt;
-  } else if (md.loss == G4R_LOSS_XE_LOGIT) {
-    loss = logf(Z) - (T - m);
-    rs[0] = m; rs[1] = Z; rs[5] = T;
-  } else if (md.loss == G4R_LOSS_BPR_MAX) {
-    const float Ap = __fdiv_rn(A, Z), Qp = __fdiv_rn(Q, Z), Dp = __fdiv_rn(D, Z);
-    loss = -logf(Ap + G4R_EPS_LOG) + md.bpreg * Qp;
-    rs[0] = m; rs[1] = Z; rs[2] = Ap; rs[3] = Qp; rs[4] = Dp; rs[5] = tt;
-  } else if (md.loss == G4R_LOSS_TOP1_MAX) {
-    const float Ap = __fdiv_rn(A, Z), Dp = __fdiv_rn(D, Z);
-    loss = Ap;
-    rs[0] = m; rs[1] = Z; rs[2] = Ap; rs[4] = Dp; rs[5] = tt;
-  } else if (md.loss == G4R_LOSS_BPR) {
-    loss = A;
-    rs[4] = D; rs[5] = tt;
-  } else {  // TOP1 (gru4rec.py:242-244): mean over the N columns, last term over M + n_sample; the reference subtracts a
-    // COLUMN from the row-mean vector, which broadcasts to [M x M] before the sum: everything is M times the row expression
-    const float c = sigmoidf_(tt * tt);
-    loss = (float)M * (__fdiv_rn(A, (float)N) - __fdiv_rn(c, (float)(M + md.S_cfg)));
-    rs[4] = D; rs[5] = tt;
-  }
-  rs[6] = loss;
-}
-
 // ------------------------------------------------------------------------------------------------
 // phase S2: combine the chunk statistics of lane b (one CTA per lane; fixed combine order => deterministic)
-// RS[b] = {m, Z, A', Q', D', t_or_targetO, loss_b}
+// RS[b] = {m, Z, A', Q', D', t_or_targetO, loss_b, 0}
 // ------------------------------------------------------------------------------------------------
 __device__ void phase_stats(const ModelDev& md, int s, int cta, int ncta, float* smem) {
   const int M = md.wM[s];
@@ -807,9 +736,7 @@ __device__ void phase_stats2a(const ModelDev& md, int s, int chunk) {
     const float m = md.RS[(size_t)b * G4R_NSTAT], Z = md.RS[(size_t)b * G4R_NSTAT + 1];
     float s1 = 0.f, f = 0.f;
     for (int j = cb; j < ce; j++) {
-      const float o = md.O[(size_t)j * md.Bld + b];
-      if (md.loss == G4R_LOSS_XE) { const float p = __fdiv_rn(expf(o - m), Z); s1 += -logf(p + G4R_EPS_LOG); f += __fdiv_rn(p, p + G4R_EPS_LOG); }
-      else s1 += logf(Z) - (o - m);
+      smooth_add_elem(md.loss, md.O[(size_t)j * md.Bld + b], m, Z, s1, f);
     }
     md.stat2[((size_t)chunk * md.B + b) * 2] = s1;
     md.stat2[((size_t)chunk * md.B + b) * 2 + 1] = f;
@@ -829,11 +756,8 @@ __device__ void phase_stats2b(const ModelDev& md, int s, int cta, int ncta, floa
       s1 = 0.f; f = 0.f;
       for (int w = 0; w < nwarp; w++) { s1 += smem[w * 2]; f += smem[w * 2 + 1]; }
       float* rs = md.RS + (size_t)b * G4R_NSTAT;
-      const float n_out = (float)(M + md.S_cfg);
-      const float c1 = 1.0f - __fdiv_rn(n_out, n_out - 1.0f) * md.smoothing, c2 = __fdiv_rn(md.smoothing, n_out - 1.0f);
       rs[3] = f;
-      if (md.loss == G4R_LOSS_XE) rs[6] = c1 * (-logf(rs[2] + G4R_EPS_LOG)) + c2 * s1;
-      else rs[6] = c1 * (logf(rs[1]) - (rs[5] - rs[0])) + c2 * s1;
+      rs[6] = smooth_loss(md, M, rs, s1);
     }
     __syncthreads();
   }
@@ -865,68 +789,6 @@ __device__ void phase_gradnorm(const ModelDev& md, int s, const float* dense_fla
   }
 }
 
-// dL/do for element (b, column j) given final row statistics (already divided by batch_size)
-__device__ __forceinline__ float loss_grad_elem(const ModelDev& md, const float* rs, float o, bool is_t, int M, int N) {
-  const float invB = __fdiv_rn(1.0f, (float)md.B);
-  if (md.smoothing > 0.f && (md.loss == G4R_LOSS_XE || md.loss == G4R_LOSS_XE_LOGIT)) {
-    // label smoothing (gru4rec.py:226-228, 232-234): loss_i = c1 * l(target) + c2 * sum_j l(j), n_out = M + n_sample
-    const float n_out = (float)(M + md.S_cfg);
-    const float c1 = 1.0f - __fdiv_rn(n_out, n_out - 1.0f) * md.smoothing, c2 = __fdiv_rn(md.smoothing, n_out - 1.0f);
-    const float p = __fdiv_rn(expf(o - rs[0]), rs[1]);
-    if (md.loss == G4R_LOSS_XE) {
-      const float f = __fdiv_rn(p, p + G4R_EPS_LOG), ft = __fdiv_rn(rs[2], rs[2] + G4R_EPS_LOG);
-      return (-c2 * f - (is_t ? c1 * ft : 0.f) + p * (c2 * rs[3] + c1 * ft)) * invB;       // rs[3] = sum_j p_j / (p_j + eps)
-    }
-    return (-(c2 + (is_t ? c1 : 0.f)) + p * (c2 * (float)N + c1)) * invB;
-  }
-  if (md.loss == G4R_LOSS_XE) {
-    const float p = __fdiv_rn(expf(o - rs[0]), rs[1]);
-    const float fac = __fdiv_rn(rs[2], rs[2] + G4R_EPS_LOG);
-    return fac * (p - (is_t ? 1.f : 0.f)) * invB;
-  }
-  if (md.loss == G4R_LOSS_XE_LOGIT) {
-    const float p = __fdiv_rn(expf(o - rs[0]), rs[1]);
-    return (p - (is_t ? 1.f : 0.f)) * invB;
-  }
-  const float y = act_fwd(md.fact, o);
-  const float fd = act_der(md.fact, o, y);
-  const float t = rs[5];
-  float dy;
-  if (md.loss == G4R_LOSS_BPR_MAX) {
-    const float Ap = rs[2], Qp = rs[3], Dp = rs[4];
-    const float invA = __fdiv_rn(1.0f, Ap + G4R_EPS_LOG);
-    if (is_t) dy = -invA * Dp;
-    else {
-      const float sj = __fdiv_rn(expf(y - rs[0]), rs[1]);
-      const float sg = sigmoidf_(t - y);
-      const float dLds = -invA * sg + md.bpreg * y * y;
-      const float mean = -invA * Ap + md.bpreg * Qp;
-      dy = sj * (dLds - mean) + invA * sj * sg * (1.f - sg) + 2.f * md.bpreg * y * sj;
-    }
-  } else if (md.loss == G4R_LOSS_TOP1_MAX) {
-    const float Ap = rs[2], Dp = rs[4];
-    if (is_t) dy = -Dp;
-    else {
-      const float sj = __fdiv_rn(expf(y - rs[0]), rs[1]);
-      const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y);
-      dy = sj * ((a1 + b1) - Ap) + sj * a1 * (1.f - a1) + sj * b1 * (1.f - b1) * 2.f * y;
-    }
-  } else if (md.loss == G4R_LOSS_BPR) {
-    if (is_t) dy = -rs[4];
-    else dy = 1.f - sigmoidf_(t - y);
-  } else {  // TOP1 (M times the row expression, see the statistics phase)
-    const float invN = __fdiv_rn(1.0f, (float)N);
-    if (is_t) {
-      const float c = sigmoidf_(t * t);
-      dy = -rs[4] * invN + c * (1.f - c) * 2.f * t * invN - __fdiv_rn(c * (1.f - c) * 2.f * t, (float)(M + md.S_cfg));
-    } else {
-      const float a1 = sigmoidf_(y - t), b1 = sigmoidf_(y * y);
-      dy = (a1 * (1.f - a1) + b1 * (1.f - b1) * 2.f * y) * invN;
-    }
-    dy *= (float)M;
-  }
-  return dy * fd * invB;
-}
 
 // ------------------------------------------------------------------------------------------------
 // phase S3: loss gradient for this chunk's columns, dSy / dby rows, partial dL/dh, then the sparse
