@@ -1,6 +1,7 @@
 """ctypes binding of libg4r.so (include/g4r.h).  There is no CPU path: loading fails loudly if the
 library is missing, and creating a handle fails loudly if no CUDA device is visible."""
 import ctypes as C
+import math
 import os
 import numpy as np
 
@@ -51,7 +52,7 @@ EXPORTS = [
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
-    'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1',
+    'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit',
 ]
 
 _lib = None
@@ -156,6 +157,7 @@ def load():
     lib.g4r_bl_sknn_fit.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32]
     lib.g4r_bl_stan_fit.argtypes = [vp, vp, i64, vp, i64, vp, vp, vp, vp, i64, i32]
     lib.g4r_bl_stan_set_w1.argtypes = [vp, vp, i64]
+    lib.g4r_bl_rules_fit.argtypes = [vp, vp, i64, vp, i64, i32, i32, C.POINTER(i64), C.POINTER(C.c_size_t), C.POINTER(C.c_float)]
     _lib = lib
     return lib
 
@@ -780,14 +782,43 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
+RULES_WEIGHTING = {'div': 0, 'same': 1}
+RULES_STEPS_MAX = 20
+KEEP_MAX = 1024             # n_sims / k / pruning bound of the row-keeping baselines
+
+
+def rules_scale(steps, weighting):
+    """L of a rules fit: lcm(1 .. steps) for SR 'div' (every L / d is an integer), 1 for SR 'same' and for AR (steps None)"""
+    L = 1
+    if steps is not None and weighting == 'div':
+        for d in range(2, steps + 1):
+            L = L * d // math.gcd(L, d)
+    return L
+
+
+def rules_bound(session_offsets, items, n_items, steps, weighting):
+    """the largest per-row bound of a rules fit's uint64 counts, as a Python int: SR occurrences * min(steps, longest session -
+    1) * L, AR (steps None) the sum of n_s over the row item's occurrences"""
+    off = np.asarray(session_offsets, dtype=np.int64)
+    it = np.asarray(items, dtype=np.int64)
+    lens = np.diff(off)
+    if not it.size:
+        return 0
+    if steps is None:
+        o = np.argsort(it, kind='stable')
+        _, first = np.unique(it[o], return_index=True)
+        return int(np.add.reduceat(np.repeat(lens, lens)[o], first).max())    # < 2^62 for fewer than 2^31 events
+    occ = int(np.bincount(it, minlength=n_items).max())
+    return occ * min(steps, max(int(lens.max()) - 1, 0)) * rules_scale(steps, weighting)
 
 
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
-    a baseline, the BPR-MF fit and factors (DESIGN §3k), and the SessionKNN and STAN indexes (DESIGN §3o, §3p).  kind: 'pop',
-    'sessionpop', 'itemknn', 'bpr', 'sknn' or 'stan'; n_keep: top_n, n_sims, n_factors or k."""
+    a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN and STAN indexes (DESIGN §3o, §3p), and the SR / AR fit
+    into ItemKNN's rows (DESIGN §3q).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr' or 'ar'; n_keep: top_n,
+    n_sims, n_factors, k or pruning."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -934,6 +965,36 @@ class Baselines(object):
             raise ValueError('stan_fit: w3 must be a non-empty 1-D table')
         self._check(self.lib.g4r_bl_stan_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(pos), _ptr(rc), _ptr(w2), _ptr(w3),
                                              w3.size, int(sample_size)))
+
+    def rules_fit(self, session_offsets, items, steps=None, weighting=None):
+        """SR (steps 1 .. 20, weighting 'div' / 'same') or AR (steps and weighting None) rows from the training events as session
+        CSR of item indices in time order; returns (pair work, scratch bytes, fit kernel ms).  Refuses a fit whose per-row bound
+        (rules_bound) reaches 2^63 before the library is called."""
+        if not 1 <= self.n_keep <= KEEP_MAX:
+            raise ValueError('rules_fit: pruning must be in 1 .. %d, not %r' % (KEEP_MAX, self.n_keep))
+        if self.kind == 'ar':
+            if steps is not None or weighting is not None:
+                raise ValueError('rules_fit: AR takes no steps or weighting')
+        else:
+            if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or not 1 <= steps <= RULES_STEPS_MAX:
+                raise ValueError('rules_fit: steps must be an integer in 1 .. %d, not %r' % (RULES_STEPS_MAX, steps))
+            if weighting not in RULES_WEIGHTING:
+                raise ValueError('rules_fit: weighting must be one of %s, not %r' % (sorted(RULES_WEIGHTING), weighting))
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        if off.ndim != 1 or off.size < 1 or it.ndim != 1:
+            raise ValueError('rules_fit: need session offsets and a 1-D item array')
+        if it.size and (it.min() < 0 or it.max() >= self.n_items):
+            raise IndexError('rules_fit: item index out of range')
+        if off[0] != 0 or off[-1] != it.size or (np.diff(off) < 0).any():
+            raise ValueError('rules_fit: session offsets must rise from 0 to the number of events')
+        if off.size - 1 > 2 ** 31 - 1 or it.size > 2 ** 31 - 1:
+            raise ValueError('rules_fit: more than 2^31 - 1 sessions or events')
+        if rules_bound(off, it, self.n_items, steps, weighting) >= 1 << 63:
+            raise ValueError('rules_fit: a row\'s weight bound reaches 2^63 (uint64 counts could overflow)')
+        pw, sb, ms = C.c_int64(), C.c_size_t(), C.c_float()
+        self._check(self.lib.g4r_bl_rules_fit(self.h, _ptr(off), off.size - 1, _ptr(it), it.size, 0 if steps is None else int(steps),
+                                              0 if weighting is None else RULES_WEIGHTING[weighting], C.byref(pw), C.byref(sb), C.byref(ms)))
+        return pw.value, sb.value, ms.value
 
     def stan_set_w1(self, w1):
         """the STAN prefix-distance table W1[0 .. n): it must cover every counted event's prefix length"""

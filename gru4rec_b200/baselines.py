@@ -1,6 +1,6 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
-signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), and session-based kNN (SessionKNN, DESIGN
-§3o; STAN, §3p) with the same surface.  ItemKNN's fit runs on the device (the
+signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
+§3o; STAN, §3p) and the rule-based baselines (SR and AR, §3q, fitted on the device) with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -487,3 +487,83 @@ class STAN(SessionKNN):
             sel = owner == q
             score[flat[sel]] = score[flat[sel]] + sims[q] * self.w3[np.abs(fpos[sel] - qr[q])]
         return score
+
+
+class _Rules(Baseline):
+    """What SR and AR share (DESIGN §3q): the training sequences, the device fit, the kept rows and predict_next from them"""
+
+    def _n_keep(self):
+        return self.pruning
+
+    def _steps(self):
+        return None, None
+
+    def fit(self, data):
+        if isinstance(self.pruning, bool) or not isinstance(self.pruning, (int, np.integer)) or not 1 <= self.pruning <= _lib.KEEP_MAX:
+            raise ValueError('pruning must be an integer in 1 .. %d, not %r' % (_lib.KEEP_MAX, self.pruning))
+        steps, weighting = self._steps()
+        idx = self._index(data)
+        sess = data[self.session_key].values
+        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
+        o = np.lexsort((data[self.time_key].values, code))      # each session's events by time, ties by row order
+        S = int(code.max()) + 1 if len(code) else 0
+        offsets = np.zeros(S + 1, np.int64)
+        offsets[1:] = np.cumsum(np.bincount(code, minlength=S))
+        self.__dict__.pop('_dev', None)
+        dev = _lib.Baselines(self._kind, self.n_items, self.pruning)
+        self.fit_stats = dev.rules_fit(offsets, idx[o], steps, weighting)
+        self.rows = dev.rows_export()
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.rows_import(*self.rows)
+
+    predict_next = ItemKNN.predict_next
+
+
+class SR(_Rules):
+    '''
+    SR(steps=10, weighting='div', pruning=20, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Sequential rules: a directed rule from an item to each item that follows it within `steps` events of a training session,
+    weighted by the distance.  This is this project's definition (DESIGN §3q); it is not claimed to match any other implementation
+    bit for bit.  A session's events are ordered by time_key (ties by row order): x_1 .. x_n, repeats kept.  w(i, j) is the sum
+    over sessions and position pairs p < q <= p + steps with x_p = i, x_q = j and i != j of f(q - p), f(d) = 1 / d ('div') or 1
+    ('same').  The device counts W = w * L exactly in uint64 (L = lcm(1 .. steps) for 'div', else 1) and divides once in float64.
+    Each item keeps its `pruning` (1 .. 1024) largest weights (ties by the smaller item index); after input x, item j scores w(x, j)
+    if kept, else 0.  SR(steps=1, weighting='same') is the first-order Markov baseline: transition counts, self-transitions
+    dropped.  After fit, `rows` holds the kept rows (ItemKNN's layout) and `fit_stats` (pair work, scratch bytes, device ms).
+    '''
+    _kind = 'sr'
+
+    def __init__(self, steps=10, weighting='div', pruning=20, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.steps = steps
+        self.weighting = weighting
+        self.pruning = pruning
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+
+    def _steps(self):
+        if isinstance(self.steps, bool) or not isinstance(self.steps, (int, np.integer)) or not 1 <= self.steps <= _lib.RULES_STEPS_MAX:
+            raise ValueError('steps must be an integer in 1 .. %d, not %r' % (_lib.RULES_STEPS_MAX, self.steps))
+        if self.weighting not in _lib.RULES_WEIGHTING:
+            raise ValueError('weighting must be one of %s, not %r' % (sorted(_lib.RULES_WEIGHTING), self.weighting))
+        return int(self.steps), self.weighting
+
+
+class AR(_Rules):
+    '''
+    AR(pruning=20, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Association rules: co-occurrence within a training session, without normalisation.  This is this project's definition (DESIGN
+    §3q).  w(i, j) = sum over sessions of occ_s(i) * occ_s(j) for i != j: every ordered pair of distinct positions holding i and
+    j counts 1 (ItemKNN's cnt counts occ_s(i) * [j in s] instead, and divides by a norm).  Rows, scores and `fit_stats` as SR's.
+    '''
+    _kind = 'ar'
+
+    def __init__(self, pruning=20, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.pruning = pruning
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key

@@ -4,7 +4,7 @@
 // nothing here touches a g4r_handle.
 #pragma once
 
-constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6;   // 4 stays unused
+constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6, BL_SR = 8, BL_AR = 9;   // 4 and 7 stay unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
@@ -17,7 +17,7 @@ struct g4r_baselines {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   bool ready = false;                                   // rows fitted / imported, or Pop scores set
-  // ItemKNN: [n_items x n_keep] rows by (sim desc, index asc) and the same rows by index asc (lookups); len [n_items]
+  // ItemKNN, SR and AR: [n_items x n_keep] rows by (sim desc, index asc) and the same rows by index asc (lookups); len [n_items]
   int *dIdx = nullptr, *dIdxI = nullptr, *dLen = nullptr;
   double *dSim = nullptr, *dSimI = nullptr;
   // Pop / SessionPop: dense scores [n_items] (0 past top_n) and the positive ones by (score desc, index asc)
@@ -63,6 +63,9 @@ struct KnnFitDev {
   int* out_idx; double* out_sim; int* out_len;
 };
 
+// the kinds whose model is ItemKNN's rows (g4r_rules.cuh fits SR and AR)
+__host__ __device__ __forceinline__ bool bl_has_rows(int kind) { return kind == BL_ITEMKNN || kind == BL_SR || kind == BL_AR; }
+
 // (score desc, index asc): the order of every kept row and list
 __device__ __forceinline__ bool bl_before(double sa, int ia, double sb, int ib) { return sa > sb || (sa == sb && ia < ib); }
 
@@ -86,43 +89,19 @@ __device__ void cta_bitonic(double* ks, int* ki, int P) {
   __syncthreads();
 }
 
-// one CTA per row from the work queue: cnt(i, .) accumulated in the CTA's dense slice (a column enters the touched list when its
-// count leaves 0), sims of the touched columns, a radix select of the n_keep largest on (sim bits, then index), a bitonic sort of
-// the kept entries, and the slice cleared on the way (atomicExch reads and zeroes each touched count)
-__global__ void __launch_bounds__(KF_THREADS) k_knn_fit(KnnFitDev d) {
+// row i of a fit (KF_THREADS threads): of the T touched columns tl[t] with values sv[t], the K largest by (value desc, index
+// asc) -- a radix select on (value bits, then index) and a bitonic sort of the kept entries -- into out_idx / out_sim (-1 / 0
+// past the kept ones) and out_len.  Only integer and bit operations: the values are copied, never computed.
+__device__ void bl_keep_row(const double* sv, const int* tl, int T, int K, int i, int* out_idx, double* out_sim, int* out_len) {
   __shared__ double sKs[KF_KEEP_MAX];
   __shared__ int sKi[KF_KEEP_MAX];
   __shared__ unsigned sHist[256];
-  __shared__ int sRow, sT, sKn, sBin, sNeed, sFull;
-  unsigned* acc = d.acc + (size_t)blockIdx.x * d.n_items;
-  int* tl = d.touched + (size_t)blockIdx.x * d.n_items;
-  double* sv = d.sims + (size_t)blockIdx.x * d.n_items;
-  const int tid = threadIdx.x, K = d.n_keep;
-  for (;;) {
-    if (tid == 0) { sRow = atomicAdd(d.next, 1); sT = 0; sKn = 0; }
-    __syncthreads();
-    if (sRow >= d.n_items) break;
-    const int i = d.order[sRow];
-    for (int64_t o = d.i_off[i] + tid; o < d.i_off[i + 1]; o += KF_THREADS) {
-      const int s = d.i_sess[o];
-      const unsigned c = (unsigned)d.i_mult[o];
-      for (int64_t e = d.s_off[s]; e < d.s_off[s + 1]; e++) {
-        const int j = d.s_item[e];
-        if (j != i && atomicAdd(&acc[j], c) == 0u) tl[atomicAdd(&sT, 1)] = j;
-      }
-    }
-    __syncthreads();
-    const int T = sT;
-    const double ai = d.a[i];
-    for (int t = tid; t < T; t += KF_THREADS) {
-      const int j = tl[t];
-      const unsigned c = atomicExch(&acc[j], 0u);
-      double nrm = __dmul_rn(ai, d.b[j]);
-      if (nrm == 0.0) nrm = 1.0;
-      sv[t] = __ddiv_rn((double)c, nrm);
-    }
-    __syncthreads();
-    // every sim is positive and finite, so its bits order like its value
+  __shared__ int sKn, sBin, sNeed, sFull;
+  const int tid = threadIdx.x;
+  if (tid == 0) sKn = 0;
+  __syncthreads();
+  {
+    // every value is positive and finite, so its bits order like its value
     unsigned long long prefix = 0ull, mask = 0ull;
     int need = K, full = 1;
     unsigned jprefix = 0u, jmask = 0u;
@@ -180,11 +159,48 @@ __global__ void __launch_bounds__(KF_THREADS) k_knn_fit(KnnFitDev d) {
     for (int q = n + tid; q < P; q += KF_THREADS) { sKs[q] = -1.0; sKi[q] = 0x7fffffff; }
     cta_bitonic<false>(sKs, sKi, P);
     for (int q = tid; q < K; q += KF_THREADS) {
-      d.out_idx[(size_t)i * K + q] = q < n ? sKi[q] : -1;
-      d.out_sim[(size_t)i * K + q] = q < n ? sKs[q] : 0.0;
+      out_idx[(size_t)i * K + q] = q < n ? sKi[q] : -1;
+      out_sim[(size_t)i * K + q] = q < n ? sKs[q] : 0.0;
     }
-    if (tid == 0) d.out_len[i] = n;
+    if (tid == 0) out_len[i] = n;
     __syncthreads();
+  }
+}
+
+// one CTA per row from the work queue: cnt(i, .) accumulated in the CTA's dense slice (a column enters the touched list when its
+// count leaves 0), sims of the touched columns, the kept entries by bl_keep_row, and the slice cleared on the way (atomicExch
+// reads and zeroes each touched count)
+__global__ void __launch_bounds__(KF_THREADS) k_knn_fit(KnnFitDev d) {
+  __shared__ int sRow, sT;
+  unsigned* acc = d.acc + (size_t)blockIdx.x * d.n_items;
+  int* tl = d.touched + (size_t)blockIdx.x * d.n_items;
+  double* sv = d.sims + (size_t)blockIdx.x * d.n_items;
+  const int tid = threadIdx.x;
+  for (;;) {
+    if (tid == 0) { sRow = atomicAdd(d.next, 1); sT = 0; }
+    __syncthreads();
+    if (sRow >= d.n_items) break;
+    const int i = d.order[sRow];
+    for (int64_t o = d.i_off[i] + tid; o < d.i_off[i + 1]; o += KF_THREADS) {
+      const int s = d.i_sess[o];
+      const unsigned c = (unsigned)d.i_mult[o];
+      for (int64_t e = d.s_off[s]; e < d.s_off[s + 1]; e++) {
+        const int j = d.s_item[e];
+        if (j != i && atomicAdd(&acc[j], c) == 0u) tl[atomicAdd(&sT, 1)] = j;
+      }
+    }
+    __syncthreads();
+    const int T = sT;
+    const double ai = d.a[i];
+    for (int t = tid; t < T; t += KF_THREADS) {
+      const int j = tl[t];
+      const unsigned c = atomicExch(&acc[j], 0u);
+      double nrm = __dmul_rn(ai, d.b[j]);
+      if (nrm == 0.0) nrm = 1.0;
+      sv[t] = __ddiv_rn((double)c, nrm);
+    }
+    __syncthreads();
+    bl_keep_row(sv, tl, T, d.n_keep, i, d.out_idx, d.out_sim, d.out_len);
   }
 }
 
@@ -596,13 +612,13 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN) {
-    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN) or 6 (STAN)";
+  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR) {
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR) or 9 (AR)";
     return G4R_ERR_INVALID;
   }
-  if (n_items < 1 || n_keep < 1 || ((kind == BL_ITEMKNN || kind == BL_SKNN || kind == BL_STAN) && n_keep > KF_KEEP_MAX) ||
+  if (n_items < 1 || n_keep < 1 || ((bl_has_rows(kind) || kind == BL_SKNN || kind == BL_STAN) && n_keep > KF_KEEP_MAX) ||
       (kind == BL_BPR && n_keep > BPR_F_MAX)) {
-    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN and STAN, <= " +
+    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR and AR, <= " +
                         std::to_string(BPR_F_MAX) + " n_factors for BPR)";
     return G4R_ERR_INVALID;
   }
@@ -622,7 +638,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   bool ok = true;
   if (kind == BL_BPR) {
     ok &= bl_alloc(&h->dI, rows) == cudaSuccess && bl_alloc(&h->dBI, n_items) == cudaSuccess;
-  } else if (kind == BL_ITEMKNN) {
+  } else if (bl_has_rows(kind)) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
   } else if (kind != BL_SKNN && kind != BL_STAN) {     // SessionKNN and STAN allocate at their fit
@@ -778,7 +794,7 @@ extern "C" int g4r_bl_set_pop(g4r_baselines* h, const double* scores, int64_t n)
 
 extern "C" int g4r_bl_rows_export(g4r_baselines* h, int32_t* idx, double* sim, int32_t* len) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind != BL_ITEMKNN || !h->ready) FAIL(G4R_ERR_STATE, "g4r_bl_rows_export: no fitted ItemKNN rows");
+  if (!bl_has_rows(h->kind) || !h->ready) FAIL(G4R_ERR_STATE, "g4r_bl_rows_export: no fitted ItemKNN, SR or AR rows");
   if (!idx || !sim || !len) FAIL(G4R_ERR_INVALID, "g4r_bl_rows_export: null argument");
   const size_t rows = (size_t)h->n_items * h->n_keep;
   cudaSetDevice(h->device);
@@ -791,7 +807,7 @@ extern "C" int g4r_bl_rows_export(g4r_baselines* h, int32_t* idx, double* sim, i
 
 extern "C" int g4r_bl_rows_import(g4r_baselines* h, const int32_t* idx, const double* sim, const int32_t* len) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind != BL_ITEMKNN) FAIL(G4R_ERR_STATE, "g4r_bl_rows_import: the handle is not an ItemKNN");
+  if (!bl_has_rows(h->kind)) FAIL(G4R_ERR_STATE, "g4r_bl_rows_import: the handle is not an ItemKNN, SR or AR");
   if (!idx || !sim || !len) FAIL(G4R_ERR_INVALID, "g4r_bl_rows_import: null argument");
   const int NI = h->n_items, K = h->n_keep;
   std::vector<int> seen(NI, -1);                        // seen[j] == i: j is already in row i
@@ -908,7 +924,7 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
     static const Fn fns[3][2] = {{k_bl_rank<BL_POP, false>, k_bl_rank<BL_POP, true>},
                                  {k_bl_rank<BL_SESSIONPOP, false>, k_bl_rank<BL_SESSIONPOP, true>},
                                  {k_bl_rank<BL_ITEMKNN, false>, k_bl_rank<BL_ITEMKNN, true>}};
-    fns[h->kind][k > 0]<<<grid, 256, 0, st>>>(d, n_sessions);
+    fns[bl_has_rows(h->kind) ? BL_ITEMKNN : h->kind][k > 0]<<<grid, 256, 0, st>>>(d, n_sessions);   // SR and AR rank as ItemKNN
     CK(cudaGetLastError());
   }
   k_bl_sums<<<1, 1024, 0, st>>>(d.counts, n_ev, dCut, n_cut, mode, dSums);

@@ -1750,5 +1750,6 @@ extern "C" int g4r_copy_item_tables(g4r_handle* h, g4r_handle* src, const float*
 #include "g4r_eval.cuh"
 #include "g4r_full.cuh"
 #include "g4r_baselines.cuh"
+#include "g4r_rules.cuh"
 #include "g4r_bpr.cuh"
 #include "g4r_sknn.cuh"

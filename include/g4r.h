@@ -448,6 +448,23 @@ int g4r_bl_stan_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_
  * correctly rounded in float64.  Lists hold the positive scores first, then every zero-score item by index. */
 int g4r_bl_stan_set_w1(g4r_baselines* b, const double* w1, int64_t n_w1);
 
+/* ---- rule-based baselines: sequential rules (SR) and association rules (AR) (DESIGN §3q) --------------------------------------
+ * g4r_bl_create(G4R_BL_SR or G4R_BL_AR, n_items, pruning (1 .. 1024), ...).  Kind 7 is not used.  The model is ItemKNN's rows:
+ * g4r_bl_rows_export / g4r_bl_rows_import take SR and AR handles, and g4r_bl_evaluate ranks them as an ItemKNN (after input x,
+ * item j scores its kept weight w(x, j), every other item 0). */
+#define G4R_BL_SR 8
+#define G4R_BL_AR 9
+/* The fit, from the training events as session CSR in time order (items[session_offsets[s] .. session_offsets[s+1]) = x_1 .. x_n).
+ * SR (steps 1 .. 20, weighting 0 'div' or 1 'same'): W(i, j) = sum over sessions and position pairs p < q <= p + steps with
+ * x_p = i != j = x_q of L / (q - p) ('div', L = lcm(1 .. steps)) or 1 ('same', L = 1).  AR (steps = weighting = 0): W(i, j) =
+ * sum over sessions of occ_s(i) * occ_s(j), i != j, L = 1.  W is counted in uint64; w = double(W) / L, each conversion and the
+ * division correctly rounded.  Each row keeps its n_keep largest positive w by (w desc, index asc).  Every argument is checked
+ * before any device write, and G4R_ERR_INVALID refuses a fit whose per-row bound (SR: occurrences * min(steps, longest session -
+ * 1) * L; AR: the sum of n_s over the row item's occurrences) reaches 2^63.  Out (may be NULL): the pair work (the pairs the fit
+ * visits), the scratch bytes of the accumulators, the device time (CUDA events) from the first kernel to the last. */
+int g4r_bl_rules_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_events,
+                     int32_t steps, int32_t weighting, int64_t* pair_work, size_t* scratch_bytes, float* device_ms);
+
 #ifdef __cplusplus
 }
 #endif
