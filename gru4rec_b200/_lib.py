@@ -52,7 +52,7 @@ EXPORTS = [
     'g4r_train_state_bytes', 'g4r_train_state_export', 'g4r_train_state_import', 'g4r_copy_item_tables',
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
-    'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit',
+    'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit', 'g4r_bl_vstan_set',
 ]
 
 _lib = None
@@ -157,6 +157,7 @@ def load():
     lib.g4r_bl_sknn_fit.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32]
     lib.g4r_bl_stan_fit.argtypes = [vp, vp, i64, vp, i64, vp, vp, vp, vp, i64, i32]
     lib.g4r_bl_stan_set_w1.argtypes = [vp, vp, i64]
+    lib.g4r_bl_vstan_set.argtypes = [vp, i32, vp, i64, vp, i64]
     lib.g4r_bl_rules_fit.argtypes = [vp, vp, i64, vp, i64, i32, i32, C.POINTER(i64), C.POINTER(C.c_size_t), C.POINTER(C.c_float)]
     _lib = lib
     return lib
@@ -782,7 +783,7 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -816,9 +817,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
-    a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN and STAN indexes (DESIGN §3o, §3p), and the SR / AR fit
-    into ItemKNN's rows (DESIGN §3q).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr' or 'ar'; n_keep: top_n,
-    n_sims, n_factors, k or pruning."""
+    a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
+    SR / AR fit into ItemKNN's rows (DESIGN §3q).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar' or
+    'vstan'; n_keep: top_n, n_sims, n_factors, k or pruning."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -952,7 +953,7 @@ class Baselines(object):
                                              SKNN_SIMILARITY[similarity]))
 
     def stan_fit(self, session_offsets, items, positions, recency, w2, w3, sample_size):
-        """the STAN index: sknn_fit's CSR and ranks, each entry's last position in its session, W2 per session (in the order of
+        """the STAN (or VSTAN) index: sknn_fit's CSR and ranks, each entry's last position in its session, W2 per session (in the order of
         session_offsets) and the W3 table"""
         off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
         pos = np.ascontiguousarray(positions, dtype=np.int32); rc = np.ascontiguousarray(recency, dtype=np.int32)
@@ -997,9 +998,22 @@ class Baselines(object):
         return pw.value, sb.value, ms.value
 
     def stan_set_w1(self, w1):
-        """the STAN prefix-distance table W1[0 .. n): it must cover every counted event's prefix length"""
+        """the STAN (or VSTAN) prefix-distance table W1[0 .. n): it must cover every counted event's prefix length"""
         w1 = np.ascontiguousarray(w1, dtype=np.float64)
         if w1.ndim != 1 or w1.size < 1:
             raise ValueError('stan_set_w1: w1 must be a non-empty 1-D table')
         self._check(self.lib.g4r_bl_stan_set_w1(self.h, _ptr(w1), w1.size))
         self.n_w1 = w1.size
+
+    def vstan_set(self, similarity, f, w4):
+        """the VSTAN settings after a stan_fit: the similarity ('cosine' or 'vector'), F per item (finite, >= 0) and the
+        neighbour table W4[0 .. n) by prefix distance, entries in [0, 1]; W4 must cover every counted event's prefix length"""
+        f = np.ascontiguousarray(f, dtype=np.float64); w4 = np.ascontiguousarray(w4, dtype=np.float64)
+        if similarity not in SKNN_SIMILARITY:
+            raise ValueError('vstan_set: similarity must be one of %s' % sorted(SKNN_SIMILARITY))
+        if f.shape != (self.n_items,) or not (np.isfinite(f) & (f >= 0.0)).all():
+            raise ValueError('vstan_set: f must hold one finite factor >= 0 per item')
+        if w4.ndim != 1 or not 1 <= w4.size <= 1 << 30 or not ((w4 >= 0.0) & (w4 <= 1.0)).all():
+            raise ValueError('vstan_set: w4 must be a non-empty 1-D table with entries in [0, 1]')
+        self._check(self.lib.g4r_bl_vstan_set(self.h, SKNN_SIMILARITY[similarity], _ptr(f), f.size, _ptr(w4), w4.size))
+        self.n_w4 = w4.size

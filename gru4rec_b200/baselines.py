@@ -1,6 +1,6 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
-§3o; STAN, §3p) and the rule-based baselines (SR and AR, §3q, fitted on the device) with the same surface.  ItemKNN's fit runs on the device (the
+§3o; STAN, §3p; VSTAN, §3r) and the rule-based baselines (SR and AR, §3q, fitted on the device) with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -408,6 +408,11 @@ class STAN(SessionKNN):
         self.current_session = None
 
     def fit(self, data):
+        self._fit_index(data)
+        self._device()
+
+    def _fit_index(self, data):
+        """the parameter checks, the index, positions, W2 and W3 on the host (no device work)"""
         if not 1 <= self.sample_size <= 8192:
             raise ValueError('sample_size must be in 1 .. 8192, not %r' % (self.sample_size,))
         if not 1 <= self.k <= min(self.sample_size, 1024):
@@ -417,7 +422,7 @@ class STAN(SessionKNN):
                 raise ValueError('%s must be in (0, inf], not %r' % (name, getattr(self, name)))
         col = data[self.time_key]
         if not pd.api.types.is_numeric_dtype(col) or pd.api.types.is_bool_dtype(col):
-            raise ValueError('STAN needs a numeric time column %r, not %s' % (self.time_key, col.dtype))
+            raise ValueError('%s needs a numeric time column %r, not %s' % (type(self).__name__, self.time_key, col.dtype))
         times = col.values
         idx = self._index(data).astype(np.int64)
         sess = data[self.session_key].values
@@ -443,7 +448,6 @@ class STAN(SessionKNN):
         self.current_session = None
         self.__dict__.pop('_dev', None)
         self.__dict__.pop('_post', None)
-        self._device()
 
     def _w1(self, n):
         return np.exp(-(np.arange(n) / float(self.lambda_spw)))
@@ -487,6 +491,93 @@ class STAN(SessionKNN):
             sel = owner == q
             score[flat[sel]] = score[flat[sel]] + sims[q] * self.w3[np.abs(fpos[sel] - qr[q])]
         return score
+
+
+class VSTAN(STAN):
+    '''
+    VSTAN(k=100, sample_size=500, similarity='cosine', lambda_spw=1.02, lambda_snh=432000.0, lambda_inh=2.05, lambda_ipw=1.02,
+          lambda_idf=1.0, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    STAN with the ideas of V-SKNN added back, in the style of VSTAN (Ludewig et al., RecSys 2019): an unnormalised ("vector")
+    similarity, a neighbour that counts less when its most recent item shared with the session lies further back in the session,
+    and IDF-weighted item scores.  This is this project's definition (DESIGN §3r); it is not claimed to match any other
+    implementation bit for bit.
+
+    Everything STAN defines stays: the index, T(s), the recency order, the candidates, p_i, q_n(j), W1, W2, W3 and r(n).  Two more
+    tables, computed by NumPy: W4[d] = exp(-(d / lambda_ipw)) for the prefix distance d, and F[j] = 1 + lambda_idf * log(n_sessions /
+    df_j), df_j the number of training sessions that contain j.  sim1 = v / sqrt(|I(c)| |I(n)|) ('cosine', STAN's) or v
+    ('vector'), v the W1 sum; sim2 = sim1 * W2[n]; the k largest sim2 (ties: the more recent) are the neighbours; g(n) = sim2 *
+    W4[t - p_r(n)]; score(j) = F[j] * (the float64 sum, in neighbour order, of g(n) * W3[|q_n(j) - q_n(r(n))|] over the neighbours
+    containing j).  lambda_ipw = inf switches W4 off and lambda_idf = 0 sets F to 1: with similarity='cosine' and both, the scores
+    are STAN's bit for bit.
+    '''
+    _kind = 'vstan'
+
+    def __init__(self, k=100, sample_size=500, similarity='cosine', lambda_spw=1.02, lambda_snh=432000.0, lambda_inh=2.05, lambda_ipw=1.02,
+                 lambda_idf=1.0, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        STAN.__init__(self, k, sample_size, lambda_spw, lambda_snh, lambda_inh, session_key, item_key, time_key)
+        self.similarity = similarity
+        self.lambda_ipw = lambda_ipw
+        self.lambda_idf = lambda_idf
+
+    def fit(self, data):
+        if self.similarity not in _lib.SKNN_SIMILARITY:
+            raise ValueError('similarity must be one of %s, not %r' % (sorted(_lib.SKNN_SIMILARITY), self.similarity))
+        if not float(self.lambda_ipw) > 0.0:
+            raise ValueError('lambda_ipw must be in (0, inf], not %r' % (self.lambda_ipw,))
+        if not 0.0 <= float(self.lambda_idf) < np.inf:
+            raise ValueError('lambda_idf must be finite and >= 0, not %r' % (self.lambda_idf,))
+        self._fit_index(data)
+        df = np.bincount(self.session_items, minlength=self.n_items)   # the sessions that contain each item
+        self.f = 1.0 + float(self.lambda_idf) * np.log(self.n_sessions / df)
+        self._device()
+
+    def _w4(self, n):
+        return np.exp(-(np.arange(n) / float(self.lambda_ipw)))
+
+    def _upload(self, dev):
+        STAN._upload(self, dev)
+        dev.vstan_set(self.similarity, self.f, self._w4(len(self.w3)))
+
+    def _cover(self, max_len):
+        STAN._cover(self, max_len)
+        dev = self._device()
+        if dev.n_w4 < max_len:
+            dev.vstan_set(self.similarity, self.f, self._w4(max_len))
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        prefix = np.asarray(prefix, dtype=np.int64)
+        t = len(prefix)
+        u, first_rev = np.unique(prefix[::-1], return_index=True)
+        last = t - first_rev                                      # 1-based position of the last occurrence
+        o = np.argsort(last)
+        ci, pos = u[o], last[o]
+        ioff, ranks, by_rank = self._postings()
+        S = self.sample_size
+        cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
+        sess = by_rank[cand]
+        starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
+        owner = np.repeat(np.arange(len(cand)), lens)
+        at = np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())
+        flat, fpos = self.session_items[at], self.positions[at]
+        w1 = self._w1(t)
+        v, qr, dr = np.zeros(len(cand)), np.zeros(len(cand), np.int64), np.zeros(len(cand), np.int64)
+        for m, i in enumerate(ci):                                # c's items in order of their last position
+            sel = flat == i
+            hit = np.zeros(len(cand), bool)
+            hit[owner[sel]] = True
+            v = v + np.where(hit, w1[t - pos[m]], 0.0)
+            qr[owner[sel]] = fpos[sel]                            # ends at the shared item with the largest p_i
+            dr[owner[sel]] = t - pos[m]
+        sim1 = v if self.similarity == 'vector' else v / np.sqrt((len(ci) * lens).astype(np.float64))
+        sims = sim1 * self.w2[sess]
+        g = sims * self._w4(t)[dr]
+        score = np.zeros(self.n_items)
+        for q in np.lexsort((cand, -sims))[:self.k]:
+            sel = owner == q
+            score[flat[sel]] = score[flat[sel]] + g[q] * self.w3[np.abs(fpos[sel] - qr[q])]
+        return score * self.f
 
 
 class _Rules(Baseline):

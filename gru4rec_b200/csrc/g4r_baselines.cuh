@@ -4,7 +4,8 @@
 // nothing here touches a g4r_handle.
 #pragma once
 
-constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6, BL_SR = 8, BL_AR = 9;   // 4 and 7 stay unused
+constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6, BL_SR = 8, BL_AR = 9,
+              BL_VSTAN = 11;                            // 4, 7 and 10 stay unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
@@ -48,6 +49,11 @@ struct g4r_baselines {
   int* dStPos = nullptr;
   double *dStW2 = nullptr, *dStW3 = nullptr, *dStW1 = nullptr;
   int64_t st_n_w1 = 0;
+  // VSTAN (the STAN index and W1 above plus): F per item and W4 by prefix distance, with the similarity (sk_sim) set by
+  // g4r_bl_vstan_set; a fit clears them, and evaluation needs them set (vs_set)
+  double *dVsF = nullptr, *dVsW4 = nullptr;
+  int64_t vs_n_w4 = 0;
+  bool vs_set = false;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -599,7 +605,7 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   for (void* p : {(void*)h->dIdx, (void*)h->dIdxI, (void*)h->dLen, (void*)h->dSim, (void*)h->dSimI, (void*)h->dPop, (void*)h->dTopS, (void*)h->dTop,
-                  (void*)h->dI, (void*)h->dBI, (void*)h->dStW1})
+                  (void*)h->dI, (void*)h->dBI, (void*)h->dStW1, (void*)h->dVsF, (void*)h->dVsW4})
     if (p) cudaFree(p);
   for (void* p : h->bpr_mem) cudaFree(p);
   for (void* p : h->sknn_mem) cudaFree(p);
@@ -612,13 +618,13 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR) {
-    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR) or 9 (AR)";
+  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR && kind != BL_VSTAN) {
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR) or 11 (VSTAN)";
     return G4R_ERR_INVALID;
   }
-  if (n_items < 1 || n_keep < 1 || ((bl_has_rows(kind) || kind == BL_SKNN || kind == BL_STAN) && n_keep > KF_KEEP_MAX) ||
+  if (n_items < 1 || n_keep < 1 || ((bl_has_rows(kind) || kind == BL_SKNN || kind == BL_STAN || kind == BL_VSTAN) && n_keep > KF_KEEP_MAX) ||
       (kind == BL_BPR && n_keep > BPR_F_MAX)) {
-    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR and AR, <= " +
+    g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR, AR and VSTAN, <= " +
                         std::to_string(BPR_F_MAX) + " n_factors for BPR)";
     return G4R_ERR_INVALID;
   }
@@ -641,7 +647,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   } else if (bl_has_rows(kind)) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
-  } else if (kind != BL_SKNN && kind != BL_STAN) {     // SessionKNN and STAN allocate at their fit
+  } else if (kind != BL_SKNN && kind != BL_STAN && kind != BL_VSTAN) {   // SessionKNN, STAN and VSTAN allocate at their fit
     ok &= bl_alloc(&h->dPop, n_items) == cudaSuccess && bl_alloc(&h->dTopS, h->n_keep) == cudaSuccess && bl_alloc(&h->dTop, h->n_keep) == cudaSuccess;
   }
   if (!ok) return bail("device allocation failed");
@@ -851,6 +857,7 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
                                int32_t* out_counts, int32_t* out_items, double* out_scores) {
   if (!h) return G4R_ERR_INVALID;
   if (!h->ready) FAIL(G4R_ERR_STATE, "g4r_bl_evaluate: the baseline is not fitted");
+  if (h->kind == BL_VSTAN && !h->vs_set) FAIL(G4R_ERR_STATE, "g4r_bl_evaluate: the VSTAN settings are not set since the last fit (g4r_bl_vstan_set)");
   if (!session_offsets || n_sessions < 0 || n_events < 0 || (n_events > 0 && !items) || !cut_off || n_cut < 1 || n_cut > 64 ||
       !recall_sum || !mrr_sum || n_cand < 0 || n_cand > INT32_MAX || (n_cand > 0 && !cand))
     FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: null or out-of-range argument");
@@ -881,7 +888,7 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   }
   const int64_t n_ev = ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
-  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN) {
+  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN || h->kind == BL_VSTAN) {
     cudaSetDevice(h->device);
     const int rc = h->kind == BL_BPR ? bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
                                                     cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)

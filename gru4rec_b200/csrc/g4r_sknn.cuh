@@ -1,6 +1,6 @@
 // g4r_sknn.cuh -- session-based kNN (S-KNN with cosine similarity, V-SKNN-style position weights, DESIGN §3o; STAN-style time
-// and position decays, §3p) on the device: the index of the training sessions and the event-parallel ranking of evaluate_gpu /
-// evaluate_events, one CTA per counted event.
+// and position decays, §3p; VSTAN-style vector similarity, match-position neighbour weights and IDF, §3r) on the device: the
+// index of the training sessions and the event-parallel ranking of evaluate_gpu / evaluate_events, one CTA per counted event.
 // Included at the end of g4r_lib.cu after g4r_baselines.cuh (the handle, BlEvalDev, bl_w, bl_noise, bl_zero_eq, bl_emit,
 // cta_bitonic, k_bl_sums, BlBufs).
 #pragma once
@@ -22,7 +22,12 @@ struct SknnEvalDev {
   // per-CTA slices of global scratch: the prefix (c_cap entries) and the neighbours' (item, neighbour) pairs (z_cap entries)
   unsigned long long* c_key; int* c_flag; int* c_item; double* c_w; int c_cap;
   unsigned long long* z_key; int* u_item; double* u_sc; double* l_sc; int* l_item; int z_cap;
+  // VSTAN (§3r): F per item (IDF) and W4 (prefix distance of the neighbour's most recent shared item)
+  const double* f; const double* w4;
 };
+
+// the instances of k_sknn_rank
+constexpr int SK_SKNN = 0, SK_STAN = 1, SK_VSTAN = 2;
 
 // in-place bitonic sort of P (a power of two) 64-bit keys, ascending, in memory the whole CTA reads
 __device__ void sk_bitonic_u64(unsigned long long* a, int P) {
@@ -95,8 +100,12 @@ __device__ __forceinline__ bool sk_scored(const int* ui, int U, int j) {
 // STAN (§3p) changes three steps: the weights of step 1 are W1[t - p], step 3 is the W1 sum over sqrt(|I(c)| |I(n)|) times W2[n],
 // and step 5 first finds each neighbour's most recent shared item r(n) and multiplies each summand by W3[|q_n(j) - q_n(r(n))|].
 // Its scored items may score exactly 0 (underflow): they are counted as scored items and listed with the zero-score items.
-template <bool STAN>
+// VSTAN (§3r) is STAN plus: step 1 keeps each compacted item's prefix distance t - p in c_flag (free once read), step 3 leaves the
+// norm out for 'vector' (d.sim), the r(n) pre-pass turns sim2(n) into g(n) = sim2(n) W4[t - p_r(n)] in place in sS after the sort,
+// and step 5 multiplies each item's neighbour-order sum once by F[j].
+template <int V>
 __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
+  constexpr bool STAN = V != SK_SKNN, VSTAN = V == SK_VSTAN;
   extern __shared__ __align__(16) unsigned char sk_smem[];
   __shared__ int sW[SK_THREADS / 32];
   __shared__ long long sRed[SK_THREADS / 32];
@@ -132,7 +141,10 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
       const bool f = q < t && cf[q];
       int tot;
       const int r = sk_rank_flag(f, sW, tot);
-      if (f) { ci[D + r] = b.items[st + q]; cw[D + r] = STAN ? d.w1[t - 1 - q] : __ddiv_rn((double)(q + 1), (double)t); }
+      if (f) {
+        ci[D + r] = b.items[st + q]; cw[D + r] = STAN ? d.w1[t - 1 - q] : __ddiv_rn((double)(q + 1), (double)t);
+        if (VSTAN) cf[D + r] = t - 1 - q;                // D + r <= q: this round's flags are read before sk_rank_flag's barrier
+      }
       D += tot;
     }
     __syncthreads();
@@ -182,25 +194,27 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
         const int x = sorted_lb(it, ns, j);
         if (x < ns && it[x] == j) { cnt++; if (STAN || d.sim) v = __dadd_rn(v, cw[m]); }
       }
-      if (STAN) v = __dmul_rn(__ddiv_rn(v, __dsqrt_rn((double)((long long)D * ns))), d.w2[r]);
+      if (STAN) v = __dmul_rn((VSTAN && d.sim) ? v : __ddiv_rn(v, __dsqrt_rn((double)((long long)D * ns))), d.w2[r]);
       else if (!d.sim) v = __ddiv_rn((double)cnt, __dsqrt_rn((double)((long long)D * ns)));
       sS[q] = v;
     }
     // 4. neighbours
     cta_bitonic<false>(sS, cand, Pn);
     const int nK = min(d.nbr, nB);
-    // 5. scores (STAN: nxt, free since the merge, holds q_n(r(n)) of neighbour n; c's items are searched from the last position)
+    // 5. scores (STAN: nxt, free since the merge, holds q_n(r(n)) of neighbour n; c's items are searched from the last position;
+    //    VSTAN: sS[n] becomes g(n))
     if (STAN) {
       for (int r = tid; r < nK; r += SK_THREADS) {
         const int64_t a0 = d.s_off[cand[r]];
         const int ns = (int)(d.s_off[cand[r] + 1] - a0);
         const int* it = d.s_item + a0;
-        int qr = 0;
+        int qr = 0, dr = 0;
         for (int m = D - 1; m >= 0; m--) {
           const int x = sorted_lb(it, ns, ci[m]);
-          if (x < ns && it[x] == ci[m]) { qr = d.s_pos[a0 + x]; break; }
+          if (x < ns && it[x] == ci[m]) { qr = d.s_pos[a0 + x]; if (VSTAN) dr = cf[m]; break; }
         }
         nxt[r] = qr;
+        if (VSTAN) sS[r] = __dmul_rn(sS[r], d.w4[dr]);
       }
     }
     if (tid == 0) sZ = 0;
@@ -234,7 +248,7 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
             acc = __dadd_rn(acc, __dmul_rn(sS[n], d.w3[abs(d.s_pos[a0 + x] - nxt[n])]));
           } else acc = __dadd_rn(acc, sS[n]);
         }
-        ui[U + r] = (int)j; us[U + r] = acc;
+        ui[U + r] = (int)j; us[U + r] = VSTAN ? __dmul_rn(acc, d.f[j]) : acc;
       }
       U += tot;
     }
@@ -305,12 +319,12 @@ __global__ void __launch_bounds__(SK_THREADS) k_sknn_rank(SknnEvalDev d) {
 // ---------------------------------------------------------------------------------------------------------------------------
 // C ABI (include/g4r.h)
 // ---------------------------------------------------------------------------------------------------------------------------
-// the index of a SessionKNN (similarity; positions, w2 and w3 null) or a STAN handle: every argument checked on the host before any device
-// write, the sessions renumbered by rank and every item's sessions built by a counting sort that visits the ranks in order
+// the index of a SessionKNN (similarity; positions, w2 and w3 null) or a STAN / VSTAN handle: every argument checked on the host before
+// any device write, the sessions renumbered by rank and every item's sessions built by a counting sort that visits the ranks in order
 static int sk_index(g4r_baselines* h, const std::string& fn, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items,
                     int64_t n_entries, const int32_t* recency, int32_t sample_size, int32_t similarity, const int32_t* positions,
                     const double* w2, const double* w3, int64_t n_w3) {
-  const bool stan = h->kind == BL_STAN;
+  const bool stan = h->kind == BL_STAN || h->kind == BL_VSTAN;
   if (!session_offsets || !recency || n_sessions < 1 || n_sessions >= INT32_MAX || n_entries < 0 || (n_entries > 0 && !items))
     FAIL(G4R_ERR_INVALID, fn + ": null argument, or n_sessions outside 1 .. 2^31 - 2");
   if (stan && (!w2 || !w3 || n_w3 < 1 || n_w3 > (1 << 30) || (n_entries > 0 && !positions)))
@@ -374,6 +388,10 @@ static int sk_index(g4r_baselines* h, const std::string& fn, const int64_t* sess
   for (void* p : h->sknn_mem) cudaFree(p);
   h->sknn_mem.clear();
   h->dSkOff = h->dSkIoff = nullptr; h->dSkItem = h->dSkIsess = h->dStPos = nullptr; h->dStW2 = h->dStW3 = nullptr;
+  if (h->kind == BL_VSTAN) {                            // a fit clears g4r_bl_vstan_set's settings
+    for (void* p : {(void*)h->dVsF, (void*)h->dVsW4}) if (p) cudaFree(p);
+    h->dVsF = h->dVsW4 = nullptr; h->vs_n_w4 = 0; h->vs_set = false;
+  }
   auto take = [&](auto** p, size_t n) { cudaError_t e = bl_alloc(p, n); if (e == cudaSuccess) h->sknn_mem.push_back(*p); else *p = nullptr; return e; };
   CK(take(&h->dSkOff, S + 1)); CK(take(&h->dSkIoff, NI + 1));
   CK(take(&h->dSkItem, n_entries)); CK(take(&h->dSkIsess, n_entries));
@@ -408,13 +426,13 @@ extern "C" int g4r_bl_stan_fit(g4r_baselines* h, const int64_t* session_offsets,
                                const int32_t* positions, const int32_t* recency, const double* w2, const double* w3, int64_t n_w3,
                                int32_t sample_size) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind != BL_STAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_fit: the handle is not a STAN");
+  if (h->kind != BL_STAN && h->kind != BL_VSTAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_fit: the handle is not a STAN or VSTAN");
   return sk_index(h, "g4r_bl_stan_fit", session_offsets, n_sessions, items, n_entries, recency, sample_size, 0, positions, w2, w3, n_w3);
 }
 
 extern "C" int g4r_bl_stan_set_w1(g4r_baselines* h, const double* w1, int64_t n_w1) {
   if (!h) return G4R_ERR_INVALID;
-  if (h->kind != BL_STAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_set_w1: the handle is not a STAN");
+  if (h->kind != BL_STAN && h->kind != BL_VSTAN) FAIL(G4R_ERR_STATE, "g4r_bl_stan_set_w1: the handle is not a STAN or VSTAN");
   if (!w1 || n_w1 < 1 || n_w1 > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_stan_set_w1: null w1, or n_w1 outside 1 .. 2^30");
   for (int64_t q = 0; q < n_w1; q++)
     if (!(w1[q] >= 0.0 && w1[q] <= 1.0)) FAIL(G4R_ERR_INVALID, "g4r_bl_stan_set_w1: w1 entries must be in [0, 1]");
@@ -428,7 +446,29 @@ extern "C" int g4r_bl_stan_set_w1(g4r_baselines* h, const double* w1, int64_t n_
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a SessionKNN or a STAN, after its argument checks: resident CTAs over the counted events, each with its own slices of
+extern "C" int g4r_bl_vstan_set(g4r_baselines* h, int32_t similarity, const double* f, int64_t n_f, const double* w4, int64_t n_w4) {
+  if (!h) return G4R_ERR_INVALID;
+  if (h->kind != BL_VSTAN) FAIL(G4R_ERR_STATE, "g4r_bl_vstan_set: the handle is not a VSTAN");
+  if (similarity != 0 && similarity != 1) FAIL(G4R_ERR_INVALID, "g4r_bl_vstan_set: similarity must be 0 (cosine) or 1 (vector)");
+  if (!f || n_f != h->n_items) FAIL(G4R_ERR_INVALID, "g4r_bl_vstan_set: null f, or n_f is not n_items");
+  for (int64_t q = 0; q < n_f; q++)
+    if (!(std::isfinite(f[q]) && f[q] >= 0.0)) FAIL(G4R_ERR_INVALID, "g4r_bl_vstan_set: f entries must be finite and >= 0");
+  if (!w4 || n_w4 < 1 || n_w4 > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_vstan_set: null w4, or n_w4 outside 1 .. 2^30");
+  for (int64_t q = 0; q < n_w4; q++)
+    if (!(w4[q] >= 0.0 && w4[q] <= 1.0)) FAIL(G4R_ERR_INVALID, "g4r_bl_vstan_set: w4 entries must be in [0, 1]");
+  cudaSetDevice(h->device);
+  for (void* p : {(void*)h->dVsF, (void*)h->dVsW4}) if (p) cudaFree(p);
+  h->dVsF = h->dVsW4 = nullptr; h->vs_n_w4 = 0; h->vs_set = false;
+  CK(bl_alloc(&h->dVsF, n_f));
+  CK(bl_alloc(&h->dVsW4, n_w4));
+  CK(cudaMemcpyAsync(h->dVsF, f, n_f * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->dVsW4, w4, n_w4 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->sk_sim = similarity; h->vs_n_w4 = n_w4; h->vs_set = true;
+  return G4R_OK;
+}
+
+// g4r_bl_evaluate of a SessionKNN, a STAN or a VSTAN, after its argument checks: resident CTAs over the counted events, each with its own slices of
 // a global scratch of at most SK_SCRATCH bytes (fewer CTAs when the slices are large; one at least)
 static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                          const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
@@ -438,11 +478,15 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
   int64_t max_len = 1;
   for (int64_t s = 0; s < n_sessions; s++) max_len = std::max(max_len, session_offsets[s + 1] - session_offsets[s]);
   if (max_len > (1 << 30) || h->sk_zmax > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a session or the neighbours' items exceed 2^30 entries");
-  const bool stan = h->kind == BL_STAN;
-  if (stan)                                             // W1 must cover the prefix distances 0 .. t - 1 of every counted event
-    for (int64_t s = 0; s < n_sessions; s++)
-      if (ev0[s + 1] > ev0[s] && session_offsets[s + 1] - session_offsets[s] - 1 > h->st_n_w1)
+  const bool stan = h->kind == BL_STAN || h->kind == BL_VSTAN, vstan = h->kind == BL_VSTAN;
+  if (stan)                                             // W1 (and W4) must cover the prefix distances 0 .. t - 1 of every counted event
+    for (int64_t s = 0; s < n_sessions; s++) {
+      const int64_t t_max = session_offsets[s + 1] - session_offsets[s] - 1;
+      if (ev0[s + 1] > ev0[s] && t_max > h->st_n_w1)
         FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a counted event's prefix is longer than the STAN W1 table (g4r_bl_stan_set_w1)");
+      if (vstan && ev0[s + 1] > ev0[s] && t_max > h->vs_n_w4)
+        FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a counted event's prefix is longer than the VSTAN W4 table (g4r_bl_vstan_set)");
+    }
   cudaStream_t st = h->stream;
   BlBufs bb;
   SknnEvalDev d{};
@@ -463,7 +507,8 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
   d.s_off = h->dSkOff; d.s_item = h->dSkItem; d.i_off = h->dSkIoff; d.i_sess = h->dSkIsess;
   d.sample = h->sk_sample; d.sim = h->sk_sim; d.nbr = h->n_keep;
   d.s_pos = h->dStPos; d.w1 = h->dStW1; d.w2 = h->dStW2; d.w3 = h->dStW3;
-  const auto kern = stan ? k_sknn_rank<true> : k_sknn_rank<false>;
+  d.f = h->dVsF; d.w4 = h->dVsW4;
+  const auto kern = vstan ? k_sknn_rank<SK_VSTAN> : stan ? k_sknn_rank<SK_STAN> : k_sknn_rank<SK_SKNN>;
   int PS = 1;
   while (PS < d.sample) PS <<= 1;
   const size_t smem = (size_t)PS * (sizeof(double) + 2 * sizeof(int)) + SK_CHUNK * sizeof(int);

@@ -465,6 +465,20 @@ int g4r_bl_stan_set_w1(g4r_baselines* b, const double* w1, int64_t n_w1);
 int g4r_bl_rules_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n_sessions, const int32_t* items, int64_t n_events,
                      int32_t steps, int32_t weighting, int64_t* pair_work, size_t* scratch_bytes, float* device_ms);
 
+/* ---- VSTAN-style session kNN (DESIGN §3r) -----------------------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_VSTAN, n_items, k (1 .. 1024), ...); kind 10 is not used.  STAN plus a vector similarity, a neighbour weight by the prefix
+ * distance of its most recent shared item and a per-item factor (IDF), all from tables the caller computes.  The index and W1 are
+ * STAN's: g4r_bl_stan_fit and g4r_bl_stan_set_w1 take a VSTAN handle. */
+#define G4R_BL_VSTAN 11
+/* similarity 0 (cosine, STAN's sim) or 1 (vector: no norm), f[0 .. n_items) the item factors (finite, >= 0), w4[0 .. n_w4) the
+ * neighbour weights by prefix distance, entries in [0, 1], n_w4 in 1 .. 2^30.  Every argument is checked before any device write;
+ * a call replaces the earlier settings, and a fit clears them: g4r_bl_evaluate of a VSTAN handle returns G4R_ERR_STATE until this
+ * has been called after the last fit, and refuses (G4R_ERR_INVALID, before any device work) a frame with a counted event whose
+ * prefix is longer than n_w4 or n_w1.  It ranks by DESIGN §3r: sim1 = v (vector) or v / sqrt(|I(c)| |I(n)|) (cosine), sim2 =
+ * sim1 * w2[n]; the neighbours are STAN's by sim2; g(n) = sim2 * w4[t - p_r(n)]; item j scores f[j] times the sum, in neighbour
+ * order, of g(n) * w3[|q_n(j) - q_n(r(n))|]; each product and sum correctly rounded in float64. */
+int g4r_bl_vstan_set(g4r_baselines* b, int32_t similarity, const double* f, int64_t n_f, const double* w4, int64_t n_w4);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,8 +1,8 @@
-"""Times STAN-style session kNN (DESIGN §3p, §5) on synthetic RSC15-shaped data (37,483 items, about 31M training events) with
+"""Times STAN- and VSTAN-style session kNN (DESIGN §3p, §3r, §5) on synthetic RSC15-shaped data (37,483 items, about 31M training events) with
 per-event times in seconds: the fit (baselines.STAN.fit on the frame: the host index, positions and decay tables, the library's
-checks and the upload), then the device call behind evaluate_gpu / evaluate_events (g4r_bl_evaluate, sums only; the host
-preparation of the frame is not timed) on about 100,000 test events at sample_size 500 and 5000 (k = 100), the same for
-SessionKNN cosine on the same data for scale, then the float64 NumPy oracle on a sample of events.  Prints one JSON line per
+checks and the upload; VSTAN's adds F and W4), then the device call behind evaluate_gpu / evaluate_events (g4r_bl_evaluate, sums only; the host
+preparation of the frame is not timed) on about 100,000 test events at sample_size 500 and 5000 (k = 100; VSTAN with the
+default lambdas for both similarities), the same for SessionKNN cosine on the same data for scale, then the float64 NumPy oracle on a sample of events.  Prints one JSON line per
 measurement, then the card's name and power limit.
 
     python scripts/stan_bench.py [--events 31000000] [--test_events 130000] [--oracle_sample 40]"""
@@ -47,6 +47,8 @@ def main():
     te_off = te_off.astype(np.int64)
     head = int(te_off[min(200, len(te_off) - 1)])
     for name, model in (('stan', baselines.STAN(k=args.k, sample_size=500)),
+                        ('vstan_cosine', baselines.VSTAN(k=args.k, sample_size=500, similarity='cosine')),
+                        ('vstan_vector', baselines.VSTAN(k=args.k, sample_size=500, similarity='vector')),
                         ('sknn_cosine', baselines.SessionKNN(k=args.k, sample_size=500, similarity='cosine'))):
         t0 = time.time()
         model.fit(frame)
@@ -54,12 +56,14 @@ def main():
              seconds=round(time.time() - t0, 3))
         dev = model._device()
         ti = model.itemidmap.reindex(te_items).values.astype(np.int32)              # ids to item indices (every id is in training)
-        if name == 'stan':
+        if name != 'sknn_cosine':
             model._cover(int(np.diff(te_off).max()))
         for sample in (500, 5000):
             t0 = time.time()
-            if name == 'stan':
+            if name != 'sknn_cosine':
                 dev.stan_fit(model.session_offsets, model.session_items, model.positions, model.recency, model.w2, model.w3, sample)
+                if name != 'stan':                                                   # the fit clears VSTAN's settings
+                    dev.vstan_set(model.similarity, model.f, model._w4(dev.n_w4))
             else:
                 dev.sknn_fit(model.session_offsets, model.session_items, model.recency, sample, 'cosine')
             up = time.time() - t0
