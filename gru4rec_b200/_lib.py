@@ -53,6 +53,7 @@ EXPORTS = [
     'g4r_bl_create', 'g4r_bl_destroy', 'g4r_bl_last_error', 'g4r_bl_knn_fit', 'g4r_bl_set_pop', 'g4r_bl_rows_export',
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
     'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit', 'g4r_bl_vstan_set',
+    'g4r_bl_narm_begin', 'g4r_bl_narm_epoch', 'g4r_bl_narm_grads', 'g4r_bl_narm_export', 'g4r_bl_narm_import', 'g4r_bl_narm_encode',
 ]
 
 _lib = None
@@ -159,6 +160,13 @@ def load():
     lib.g4r_bl_stan_set_w1.argtypes = [vp, vp, i64]
     lib.g4r_bl_vstan_set.argtypes = [vp, i32, vp, i64, vp, i64]
     lib.g4r_bl_rules_fit.argtypes = [vp, vp, i64, vp, i64, i32, i32, C.POINTER(i64), C.POINTER(C.c_size_t), C.POINTER(C.c_float)]
+    u32, f32 = C.c_uint32, C.c_float
+    lib.g4r_bl_narm_begin.argtypes = [vp, i32, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_narm_epoch.argtypes = [vp, vp, i64, u32, f32, f32, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_narm_grads.argtypes = [vp, vp, i32, u32, i64, f32, f32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_narm_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_narm_import.argtypes = [vp, i32, i32, vp, i64]
+    lib.g4r_bl_narm_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -783,7 +791,7 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -818,8 +826,8 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar' or
-    'vstan'; n_keep: top_n, n_sims, n_factors, k or pruning."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM fit and parameters (DESIGN §3s).  kind: 'pop', 'sessionpop',
+    'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan' or 'narm'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1017,3 +1025,58 @@ class Baselines(object):
             raise ValueError('vstan_set: w4 must be a non-empty 1-D table with entries in [0, 1]')
         self._check(self.lib.g4r_bl_vstan_set(self.h, SKNN_SIMILARITY[similarity], _ptr(f), f.size, _ptr(w4), w4.size))
         self.n_w4 = w4.size
+
+    # ---- NARM (DESIGN §3s) ----
+    def narm_n_params(self, hidden):
+        d, H = self.n_keep, int(hidden)
+        return self.n_items * d + 5 * d * H + 5 * H * H + 4 * H
+
+    def _narm_params(self, hidden, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        if th.size != self.narm_n_params(hidden):
+            raise ValueError('narm: need %d parameters (n_items d + 5 d H + 5 H^2 + 4 H), not %d' % (self.narm_n_params(hidden), th.size))
+        return th
+
+    def narm_begin(self, hidden, max_len, batch_size, piece_offsets, items, params):
+        """starts a NARM fit: the training pieces (CSR of item indices, 2 .. max_len events each) and the initial flat parameters"""
+        off = np.ascontiguousarray(piece_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._narm_params(hidden, params)
+        self._check(self.lib.g4r_bl_narm_begin(self.h, int(hidden), int(max_len), int(batch_size), _ptr(off), off.size - 1, _ptr(it), it.size,
+                                               _ptr(th), th.size))
+        self.narm_hidden, self.narm_batch = int(hidden), int(batch_size)
+
+    def narm_epoch(self, order, seed, learning_rate, dropout_emb, dropout_ct):
+        """one epoch over the pieces in `order`; returns (per-step losses float32, device ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32)
+        losses = np.zeros(-(-od.size // self.narm_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_narm_epoch(self.h, _ptr(od), od.size, int(seed) & 0xffffffff, float(learning_rate), float(dropout_emb),
+                                               float(dropout_ct), _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def narm_grads(self, pieces, seed, step, dropout_emb, dropout_ct):
+        """(loss, flat gradient float32) of one mini-batch of pieces at the current parameters, without an update"""
+        pc = np.ascontiguousarray(pieces, dtype=np.int32)
+        g = np.empty(self.narm_n_params(self.narm_hidden), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_narm_grads(self.h, _ptr(pc), pc.size, int(seed) & 0xffffffff, int(step), float(dropout_emb), float(dropout_ct),
+                                               C.byref(loss), _ptr(g)))
+        return loss.value, g
+
+    def narm_export(self):
+        th = np.empty(self.narm_n_params(self.narm_hidden), np.float32)
+        self._check(self.lib.g4r_bl_narm_export(self.h, _ptr(th), th.size))
+        return th
+
+    def narm_import(self, hidden, max_len, params):
+        th = self._narm_params(hidden, params)
+        self._check(self.lib.g4r_bl_narm_import(self.h, int(hidden), int(max_len), _ptr(th), th.size))
+        self.narm_hidden = int(hidden)
+
+    def narm_encode(self, items, session_offsets, n_history=None):
+        """every counted event's q [n, d_e] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_narm_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q

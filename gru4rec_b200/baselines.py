@@ -1,6 +1,7 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
-§3o; STAN, §3p; VSTAN, §3r) and the rule-based baselines (SR and AR, §3q, fitted on the device) with the same surface.  ItemKNN's fit runs on the device (the
+§3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s, trained
+on the device) with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -658,3 +659,193 @@ class AR(_Rules):
         self.session_key = session_key
         self.item_key = item_key
         self.time_key = time_key
+
+
+def narm_pieces(offsets, items, max_len):
+    """(piece offsets int64, piece items int32): every session of >= 2 events (items[offsets[s] .. offsets[s+1]) in time order)
+    cut into pieces of at most max_len events, consecutive pieces overlapping by one event, so that every (input, next item)
+    pair lies in exactly one piece; pieces in session order"""
+    off = np.asarray(offsets, dtype=np.int64)
+    items = np.asarray(items)
+    lens = np.diff(off)
+    m = int(max_len) - 1
+    npc = np.where(lens >= 2, (lens - 1 + m - 1) // m, 0)
+    sess = np.repeat(np.arange(len(lens)), npc)
+    k = np.arange(int(npc.sum())) - np.repeat(np.cumsum(npc) - npc, npc)
+    start = off[sess] + k * m
+    plen = np.minimum(start + int(max_len), off[sess + 1]) - start
+    poff = np.zeros(len(plen) + 1, np.int64)
+    poff[1:] = np.cumsum(plen)
+    at = np.repeat(start - poff[:-1], plen) + np.arange(int(poff[-1]))
+    return poff, items[at].astype(np.int32)
+
+
+NARM_PARAMS = ('E', 'Wx', 'Wrz', 'Wh', 'Bh', 'A1', 'A2', 'v', 'B')
+
+
+def narm_shapes(n_items, d, H):
+    """the parameters in the order of the flat vector (DESIGN §3s)"""
+    return dict(E=(n_items, d), Wx=(d, 3 * H), Wrz=(H, 2 * H), Wh=(H, H), Bh=(3 * H,), A1=(H, H), A2=(H, H), v=(H,), B=(d, 2 * H))
+
+
+def narm_unpack(flat, n_items, d, H):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in narm_shapes(n_items, d, H).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def narm_init(n_items, d, H, rs):
+    """the initial parameters, float32 flat: in the order of the vector each matrix [r x c] (v as [H x 1]) drawn from
+    rs.uniform(-s, s) with s = sqrt(6 / (r + c)); Bh is 0 and takes no draw"""
+    parts = []
+    for name, shp in narm_shapes(n_items, d, H).items():
+        if name == 'Bh':
+            parts.append(np.zeros(shp))
+            continue
+        r, c = (shp[0], 1) if len(shp) == 1 else shp
+        s = np.sqrt(6.0 / (r + c))
+        parts.append(rs.uniform(-s, s, size=shp))
+    return np.concatenate([p.ravel() for p in parts]).astype(np.float32)
+
+
+def _sig(x):
+    return 1.0 / (1.0 + np.exp(-x))
+
+
+def narm_encode(p, x):
+    """q (float64) of the inputs x (item indices, oldest first) in eval mode: p maps the parameter names to float64 arrays"""
+    H = p['Wh'].shape[0]
+    h = np.zeros(H)
+    hs = []
+    for it in x:
+        vec = p['E'][it] @ p['Wx'] + p['Bh']
+        rz = _sig(vec[H:] + h @ p['Wrz'])
+        r, z = rz[:H], rz[H:]
+        ht = np.tanh((h * r) @ p['Wh'] + vec[:H])
+        h = (1.0 - z) * h + z * ht
+        hs.append(h)
+    hs = np.array(hs)
+    alpha = _sig(p['A1'] @ h + hs @ p['A2'].T) @ p['v']
+    return p['B'] @ np.concatenate([h, alpha @ hs])
+
+
+class NARM(Baseline):
+    '''
+    NARM(embedding=50, hidden=100, n_epochs=10, batch_size=512, learning_rate=0.001, dropout_emb=0.25, dropout_ct=0.5, max_len=50,
+         seed=42, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Neural attentive session model in the style of NARM (Li et al., CIKM 2017), trained on the device with full-catalogue
+    cross-entropy and Adam.  This is this project's definition (DESIGN §3s); no parity with another framework is claimed.
+
+    One item table E [n_items x embedding] is the input embedding and the decoder's item side.  For the last max_len inputs x_1 ..
+    x_t of a session prefix: h_1 .. h_t is GRU4Rec's GRU cell over E[x] from a zero state, alpha_j = v . sig(A1 h_t + A2 h_j),
+    c = [h_t ; sum_j alpha_j h_j], q = B c and item i scores E[i] . q.  Training cuts each session (events by time_key, ties by
+    row order) into pieces of at most max_len events overlapping by one, encodes each piece causally, and per mini-batch of
+    batch_size pieces takes one Adam step on the mean cross-entropy, with dropout_emb on the embeddings and dropout_ct on c.
+    The parameters are float32 and drawn, like the epochs' piece orders, from np.random.RandomState(seed).  fit prints the
+    epoch's mean loss; `fit_stats` holds per epoch (mean loss, device ms, per-step losses).  predict_next computes the scores on
+    the host in float64 from the float32 parameters.
+    '''
+    _kind = 'narm'
+
+    def __init__(self, embedding=50, hidden=100, n_epochs=10, batch_size=512, learning_rate=0.001, dropout_emb=0.25, dropout_ct=0.5,
+                 max_len=50, seed=42, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.hidden = hidden
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.dropout_emb = dropout_emb
+        self.dropout_ct = dropout_ct
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        def integer(name, lo, hi):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+                raise ValueError('%s must be an integer in %d .. %d, not %r' % (name, lo, hi, v))
+        integer('embedding', 1, 1024)
+        integer('hidden', 1, 1024)
+        integer('n_epochs', 0, 1 << 30)
+        integer('batch_size', 1, 1 << 20)
+        integer('max_len', 2, 512)
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+        for name in ('dropout_emb', 'dropout_ct'):
+            if not 0.0 <= float(getattr(self, name)) < 1.0:
+                raise ValueError('%s must be in [0, 1), not %r' % (name, getattr(self, name)))
+
+    def pieces(self, data):
+        """(piece offsets, piece items) of the training data, after the item index (_index)"""
+        idx = self._index(data)
+        sess = data[self.session_key].values
+        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
+        o = np.lexsort((data[self.time_key].values, code))      # each session's events by time, ties by row order
+        S = int(code.max()) + 1 if len(code) else 0
+        offsets = np.zeros(S + 1, np.int64)
+        offsets[1:] = np.cumsum(np.bincount(code, minlength=S))
+        return narm_pieces(offsets, idx[o], self.max_len)
+
+    def fit(self, data):
+        self._check()
+        poff, pitems = self.pieces(data)
+        if len(poff) < 2:
+            raise ValueError('NARM needs a training session of at least 2 events')
+        rs = np.random.RandomState(self.seed)
+        params = narm_init(self.n_items, self.embedding, self.hidden, rs)
+        self.__dict__.pop('_dev', None)
+        self.__dict__.pop('_p64', None)
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.narm_begin(self.hidden, self.max_len, self.batch_size, poff, pitems, params)
+        self.fit_stats = []
+        for epoch in range(self.n_epochs):
+            losses, ms = dev.narm_epoch(rs.permutation(len(poff) - 1), self.seed, self.learning_rate, self.dropout_emb, self.dropout_ct)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.narm_export()
+        dev.narm_import(self.hidden, self.max_len, self.params)   # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.narm_import(self.hidden, self.max_len, self.params)
+
+    def __getstate__(self):
+        state = Baseline.__getstate__(self)
+        state.pop('_p64', None)
+        return state
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            p = self._p64 = {k: v.astype(np.float64) for k, v in narm_unpack(self.params, self.n_items, self.embedding, self.hidden).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['E'] @ narm_encode(p, list(prefix)[-self.max_len:])
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        x = self.itemidmap[input_item_id]
+        if self.current_session is None or self.current_session != session_id:
+            self.current_session = session_id
+            self.session = [x]
+        else:
+            self.session.append(x)
+        score = self.score_prefix(self.session)
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)

@@ -5,12 +5,21 @@
 #pragma once
 
 constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6, BL_SR = 8, BL_AR = 9,
-              BL_VSTAN = 11;                            // 4, 7 and 10 stay unused
+              BL_VSTAN = 11, BL_NARM = 12;              // 4, 7 and 10 stay unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
 constexpr size_t KF_SCRATCH = (size_t)512 << 20;        // dense accumulators of the fit's resident CTAs
 constexpr unsigned BL_TIE_SEED = 0x6A09E667U;           // key of the tiebreaking noise (fixed: evaluations are reproducible)
+
+// NARM's device scratch (g4r_narm.cuh): per position indices, the carved float arrays, the logits, split partials, the
+// sort of the input embeddings' rows, per slot the plan
+struct NmScratch {
+  int *PX = nullptr, *PY = nullptr, *PS = nullptr;
+  float* f = nullptr; float* S = nullptr; float* part = nullptr;
+  unsigned long long *keys = nullptr, *keys2 = nullptr; unsigned char* cub = nullptr; size_t cub_bytes = 0;
+  long long* pstart = nullptr; int *plen = nullptr, *poff = nullptr;
+};
 
 struct g4r_baselines {
   int kind = 0, n_items = 0, n_keep = 0, device = 0, n_sm = 132;
@@ -54,6 +63,18 @@ struct g4r_baselines {
   double *dVsF = nullptr, *dVsW4 = nullptr;
   int64_t vs_n_w4 = 0;
   bool vs_set = false;
+  // NARM (g4r_narm.cuh): the flat float32 parameters, a device 1.0f, and dI = double(E), dBI = 0 for bpr_evaluate; the fit's
+  // gradient, Adam moments, training pieces and scratch (nm_mem, from g4r_bl_narm_begin until an import or the destroy)
+  float *dNmTh = nullptr, *dNmOne = nullptr, *dNmG = nullptr, *dNmM = nullptr, *dNmV = nullptr, *dNmLoss = nullptr;
+  int* dNmItems = nullptr;
+  int nm_H = 0, nm_len = 0, nm_bs = 0;
+  size_t nm_n = 0;
+  long long nm_Pmax = 0;
+  int64_t nm_step = 0;                                  // Adam steps since the fit began
+  bool nm_fit = false;
+  std::vector<int64_t> nm_off;                          // the training pieces' offsets (host)
+  std::vector<void*> nm_mem;
+  NmScratch nm_s;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -605,9 +626,10 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   for (void* p : {(void*)h->dIdx, (void*)h->dIdxI, (void*)h->dLen, (void*)h->dSim, (void*)h->dSimI, (void*)h->dPop, (void*)h->dTopS, (void*)h->dTop,
-                  (void*)h->dI, (void*)h->dBI, (void*)h->dStW1, (void*)h->dVsF, (void*)h->dVsW4})
+                  (void*)h->dI, (void*)h->dBI, (void*)h->dStW1, (void*)h->dVsF, (void*)h->dVsW4, (void*)h->dNmTh, (void*)h->dNmOne})
     if (p) cudaFree(p);
   for (void* p : h->bpr_mem) cudaFree(p);
+  for (void* p : h->nm_mem) cudaFree(p);
   for (void* p : h->sknn_mem) cudaFree(p);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -618,14 +640,14 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR && kind != BL_VSTAN) {
-    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR) or 11 (VSTAN)";
+  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR && kind != BL_VSTAN && kind != BL_NARM) {
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR), 11 (VSTAN) or 12 (NARM)";
     return G4R_ERR_INVALID;
   }
   if (n_items < 1 || n_keep < 1 || ((bl_has_rows(kind) || kind == BL_SKNN || kind == BL_STAN || kind == BL_VSTAN) && n_keep > KF_KEEP_MAX) ||
-      (kind == BL_BPR && n_keep > BPR_F_MAX)) {
+      ((kind == BL_BPR || kind == BL_NARM) && n_keep > BPR_F_MAX)) {
     g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR, AR and VSTAN, <= " +
-                        std::to_string(BPR_F_MAX) + " n_factors for BPR)";
+                        std::to_string(BPR_F_MAX) + " n_factors for BPR and embedding for NARM)";
     return G4R_ERR_INVALID;
   }
   int dev_count = 0;
@@ -647,7 +669,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   } else if (bl_has_rows(kind)) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
-  } else if (kind != BL_SKNN && kind != BL_STAN && kind != BL_VSTAN) {   // SessionKNN, STAN and VSTAN allocate at their fit
+  } else if (kind != BL_SKNN && kind != BL_STAN && kind != BL_VSTAN && kind != BL_NARM) {   // SessionKNN, STAN, VSTAN and NARM allocate at their fit
     ok &= bl_alloc(&h->dPop, n_items) == cudaSuccess && bl_alloc(&h->dTopS, h->n_keep) == cudaSuccess && bl_alloc(&h->dTop, h->n_keep) == cudaSuccess;
   }
   if (!ok) return bail("device allocation failed");
@@ -845,7 +867,11 @@ extern "C" int g4r_bl_rows_import(g4r_baselines* h, const int32_t* idx, const do
 static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_bpr.cuh
+                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores, const float* qev);   // g4r_bpr.cuh
+static int narm_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
+                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
+                         double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_narm.cuh
 static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                          const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
                          const std::vector<int>& mult, const std::vector<int>& cdist, long long wtot, int32_t exclude_seen, int32_t k,
@@ -888,10 +914,12 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   }
   const int64_t n_ev = ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
-  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN || h->kind == BL_VSTAN) {
+  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN || h->kind == BL_VSTAN || h->kind == BL_NARM) {
     cudaSetDevice(h->device);
     const int rc = h->kind == BL_BPR ? bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
-                                                    cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)
+                                                    cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores, nullptr)
+                   : h->kind == BL_NARM ? narm_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
+                                                        cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)
                                      : sknn_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
                                                      cdist, wtot, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores);
     if (rc == G4R_OK && n_counted) *n_counted = n_ev;

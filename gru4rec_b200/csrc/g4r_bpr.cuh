@@ -227,6 +227,23 @@ __global__ void __launch_bounds__(256) k_bpr_uvec(BprEvalDev d, int64_t s0, int6
   }
 }
 
+// NARM (g4r_narm.cuh): as k_bpr_uvec, with each counted event's vector the encoder's q[e] (float32, converted exactly)
+__global__ void __launch_bounds__(256) k_narm_uvec(BprEvalDev d, const float* qev, int64_t s0, int64_t s1) {
+  const int lane = threadIdx.x & 31;
+  const int64_t s = s0 + (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (s >= s1) return;
+  const int64_t st = d.off[s], en = d.off[s + 1];
+  const int64_t p0 = st + max(d.nh ? d.nh[s] : 0, 1) - 1;
+  const long long e0 = d.ev0[s];
+  for (int64_t p = p0; p + 1 < en; p++) {
+    const long long e = e0 + (p - p0);
+    if (e >= d.E0 + d.nb) break;
+    if (e < d.E0) continue;
+    for (int f = lane; f < d.F; f += 32) d.uvec[(size_t)(e - d.E0) * d.F + f] = (double)qev[(size_t)e * d.F + f];
+    if (lane == 0) { d.pos[e - d.E0] = p; d.st[e - d.E0] = st; }
+  }
+}
+
 // thread per block event: the target's compared value, by the function the tile uses
 __global__ void k_bpr_target(BprEvalDev d) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -594,11 +611,12 @@ extern "C" int g4r_bl_bpr_import(g4r_baselines* h, const double* I, const double
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a BPR, after its argument checks: the counted events in blocks of bounded scratch
+// g4r_bl_evaluate of a BPR, after its argument checks: the counted events in blocks of bounded scratch.  qev (NARM): the
+// counted events' vectors [n_ev x F] on the device, which replace the session means
 static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores) {
+                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores, const float* qev) {
   const int NI = h->n_items, F = h->n_keep;
   const int64_t n_ev = ev0[n_sessions];
   cudaStream_t st = h->stream;
@@ -636,7 +654,8 @@ static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events
     // the sessions with counted events in [E0, E0 + nb)
     const int64_t s0 = std::upper_bound(ev0.begin(), ev0.begin() + n_sessions + 1, (int64_t)E0) - ev0.begin() - 1;
     const int64_t s1 = std::lower_bound(ev0.begin(), ev0.begin() + n_sessions + 1, (int64_t)(E0 + nb)) - ev0.begin();
-    k_bpr_uvec<<<(unsigned)((s1 - s0 + 7) / 8), 256, 0, st>>>(d, s0, s1);
+    if (qev) k_narm_uvec<<<(unsigned)((s1 - s0 + 7) / 8), 256, 0, st>>>(d, qev, s0, s1);
+    else k_bpr_uvec<<<(unsigned)((s1 - s0 + 7) / 8), 256, 0, st>>>(d, s0, s1);
     k_bpr_target<<<(nb + 255) / 256, 256, 0, st>>>(d);
     const unsigned gx = (unsigned)((nb + BT_E - 1) / BT_E);
     const int chunks = std::max(1, std::min(n_tiles, (int)((4 * h->n_sm + gx - 1) / gx)));

@@ -479,6 +479,41 @@ int g4r_bl_rules_fit(g4r_baselines* b, const int64_t* session_offsets, int64_t n
  * order, of g(n) * w3[|q_n(j) - q_n(r(n))|]; each product and sum correctly rounded in float64. */
 int g4r_bl_vstan_set(g4r_baselines* b, int32_t similarity, const double* f, int64_t n_f, const double* w4, int64_t n_w4);
 
+/* ---- NARM neural session baseline (DESIGN §3s) -----------------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_NARM, n_items, d_e (1 .. 1024), ...).  The model is one flat float32 vector: E [n_items x d_e], Wx
+ * [d_e x 3H], Wrz [H x 2H], Wh [H x H], Bh [3H], A1 [H x H], A2 [H x H], v [H], B [d_e x 2H], n_params = n_items d_e + 5 d_e H +
+ * 5 H^2 + 4 H.  For inputs x_1 .. x_t: h_j the GRU of GRU4Rec's cell over E[x] from a zero state, alpha_j = v . sig(A1 h_t +
+ * A2 h_j), c = [h_t ; sum_j alpha_j h_j], q = B c, score(i) = E[i] . q. */
+#define G4R_BL_NARM 12
+/* Begins a fit: hidden 1 .. 1024, max_len 2 .. 512, batch_size >= 1, the training pieces as CSR (items[piece_offsets[k] ..
+ * piece_offsets[k+1]), 2 .. max_len events each: inputs are every event but the last, targets every event but the first) and the
+ * initial parameters.  Adam's moments start at 0.  Every argument is checked before any device write; G4R_ERR_CUDA with a message
+ * naming the sizes if the device cannot hold the largest batch's logits (positions x n_items floats) and scratch. */
+int g4r_bl_narm_begin(g4r_baselines* b, int32_t hidden, int32_t max_len, int32_t batch_size, const int64_t* piece_offsets, int64_t n_pieces,
+                      const int32_t* items, int64_t n_entries, const float* params, int64_t n_params);
+/* One epoch: mini-batches of batch_size consecutive entries of order (piece indices; the last batch may be smaller), each the mean
+ * full-catalogue cross-entropy over its positions and one Adam step (b1 0.9, b2 0.999, eps 1e-8, bias-corrected) on every
+ * parameter, with dropout masks of global step = the steps since g4r_bl_narm_begin.  No host round trip inside.  A batch may
+ * hold at most as many positions (inputs) as the batch_size longest distinct pieces, the scratch g4r_bl_narm_begin sized: a
+ * batch that repeats a long piece past that bound refuses the call (G4R_ERR_INVALID) before any device write.  Out (may be
+ * NULL): losses[ceil(n_order / batch_size)] and the device time (CUDA events). */
+int g4r_bl_narm_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, uint32_t seed, float learning_rate, float dropout_emb,
+                      float dropout_ct, float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size pieces at the current parameters, without an update: the mean loss and the gradient of every
+ * parameter (n_params floats, the parameters' layout), dropout masks of global step `step`.  The pieces obey
+ * g4r_bl_narm_epoch's bound on a batch's positions. */
+int g4r_bl_narm_grads(g4r_baselines* b, const int32_t* pieces, int32_t n, uint32_t seed, int64_t step, float dropout_emb, float dropout_ct,
+                      float* loss, float* grads);
+/* The parameters (n_params floats). */
+int g4r_bl_narm_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (a model loaded from a pickle); ends any fit in progress. */
+int g4r_bl_narm_import(g4r_baselines* b, int32_t hidden, int32_t max_len, const float* params, int64_t n_params);
+/* Every counted event's q (eval mode, the last max_len inputs of items[start .. p]) in g4r_bl_evaluate's order: q [n_q x d_e],
+ * n_q the number of counted events.  g4r_bl_evaluate of a NARM handle ranks these q as a BPR handle ranks its session vectors,
+ * with I = double(E) and bI = 0. */
+int g4r_bl_narm_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                       const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif
