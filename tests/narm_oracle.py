@@ -204,9 +204,19 @@ def train(th0, shape, piece_list, orders, batch_size, lr, seed, p_emb, p_ct, max
 
 
 def encode(p, prefix, max_len):
-    """eval-mode q of a prefix: the last max_len inputs through piece_forward, its last position"""
-    _, q = piece_forward(p, list(prefix)[-max_len:])
-    return q[-1]
+    """eval-mode q of a prefix: the GRU over its last max_len inputs, then the attention and q of the last position only (the
+    others' are not needed, and at max_len 512 the whole triangle would cost [n, n, H] doubles per event)"""
+    H = p['Wh'].shape[0]
+    h, HS = np.zeros(H), []
+    for x in list(prefix)[-max_len:]:
+        vec = p['E'][x] @ p['Wx'] + p['Bh']
+        rz = _sig(vec[H:] + h @ p['Wrz'])
+        r, z = rz[:H], rz[H:]
+        h = (1.0 - z) * h + z * np.tanh((h * r) @ p['Wh'] + vec[:H])
+        HS.append(h)
+    HS = np.array(HS)
+    alpha = _sig(HS[-1] @ p['A1'].T + HS @ p['A2'].T) @ p['v']
+    return p['B'] @ np.concatenate([HS[-1], alpha @ HS])
 
 
 def encode_events(p, items, offsets, n_history, max_len):
