@@ -19,6 +19,11 @@ class Baseline(object):
     error_during_train = False
     _kind = None
     _world = staticmethod(_GRU4Rec._world)
+    _caches = ('_dev', '_post', '_p64')          # built on first use from the fitted model; never pickled, dropped by fit
+
+    def _drop_caches(self):
+        for name in self._caches:
+            self.__dict__.pop(name, None)
 
     def _index(self, data):
         """itemidmap / n_items from the training data; returns the item index of every row"""
@@ -27,6 +32,36 @@ class Baseline(object):
         self.n_items = len(itemids)
         self.itemidmap = pd.Series(data=np.arange(self.n_items), index=itemids)
         return pd.Index(itemids).get_indexer(ids)
+
+    def _sessions(self, data, order=None):
+        """the session index of the training data, after the item index (_index): (item index of every row, session code of
+        every row with the sessions in order of first appearance, session CSR offsets [n_sessions + 1], event order).  The event
+        order groups the rows by session, each session's events in row order (order='rows') or by time_key with ties by row
+        order (order='time'); it is None for order=None"""
+        idx = self._index(data)
+        sess = data[self.session_key].values
+        code = pd.Index(pd.unique(sess)).get_indexer(sess)
+        S = int(code.max()) + 1 if len(code) else 0
+        offsets = np.zeros(S + 1, np.int64)
+        offsets[1:] = np.cumsum(np.bincount(code, minlength=S))
+        if order is None:
+            return idx, code, offsets, None
+        o = np.argsort(code, kind='stable') if order == 'rows' else np.lexsort((data[self.time_key].values, code))
+        return idx, code, offsets, o
+
+    def _prefix(self, session_id, x):
+        """the session's inputs so far with x appended, or [x] when session_id is not the current session"""
+        if self.current_session is None or self.current_session != session_id:
+            self.current_session = session_id
+            self.session = [x]
+        else:
+            self.session.append(x)
+        return self.session
+
+    def _integer(self, name, lo, hi):
+        v = getattr(self, name)
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+            raise ValueError('%s must be an integer in %d .. %d, not %r' % (name, lo, hi, v))
 
     def _n_keep(self):
         raise NotImplementedError
@@ -47,7 +82,8 @@ class Baseline(object):
 
     def __getstate__(self):
         state = self.__dict__.copy()
-        state.pop('_dev', None)
+        for name in self._caches:
+            state.pop(name, None)
         return state
 
 
@@ -82,7 +118,7 @@ class Pop(Baseline):
 
     def fit(self, data):
         self.pop_scores = _pop_scores(self, data)
-        self.__dict__.pop('_dev', None)
+        self._drop_caches()
 
     def _n_keep(self):
         return self.top_n
@@ -153,15 +189,10 @@ class ItemKNN(Baseline):
         return a, b
 
     def fit(self, data):
-        idx = self._index(data)
-        sess = data[self.session_key].values
-        codes = pd.Index(pd.unique(sess)).get_indexer(sess)
-        order = np.argsort(codes, kind='stable')                   # session CSR of the item indices
-        offsets = np.zeros(codes.max() + 2 if len(codes) else 1, dtype=np.int64)
-        offsets[1:] = np.cumsum(np.bincount(codes, minlength=len(offsets) - 1))
+        idx, _, offsets, order = self._sessions(data, 'rows')
         supp = np.bincount(idx, minlength=self.n_items).astype(np.int64)
         a, b = self.norm_factors(supp)
-        self.__dict__.pop('_dev', None)
+        self._drop_caches()
         dev = _lib.Baselines(self._kind, self.n_items, self.n_sims)
         self.fit_stats = dev.knn_fit(offsets, idx[order], a, b)
         self.rows = dev.rows_export()
@@ -231,7 +262,7 @@ class BPR(Baseline):
         data = pd.merge(data, pd.DataFrame({self.item_key: itemids, 'ItemIdx': np.arange(self.n_items)}), on=self.item_key, how='inner')
         data = pd.merge(data, pd.DataFrame({self.session_key: sessionids, 'SessionIdx': np.arange(self.n_sessions)}), on=self.session_key, how='inner')
         self.init(data)
-        self.__dict__.pop('_dev', None)
+        self._drop_caches()
         dev = _lib.Baselines(self._kind, self.n_items, self.n_factors)
         dev.bpr_begin(data.SessionIdx.values, data.ItemIdx.values, self.n_sessions, self.U, self.I, self.bI)
         self.fit_stats = []
@@ -250,13 +281,7 @@ class BPR(Baseline):
         dev.bpr_import(self.I, self.bI)
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
-        iidx = self.itemidmap[input_item_id]
-        if self.current_session is None or self.current_session != session_id:
-            self.current_session = session_id
-            self.session = [iidx]
-        else:
-            self.session.append(iidx)
-        uF = self.I[self.session].mean(axis=0)
+        uF = self.I[self._prefix(session_id, self.itemidmap[input_item_id])].mean(axis=0)
         iIdxs = self.itemidmap[predict_for_item_ids]
         return pd.Series(data=self.I[iIdxs].dot(uF) + self.bI[iIdxs], index=predict_for_item_ids)
 
@@ -292,37 +317,40 @@ class SessionKNN(Baseline):
     def _n_keep(self):
         return self.k
 
-    def fit(self, data):
+    def _check_similarity(self):
         if self.similarity not in _lib.SKNN_SIMILARITY:
             raise ValueError('similarity must be one of %s, not %r' % (sorted(_lib.SKNN_SIMILARITY), self.similarity))
+
+    def _check_neighbours(self):
         if not 1 <= self.sample_size <= 8192:
             raise ValueError('sample_size must be in 1 .. 8192, not %r' % (self.sample_size,))
         if not 1 <= self.k <= min(self.sample_size, 1024):
             raise ValueError('k must be in 1 .. min(sample_size, 1024), not %r' % (self.k,))
-        idx = self._index(data).astype(np.int64)
-        sess = data[self.session_key].values
-        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
-        self.n_sessions = S = int(code.max()) + 1 if len(code) else 0
-        T = pd.Series(data[self.time_key].values).groupby(code).max().values
-        order = np.argsort(-T, kind='stable')                    # T descending, ties by first appearance
+
+    def _recency(self, code, times):
+        """T per session (the largest time of its events); sets n_sessions and the recency ranks (T descending, ties by first
+        appearance)"""
+        T = pd.Series(times).groupby(code).max().values
+        self.n_sessions = S = len(T)
         self.recency = np.empty(S, np.int32)
-        self.recency[order] = np.arange(S, dtype=np.int32)
-        pairs = np.unique(code.astype(np.int64) * self.n_items + idx)   # (session, item) distinct, items ascending per session
+        self.recency[np.argsort(-T, kind='stable')] = np.arange(S, dtype=np.int32)
+        return T
+
+    def fit(self, data):
+        self._check_similarity()
+        self._check_neighbours()
+        idx, code, _, _ = self._sessions(data)
+        self._recency(code, data[self.time_key].values)
+        pairs = np.unique(code.astype(np.int64) * self.n_items + idx.astype(np.int64))   # (session, item) distinct, items ascending per session
         self.session_items = (pairs % self.n_items).astype(np.int32)
-        self.session_offsets = np.zeros(S + 1, np.int64)
-        self.session_offsets[1:] = np.cumsum(np.bincount(pairs // self.n_items, minlength=S))
+        self.session_offsets = np.zeros(self.n_sessions + 1, np.int64)
+        self.session_offsets[1:] = np.cumsum(np.bincount(pairs // self.n_items, minlength=self.n_sessions))
         self.current_session = None
-        self.__dict__.pop('_dev', None)
-        self.__dict__.pop('_post', None)
+        self._drop_caches()
         self._device()
 
     def _upload(self, dev):
         dev.sknn_fit(self.session_offsets, self.session_items, self.recency, self.sample_size, self.similarity)
-
-    def __getstate__(self):
-        state = Baseline.__getstate__(self)
-        state.pop('_post', None)
-        return state
 
     def _postings(self):
         """(per item offsets, the ranks of its sessions ascending, the session of each rank), built on first use"""
@@ -335,43 +363,55 @@ class SessionKNN(Baseline):
             post = self._post = (ioff, rank[o], np.argsort(self.recency))
         return post
 
-    def score_prefix(self, prefix):
-        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+    def _knn_scores(self, prefix, weight, normalise, w2=None, w3=None, w4=None, f=None):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last), from the
+        candidates and the k neighbours every kNN baseline shares.  Each class supplies: weight(t, p), the weight of a shared
+        item whose last position in the prefix is p; normalise, whether v / sqrt(|I(c)| |I(n)|) is the similarity (else v, the
+        weights' sum); W2 per session; W3 by distance inside a neighbour (None: no positions); W4(t), the table by the prefix
+        distance of the neighbour's most recent shared item; F per item"""
         prefix = np.asarray(prefix, dtype=np.int64)
         t = len(prefix)
         u, first_rev = np.unique(prefix[::-1], return_index=True)
         last = t - first_rev                                      # 1-based position of the last occurrence
         o = np.argsort(last)
         ci, pos = u[o], last[o]
+        wp = weight(t, pos)
         ioff, ranks, by_rank = self._postings()
         S = self.sample_size
         cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
         sess = by_rank[cand]
         starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
         owner = np.repeat(np.arange(len(cand)), lens)
-        flat = self.session_items[np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())]
-        sims, cnt = np.zeros(len(cand)), np.zeros(len(cand), np.int64)
+        at = np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())
+        flat = self.session_items[at]
+        fpos = None if w3 is None else self.positions[at]
+        v, qr, dr = np.zeros(len(cand)), np.zeros(len(cand), np.int64), np.zeros(len(cand), np.int64)
         for m, i in enumerate(ci):                                # c's items in order of their last position
+            sel = flat == i
             hit = np.zeros(len(cand), bool)
-            hit[owner[flat == i]] = True
-            cnt += hit
-            sims = sims + np.where(hit, pos[m] / t, 0.0)
-        if self.similarity == 'cosine':
-            sims = cnt / np.sqrt((len(ci) * lens).astype(np.float64))
+            hit[owner[sel]] = True
+            v = v + np.where(hit, wp[m], 0.0)
+            if w3 is not None:
+                qr[owner[sel]] = fpos[sel]                        # ends at the shared item with the largest p_i
+                dr[owner[sel]] = t - pos[m]
+        sims = v / np.sqrt((len(ci) * lens).astype(np.float64)) if normalise else v
+        if w2 is not None:
+            sims = sims * w2[sess]
+        g = sims if w4 is None else sims * w4(t)[dr]
         score = np.zeros(self.n_items)
         for q in np.lexsort((cand, -sims))[:self.k]:
-            j = flat[owner == q]
-            score[j] = score[j] + sims[q]
-        return score
+            sel = owner == q
+            score[flat[sel]] = score[flat[sel]] + (g[q] if w3 is None else g[q] * w3[np.abs(fpos[sel] - qr[q])])
+        return score if f is None else score * f
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        if self.similarity == 'cosine':
+            return self._knn_scores(prefix, lambda t, p: np.ones(len(p)), True)
+        return self._knn_scores(prefix, lambda t, p: p / t, False)
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
-        x = self.itemidmap[input_item_id]
-        if self.current_session is None or self.current_session != session_id:
-            self.current_session = session_id
-            self.session = [x]
-        else:
-            self.session.append(x)
-        score = self.score_prefix(self.session)
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
         return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
 
 
@@ -414,29 +454,19 @@ class STAN(SessionKNN):
 
     def _fit_index(self, data):
         """the parameter checks, the index, positions, W2 and W3 on the host (no device work)"""
-        if not 1 <= self.sample_size <= 8192:
-            raise ValueError('sample_size must be in 1 .. 8192, not %r' % (self.sample_size,))
-        if not 1 <= self.k <= min(self.sample_size, 1024):
-            raise ValueError('k must be in 1 .. min(sample_size, 1024), not %r' % (self.k,))
+        self._check_neighbours()
         for name in ('lambda_spw', 'lambda_snh', 'lambda_inh'):
             if not float(getattr(self, name)) > 0.0:
                 raise ValueError('%s must be in (0, inf], not %r' % (name, getattr(self, name)))
         col = data[self.time_key]
         if not pd.api.types.is_numeric_dtype(col) or pd.api.types.is_bool_dtype(col):
             raise ValueError('%s needs a numeric time column %r, not %s' % (type(self).__name__, self.time_key, col.dtype))
-        times = col.values
-        idx = self._index(data).astype(np.int64)
-        sess = data[self.session_key].values
-        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
-        self.n_sessions = S = int(code.max()) + 1 if len(code) else 0
-        T = pd.Series(times).groupby(code).max().values
-        order = np.argsort(-T, kind='stable')                    # T descending, ties by first appearance
-        self.recency = np.empty(S, np.int32)
-        self.recency[order] = np.arange(S, dtype=np.int32)
-        lens = np.bincount(code, minlength=S)
-        o = np.lexsort((times, code))                            # each session's events by time, ties by row order
-        pos = np.arange(len(o)) - np.repeat(np.cumsum(lens) - lens, lens) + 1
-        key = code[o].astype(np.int64) * self.n_items + idx[o]
+        idx, code, offsets, o = self._sessions(data, 'time')
+        T = self._recency(code, col.values)
+        S = self.n_sessions
+        lens = np.diff(offsets)
+        pos = np.arange(len(o)) - np.repeat(offsets[:-1], lens) + 1
+        key = code[o].astype(np.int64) * self.n_items + idx[o].astype(np.int64)
         o2 = np.lexsort((pos, key))
         key, pos = key[o2], pos[o2]
         last = np.r_[key[1:] != key[:-1], True]                  # (session, item) distinct, items ascending; its last position
@@ -447,8 +477,7 @@ class STAN(SessionKNN):
         self.w2 = np.exp(-((T.max() - T).astype(np.float64) / float(self.lambda_snh)))
         self.w3 = np.exp(-(np.arange(int(lens.max())) / float(self.lambda_inh)))
         self.current_session = None
-        self.__dict__.pop('_dev', None)
-        self.__dict__.pop('_post', None)
+        self._drop_caches()
 
     def _w1(self, n):
         return np.exp(-(np.arange(n) / float(self.lambda_spw)))
@@ -464,34 +493,7 @@ class STAN(SessionKNN):
 
     def score_prefix(self, prefix):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
-        prefix = np.asarray(prefix, dtype=np.int64)
-        t = len(prefix)
-        u, first_rev = np.unique(prefix[::-1], return_index=True)
-        last = t - first_rev                                      # 1-based position of the last occurrence
-        o = np.argsort(last)
-        ci, pos = u[o], last[o]
-        ioff, ranks, by_rank = self._postings()
-        S = self.sample_size
-        cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
-        sess = by_rank[cand]
-        starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
-        owner = np.repeat(np.arange(len(cand)), lens)
-        at = np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())
-        flat, fpos = self.session_items[at], self.positions[at]
-        w1 = self._w1(t)
-        v, qr = np.zeros(len(cand)), np.zeros(len(cand), np.int64)
-        for m, i in enumerate(ci):                                # c's items in order of their last position
-            sel = flat == i
-            hit = np.zeros(len(cand), bool)
-            hit[owner[sel]] = True
-            v = v + np.where(hit, w1[t - pos[m]], 0.0)
-            qr[owner[sel]] = fpos[sel]                            # ends at the shared item with the largest p_i
-        sims = v / np.sqrt((len(ci) * lens).astype(np.float64)) * self.w2[sess]
-        score = np.zeros(self.n_items)
-        for q in np.lexsort((cand, -sims))[:self.k]:
-            sel = owner == q
-            score[flat[sel]] = score[flat[sel]] + sims[q] * self.w3[np.abs(fpos[sel] - qr[q])]
-        return score
+        return self._knn_scores(prefix, lambda t, p: self._w1(t)[t - p], True, self.w2, self.w3)
 
 
 class VSTAN(STAN):
@@ -522,8 +524,7 @@ class VSTAN(STAN):
         self.lambda_idf = lambda_idf
 
     def fit(self, data):
-        if self.similarity not in _lib.SKNN_SIMILARITY:
-            raise ValueError('similarity must be one of %s, not %r' % (sorted(_lib.SKNN_SIMILARITY), self.similarity))
+        self._check_similarity()
         if not float(self.lambda_ipw) > 0.0:
             raise ValueError('lambda_ipw must be in (0, inf], not %r' % (self.lambda_ipw,))
         if not 0.0 <= float(self.lambda_idf) < np.inf:
@@ -548,37 +549,7 @@ class VSTAN(STAN):
 
     def score_prefix(self, prefix):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
-        prefix = np.asarray(prefix, dtype=np.int64)
-        t = len(prefix)
-        u, first_rev = np.unique(prefix[::-1], return_index=True)
-        last = t - first_rev                                      # 1-based position of the last occurrence
-        o = np.argsort(last)
-        ci, pos = u[o], last[o]
-        ioff, ranks, by_rank = self._postings()
-        S = self.sample_size
-        cand = np.unique(np.concatenate([ranks[ioff[i]:ioff[i] + min(ioff[i + 1] - ioff[i], S)] for i in ci]))[:S]
-        sess = by_rank[cand]
-        starts, lens = self.session_offsets[sess], np.diff(self.session_offsets)[sess]
-        owner = np.repeat(np.arange(len(cand)), lens)
-        at = np.repeat(starts - np.r_[0, np.cumsum(lens)[:-1]], lens) + np.arange(lens.sum())
-        flat, fpos = self.session_items[at], self.positions[at]
-        w1 = self._w1(t)
-        v, qr, dr = np.zeros(len(cand)), np.zeros(len(cand), np.int64), np.zeros(len(cand), np.int64)
-        for m, i in enumerate(ci):                                # c's items in order of their last position
-            sel = flat == i
-            hit = np.zeros(len(cand), bool)
-            hit[owner[sel]] = True
-            v = v + np.where(hit, w1[t - pos[m]], 0.0)
-            qr[owner[sel]] = fpos[sel]                            # ends at the shared item with the largest p_i
-            dr[owner[sel]] = t - pos[m]
-        sim1 = v if self.similarity == 'vector' else v / np.sqrt((len(ci) * lens).astype(np.float64))
-        sims = sim1 * self.w2[sess]
-        g = sims * self._w4(t)[dr]
-        score = np.zeros(self.n_items)
-        for q in np.lexsort((cand, -sims))[:self.k]:
-            sel = owner == q
-            score[flat[sel]] = score[flat[sel]] + g[q] * self.w3[np.abs(fpos[sel] - qr[q])]
-        return score * self.f
+        return self._knn_scores(prefix, lambda t, p: self._w1(t)[t - p], self.similarity != 'vector', self.w2, self.w3, self._w4, self.f)
 
 
 class _Rules(Baseline):
@@ -591,17 +562,10 @@ class _Rules(Baseline):
         return None, None
 
     def fit(self, data):
-        if isinstance(self.pruning, bool) or not isinstance(self.pruning, (int, np.integer)) or not 1 <= self.pruning <= _lib.KEEP_MAX:
-            raise ValueError('pruning must be an integer in 1 .. %d, not %r' % (_lib.KEEP_MAX, self.pruning))
+        self._integer('pruning', 1, _lib.KEEP_MAX)
         steps, weighting = self._steps()
-        idx = self._index(data)
-        sess = data[self.session_key].values
-        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
-        o = np.lexsort((data[self.time_key].values, code))      # each session's events by time, ties by row order
-        S = int(code.max()) + 1 if len(code) else 0
-        offsets = np.zeros(S + 1, np.int64)
-        offsets[1:] = np.cumsum(np.bincount(code, minlength=S))
-        self.__dict__.pop('_dev', None)
+        idx, _, offsets, o = self._sessions(data, 'time')
+        self._drop_caches()
         dev = _lib.Baselines(self._kind, self.n_items, self.pruning)
         self.fit_stats = dev.rules_fit(offsets, idx[o], steps, weighting)
         self.rows = dev.rows_export()
@@ -637,8 +601,7 @@ class SR(_Rules):
         self.time_key = time_key
 
     def _steps(self):
-        if isinstance(self.steps, bool) or not isinstance(self.steps, (int, np.integer)) or not 1 <= self.steps <= _lib.RULES_STEPS_MAX:
-            raise ValueError('steps must be an integer in 1 .. %d, not %r' % (_lib.RULES_STEPS_MAX, self.steps))
+        self._integer('steps', 1, _lib.RULES_STEPS_MAX)
         if self.weighting not in _lib.RULES_WEIGHTING:
             raise ValueError('weighting must be one of %s, not %r' % (sorted(_lib.RULES_WEIGHTING), self.weighting))
         return int(self.steps), self.weighting
@@ -772,15 +735,11 @@ class NARM(Baseline):
         return self.embedding
 
     def _check(self):
-        def integer(name, lo, hi):
-            v = getattr(self, name)
-            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
-                raise ValueError('%s must be an integer in %d .. %d, not %r' % (name, lo, hi, v))
-        integer('embedding', 1, 1024)
-        integer('hidden', 1, 1024)
-        integer('n_epochs', 0, 1 << 30)
-        integer('batch_size', 1, 1 << 20)
-        integer('max_len', 2, 512)
+        self._integer('embedding', 1, 1024)
+        self._integer('hidden', 1, 1024)
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 2, 512)
         if not 0.0 < float(self.learning_rate) < np.inf:
             raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
         for name in ('dropout_emb', 'dropout_ct'):
@@ -789,13 +748,7 @@ class NARM(Baseline):
 
     def pieces(self, data):
         """(piece offsets, piece items) of the training data, after the item index (_index)"""
-        idx = self._index(data)
-        sess = data[self.session_key].values
-        code = pd.Index(pd.unique(sess)).get_indexer(sess)        # sessions in order of first appearance
-        o = np.lexsort((data[self.time_key].values, code))      # each session's events by time, ties by row order
-        S = int(code.max()) + 1 if len(code) else 0
-        offsets = np.zeros(S + 1, np.int64)
-        offsets[1:] = np.cumsum(np.bincount(code, minlength=S))
+        idx, _, offsets, o = self._sessions(data, 'time')
         return narm_pieces(offsets, idx[o], self.max_len)
 
     def fit(self, data):
@@ -805,8 +758,7 @@ class NARM(Baseline):
             raise ValueError('NARM needs a training session of at least 2 events')
         rs = np.random.RandomState(self.seed)
         params = narm_init(self.n_items, self.embedding, self.hidden, rs)
-        self.__dict__.pop('_dev', None)
-        self.__dict__.pop('_p64', None)
+        self._drop_caches()
         dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
         dev.narm_begin(self.hidden, self.max_len, self.batch_size, poff, pitems, params)
         self.fit_stats = []
@@ -823,11 +775,6 @@ class NARM(Baseline):
     def _upload(self, dev):
         dev.narm_import(self.hidden, self.max_len, self.params)
 
-    def __getstate__(self):
-        state = Baseline.__getstate__(self)
-        state.pop('_p64', None)
-        return state
-
     def params64(self):
         """name -> float64 copy of each parameter"""
         p = self.__dict__.get('_p64')
@@ -841,11 +788,5 @@ class NARM(Baseline):
         return p['E'] @ narm_encode(p, list(prefix)[-self.max_len:])
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
-        x = self.itemidmap[input_item_id]
-        if self.current_session is None or self.current_session != session_id:
-            self.current_session = session_id
-            self.session = [x]
-        else:
-            self.session.append(x)
-        score = self.score_prefix(self.session)
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
         return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)

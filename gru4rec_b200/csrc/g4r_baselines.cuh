@@ -63,7 +63,7 @@ struct g4r_baselines {
   double *dVsF = nullptr, *dVsW4 = nullptr;
   int64_t vs_n_w4 = 0;
   bool vs_set = false;
-  // NARM (g4r_narm.cuh): the flat float32 parameters, a device 1.0f, and dI = double(E), dBI = 0 for bpr_evaluate; the fit's
+  // NARM (g4r_narm.cuh): the flat float32 parameters, a device 1.0f, and dI = double(E), dBI = 0 for bpr_blocks; the fit's
   // gradient, Adam moments, training pieces and scratch (nm_mem, from g4r_bl_narm_begin until an import or the destroy)
   float *dNmTh = nullptr, *dNmOne = nullptr, *dNmG = nullptr, *dNmM = nullptr, *dNmV = nullptr, *dNmLoss = nullptr;
   int* dNmItems = nullptr;
@@ -90,8 +90,33 @@ struct KnnFitDev {
   int* out_idx; double* out_sim; int* out_len;
 };
 
-// the kinds whose model is ItemKNN's rows (g4r_rules.cuh fits SR and AR)
-__host__ __device__ __forceinline__ bool bl_has_rows(int kind) { return kind == BL_ITEMKNN || kind == BL_SR || kind == BL_AR; }
+// what g4r_bl_create and g4r_bl_evaluate know of each kind: its n_keep bound, the model storage the handle allocates at its
+// creation (NONE: at the fit) and the function that ranks an evaluation (null: no such kind)
+struct BlCall;
+static int bl_rank_list(g4r_baselines* h, BlCall& c);  // k_bl_rank (below)
+static int bpr_rank(g4r_baselines* h, BlCall& c);      // g4r_bpr.cuh
+static int sknn_rank(g4r_baselines* h, BlCall& c);     // g4r_sknn.cuh
+static int narm_rank(g4r_baselines* h, BlCall& c);     // g4r_narm.cuh
+enum BlStore { BL_STORE_NONE, BL_STORE_ROWS, BL_STORE_POP, BL_STORE_BPR };
+struct BlKind { int keep_max; BlStore store; int (*rank)(g4r_baselines*, BlCall&); };
+constexpr BlKind BL_KINDS[] = {
+    {INT32_MAX, BL_STORE_POP, bl_rank_list},            // 0 Pop
+    {INT32_MAX, BL_STORE_POP, bl_rank_list},            // 1 SessionPop
+    {KF_KEEP_MAX, BL_STORE_ROWS, bl_rank_list},         // 2 ItemKNN
+    {BPR_F_MAX, BL_STORE_BPR, bpr_rank},                // 3 BPR
+    {0, BL_STORE_NONE, nullptr},
+    {KF_KEEP_MAX, BL_STORE_NONE, sknn_rank},            // 5 SessionKNN
+    {KF_KEEP_MAX, BL_STORE_NONE, sknn_rank},            // 6 STAN
+    {0, BL_STORE_NONE, nullptr},
+    {KF_KEEP_MAX, BL_STORE_ROWS, bl_rank_list},         // 8 SR (g4r_rules.cuh; its rows rank as ItemKNN's)
+    {KF_KEEP_MAX, BL_STORE_ROWS, bl_rank_list},         // 9 AR
+    {0, BL_STORE_NONE, nullptr},
+    {KF_KEEP_MAX, BL_STORE_NONE, sknn_rank},            // 11 VSTAN
+    {BPR_F_MAX, BL_STORE_NONE, narm_rank},              // 12 NARM
+};
+static bool bl_kind_ok(int kind) { return kind >= 0 && kind < (int)(sizeof(BL_KINDS) / sizeof(BL_KINDS[0])) && BL_KINDS[kind].rank; }
+// the kinds whose model is ItemKNN's rows
+static bool bl_has_rows(int kind) { return BL_KINDS[kind].store == BL_STORE_ROWS; }
 
 // (score desc, index asc): the order of every kept row and list
 __device__ __forceinline__ bool bl_before(double sa, int ia, double sb, int ib) { return sa > sb || (sa == sb && ia < ib); }
@@ -640,12 +665,12 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
-  if ((kind < BL_POP || kind > BL_BPR) && kind != BL_SKNN && kind != BL_STAN && kind != BL_SR && kind != BL_AR && kind != BL_VSTAN && kind != BL_NARM) {
+  if (!bl_kind_ok(kind)) {
     g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR), 11 (VSTAN) or 12 (NARM)";
     return G4R_ERR_INVALID;
   }
-  if (n_items < 1 || n_keep < 1 || ((bl_has_rows(kind) || kind == BL_SKNN || kind == BL_STAN || kind == BL_VSTAN) && n_keep > KF_KEEP_MAX) ||
-      ((kind == BL_BPR || kind == BL_NARM) && n_keep > BPR_F_MAX)) {
+  const BlStore store = BL_KINDS[kind].store;
+  if (n_items < 1 || n_keep < 1 || n_keep > BL_KINDS[kind].keep_max) {
     g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR, AR and VSTAN, <= " +
                         std::to_string(BPR_F_MAX) + " n_factors for BPR and embedding for NARM)";
     return G4R_ERR_INVALID;
@@ -656,7 +681,7 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
     return G4R_ERR_CUDA;
   }
   g4r_baselines* h = new g4r_baselines();
-  h->kind = kind; h->n_items = n_items; h->n_keep = (kind >= BL_ITEMKNN) ? n_keep : std::min(n_keep, n_items); h->device = device;
+  h->kind = kind; h->n_items = n_items; h->n_keep = store == BL_STORE_POP ? std::min(n_keep, n_items) : n_keep; h->device = device;
   auto bail = [&](const char* m) { g_bl_create_error = m; g4r_bl_destroy(h); return G4R_ERR_CUDA; };
   if (cudaSetDevice(device) != cudaSuccess) return bail("cudaSetDevice failed");
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
@@ -664,12 +689,12 @@ extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int3
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1);
   const size_t rows = (size_t)n_items * h->n_keep;
   bool ok = true;
-  if (kind == BL_BPR) {
+  if (store == BL_STORE_BPR) {
     ok &= bl_alloc(&h->dI, rows) == cudaSuccess && bl_alloc(&h->dBI, n_items) == cudaSuccess;
-  } else if (bl_has_rows(kind)) {
+  } else if (store == BL_STORE_ROWS) {
     ok &= bl_alloc(&h->dIdx, rows) == cudaSuccess && bl_alloc(&h->dIdxI, rows) == cudaSuccess && bl_alloc(&h->dLen, n_items) == cudaSuccess;
     ok &= bl_alloc(&h->dSim, rows) == cudaSuccess && bl_alloc(&h->dSimI, rows) == cudaSuccess;
-  } else if (kind != BL_SKNN && kind != BL_STAN && kind != BL_VSTAN && kind != BL_NARM) {   // SessionKNN, STAN, VSTAN and NARM allocate at their fit
+  } else if (store == BL_STORE_POP) {
     ok &= bl_alloc(&h->dPop, n_items) == cudaSuccess && bl_alloc(&h->dTopS, h->n_keep) == cudaSuccess && bl_alloc(&h->dTop, h->n_keep) == cudaSuccess;
   }
   if (!ok) return bail("device allocation failed");
@@ -690,16 +715,90 @@ struct BlBufs {
   ~BlBufs() { for (void* q : p) cudaFree(q); }
 };
 
+// one g4r_bl_evaluate call after its argument checks: the counted events and the candidates on the host, their device copies, the
+// outputs every kind's ranking fills (counts [2 x n_ev], lists [n_ev x k]) and the owner of the call's device buffers
+struct BlCall {
+  const int32_t* items; int64_t n_events; const int64_t* off; int64_t n_sessions; const int32_t* n_history;
+  int mode, k; bool exclude;
+  std::vector<int64_t> ev0;                             // counted events before each session [n_sessions + 1]
+  int64_t n_ev;
+  std::vector<int> mult, cdist;                         // candidates: multiplicities [n_items], distinct ascending (empty: every item)
+  long long wtot;
+  BlBufs bb;
+  const int *d_items = nullptr, *d_nh = nullptr, *d_mult = nullptr, *d_cdist = nullptr;
+  const int64_t *d_off = nullptr, *d_ev0 = nullptr;
+  int *counts = nullptr, *out_items = nullptr;
+  double* out_scores = nullptr;
+  // the call's part of k_bl_rank's and k_sknn_rank's arguments
+  BlEvalDev bl(int n_items) const {
+    BlEvalDev d{};
+    d.n_items = n_items; d.mode = mode; d.k = k; d.exclude = exclude; d.wtot = wtot;
+    d.items = d_items; d.off = d_off; d.nh = d_nh; d.ev0 = d_ev0;
+    d.mult = d_mult; d.cdist = d_cdist; d.n_cdist = (int)cdist.size();
+    d.counts = counts; d.out_items = out_items; d.out_scores = out_scores;
+    return d;
+  }
+};
+
+// the counted events before each session, ev0 [n_sessions + 1]: a session counts its events after the first max(n_history, 1)
+static int bl_counted(g4r_baselines* h, const char* fn, const int64_t* off, int64_t n_sessions, const int32_t* n_history, std::vector<int64_t>& ev0) {
+  ev0.assign(n_sessions + 1, 0);
+  for (int64_t s = 0; s < n_sessions; s++) {
+    const int64_t len = off[s + 1] - off[s], hs = n_history ? n_history[s] : 0;
+    if (hs < 0 || hs > len) FAIL(G4R_ERR_INVALID, std::string(fn) + ": n_history entry out of range");
+    ev0[s + 1] = ev0[s] + std::max<int64_t>(0, len - std::max<int64_t>(hs, 1));
+  }
+  return G4R_OK;
+}
+
 static bool bl_offsets_ok(const int64_t* off, int64_t n_sessions, int64_t n_events) {
   if (off[0] != 0 || off[n_sessions] != n_events) return false;
   for (int64_t s = 0; s < n_sessions; s++) if (off[s + 1] < off[s]) return false;
   return true;
 }
 
-static int bl_sort_rows(g4r_baselines* h) {
+static cudaError_t bl_sort_rows(g4r_baselines* h) {
   k_knn_by_index<<<h->n_items, KF_THREADS, 0, h->stream>>>(h->dIdx, h->dSim, h->dLen, h->n_keep, h->dIdxI, h->dSimI);
-  CK(cudaGetLastError());
+  return cudaGetLastError();
+}
+
+// the row fits (ItemKNN here, SR and AR in g4r_rules.cuh): resident CTAs, each with a dense slice of n_items accumulators of
+// acc_size bytes, touched columns and values, within KF_SCRATCH
+static int bl_fit_grid(const g4r_baselines* h, size_t acc_size, size_t* scratch_bytes) {
+  const size_t per_cta = (size_t)h->n_items * (acc_size + sizeof(int) + sizeof(double));
+  const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)4 * h->n_sm, KF_SCRATCH / per_cta));
+  if (scratch_bytes) *scratch_bytes = per_cta * grid;
+  return grid;
+}
+
+// exclusive scan out[0 .. n] of in[0 .. n); tot holds (n + SCAN_B - 1) / SCAN_B block totals
+static cudaError_t bl_scan(const long long* in, int64_t n, long long* out, long long* tot, cudaStream_t st) {
+  const int64_t nb = (n + SCAN_B - 1) / SCAN_B;
+  if (!nb) return cudaMemsetAsync(out, 0, sizeof(long long), st);
+  k_scan_block<<<(unsigned)nb, SCAN_B, 0, st>>>(in, n, out, tot);
+  k_scan_tot<<<1, 1, 0, st>>>(tot, nb);
+  k_scan_add<<<(unsigned)nb, SCAN_B, 0, st>>>(out, n, tot);
+  return cudaSuccess;
+}
+
+// the rows 0 .. n - 1 by decreasing pair work: the work buckets (bkt [65], zeroed) into order [n]
+static void bl_row_order(const unsigned long long* work, int n, unsigned* bkt, int* order, cudaStream_t st) {
+  const unsigned g = (unsigned)((n + 255) / 256);
+  k_kp_bucket_count<<<g, 256, 0, st>>>(work, n, bkt);
+  k_kp_bucket_start<<<1, 1, 0, st>>>(bkt);
+  k_kp_bucket_place<<<g, 256, 0, st>>>(work, n, bkt, order);
+}
+
+// the end of a row fit, after its k_*_fit launch: the rows by index, the end event, the pair work and the device time since ev0
+static int bl_fit_end(g4r_baselines* h, const unsigned long long* pairs, int64_t* pair_work, float* device_ms) {
+  CK(bl_sort_rows(h));
+  CK(cudaEventRecord(h->ev1, h->stream));
+  unsigned long long hp = 0;
+  CK(cudaMemcpyAsync(&hp, pairs, sizeof(hp), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
+  if (device_ms) CK(cudaEventElapsedTime(device_ms, h->ev0, h->ev1));
+  if (pair_work) *pair_work = (int64_t)hp;
+  h->ready = true;
   return G4R_OK;
 }
 
@@ -717,14 +816,12 @@ extern "C" int g4r_bl_knn_fit(g4r_baselines* h, const int64_t* session_offsets, 
   if (n_sessions > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_knn_fit: more than 2^31 - 1 sessions");
   int64_t max_len = 0;
   for (int64_t s = 0; s < n_sessions; s++) max_len = std::max(max_len, session_offsets[s + 1] - session_offsets[s]);
-  const size_t per_cta = (size_t)NI * (sizeof(unsigned) + sizeof(int) + sizeof(double));
-  const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)4 * h->n_sm, KF_SCRATCH / per_cta));
-  if (scratch_bytes) *scratch_bytes = per_cta * grid;
-  int cap = 1;                                          // long sessions: one padded session per CTA of k_kp_sort_long
+  const int grid = bl_fit_grid(h, sizeof(unsigned), scratch_bytes);
+  int cap = 1;                                         // long sessions: one padded session per CTA of k_kp_sort_long
   while (cap < max_len) cap <<= 1;
   const int grid_long = max_len > KP_SHORT ? (int)std::max<size_t>(1, std::min<size_t>((size_t)2 * h->n_sm, ((size_t)256 << 20) / ((size_t)cap * 4))) : 0;
   const int64_t S = n_sessions, E = n_events;
-  const unsigned gs = (unsigned)((S + 7) / 8), gi = (unsigned)((NI + 255) / 256);
+  const unsigned gs = (unsigned)((S + 7) / 8);
   const int64_t nbS = (S + SCAN_B - 1) / SCAN_B, nbI = (NI + SCAN_B - 1) / SCAN_B;
   cudaSetDevice(h->device);
   cudaStream_t st = h->stream;
@@ -765,33 +862,16 @@ extern "C" int g4r_bl_knn_fit(g4r_baselines* h, const int64_t* session_offsets, 
     if (grid_long) k_kp_sort_long<<<grid_long, KF_THREADS, 0, st>>>(dOff, dItems, srt, long_list, n_long, scratch, cap);
     k_kp_count<<<gs, 256, 0, st>>>(dOff, S, srt, s_cnt);
   }
-  if (nbS) {
-    k_scan_block<<<(unsigned)nbS, SCAN_B, 0, st>>>(s_cnt, S, s_off, tot);
-    k_scan_tot<<<1, 1, 0, st>>>(tot, nbS);
-    k_scan_add<<<(unsigned)nbS, SCAN_B, 0, st>>>(s_off, S, tot);
-  } else CK(cudaMemsetAsync(s_off, 0, sizeof(long long), st));
+  CK(bl_scan(s_cnt, S, s_off, tot, st));
   if (S > 0) k_kp_emit<<<gs, 256, 0, st>>>(dOff, S, srt, (const int64_t*)s_off, s_item, s_mult, i_cnt, work, pairs);
-  k_scan_block<<<(unsigned)nbI, SCAN_B, 0, st>>>((const long long*)i_cnt, NI, i_off, tot);
-  k_scan_tot<<<1, 1, 0, st>>>(tot, nbI);
-  k_scan_add<<<(unsigned)nbI, SCAN_B, 0, st>>>(i_off, NI, tot);
+  CK(bl_scan((const long long*)i_cnt, NI, i_off, tot, st));
   if (S > 0) k_kp_occ<<<gs, 256, 0, st>>>((const int64_t*)s_off, S, s_item, s_mult, (const int64_t*)i_off, i_fill, i_sess, i_mult);
-  k_kp_bucket_count<<<gi, 256, 0, st>>>(work, NI, bkt);
-  k_kp_bucket_start<<<1, 1, 0, st>>>(bkt);
-  k_kp_bucket_place<<<gi, 256, 0, st>>>(work, NI, bkt, order);
+  bl_row_order(work, NI, bkt, order, st);
   d.s_off = (const int64_t*)s_off; d.s_item = s_item; d.i_off = (const int64_t*)i_off; d.i_sess = i_sess; d.i_mult = i_mult;
   d.order = order; d.next = next; d.n_items = NI; d.n_keep = K;
   d.out_idx = h->dIdx; d.out_sim = h->dSim; d.out_len = h->dLen;
   k_knn_fit<<<grid, KF_THREADS, 0, st>>>(d);
-  k_knn_by_index<<<NI, KF_THREADS, 0, st>>>(h->dIdx, h->dSim, h->dLen, K, h->dIdxI, h->dSimI);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(h->ev1, st));
-  unsigned long long hp = 0;
-  CK(cudaMemcpyAsync(&hp, pairs, sizeof(hp), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (device_ms) CK(cudaEventElapsedTime(device_ms, h->ev0, h->ev1));
-  if (pair_work) *pair_work = (int64_t)hp;
-  h->ready = true;
-  return G4R_OK;
+  return bl_fit_end(h, pairs, pair_work, device_ms);
 }
 
 extern "C" int g4r_bl_set_pop(g4r_baselines* h, const double* scores, int64_t n) {
@@ -858,24 +938,36 @@ extern "C" int g4r_bl_rows_import(g4r_baselines* h, const int32_t* idx, const do
   CK(cudaMemcpyAsync(h->dIdx, idx, rows * sizeof(int), cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(h->dSim, sim, rows * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(h->dLen, len, NI * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  int rc = bl_sort_rows(h);
-  if (rc) return rc;
+  CK(bl_sort_rows(h));
+  CK(cudaStreamSynchronize(h->stream));
   h->ready = true;
   return G4R_OK;
 }
 
-static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                        const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                        const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores, const float* qev);   // g4r_bpr.cuh
-static int narm_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                         double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_narm.cuh
-static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                         const std::vector<int>& mult, const std::vector<int>& cdist, long long wtot, int32_t exclude_seen, int32_t k,
-                         double* recall_sum, double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores);   // g4r_sknn.cuh
+// Pop, SessionPop, ItemKNN, SR and AR: k_bl_rank, warp per session (SR and AR rank as ItemKNN)
+static int bl_rank_list(g4r_baselines* h, BlCall& c) {
+  // competitor weights of the Pop list: prefix sums along (score desc, index asc)
+  std::vector<long long> topW(h->hTop.size() + 1, 0);
+  for (size_t r = 0; r < h->hTop.size(); r++) topW[r + 1] = topW[r] + (c.mult.empty() ? 1 : c.mult[h->hTop[r]]);
+  cudaStream_t st = h->stream;
+  BlEvalDev d = c.bl(h->n_items);
+  d.K = h->n_keep; d.n_top = (int)h->hTop.size();
+  CK(c.bb.take(&d.pl_item, c.n_events));
+  CK(c.bb.take(&d.pl_cnt, c.n_events));
+  CK(c.bb.put(&d.topW, topW.data(), topW.size(), st));
+  d.rIdx = h->dIdx; d.rSim = h->dSim; d.rLen = h->dLen; d.rIdxI = h->dIdxI; d.rSimI = h->dSimI;
+  d.pop = h->dPop; d.top = h->dTop; d.topS = h->dTopS;
+  if (c.n_sessions > 0) {
+    const unsigned grid = (unsigned)((c.n_sessions + 7) / 8);
+    using Fn = void (*)(BlEvalDev, int64_t);
+    static const Fn fns[3][2] = {{k_bl_rank<BL_POP, false>, k_bl_rank<BL_POP, true>},
+                                 {k_bl_rank<BL_SESSIONPOP, false>, k_bl_rank<BL_SESSIONPOP, true>},
+                                 {k_bl_rank<BL_ITEMKNN, false>, k_bl_rank<BL_ITEMKNN, true>}};
+    fns[bl_has_rows(h->kind) ? BL_ITEMKNN : h->kind][c.k > 0]<<<grid, 256, 0, st>>>(d, c.n_sessions);
+    CK(cudaGetLastError());
+  }
+  return G4R_OK;
+}
 
 extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                                const int32_t* n_history, int32_t mode, const int32_t* cut_off, int32_t n_cut, const int32_t* cand,
@@ -891,88 +983,53 @@ extern "C" int g4r_bl_evaluate(g4r_baselines* h, const int32_t* items, int64_t n
   if (!bl_offsets_ok(session_offsets, n_sessions, n_events)) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: session offsets must rise from 0 to n_events");
   const int NI = h->n_items;
   for (int64_t e = 0; e < n_events; e++) if (items[e] < 0 || items[e] >= NI) FAIL(G4R_ERR_INDEX, "g4r_bl_evaluate: item index out of range");
-  std::vector<int> mult, cdist;
-  long long wtot = NI;
+  BlCall c{items, n_events, session_offsets, n_sessions, n_history, mode, k, exclude_seen != 0};
+  c.wtot = NI;
   if (n_cand > 0) {
-    mult.assign(NI, 0);
+    c.mult.assign(NI, 0);
     for (int64_t q = 0; q < n_cand; q++) {
       if (cand[q] < 0 || cand[q] >= NI) FAIL(G4R_ERR_INDEX, "g4r_bl_evaluate: candidate item index out of range");
-      if (mult[cand[q]]++ == 0) cdist.push_back(cand[q]);
+      if (c.mult[cand[q]]++ == 0) c.cdist.push_back(cand[q]);
     }
-    std::sort(cdist.begin(), cdist.end());
-    wtot = n_cand;
+    std::sort(c.cdist.begin(), c.cdist.end());
+    c.wtot = n_cand;
   }
-  const int n_distinct = n_cand > 0 ? (int)cdist.size() : NI;
+  const int n_distinct = n_cand > 0 ? (int)c.cdist.size() : NI;
   if (k < 0 || k > std::min(n_distinct, 1024) || (k > 0 && (!out_items || !out_scores)))
     FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: k must be in 0 .. min(distinct candidates, 1024), with output lists when k > 0");
-  std::vector<int64_t> ev0(n_sessions + 1, 0);
-  for (int64_t s = 0; s < n_sessions; s++) {
-    const int64_t len = session_offsets[s + 1] - session_offsets[s];
-    const int64_t hs = n_history ? n_history[s] : 0;
-    if (hs < 0 || hs > len) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: n_history entry out of range");
-    ev0[s + 1] = ev0[s] + std::max<int64_t>(0, len - std::max<int64_t>(hs, 1));
-  }
-  const int64_t n_ev = ev0[n_sessions];
+  int rc = bl_counted(h, "g4r_bl_evaluate", session_offsets, n_sessions, n_history, c.ev0);
+  if (rc) return rc;
+  const int64_t n_ev = c.n_ev = c.ev0[n_sessions];
   if (n_ev > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: more than 2^31 - 1 counted events");
-  if (h->kind == BL_BPR || h->kind == BL_SKNN || h->kind == BL_STAN || h->kind == BL_VSTAN || h->kind == BL_NARM) {
-    cudaSetDevice(h->device);
-    const int rc = h->kind == BL_BPR ? bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
-                                                    cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores, nullptr)
-                   : h->kind == BL_NARM ? narm_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
-                                                        cdist, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores)
-                                     : sknn_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult,
-                                                     cdist, wtot, exclude_seen, k, recall_sum, mrr_sum, out_counts, out_items, out_scores);
-    if (rc == G4R_OK && n_counted) *n_counted = n_ev;
-    return rc;
-  }
-  // competitor weights of the Pop list: prefix sums along (score desc, index asc)
-  std::vector<long long> topW(h->hTop.size() + 1, 0);
-  for (size_t r = 0; r < h->hTop.size(); r++) topW[r + 1] = topW[r] + (n_cand > 0 ? mult[h->hTop[r]] : 1);
   cudaSetDevice(h->device);
   cudaStream_t st = h->stream;
-  BlBufs bb;
-  BlEvalDev d{};
-  d.n_items = NI; d.K = h->n_keep; d.n_top = (int)h->hTop.size(); d.mode = mode; d.k = k; d.exclude = exclude_seen != 0;
-  const int* dCut = nullptr; double* dSums = nullptr;
-  CK(bb.put(&d.items, items, n_events, st));
-  CK(bb.put(&d.off, session_offsets, n_sessions + 1, st));
-  if (n_history) CK(bb.put(&d.nh, n_history, n_sessions, st));
-  CK(bb.put(&d.ev0, ev0.data(), n_sessions, st));
-  CK(bb.take(&d.pl_item, n_events));
-  CK(bb.take(&d.pl_cnt, n_events));
-  CK(bb.put(&d.topW, topW.data(), topW.size(), st));
+  CK(c.bb.put(&c.d_items, items, n_events, st));
+  CK(c.bb.put(&c.d_off, session_offsets, n_sessions + 1, st));
+  if (n_history) CK(c.bb.put(&c.d_nh, n_history, n_sessions, st));
+  CK(c.bb.put(&c.d_ev0, c.ev0.data(), n_sessions + 1, st));
   if (n_cand > 0) {
-    CK(bb.put(&d.mult, mult.data(), mult.size(), st));
-    CK(bb.put(&d.cdist, cdist.data(), cdist.size(), st));
-    d.n_cdist = (int)cdist.size();
+    CK(c.bb.put(&c.d_mult, c.mult.data(), c.mult.size(), st));
+    CK(c.bb.put(&c.d_cdist, c.cdist.data(), c.cdist.size(), st));
   }
-  d.wtot = wtot;
-  d.rIdx = h->dIdx; d.rSim = h->dSim; d.rLen = h->dLen; d.rIdxI = h->dIdxI; d.rSimI = h->dSimI;
-  d.pop = h->dPop; d.top = h->dTop; d.topS = h->dTopS;
-  CK(bb.take(&d.counts, (size_t)2 * n_ev));
-  if (k) { CK(bb.take(&d.out_items, (size_t)n_ev * k)); CK(bb.take(&d.out_scores, (size_t)n_ev * k)); }
-  CK(bb.put(&dCut, cut_off, n_cut, st));
-  CK(bb.take(&dSums, 128));
-  if (n_sessions > 0) {
-    const unsigned grid = (unsigned)((n_sessions + 7) / 8);
-    using Fn = void (*)(BlEvalDev, int64_t);
-    static const Fn fns[3][2] = {{k_bl_rank<BL_POP, false>, k_bl_rank<BL_POP, true>},
-                                 {k_bl_rank<BL_SESSIONPOP, false>, k_bl_rank<BL_SESSIONPOP, true>},
-                                 {k_bl_rank<BL_ITEMKNN, false>, k_bl_rank<BL_ITEMKNN, true>}};
-    fns[bl_has_rows(h->kind) ? BL_ITEMKNN : h->kind][k > 0]<<<grid, 256, 0, st>>>(d, n_sessions);   // SR and AR rank as ItemKNN
-    CK(cudaGetLastError());
-  }
-  k_bl_sums<<<1, 1024, 0, st>>>(d.counts, n_ev, dCut, n_cut, mode, dSums);
+  CK(c.bb.take(&c.counts, (size_t)2 * n_ev));
+  if (k) { CK(c.bb.take(&c.out_items, (size_t)n_ev * k)); CK(c.bb.take(&c.out_scores, (size_t)n_ev * k)); }
+  rc = BL_KINDS[h->kind].rank(h, c);
+  if (rc) return rc;
+  // every kind: Recall / MRR from the counts, and the outputs
+  const int* dCut = nullptr; double* dSums = nullptr;
+  CK(c.bb.put(&dCut, cut_off, n_cut, st));
+  CK(c.bb.take(&dSums, 128));
+  k_bl_sums<<<1, 1024, 0, st>>>(c.counts, n_ev, dCut, n_cut, mode, dSums);
   CK(cudaGetLastError());
   std::vector<double> sums(2 * n_cut);
   CK(cudaMemcpyAsync(sums.data(), dSums, 2 * n_cut * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (out_counts && n_ev) CK(cudaMemcpyAsync(out_counts, d.counts, (size_t)2 * n_ev * sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (out_counts && n_ev) CK(cudaMemcpyAsync(out_counts, c.counts, (size_t)2 * n_ev * sizeof(int), cudaMemcpyDeviceToHost, st));
   if (k && n_ev) {
-    CK(cudaMemcpyAsync(out_items, d.out_items, (size_t)n_ev * k * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(out_scores, d.out_scores, (size_t)n_ev * k * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(out_items, c.out_items, (size_t)n_ev * k * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(out_scores, c.out_scores, (size_t)n_ev * k * sizeof(double), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
-  for (int c = 0; c < n_cut; c++) { recall_sum[c] = sums[c]; mrr_sum[c] = sums[n_cut + c]; }
+  for (int q = 0; q < n_cut; q++) { recall_sum[q] = sums[q]; mrr_sum[q] = sums[n_cut + q]; }
   if (n_counted) *n_counted = n_ev;
   return G4R_OK;
 }

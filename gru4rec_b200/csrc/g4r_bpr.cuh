@@ -611,42 +611,31 @@ extern "C" int g4r_bl_bpr_import(g4r_baselines* h, const double* I, const double
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a BPR, after its argument checks: the counted events in blocks of bounded scratch.  qev (NARM): the
-// counted events' vectors [n_ev x F] on the device, which replace the session means
-static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                        const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                        const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                        double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores, const float* qev) {
+// BPR's ranking of a g4r_bl_evaluate call: the counted events in blocks of bounded scratch.  qev (NARM): the counted events'
+// vectors [n_ev x F] on the device, which replace the session means
+static int bpr_blocks(g4r_baselines* h, BlCall& c, const float* qev) {
   const int NI = h->n_items, F = h->n_keep;
-  const int64_t n_ev = ev0[n_sessions];
+  const int64_t n_ev = c.n_ev, n_sessions = c.n_sessions;
   cudaStream_t st = h->stream;
-  BlBufs bb;
   BprEvalDev d{};
-  d.I = h->dI; d.bI = h->dBI; d.F = F; d.n_items = NI; d.mode = mode; d.exclude = exclude_seen != 0; d.k = k;
-  CK(bb.put(&d.items, items, n_events, st));
-  CK(bb.put(&d.off, session_offsets, n_sessions + 1, st));
-  if (n_history) CK(bb.put(&d.nh, n_history, n_sessions, st));
-  CK(bb.put(&d.ev0, ev0.data(), n_sessions + 1, st));
-  d.n_comp = NI;
-  if (!cdist.empty()) {
-    CK(bb.put(&d.mult, mult.data(), mult.size(), st));
-    CK(bb.put(&d.comp, cdist.data(), cdist.size(), st));
-    d.n_comp = (int)cdist.size();
-  }
+  d.I = h->dI; d.bI = h->dBI; d.F = F; d.n_items = NI; d.mode = c.mode; d.exclude = c.exclude; d.k = c.k;
+  d.items = c.d_items; d.off = c.d_off; d.nh = c.d_nh; d.ev0 = c.d_ev0;
+  d.mult = c.d_mult; d.comp = c.d_cdist; d.n_comp = c.cdist.empty() ? NI : (int)c.cdist.size();
   unsigned char* first = nullptr;
   if (d.exclude) {
-    CK(bb.take(&first, n_events));
+    CK(c.bb.take(&first, c.n_events));
     if (n_sessions > 0) k_bpr_first<<<(unsigned)((n_sessions + 7) / 8), 256, 0, st>>>(d.items, d.off, n_sessions, first);
     d.first = first;
   }
-  CK(bb.take(&d.counts, (size_t)2 * n_ev));
+  d.counts = c.counts; d.out_items = c.out_items; d.out_scores = c.out_scores;
   CK(cudaMemsetAsync(d.counts, 0, (size_t)2 * n_ev * sizeof(int), st));
-  if (k) { CK(bb.take(&d.out_items, (size_t)n_ev * k)); CK(bb.take(&d.out_scores, (size_t)n_ev * k)); }
+  const int k = c.k;
   int64_t blk = std::max<int64_t>(1, std::min<int64_t>(65536, (int64_t)(BPR_SCRATCH / ((size_t)8 * F))));
   if (k) blk = std::max<int64_t>(1, std::min<int64_t>(blk, (int64_t)(BPR_SCRATCH / ((size_t)8 * d.n_comp))));
   blk = std::min<int64_t>(blk, std::max<int64_t>(n_ev, 1));
-  CK(bb.take(&d.uvec, (size_t)blk * F)); CK(bb.take(&d.pos, blk)); CK(bb.take(&d.st, blk)); CK(bb.take(&d.tsc, blk));
-  if (k) CK(bb.take(&d.scores, (size_t)blk * d.n_comp));
+  CK(c.bb.take(&d.uvec, (size_t)blk * F)); CK(c.bb.take(&d.pos, blk)); CK(c.bb.take(&d.st, blk)); CK(c.bb.take(&d.tsc, blk));
+  if (k) CK(c.bb.take(&d.scores, (size_t)blk * d.n_comp));
+  const std::vector<int64_t>& ev0 = c.ev0;
   const int n_tiles = (d.n_comp + BT_J - 1) / BT_J;
   for (int64_t E0 = 0; E0 < n_ev; E0 += blk) {
     const int nb = (int)std::min<int64_t>(blk, n_ev - E0);
@@ -670,19 +659,7 @@ static int bpr_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events
     if (k) k_bpr_select<<<nb, KF_THREADS, 0, st>>>(d);
     CK(cudaGetLastError());
   }
-  const int* dCut = nullptr; double* dSums = nullptr;
-  CK(bb.put(&dCut, cut_off, n_cut, st));
-  CK(bb.take(&dSums, 128));
-  k_bl_sums<<<1, 1024, 0, st>>>(d.counts, n_ev, dCut, n_cut, mode, dSums);
-  CK(cudaGetLastError());
-  std::vector<double> sums(2 * n_cut);
-  CK(cudaMemcpyAsync(sums.data(), dSums, 2 * n_cut * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (out_counts && n_ev) CK(cudaMemcpyAsync(out_counts, d.counts, (size_t)2 * n_ev * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (k && n_ev) {
-    CK(cudaMemcpyAsync(out_items, d.out_items, (size_t)n_ev * k * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(out_scores, d.out_scores, (size_t)n_ev * k * sizeof(double), cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  for (int c = 0; c < n_cut; c++) { recall_sum[c] = sums[c]; mrr_sum[c] = sums[n_cut + c]; }
   return G4R_OK;
 }
+
+static int bpr_rank(g4r_baselines* h, BlCall& c) { return bpr_blocks(h, c, nullptr); }

@@ -1,8 +1,8 @@
 // g4r_narm.cuh -- the NARM neural session baseline on the device (DESIGN §3s): a GRU encoder with NARM's item-level attention,
 // a bilinear decoder against the item table and full-catalogue cross-entropy, trained with dense Adam; and the eval-mode encoder
-// that feeds bpr_evaluate's per-event vectors.  Every reduction runs in a fixed order (no floating-point atomics), so a fit is
+// that feeds per-event vectors to BPR's ranking.  Every reduction runs in a fixed order (no floating-point atomics), so a fit is
 // bitwise reproducible and independent of grid sizes.  Included at the end of g4r_lib.cu after g4r_bpr.cuh (BprEvalDev,
-// bpr_evaluate) and g4r_kernels.cuh (drop_scale).
+// bpr_blocks) and g4r_kernels.cuh (drop_scale).
 #pragma once
 
 constexpr int NM_BM = 64, NM_BN = 64, NM_BK = 16;       // product tile: rows x columns x k per shared-memory stage
@@ -478,7 +478,7 @@ static bool nm_finite(const float* v, size_t n) {
   return true;
 }
 
-// the model buffers of a NARM handle: parameters, double(E) and zero biases for bpr_evaluate, a device 1.0f
+// the model buffers of a NARM handle: parameters, double(E) and zero biases for bpr_blocks, a device 1.0f
 static int nm_set_model(g4r_baselines* h, int32_t hidden, int32_t max_len, const float* params, int64_t n_params, const char* who) {
   if (!params) FAIL(G4R_ERR_INVALID, std::string(who) + ": null parameters");
   if (hidden < 1 || hidden > NM_H_MAX || max_len < 2 || max_len > NM_LEN_MAX)
@@ -758,35 +758,27 @@ extern "C" int g4r_bl_narm_encode(g4r_baselines* h, const int32_t* items, int64_
     FAIL(G4R_ERR_INVALID, "g4r_bl_narm_encode: null or out-of-range argument");
   if (!bl_offsets_ok(session_offsets, n_sessions, n_events)) FAIL(G4R_ERR_INVALID, "g4r_bl_narm_encode: session offsets must rise from 0 to n_events");
   for (int64_t e = 0; e < n_events; e++) if (items[e] < 0 || items[e] >= h->n_items) FAIL(G4R_ERR_INDEX, "g4r_bl_narm_encode: item index out of range");
-  std::vector<int64_t> ev0(n_sessions + 1, 0);
-  for (int64_t s = 0; s < n_sessions; s++) {
-    const int64_t len = session_offsets[s + 1] - session_offsets[s], hs = n_history ? n_history[s] : 0;
-    if (hs < 0 || hs > len) FAIL(G4R_ERR_INVALID, "g4r_bl_narm_encode: n_history entry out of range");
-    ev0[s + 1] = ev0[s] + std::max<int64_t>(0, len - std::max<int64_t>(hs, 1));
-  }
+  std::vector<int64_t> ev0;
+  int rc = bl_counted(h, "g4r_bl_narm_encode", session_offsets, n_sessions, n_history, ev0);
+  if (rc) return rc;
   if (n_q != ev0[n_sessions]) FAIL(G4R_ERR_INVALID, "g4r_bl_narm_encode: n_q must be the number of counted events");
   if (n_q > INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_narm_encode: more than 2^31 - 1 counted events");
   cudaSetDevice(h->device);
   BlBufs bb;
   float* dq = nullptr;
   CK(bb.take(&dq, (size_t)n_q * h->n_keep));
-  const int rc = nm_encode_events(h, items, n_events, session_offsets, n_sessions, n_history, ev0, dq);
+  rc = nm_encode_events(h, items, n_events, session_offsets, n_sessions, n_history, ev0, dq);
   if (rc) return rc;
   if (n_q) CK(cudaMemcpyAsync(q, dq, (size_t)n_q * h->n_keep * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a NARM, after its argument checks: every counted event's q, then BPR's ranking with I = double(E), bI = 0
-static int narm_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                         const std::vector<int>& mult, const std::vector<int>& cdist, int32_t exclude_seen, int32_t k, double* recall_sum,
-                         double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores) {
-  BlBufs bb;
+// the ranking of a g4r_bl_evaluate call of a NARM: every counted event's q, then BPR's ranking with I = double(E), bI = 0
+static int narm_rank(g4r_baselines* h, BlCall& c) {
   float* dq = nullptr;
-  CK(bb.take(&dq, (size_t)ev0[n_sessions] * h->n_keep));
-  const int rc = nm_encode_events(h, items, n_events, session_offsets, n_sessions, n_history, ev0, dq);
+  CK(c.bb.take(&dq, (size_t)c.n_ev * h->n_keep));
+  const int rc = nm_encode_events(h, c.items, c.n_events, c.off, c.n_sessions, c.n_history, c.ev0, dq);
   if (rc) return rc;
-  return bpr_evaluate(h, items, n_events, session_offsets, n_sessions, n_history, ev0, mode, cut_off, n_cut, mult, cdist, exclude_seen, k,
-                      recall_sum, mrr_sum, out_counts, out_items, out_scores, dq);
+  return bpr_blocks(h, c, dq);
 }

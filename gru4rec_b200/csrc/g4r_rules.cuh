@@ -1,7 +1,7 @@
 // g4r_rules.cuh -- the rule-based session baselines on the device (DESIGN §3q): sequential rules (SR) and association rules (AR).
 // The fit counts, per item i, the weighted pairs (i, j) of the training sessions in uint64 and keeps each row's `pruning` largest
 // weights in ItemKNN's row layout; g4r_bl_evaluate ranks SR / AR handles with the ItemKNN instance of k_bl_rank.  Included from
-// g4r_lib.cu after g4r_baselines.cuh (KF_*, k_scan_*, k_kp_bucket_*, bl_keep_row, k_knn_by_index, the handle).
+// g4r_lib.cu after g4r_baselines.cuh (KF_*, bl_fit_grid, bl_scan, bl_row_order, bl_keep_row, bl_fit_end, the handle).
 #pragma once
 
 constexpr int RULES_STEPS_MAX = 20;
@@ -126,12 +126,9 @@ extern "C" int g4r_bl_rules_fit(g4r_baselines* h, const int64_t* session_offsets
       bound[items[e]] += ar ? (unsigned __int128)(session_offsets[s + 1] - session_offsets[s]) : per;
   for (int i = 0; i < NI; i++)
     if (bound[i] >= ((unsigned __int128)1 << 63)) FAIL(G4R_ERR_INVALID, "g4r_bl_rules_fit: a row's weight bound reaches 2^63 (uint64 counts could overflow)");
-  const size_t per_cta = (size_t)NI * (sizeof(unsigned long long) + sizeof(int) + sizeof(double));
-  const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)4 * h->n_sm, KF_SCRATCH / per_cta));
-  if (scratch_bytes) *scratch_bytes = per_cta * grid;
+  const int grid = bl_fit_grid(h, sizeof(unsigned long long), scratch_bytes);
   const int64_t S = n_sessions, E = n_events;
-  const unsigned gs = (unsigned)((S + 7) / 8), gi = (unsigned)((NI + 255) / 256), ge = (unsigned)((E + 255) / 256);
-  const int64_t nbI = (NI + SCAN_B - 1) / SCAN_B;
+  const unsigned gs = (unsigned)((S + 7) / 8), ge = (unsigned)((E + 255) / 256);
   cudaSetDevice(h->device);
   cudaStream_t st = h->stream;
   BlBufs bb;
@@ -144,7 +141,7 @@ extern "C" int g4r_bl_rules_fit(g4r_baselines* h, const int64_t* session_offsets
   CK(bb.put(&dItems, items, E, st));
   CK(bb.put(&dOff, session_offsets, S + 1, st));
   CK(bb.take(&ev_sess, E)); CK(bb.take(&i_pos, E));
-  CK(bb.take(&i_cnt, NI)); CK(bb.take(&work, NI)); CK(bb.take(&pairs, 1)); CK(bb.take(&i_off, NI + 1)); CK(bb.take(&tot, nbI));
+  CK(bb.take(&i_cnt, NI)); CK(bb.take(&work, NI)); CK(bb.take(&pairs, 1)); CK(bb.take(&i_off, NI + 1)); CK(bb.take(&tot, (NI + SCAN_B - 1) / SCAN_B));
   CK(bb.take(&i_fill, NI)); CK(bb.take(&bkt, 65)); CK(bb.take(&order, NI)); CK(bb.take(&next, 1));
   CK(bb.take(&d.acc, (size_t)NI * grid));
   CK(bb.take(&d.touched, (size_t)NI * grid));
@@ -164,27 +161,14 @@ extern "C" int g4r_bl_rules_fit(g4r_baselines* h, const int64_t* session_offsets
     if (ar) k_rules_events<true><<<gs, 256, 0, st>>>(dOff, S, dItems, steps, ev_sess, i_cnt, work, pairs);
     else k_rules_events<false><<<gs, 256, 0, st>>>(dOff, S, dItems, steps, ev_sess, i_cnt, work, pairs);
   }
-  k_scan_block<<<(unsigned)nbI, SCAN_B, 0, st>>>((const long long*)i_cnt, NI, i_off, tot);
-  k_scan_tot<<<1, 1, 0, st>>>(tot, nbI);
-  k_scan_add<<<(unsigned)nbI, SCAN_B, 0, st>>>(i_off, NI, tot);
+  CK(bl_scan((const long long*)i_cnt, NI, i_off, tot, st));
   if (E > 0) k_rules_place<<<ge, 256, 0, st>>>(dItems, E, (const int64_t*)i_off, i_fill, i_pos);
-  k_kp_bucket_count<<<gi, 256, 0, st>>>(work, NI, bkt);
-  k_kp_bucket_start<<<1, 1, 0, st>>>(bkt);
-  k_kp_bucket_place<<<gi, 256, 0, st>>>(work, NI, bkt, order);
+  bl_row_order(work, NI, bkt, order, st);
   d.off = dOff; d.items = dItems; d.ev_sess = ev_sess; d.i_off = (const int64_t*)i_off; d.i_pos = i_pos;
   d.order = order; d.next = next; d.n_items = NI; d.n_keep = K; d.steps = steps; d.L = (double)L;
   for (int q = 1; q <= RULES_STEPS_MAX; q++) d.inc[q] = (!ar && weighting == 0) ? L / (unsigned long long)q : 1ull;
   d.out_idx = h->dIdx; d.out_sim = h->dSim; d.out_len = h->dLen;
   if (ar) k_rules_fit<true><<<grid, KF_THREADS, 0, st>>>(d);
   else k_rules_fit<false><<<grid, KF_THREADS, 0, st>>>(d);
-  k_knn_by_index<<<NI, KF_THREADS, 0, st>>>(h->dIdx, h->dSim, h->dLen, K, h->dIdxI, h->dSimI);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(h->ev1, st));
-  unsigned long long hp = 0;
-  CK(cudaMemcpyAsync(&hp, pairs, sizeof(hp), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (device_ms) CK(cudaEventElapsedTime(device_ms, h->ev0, h->ev1));
-  if (pair_work) *pair_work = (int64_t)hp;
-  h->ready = true;
-  return G4R_OK;
+  return bl_fit_end(h, pairs, pair_work, device_ms);
 }

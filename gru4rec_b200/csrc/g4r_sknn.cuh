@@ -468,13 +468,13 @@ extern "C" int g4r_bl_vstan_set(g4r_baselines* h, int32_t similarity, const doub
   return G4R_OK;
 }
 
-// g4r_bl_evaluate of a SessionKNN, a STAN or a VSTAN, after its argument checks: resident CTAs over the counted events, each with its own slices of
-// a global scratch of at most SK_SCRATCH bytes (fewer CTAs when the slices are large; one at least)
-static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
-                         const int32_t* n_history, const std::vector<int64_t>& ev0, int32_t mode, const int32_t* cut_off, int32_t n_cut,
-                         const std::vector<int>& mult, const std::vector<int>& cdist, long long wtot, int32_t exclude_seen, int32_t k,
-                         double* recall_sum, double* mrr_sum, int32_t* out_counts, int32_t* out_items, double* out_scores) {
-  const int64_t n_ev = ev0[n_sessions];
+// the ranking of a g4r_bl_evaluate call of a SessionKNN, a STAN or a VSTAN: resident CTAs over the counted events, each with its own
+// slices of a global scratch of at most SK_SCRATCH bytes (fewer CTAs when the slices are large; one at least)
+static int sknn_rank(g4r_baselines* h, BlCall& c) {
+  const int64_t n_ev = c.n_ev, n_sessions = c.n_sessions;
+  const int64_t* session_offsets = c.off;
+  const std::vector<int64_t>& ev0 = c.ev0;
+  const int k = c.k;
   int64_t max_len = 1;
   for (int64_t s = 0; s < n_sessions; s++) max_len = std::max(max_len, session_offsets[s + 1] - session_offsets[s]);
   if (max_len > (1 << 30) || h->sk_zmax > (1 << 30)) FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a session or the neighbours' items exceed 2^30 entries");
@@ -488,21 +488,9 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
         FAIL(G4R_ERR_INVALID, "g4r_bl_evaluate: a counted event's prefix is longer than the VSTAN W4 table (g4r_bl_vstan_set)");
     }
   cudaStream_t st = h->stream;
-  BlBufs bb;
+  BlBufs& bb = c.bb;
   SknnEvalDev d{};
-  BlEvalDev& b = d.bl;
-  b.n_items = h->n_items; b.mode = mode; b.k = k; b.exclude = exclude_seen != 0; b.wtot = wtot;
-  CK(bb.put(&b.items, items, n_events, st));
-  CK(bb.put(&b.off, session_offsets, n_sessions + 1, st));
-  if (n_history) CK(bb.put(&b.nh, n_history, n_sessions, st));
-  CK(bb.put(&b.ev0, ev0.data(), n_sessions + 1, st));
-  if (!cdist.empty()) {
-    CK(bb.put(&b.mult, mult.data(), mult.size(), st));
-    CK(bb.put(&b.cdist, cdist.data(), cdist.size(), st));
-    b.n_cdist = (int)cdist.size();
-  }
-  CK(bb.take(&b.counts, (size_t)2 * n_ev));
-  if (k) { CK(bb.take(&b.out_items, (size_t)n_ev * k)); CK(bb.take(&b.out_scores, (size_t)n_ev * k)); }
+  d.bl = c.bl(h->n_items);
   d.n_ev = n_ev; d.n_sess = n_sessions;
   d.s_off = h->dSkOff; d.s_item = h->dSkItem; d.i_off = h->dSkIoff; d.i_sess = h->dSkIsess;
   d.sample = h->sk_sample; d.sim = h->sk_sim; d.nbr = h->n_keep;
@@ -530,19 +518,5 @@ static int sknn_evaluate(g4r_baselines* h, const int32_t* items, int64_t n_event
     kern<<<(unsigned)grid, SK_THREADS, smem, st>>>(d);
     CK(cudaGetLastError());
   }
-  const int* dCut = nullptr; double* dSums = nullptr;
-  CK(bb.put(&dCut, cut_off, n_cut, st));
-  CK(bb.take(&dSums, 128));
-  k_bl_sums<<<1, 1024, 0, st>>>(b.counts, n_ev, dCut, n_cut, mode, dSums);
-  CK(cudaGetLastError());
-  std::vector<double> sums(2 * n_cut);
-  CK(cudaMemcpyAsync(sums.data(), dSums, 2 * n_cut * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (out_counts && n_ev) CK(cudaMemcpyAsync(out_counts, b.counts, (size_t)2 * n_ev * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (k && n_ev) {
-    CK(cudaMemcpyAsync(out_items, b.out_items, (size_t)n_ev * k * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(out_scores, b.out_scores, (size_t)n_ev * k * sizeof(double), cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  for (int c = 0; c < n_cut; c++) { recall_sum[c] = sums[c]; mrr_sum[c] = sums[n_cut + c]; }
   return G4R_OK;
 }
