@@ -54,6 +54,8 @@ EXPORTS = [
     'g4r_bl_rows_import', 'g4r_bl_evaluate', 'g4r_bl_bpr_begin', 'g4r_bl_bpr_iterate', 'g4r_bl_bpr_export', 'g4r_bl_bpr_import',
     'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit', 'g4r_bl_vstan_set',
     'g4r_bl_narm_begin', 'g4r_bl_narm_epoch', 'g4r_bl_narm_grads', 'g4r_bl_narm_export', 'g4r_bl_narm_import', 'g4r_bl_narm_encode',
+    'g4r_bl_sasrec_begin', 'g4r_bl_sasrec_epoch', 'g4r_bl_sasrec_grads', 'g4r_bl_sasrec_export', 'g4r_bl_sasrec_import',
+    'g4r_bl_sasrec_encode',
 ]
 
 _lib = None
@@ -167,6 +169,12 @@ def load():
     lib.g4r_bl_narm_export.argtypes = [vp, vp, i64]
     lib.g4r_bl_narm_import.argtypes = [vp, i32, i32, vp, i64]
     lib.g4r_bl_narm_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
+    lib.g4r_bl_sasrec_begin.argtypes = [vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_sasrec_epoch.argtypes = [vp, vp, i64, u32, f32, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_sasrec_grads.argtypes = [vp, vp, i32, u32, i64, f32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_sasrec_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_sasrec_import.argtypes = [vp, i32, i32, i32, vp, i64]
+    lib.g4r_bl_sasrec_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -791,7 +799,7 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -826,8 +834,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM fit and parameters (DESIGN §3s).  kind: 'pop', 'sessionpop',
-    'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan' or 'narm'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM and SASRec fits and parameters (DESIGN §3s, §3t).  kind: 'pop',
+    'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm' or 'sasrec'; n_keep: top_n, n_sims, n_factors, k,
+    pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1079,4 +1088,61 @@ class Baselines(object):
         n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
         q = np.empty((n, self.n_keep), np.float32)
         self._check(self.lib.g4r_bl_narm_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q
+
+    # ---- SASRec (DESIGN §3t) ----
+    def sasrec_n_params(self, n_blocks, max_len):
+        d = self.n_keep
+        return self.n_items * d + int(max_len) * d + int(n_blocks) * (6 * d * d + 10 * d) + 2 * d
+
+    def _sasrec_params(self, n_blocks, max_len, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        n = self.sasrec_n_params(n_blocks, max_len)
+        if th.size != n:
+            raise ValueError('sasrec: need %d parameters (n_items d + max_len d + n_blocks (6 d^2 + 10 d) + 2 d), not %d' % (n, th.size))
+        return th
+
+    def sasrec_begin(self, n_blocks, n_heads, max_len, batch_size, piece_offsets, items, params):
+        """starts a SASRec fit: the training pieces (CSR of item indices, 2 .. max_len + 1 events each) and the initial flat
+        parameters"""
+        off = np.ascontiguousarray(piece_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._sasrec_params(n_blocks, max_len, params)
+        self._check(self.lib.g4r_bl_sasrec_begin(self.h, int(n_blocks), int(n_heads), int(max_len), int(batch_size), _ptr(off), off.size - 1,
+                                                 _ptr(it), it.size, _ptr(th), th.size))
+        self.sasrec_shape, self.sasrec_batch = (int(n_blocks), int(max_len)), int(batch_size)
+
+    def sasrec_epoch(self, order, seed, learning_rate, dropout):
+        """one epoch over the pieces in `order`; returns (per-step losses float32, device ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32)
+        losses = np.zeros(-(-od.size // self.sasrec_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_sasrec_epoch(self.h, _ptr(od), od.size, int(seed) & 0xffffffff, float(learning_rate), float(dropout),
+                                                 _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def sasrec_grads(self, pieces, seed, step, dropout):
+        """(loss, flat gradient float32) of one mini-batch of pieces at the current parameters, without an update"""
+        pc = np.ascontiguousarray(pieces, dtype=np.int32)
+        g = np.empty(self.sasrec_n_params(*self.sasrec_shape), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_sasrec_grads(self.h, _ptr(pc), pc.size, int(seed) & 0xffffffff, int(step), float(dropout), C.byref(loss),
+                                                 _ptr(g)))
+        return loss.value, g
+
+    def sasrec_export(self):
+        th = np.empty(self.sasrec_n_params(*self.sasrec_shape), np.float32)
+        self._check(self.lib.g4r_bl_sasrec_export(self.h, _ptr(th), th.size))
+        return th
+
+    def sasrec_import(self, n_blocks, n_heads, max_len, params):
+        th = self._sasrec_params(n_blocks, max_len, params)
+        self._check(self.lib.g4r_bl_sasrec_import(self.h, int(n_blocks), int(n_heads), int(max_len), _ptr(th), th.size))
+        self.sasrec_shape = (int(n_blocks), int(max_len))
+
+    def sasrec_encode(self, items, session_offsets, n_history=None):
+        """every counted event's q [n, d] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_sasrec_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
         return q

@@ -1,7 +1,7 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
-§3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s, trained
-on the device) with the same surface.  ItemKNN's fit runs on the device (the
+§3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s) and SASRec
+(§3t), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -786,6 +786,184 @@ class NARM(Baseline):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
         p = self.params64()
         return p['E'] @ narm_encode(p, list(prefix)[-self.max_len:])
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+SASREC_BLOCK = ('g1', 'c1', 'Wq', 'bq', 'Wk', 'bk', 'Wv', 'bv', 'Wo', 'bo', 'g2', 'c2', 'W1', 'b1', 'W2', 'b2')
+SASREC_LN_EPS = 1e-8
+
+
+def sasrec_shapes(n_items, d, n_blocks, max_len):
+    """the parameters in the order of the flat vector (DESIGN §3t): E, Pe, per block b the SASREC_BLOCK names with suffix _b
+    (W*: [d x d], the rest [d]), gf, cf"""
+    out = dict(E=(n_items, d), Pe=(max_len, d))
+    for b in range(n_blocks):
+        for name in SASREC_BLOCK:
+            out['%s_%d' % (name, b)] = (d, d) if name[0] == 'W' else (d,)
+    out['gf'], out['cf'] = (d,), (d,)
+    return out
+
+
+def sasrec_unpack(flat, n_items, d, n_blocks, max_len):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in sasrec_shapes(n_items, d, n_blocks, max_len).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def sasrec_init(n_items, d, n_blocks, max_len, rs):
+    """the initial parameters, float32 flat: in the order of the vector each matrix [r x c] (E and Pe included) drawn from
+    rs.uniform(-s, s) with s = sqrt(6 / (r + c)); biases 0 and gains 1, without draws"""
+    parts = []
+    for name, shp in sasrec_shapes(n_items, d, n_blocks, max_len).items():
+        if len(shp) == 2:
+            s = np.sqrt(6.0 / (shp[0] + shp[1]))
+            parts.append(rs.uniform(-s, s, size=shp))
+        else:
+            parts.append(np.full(shp, 1.0 if name[0] == 'g' else 0.0))
+    return np.concatenate([p.ravel() for p in parts]).astype(np.float32)
+
+
+def sasrec_scales(d, n_heads):
+    """(s_d, s_h): the float32 of sqrt(d) and of 1 / sqrt(d / n_heads), as float64"""
+    return float(np.float32(np.sqrt(float(d)))), float(np.float32(1.0 / np.sqrt(float(d // n_heads))))
+
+
+def _layer_norm(x, g, c):
+    mu = x.mean(axis=-1, keepdims=True)
+    var = ((x - mu) ** 2).mean(axis=-1, keepdims=True)
+    return g * (x - mu) / np.sqrt(var + SASREC_LN_EPS) + c
+
+
+def sasrec_encode(p, x, n_heads):
+    """q (float64) of the inputs x (item indices, oldest first, at most max_len) in eval mode: p maps the parameter names to
+    float64 arrays"""
+    d = p['E'].shape[1]
+    dh = d // n_heads
+    sd, sh = sasrec_scales(d, n_heads)
+    n = len(x)
+    h = p['E'][list(x)] * sd + p['Pe'][:n]
+    causal = np.tril(np.ones((n, n), bool))
+    b = 0
+    while 'g1_%d' % b in p:
+        w = {name: p['%s_%d' % (name, b)] for name in SASREC_BLOCK}
+        u = _layer_norm(h, w['g1'], w['c1'])
+        Q, K, V = u @ w['Wq'] + w['bq'], u @ w['Wk'] + w['bk'], u @ w['Wv'] + w['bv']
+        A = np.empty_like(h)
+        for k in range(n_heads):
+            cs = slice(k * dh, (k + 1) * dh)
+            S = np.where(causal, (Q[:, cs] @ K[:, cs].T) * sh, -np.inf)
+            P = np.exp(S - S.max(axis=1, keepdims=True))
+            A[:, cs] = (P / P.sum(axis=1, keepdims=True)) @ V[:, cs]
+        a = h + A @ w['Wo'] + w['bo']
+        h = a + np.maximum(_layer_norm(a, w['g2'], w['c2']) @ w['W1'] + w['b1'], 0.0) @ w['W2'] + w['b2']
+        b += 1
+    return _layer_norm(h[-1], p['gf'], p['cf'])
+
+
+class SASRec(Baseline):
+    '''
+    SASRec(embedding=50, n_blocks=2, n_heads=1, n_epochs=10, batch_size=128, learning_rate=0.001, dropout=0.2, max_len=50, seed=42,
+           session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Self-attentive sequential recommender in the style of SASRec (Kang & McAuley, ICDM 2018), trained on the device with
+    full-catalogue cross-entropy and Adam.  This is this project's definition (DESIGN §3t); no parity with another framework is
+    claimed.
+
+    One item table E [n_items x embedding] is the input embedding and the output item side.  For the last max_len inputs x_0 ..
+    x_(n-1) of a session prefix: h_t = E[x_t] sqrt(d) + Pe[t]; n_blocks pre-LN Transformer blocks, each causal multi-head
+    attention (n_heads heads) and a position-wise ReLU FFN with residuals; q_t = LN(h_t) and item i scores E[i] . q.  Training
+    cuts each session (events by time_key, ties by row order) into pieces of at most max_len + 1 events overlapping by one,
+    encodes each piece causally, and per mini-batch of batch_size pieces takes one Adam step on the mean cross-entropy over its
+    positions, with dropout on h0 and on both residual branches of every block.  The parameters are float32 and drawn, like the
+    epochs' piece orders, from np.random.RandomState(seed).  fit prints the epoch's mean loss; `fit_stats` holds per epoch (mean
+    loss, device ms, per-step losses).  predict_next computes the scores on the host in float64 from the float32 parameters.
+    '''
+    _kind = 'sasrec'
+
+    def __init__(self, embedding=50, n_blocks=2, n_heads=1, n_epochs=10, batch_size=128, learning_rate=0.001, dropout=0.2, max_len=50,
+                 seed=42, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.n_blocks = n_blocks
+        self.n_heads = n_heads
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.dropout = dropout
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        self._integer('embedding', 1, 1024)
+        self._integer('n_heads', 1, self.embedding)
+        if self.embedding % self.n_heads:
+            raise ValueError('n_heads must divide embedding, not %r into %r' % (self.n_heads, self.embedding))
+        self._integer('n_blocks', 1, 8)
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 1, 512)
+        if (self.n_blocks + 1) * self.batch_size * self.max_len * self.embedding >= 1 << 32:
+            raise ValueError('(n_blocks + 1) * batch_size * max_len * embedding must stay below 2^32 (dropout indices)')
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+        if not 0.0 <= float(self.dropout) < 1.0:
+            raise ValueError('dropout must be in [0, 1), not %r' % (self.dropout,))
+
+    def pieces(self, data):
+        """(piece offsets, piece items) of the training data, after the item index (_index): pieces of at most max_len inputs"""
+        idx, _, offsets, o = self._sessions(data, 'time')
+        return narm_pieces(offsets, idx[o], self.max_len + 1)
+
+    def fit(self, data):
+        self._check()
+        poff, pitems = self.pieces(data)
+        if len(poff) < 2:
+            raise ValueError('SASRec needs a training session of at least 2 events')
+        rs = np.random.RandomState(self.seed)
+        params = sasrec_init(self.n_items, self.embedding, self.n_blocks, self.max_len, rs)
+        self._drop_caches()
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.sasrec_begin(self.n_blocks, self.n_heads, self.max_len, self.batch_size, poff, pitems, params)
+        self.fit_stats = []
+        for epoch in range(self.n_epochs):
+            losses, ms = dev.sasrec_epoch(rs.permutation(len(poff) - 1), self.seed, self.learning_rate, self.dropout)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.sasrec_export()
+        self._upload(dev)                        # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.sasrec_import(self.n_blocks, self.n_heads, self.max_len, self.params)
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            flat = self.params
+            p = self._p64 = {k: v.astype(np.float64) for k, v in
+                             sasrec_unpack(flat, self.n_items, self.embedding, self.n_blocks, self.max_len).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['E'] @ sasrec_encode(p, list(prefix)[-self.max_len:], self.n_heads)
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
         score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))

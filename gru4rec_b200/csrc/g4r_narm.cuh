@@ -689,44 +689,23 @@ extern "C" int g4r_bl_narm_epoch(g4r_baselines* h, const int32_t* order, int64_t
   return G4R_OK;
 }
 
-// every counted event's q (eval mode: no dropout; the last max_len inputs of its prefix) into qev [n_ev x d] on the device
-static int nm_encode_events(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* off, int64_t n_sessions, const int32_t* n_history,
-                            const std::vector<int64_t>& ev0, float* qev) {
-  const int dd = h->n_keep, H = h->nm_H, len = h->nm_len;
-  cudaStream_t st = h->stream;
-  BlBufs bb;
-  NmScratch s;
-  auto take = [&](auto** p, size_t n) { return bb.take(p, n); };
-  CK(nm_scratch(take, s, NM_EVAL_PAIRS, NM_EVAL_PAIRS, dd, H, len, h->n_items, false));
-  const int* dItems = nullptr;
-  CK(bb.put(&dItems, items, n_events, st));
-  int *dEv = nullptr, *dPair = nullptr;
-  CK(bb.take(&dEv, NM_EVAL_PAIRS)); CK(bb.take(&dPair, NM_EVAL_PAIRS));
-  NmDev d{};
-  nm_bind(d, s, h->dNmTh, nm_layout(h->n_items, dd, H), h->n_items, dd, H, len);
-  nm_carve(d, s.f, NM_EVAL_PAIRS, dd, H, len);
-  d.items = dItems; d.train = 0; d.re = 1.f; d.rc = 1.f;
+// the encoder pieces of an evaluation's counted events, in chunks of at most cap positions and cap pieces: per session one piece
+// from its start covers the prefixes of <= len inputs, and each longer prefix takes a window of its last len inputs.  The encoder
+// hook flush(ps, pl, po, ev, pair, P) encodes one chunk: per piece its start, inputs and position offset, per counted event of
+// the chunk its index and position, and the chunk's positions.  NARM and SASRec share it.
+template <class Flush>
+static int nm_event_chunks(int len, int cap, const int64_t* off, int64_t n_sessions, const int32_t* n_history, const std::vector<int64_t>& ev0,
+                           Flush flush) {
   std::vector<long long> ps; std::vector<int> pl, po, ev, pair;
   int P = 0;
-  auto flush = [&]() -> int {
+  auto emit = [&]() -> int {
     if (ps.empty()) return G4R_OK;
-    const int nb = (int)ps.size();
-    CK(cudaMemcpyAsync(s.pstart, ps.data(), nb * sizeof(long long), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(s.plen, pl.data(), nb * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(s.poff, po.data(), nb * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dEv, ev.data(), ev.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dPair, pair.data(), pair.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    d.nb = nb; d.P = P;
-    nm_encode(st, d, s.part);
-    const int ne = (int)ev.size();
-    k_nm_pick<<<(unsigned)(((long long)ne * dd + 255) / 256), 256, 0, st>>>(d.Q, dEv, dPair, ne, dd, qev);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(st));                      // the host arrays are reused by the next chunk
+    const int rc = flush(ps, pl, po, ev, pair, P);
     ps.clear(); pl.clear(); po.clear(); ev.clear(); pair.clear(); P = 0;
-    return G4R_OK;
+    return rc;
   };
   auto piece = [&](long long start, int n) -> int {
-    if (P + n > NM_EVAL_PAIRS || (int)ps.size() >= NM_EVAL_PAIRS) { const int rc = flush(); if (rc) return rc; }
+    if (P + n > cap || (int)ps.size() >= cap) { const int rc = emit(); if (rc) return rc; }
     ps.push_back(start); pl.push_back(n); po.push_back(P); P += n;
     return G4R_OK;
   };
@@ -747,7 +726,43 @@ static int nm_encode_events(g4r_baselines* h, const int32_t* items, int64_t n_ev
       ev.push_back((int)(ev0[sI] + i - i0)); pair.push_back(po.back() + len - 1);
     }
   }
-  return flush();
+  return emit();
+}
+
+// every counted event's q (eval mode: no dropout; the last max_len inputs of its prefix) into qev [n_ev x d] on the device
+static int nm_encode_events(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* off, int64_t n_sessions, const int32_t* n_history,
+                            const std::vector<int64_t>& ev0, float* qev) {
+  const int dd = h->n_keep, H = h->nm_H, len = h->nm_len;
+  cudaStream_t st = h->stream;
+  BlBufs bb;
+  NmScratch s;
+  auto take = [&](auto** p, size_t n) { return bb.take(p, n); };
+  CK(nm_scratch(take, s, NM_EVAL_PAIRS, NM_EVAL_PAIRS, dd, H, len, h->n_items, false));
+  const int* dItems = nullptr;
+  CK(bb.put(&dItems, items, n_events, st));
+  int *dEv = nullptr, *dPair = nullptr;
+  CK(bb.take(&dEv, NM_EVAL_PAIRS)); CK(bb.take(&dPair, NM_EVAL_PAIRS));
+  NmDev d{};
+  nm_bind(d, s, h->dNmTh, nm_layout(h->n_items, dd, H), h->n_items, dd, H, len);
+  nm_carve(d, s.f, NM_EVAL_PAIRS, dd, H, len);
+  d.items = dItems; d.train = 0; d.re = 1.f; d.rc = 1.f;
+  auto flush = [&](const std::vector<long long>& ps, const std::vector<int>& pl, const std::vector<int>& po, const std::vector<int>& ev,
+                   const std::vector<int>& pair, int P) -> int {
+    const int nb = (int)ps.size();
+    CK(cudaMemcpyAsync(s.pstart, ps.data(), nb * sizeof(long long), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(s.plen, pl.data(), nb * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(s.poff, po.data(), nb * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dEv, ev.data(), ev.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dPair, pair.data(), pair.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    d.nb = nb; d.P = P;
+    nm_encode(st, d, s.part);
+    const int ne = (int)ev.size();
+    k_nm_pick<<<(unsigned)(((long long)ne * dd + 255) / 256), 256, 0, st>>>(d.Q, dEv, dPair, ne, dd, qev);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));                      // the host arrays are reused by the next chunk
+    return G4R_OK;
+  };
+  return nm_event_chunks(len, NM_EVAL_PAIRS, off, n_sessions, n_history, ev0, flush);
 }
 
 extern "C" int g4r_bl_narm_encode(g4r_baselines* h, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,

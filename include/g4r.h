@@ -514,6 +514,36 @@ int g4r_bl_narm_import(g4r_baselines* b, int32_t hidden, int32_t max_len, const 
 int g4r_bl_narm_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                        const int32_t* n_history, float* q, int64_t n_q);
 
+/* ---- SASRec self-attentive session baseline (DESIGN §3t) -------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_SASREC, n_items, d (1 .. 1024), ...).  The model is one flat float32 vector: E [n_items x d] (the input
+ * embedding and the output item side), Pe [max_len x d], per block g1, c1 [d], Wq, bq, Wk, bk, Wv, bv, Wo, bo ([d x d], [d]), g2,
+ * c2 [d], W1, b1, W2, b2 ([d x d], [d]), then gf, cf [d]; n_params = n_items d + max_len d + n_blocks (6 d^2 + 10 d) + 2 d.  For
+ * inputs x_0 .. x_(n-1): h_t = E[x_t] s_d + Pe[t]; per block u = LN1(h), causal multi-head softmax attention over u Wq + bq,
+ * u Wk + bk, u Wv + bv with scale s_h, a = h + A Wo + bo, h = a + relu(LN2(a) W1 + b1) W2 + b2; q_t = LNf(h_t), score(i) = E[i] . q.
+ * LN(x) = g (x - mean) / sqrt(var + 1e-8) + c over d; s_d and s_h the float32 of sqrt(d) and 1 / sqrt(d / n_heads). */
+#define G4R_BL_SASREC 13
+/* Begins a fit: n_blocks 1 .. 8, n_heads dividing d, max_len 1 .. 512, batch_size >= 1 with (n_blocks + 1) batch_size max_len d
+ * < 2^32, the training pieces as CSR (2 .. max_len + 1 events each: inputs every event but the last, targets every event but the
+ * first) and the initial parameters.  Adam's moments start at 0.  Every argument is checked before any device write; G4R_ERR_CUDA
+ * with a message naming the sizes if the device cannot hold the largest batch's logits and activations. */
+int g4r_bl_sasrec_begin(g4r_baselines* b, int32_t n_blocks, int32_t n_heads, int32_t max_len, int32_t batch_size, const int64_t* piece_offsets,
+                        int64_t n_pieces, const int32_t* items, int64_t n_entries, const float* params, int64_t n_params);
+/* One epoch, as g4r_bl_narm_epoch: mini-batches of batch_size consecutive entries of order, the mean full-catalogue cross-entropy
+ * over the batch's positions and one Adam step each, dropout (rate in [0, 1)) on h0 and on both residual branches of every block.
+ * A batch past the positions of the batch_size longest distinct pieces is refused before any device write. */
+int g4r_bl_sasrec_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, uint32_t seed, float learning_rate, float dropout,
+                        float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size pieces at the current parameters, without an update: the mean loss and every gradient. */
+int g4r_bl_sasrec_grads(g4r_baselines* b, const int32_t* pieces, int32_t n, uint32_t seed, int64_t step, float dropout, float* loss,
+                        float* grads);
+int g4r_bl_sasrec_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (finite); ends any fit in progress. */
+int g4r_bl_sasrec_import(g4r_baselines* b, int32_t n_blocks, int32_t n_heads, int32_t max_len, const float* params, int64_t n_params);
+/* Every counted event's q (eval mode, the last max_len inputs of items[start .. p], positions counted from the first of them) in
+ * g4r_bl_evaluate's order.  g4r_bl_evaluate of a SASRec handle ranks these q as NARM's, with I = double(E) and bI = 0. */
+int g4r_bl_sasrec_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                         const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif
