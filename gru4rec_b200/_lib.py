@@ -55,7 +55,8 @@ EXPORTS = [
     'g4r_bl_sknn_fit', 'g4r_bl_stan_fit', 'g4r_bl_stan_set_w1', 'g4r_bl_rules_fit', 'g4r_bl_vstan_set',
     'g4r_bl_narm_begin', 'g4r_bl_narm_epoch', 'g4r_bl_narm_grads', 'g4r_bl_narm_export', 'g4r_bl_narm_import', 'g4r_bl_narm_encode',
     'g4r_bl_sasrec_begin', 'g4r_bl_sasrec_epoch', 'g4r_bl_sasrec_grads', 'g4r_bl_sasrec_export', 'g4r_bl_sasrec_import',
-    'g4r_bl_sasrec_encode',
+    'g4r_bl_sasrec_encode', 'g4r_bl_srgnn_begin', 'g4r_bl_srgnn_epoch', 'g4r_bl_srgnn_grads', 'g4r_bl_srgnn_export',
+    'g4r_bl_srgnn_import', 'g4r_bl_srgnn_encode',
 ]
 
 _lib = None
@@ -175,6 +176,12 @@ def load():
     lib.g4r_bl_sasrec_export.argtypes = [vp, vp, i64]
     lib.g4r_bl_sasrec_import.argtypes = [vp, i32, i32, i32, vp, i64]
     lib.g4r_bl_sasrec_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
+    lib.g4r_bl_srgnn_begin.argtypes = [vp, i32, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_srgnn_epoch.argtypes = [vp, vp, i64, f32, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_srgnn_grads.argtypes = [vp, vp, i32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_srgnn_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_srgnn_import.argtypes = [vp, i32, i32, vp, i64]
+    lib.g4r_bl_srgnn_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -799,7 +806,7 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -834,9 +841,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM and SASRec fits and parameters (DESIGN §3s, §3t).  kind: 'pop',
-    'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm' or 'sasrec'; n_keep: top_n, n_sims, n_factors, k,
-    pruning or embedding."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec and SR-GNN fits and parameters (DESIGN §3s, §3t, §3u).
+    kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec' or 'srgnn'; n_keep: top_n,
+    n_sims, n_factors, k, pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1145,4 +1152,58 @@ class Baselines(object):
         n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
         q = np.empty((n, self.n_keep), np.float32)
         self._check(self.lib.g4r_bl_sasrec_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q
+
+    # ---- SR-GNN (DESIGN §3u) ----
+    def srgnn_n_params(self):
+        d = self.n_keep
+        return self.n_items * d + 15 * d * d + 14 * d
+
+    def _srgnn_params(self, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        n = self.srgnn_n_params()
+        if th.size != n:
+            raise ValueError('srgnn: need %d parameters (n_items d + 15 d^2 + 14 d), not %d' % (n, th.size))
+        return th
+
+    def srgnn_begin(self, step, max_len, batch_size, session_offsets, items, params):
+        """starts an SR-GNN fit: the training sessions (CSR of item indices, events in time order) and the initial flat parameters.
+        The samples are every (prefix, next item) pair in session order"""
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._srgnn_params(params)
+        self._check(self.lib.g4r_bl_srgnn_begin(self.h, int(step), int(max_len), int(batch_size), _ptr(off), off.size - 1, _ptr(it), it.size,
+                                                _ptr(th), th.size))
+        self.srgnn_batch = int(batch_size)
+
+    def srgnn_epoch(self, order, learning_rate, l2):
+        """one epoch over the samples in `order`; returns (per-step losses float32, device ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32)
+        losses = np.zeros(-(-od.size // self.srgnn_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_srgnn_epoch(self.h, _ptr(od), od.size, float(learning_rate), float(l2), _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def srgnn_grads(self, samples):
+        """(loss, flat gradient of the loss float32) of one mini-batch of samples at the current parameters, without an update"""
+        sm = np.ascontiguousarray(samples, dtype=np.int32)
+        g = np.empty(self.srgnn_n_params(), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_srgnn_grads(self.h, _ptr(sm), sm.size, C.byref(loss), _ptr(g)))
+        return loss.value, g
+
+    def srgnn_export(self):
+        th = np.empty(self.srgnn_n_params(), np.float32)
+        self._check(self.lib.g4r_bl_srgnn_export(self.h, _ptr(th), th.size))
+        return th
+
+    def srgnn_import(self, step, max_len, params):
+        th = self._srgnn_params(params)
+        self._check(self.lib.g4r_bl_srgnn_import(self.h, int(step), int(max_len), _ptr(th), th.size))
+
+    def srgnn_encode(self, items, session_offsets, n_history=None):
+        """every counted event's s_h [n, d] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_srgnn_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
         return q

@@ -1,7 +1,7 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
-§3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s) and SASRec
-(§3t), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
+§3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s), SASRec
+(§3t) and SR-GNN (§3u), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -964,6 +964,176 @@ class SASRec(Baseline):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
         p = self.params64()
         return p['E'] @ sasrec_encode(p, list(prefix)[-self.max_len:], self.n_heads)
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+SRGNN_PARAMS = ('E', 'W_in', 'W_out', 'b_in', 'b_out', 'b_iah', 'b_oah', 'W_ih', 'b_ih', 'W_hh', 'b_hh', 'W1', 'W2', 'b1', 'b2', 'q', 'W3', 'b3')
+
+
+def srgnn_shapes(n_items, d):
+    """the parameters in the order of the flat vector (DESIGN §3u)"""
+    sq, v = (d, d), (d,)
+    return dict(E=(n_items, d), W_in=sq, W_out=sq, b_in=v, b_out=v, b_iah=v, b_oah=v, W_ih=(2 * d, 3 * d), b_ih=(3 * d,), W_hh=(d, 3 * d),
+                b_hh=(3 * d,), W1=sq, W2=sq, b1=v, b2=v, q=v, W3=(2 * d, d), b3=v)
+
+
+def srgnn_unpack(flat, n_items, d):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in srgnn_shapes(n_items, d).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def srgnn_init(n_items, d, rs):
+    """the initial parameters, float32 flat: every entry (biases and E included), in the order of the vector, drawn from
+    rs.uniform(-s, s) with s = 1 / sqrt(d)"""
+    s = 1.0 / np.sqrt(d)
+    n = sum(int(np.prod(shp)) for shp in srgnn_shapes(n_items, d).values())
+    return rs.uniform(-s, s, size=n).astype(np.float32)
+
+
+def srgnn_graph(x):
+    """the graph of inputs x: (nodes: the distinct items ascending, alias: the node of each position, A_in, A_out [K x K]) with
+    an edge u -> v for each consecutive pair (a repeat once, self-loops kept), A_in[v][u] = 1 / indeg(v), A_out[u][v] =
+    1 / outdeg(u) and zero rows for nodes without such edges"""
+    nodes, alias = np.unique(np.asarray(x, dtype=np.int64), return_inverse=True)
+    K = len(nodes)
+    adj = np.zeros((K, K))
+    adj[alias[:-1], alias[1:]] = 1.0
+    indeg, outdeg = adj.sum(axis=0), adj.sum(axis=1)
+    a_in = adj.T / np.where(indeg > 0, indeg, 1.0)[:, None]
+    a_out = adj / np.where(outdeg > 0, outdeg, 1.0)[:, None]
+    return nodes, alias, a_in, a_out
+
+
+def srgnn_encode(p, x, step):
+    """s_h (float64) of the inputs x (item indices, oldest first, at most max_len): p maps the parameter names to float64 arrays"""
+    d = p['E'].shape[1]
+    nodes, alias, a_in, a_out = srgnn_graph(x)
+    H = p['E'][nodes]
+    for _ in range(step):
+        a = np.concatenate([a_in @ (H @ p['W_in'] + p['b_in']) + p['b_iah'], a_out @ (H @ p['W_out'] + p['b_out']) + p['b_oah']], axis=1)
+        gi, gh = a @ p['W_ih'] + p['b_ih'], H @ p['W_hh'] + p['b_hh']
+        r = _sig(gi[:, :d] + gh[:, :d])
+        z = _sig(gi[:, d:2 * d] + gh[:, d:2 * d])
+        n = np.tanh(gi[:, 2 * d:] + r * gh[:, 2 * d:])
+        H = n + z * (H - n)
+    h = H[alias]
+    alpha = _sig(h[-1] @ p['W1'] + p['b1'] + h @ p['W2'] + p['b2']) @ p['q']
+    return np.concatenate([alpha @ h, h[-1]]) @ p['W3'] + p['b3']
+
+
+class SRGNN(Baseline):
+    '''
+    SRGNN(embedding=100, step=1, n_epochs=10, batch_size=100, learning_rate=0.001, lr_decay=0.1, lr_decay_step=3, l2=1e-5, max_len=50,
+          seed=42, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Session-graph model in the style of SR-GNN (Wu et al., AAAI 2019), trained on the device with full-catalogue cross-entropy and
+    Adam.  This is this project's definition (DESIGN §3u); no parity with another framework is claimed.
+
+    One item table E [n_items x embedding] is the node embedding and the scored item side.  The last max_len inputs of a session
+    prefix become a directed graph of their distinct items (an edge per consecutive pair, a repeat once) with in- and
+    out-adjacency normalised by degree; `step` gated propagation steps with shared weights update the node states; the hybrid
+    readout s_h = W3 [s_g ; s_l] + b3 joins the last position's state s_l with s_g = sum_t alpha_t h_t, alpha_t = q . sig(W1 s_l +
+    b1 + W2 h_t + b2); item i scores E[i] . s_h.  Training takes every (prefix, next item) pair of every session (events by
+    time_key, ties by row order) as its own sample, and per mini-batch of batch_size samples one Adam step on the mean
+    cross-entropy plus l2 theta (coupled L2), at learning_rate lr_decay^(epoch // lr_decay_step).  The parameters are float32
+    and drawn, like the epochs' sample orders, from np.random.RandomState(seed).  fit prints the epoch's mean loss;
+    `fit_stats` holds per epoch (mean loss, device ms, per-step losses).  predict_next computes the scores on the host in float64
+    from the float32 parameters.
+    '''
+    _kind = 'srgnn'
+
+    def __init__(self, embedding=100, step=1, n_epochs=10, batch_size=100, learning_rate=0.001, lr_decay=0.1, lr_decay_step=3, l2=1e-5,
+                 max_len=50, seed=42, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.step = step
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.lr_decay = lr_decay
+        self.lr_decay_step = lr_decay_step
+        self.l2 = l2
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        self._integer('embedding', 1, 1024)
+        self._integer('step', 1, 8)
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 1, 512)
+        self._integer('lr_decay_step', 1, 1 << 30)
+        if self.batch_size * self.max_len * (self.step + 1) * 3 * self.embedding >= 1 << 31:
+            raise ValueError('batch_size * max_len * (step + 1) * 3 * embedding must stay below 2^31 (flat indices of a batch)')
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+        if not 0.0 < float(self.lr_decay) < np.inf:
+            raise ValueError('lr_decay must be finite and > 0, not %r' % (self.lr_decay,))
+        if not 0.0 <= float(self.l2) < np.inf:
+            raise ValueError('l2 must be finite and >= 0, not %r' % (self.l2,))
+
+    def sessions(self, data):
+        """(session offsets, items in time order) of the training data, after the item index (_index)"""
+        idx, _, offsets, o = self._sessions(data, 'time')
+        return offsets, idx[o].astype(np.int32)
+
+    def learning_rates(self):
+        """the learning rate of each epoch: learning_rate lr_decay^(epoch // lr_decay_step), as the float32 the device takes"""
+        return [float(np.float32(self.learning_rate * self.lr_decay ** (e // self.lr_decay_step))) for e in range(self.n_epochs)]
+
+    def fit(self, data):
+        self._check()
+        offsets, items = self.sessions(data)
+        n_samples = int(np.maximum(np.diff(offsets) - 1, 0).sum())
+        if n_samples < 1:
+            raise ValueError('SRGNN needs a training session of at least 2 events')
+        rates = self.learning_rates()
+        if not all(0.0 < r < np.inf for r in rates):
+            raise ValueError('every epoch\'s learning rate must be finite and > 0 in float32, not %r' % (rates,))
+        rs = np.random.RandomState(self.seed)
+        params = srgnn_init(self.n_items, self.embedding, rs)
+        self._drop_caches()
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.srgnn_begin(self.step, self.max_len, self.batch_size, offsets, items, params)
+        self.fit_stats = []
+        for epoch, lr in enumerate(rates):
+            losses, ms = dev.srgnn_epoch(rs.permutation(n_samples), lr, self.l2)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.srgnn_export()
+        self._upload(dev)                        # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.srgnn_import(self.step, self.max_len, self.params)
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            p = self._p64 = {k: v.astype(np.float64) for k, v in srgnn_unpack(self.params, self.n_items, self.embedding).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['E'] @ srgnn_encode(p, list(prefix)[-self.max_len:], self.step)
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
         score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))

@@ -544,6 +544,37 @@ int g4r_bl_sasrec_import(g4r_baselines* b, int32_t n_blocks, int32_t n_heads, in
 int g4r_bl_sasrec_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                          const int32_t* n_history, float* q, int64_t n_q);
 
+/* ---- SR-GNN session-graph baseline (DESIGN §3u) -----------------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_SRGNN, n_items, d (1 .. 1024), ...).  The model is one flat float32 vector: E [n_items x d] (the node
+ * embedding and the scored item side), W_in, W_out [d x d], b_in, b_out, b_iah, b_oah [d], W_ih [2d x 3d], b_ih [3d], W_hh [d x 3d],
+ * b_hh [3d], W1, W2 [d x d], b1, b2, q [d], W3 [2d x d], b3 [d]; n_params = n_items d + 15 d^2 + 14 d.  For the last max_len inputs
+ * x_1 .. x_n of a prefix: the nodes are its distinct items ascending, edges u -> v for each consecutive pair (a repeat once,
+ * self-loops kept), A_in[v][u] = 1 / indeg(v), A_out[u][v] = 1 / outdeg(u); from H = E[nodes], `step` times
+ * a = [A_in (H W_in + b_in) + b_iah ; A_out (H W_out + b_out) + b_oah], gi = a W_ih + b_ih, gh = H W_hh + b_hh in (r, z, n) thirds,
+ * r = sig(gi_r + gh_r), z = sig(gi_z + gh_z), n = tanh(gi_n + r gh_n), H = n + z (H - n); then h_t = H[node of x_t], s_l = h_n,
+ * alpha_t = q . sig(s_l W1 + b1 + h_t W2 + b2), s_g = sum_t alpha_t h_t, s_h = [s_g ; s_l] W3 + b3 and score(i) = E[i] . s_h. */
+#define G4R_BL_SRGNN 15
+/* Begins a fit: step 1 .. 8, max_len 1 .. 512, batch_size >= 1 with batch_size max_len (step + 1) 3 d < 2^31, the training
+ * sessions as CSR (events in time order) and the initial parameters.  The samples are every (prefix, next item) pair in session
+ * order, the prefix cut to its last max_len inputs: sample k of g4r_bl_srgnn_epoch / _grads counts them from 0.  Adam's moments
+ * start at 0.  Every argument is checked before any device write; G4R_ERR_CUDA with a message naming the sizes if the device
+ * cannot hold the largest batch's logits and activations. */
+int g4r_bl_srgnn_begin(g4r_baselines* b, int32_t step, int32_t max_len, int32_t batch_size, const int64_t* session_offsets, int64_t n_sessions,
+                       const int32_t* items, int64_t n_entries, const float* params, int64_t n_params);
+/* One epoch: mini-batches of batch_size consecutive samples of order, the mean full-catalogue cross-entropy over the batch's
+ * samples and one Adam step each (NARM's constants) on gradient + l2 theta over every parameter.  A batch past the positions
+ * of the batch_size longest samples is refused before any device write. */
+int g4r_bl_srgnn_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, float learning_rate, float l2, float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size samples at the current parameters, without an update: the mean loss and its gradient (no L2). */
+int g4r_bl_srgnn_grads(g4r_baselines* b, const int32_t* samples, int32_t n, float* loss, float* grads);
+int g4r_bl_srgnn_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (finite); ends any fit in progress. */
+int g4r_bl_srgnn_import(g4r_baselines* b, int32_t step, int32_t max_len, const float* params, int64_t n_params);
+/* Every counted event's s_h (the graph of the last max_len inputs of items[start .. p]) in g4r_bl_evaluate's order.
+ * g4r_bl_evaluate of an SR-GNN handle ranks these s_h as NARM's q, with I = double(E) and bI = 0. */
+int g4r_bl_srgnn_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                        const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif
