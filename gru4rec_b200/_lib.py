@@ -56,7 +56,8 @@ EXPORTS = [
     'g4r_bl_narm_begin', 'g4r_bl_narm_epoch', 'g4r_bl_narm_grads', 'g4r_bl_narm_export', 'g4r_bl_narm_import', 'g4r_bl_narm_encode',
     'g4r_bl_sasrec_begin', 'g4r_bl_sasrec_epoch', 'g4r_bl_sasrec_grads', 'g4r_bl_sasrec_export', 'g4r_bl_sasrec_import',
     'g4r_bl_sasrec_encode', 'g4r_bl_srgnn_begin', 'g4r_bl_srgnn_epoch', 'g4r_bl_srgnn_grads', 'g4r_bl_srgnn_export',
-    'g4r_bl_srgnn_import', 'g4r_bl_srgnn_encode',
+    'g4r_bl_srgnn_import', 'g4r_bl_srgnn_encode', 'g4r_bl_stamp_begin', 'g4r_bl_stamp_epoch', 'g4r_bl_stamp_grads', 'g4r_bl_stamp_export',
+    'g4r_bl_stamp_import', 'g4r_bl_stamp_encode',
 ]
 
 _lib = None
@@ -182,6 +183,12 @@ def load():
     lib.g4r_bl_srgnn_export.argtypes = [vp, vp, i64]
     lib.g4r_bl_srgnn_import.argtypes = [vp, i32, i32, vp, i64]
     lib.g4r_bl_srgnn_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
+    lib.g4r_bl_stamp_begin.argtypes = [vp, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_stamp_epoch.argtypes = [vp, vp, i64, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_stamp_grads.argtypes = [vp, vp, i32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_stamp_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_stamp_import.argtypes = [vp, i32, vp, i64]
+    lib.g4r_bl_stamp_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -806,7 +813,7 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15, 'stamp': 17}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -841,9 +848,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec and SR-GNN fits and parameters (DESIGN §3s, §3t, §3u).
-    kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec' or 'srgnn'; n_keep: top_n,
-    n_sims, n_factors, k, pruning or embedding."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec, SR-GNN and STAMP fits and parameters (DESIGN §3s, §3t,
+    §3u, §3v).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec', 'srgnn' or
+    'stamp'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1206,4 +1213,57 @@ class Baselines(object):
         n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
         q = np.empty((n, self.n_keep), np.float32)
         self._check(self.lib.g4r_bl_srgnn_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q
+
+    # ---- STAMP (DESIGN §3v) ----
+    def stamp_n_params(self):
+        d = self.n_keep
+        return self.n_items * d + 5 * d * d + 4 * d
+
+    def _stamp_params(self, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        n = self.stamp_n_params()
+        if th.size != n:
+            raise ValueError('stamp: need %d parameters (n_items d + 5 d^2 + 4 d), not %d' % (n, th.size))
+        return th
+
+    def stamp_begin(self, max_len, batch_size, session_offsets, items, params):
+        """starts a STAMP fit: the training sessions (CSR of item indices, events in time order) and the initial flat parameters.
+        The samples are every (prefix, next item) pair in session order"""
+        off = np.ascontiguousarray(session_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._stamp_params(params)
+        self._check(self.lib.g4r_bl_stamp_begin(self.h, int(max_len), int(batch_size), _ptr(off), off.size - 1, _ptr(it), it.size, _ptr(th), th.size))
+        self.stamp_batch = int(batch_size)
+
+    def stamp_epoch(self, order, learning_rate):
+        """one epoch over the samples in `order`; returns (per-step losses float32, device ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32)
+        losses = np.zeros(-(-od.size // self.stamp_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_stamp_epoch(self.h, _ptr(od), od.size, float(learning_rate), _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def stamp_grads(self, samples):
+        """(loss, flat gradient of the loss float32) of one mini-batch of samples at the current parameters, without an update"""
+        sm = np.ascontiguousarray(samples, dtype=np.int32)
+        g = np.empty(self.stamp_n_params(), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_stamp_grads(self.h, _ptr(sm), sm.size, C.byref(loss), _ptr(g)))
+        return loss.value, g
+
+    def stamp_export(self):
+        th = np.empty(self.stamp_n_params(), np.float32)
+        self._check(self.lib.g4r_bl_stamp_export(self.h, _ptr(th), th.size))
+        return th
+
+    def stamp_import(self, max_len, params):
+        th = self._stamp_params(params)
+        self._check(self.lib.g4r_bl_stamp_import(self.h, int(max_len), _ptr(th), th.size))
+
+    def stamp_encode(self, items, session_offsets, n_history=None):
+        """every counted event's q [n, d] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_stamp_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
         return q

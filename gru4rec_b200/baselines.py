@@ -1,7 +1,7 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
 §3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s), SASRec
-(§3t) and SR-GNN (§3u), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
+(§3t), SR-GNN (§3u) and STAMP (§3v), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
 co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
@@ -1134,6 +1134,138 @@ class SRGNN(Baseline):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
         p = self.params64()
         return p['E'] @ srgnn_encode(p, list(prefix)[-self.max_len:], self.step)
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+STAMP_PARAMS = ('E', 'W1', 'W2', 'W3', 'b_a', 'w0', 'Ws', 'bs', 'Wt', 'bt')
+STAMP_BIASES = ('b_a', 'bs', 'bt')
+
+
+def stamp_shapes(n_items, d):
+    """the parameters in the order of the flat vector (DESIGN §3v)"""
+    sq, v = (d, d), (d,)
+    return dict(E=(n_items, d), W1=sq, W2=sq, W3=sq, b_a=v, w0=v, Ws=sq, bs=v, Wt=sq, bt=v)
+
+
+def stamp_unpack(flat, n_items, d):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in stamp_shapes(n_items, d).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def stamp_init(n_items, d, init_std, rs):
+    """the initial parameters, float32 flat: in the order of the vector every weight (E and w0 included) drawn from
+    rs.normal(0, init_std); the biases b_a, bs and bt are 0 and take no draw"""
+    parts = [np.zeros(shp) if name in STAMP_BIASES else rs.normal(0.0, init_std, size=shp) for name, shp in stamp_shapes(n_items, d).items()]
+    return np.concatenate([p.ravel() for p in parts]).astype(np.float32)
+
+
+def stamp_encode(p, x):
+    """q (float64) of the inputs x (item indices, oldest first, at most max_len): p maps the parameter names to float64 arrays"""
+    X = p['E'][list(x)]
+    mt, ms = X[-1], X.mean(axis=0)
+    a = _sig(X @ p['W1'] + mt @ p['W2'] + ms @ p['W3'] + p['b_a']) @ p['w0']
+    return np.tanh(a @ X @ p['Ws'] + p['bs']) * np.tanh(mt @ p['Wt'] + p['bt'])
+
+
+class STAMP(Baseline):
+    '''
+    STAMP(embedding=100, n_epochs=10, batch_size=512, learning_rate=0.005, init_std=0.05, max_len=50, seed=42, session_key='SessionId',
+          item_key='ItemId', time_key='Time')
+
+    Short-term attention/memory priority model in the style of STAMP (Liu et al., KDD 2018), trained on the device with
+    full-catalogue cross-entropy and Adam.  This is this project's definition (DESIGN §3v); no parity with another framework is
+    claimed.
+
+    One item table E [n_items x embedding] is the input embedding and the scored item side.  For the last max_len inputs x_1 ..
+    x_n of a session prefix: the session mean m_s, the last click m_t = x_n, the attention a_i = w0 . sig(x_i W1 + m_t W2 + m_s W3
+    + b_a) (not normalised), m_a = sum_i a_i x_i, h_s = tanh(m_a Ws + bs), h_t = tanh(m_t Wt + bt) and q = h_s * h_t; item i scores
+    E[i] . q (the paper's sigmoid around it is left out: it does not change a ranking).  Training takes every (prefix, next item)
+    pair of every session (events by time_key, ties by row order) as its own sample, and per mini-batch of batch_size samples one
+    Adam step on the mean cross-entropy.  The weights are float32 and drawn from N(0, init_std^2), the biases 0; the draws and
+    the epochs' sample orders come from np.random.RandomState(seed).  fit prints the epoch's mean loss; `fit_stats` holds per
+    epoch (mean loss, device ms, per-step losses).  predict_next computes the scores on the host in float64 from the float32
+    parameters.
+    '''
+    _kind = 'stamp'
+
+    def __init__(self, embedding=100, n_epochs=10, batch_size=512, learning_rate=0.005, init_std=0.05, max_len=50, seed=42,
+                 session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.init_std = init_std
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        self._integer('embedding', 1, 1024)
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 1, 512)
+        if self.batch_size * self.max_len * 2 * self.embedding >= 1 << 31:
+            raise ValueError('batch_size * max_len * 2 * embedding must stay below 2^31 (flat indices of a batch)')
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+        if not 0.0 < float(self.init_std) < np.inf:
+            raise ValueError('init_std must be finite and > 0, not %r' % (self.init_std,))
+
+    def sessions(self, data):
+        """(session offsets, items in time order) of the training data, after the item index (_index)"""
+        idx, _, offsets, o = self._sessions(data, 'time')
+        return offsets, idx[o].astype(np.int32)
+
+    def fit(self, data):
+        self._check()
+        offsets, items = self.sessions(data)
+        n_samples = int(np.maximum(np.diff(offsets) - 1, 0).sum())
+        if n_samples < 1:
+            raise ValueError('STAMP needs a training session of at least 2 events')
+        rs = np.random.RandomState(self.seed)
+        params = stamp_init(self.n_items, self.embedding, self.init_std, rs)
+        self._drop_caches()
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.stamp_begin(self.max_len, self.batch_size, offsets, items, params)
+        self.fit_stats = []
+        for epoch in range(self.n_epochs):
+            losses, ms = dev.stamp_epoch(rs.permutation(n_samples), self.learning_rate)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.stamp_export()
+        self._upload(dev)                        # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.stamp_import(self.max_len, self.params)
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            p = self._p64 = {k: v.astype(np.float64) for k, v in stamp_unpack(self.params, self.n_items, self.embedding).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['E'] @ stamp_encode(p, list(prefix)[-self.max_len:])
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
         score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))

@@ -457,6 +457,26 @@ extern "C" int g4r_bl_srgnn_export(g4r_baselines* h, float* params, int64_t n_pa
   return G4R_OK;
 }
 
+// the samples of a fit (SR-GNN's and STAMP's): per session every (prefix, next item) pair, the prefix cut to its last max_len
+// inputs; per sample its first input and its inputs
+static void sg_samples(const int64_t* off, int64_t n_sessions, int max_len, std::vector<int64_t>& s0, std::vector<int>& sn) {
+  for (int64_t s = 0; s < n_sessions; s++)
+    for (int64_t j = 1; j < off[s + 1] - off[s]; j++) {
+      const int64_t a = std::max<int64_t>(0, j - max_len);
+      s0.push_back(off[s] + a); sn.push_back((int)(j - a));
+    }
+}
+
+// the positions of the largest batch: the batch_size longest samples
+static long long sg_longest(const std::vector<int>& sn, int batch_size) {
+  std::vector<int> srt(sn);
+  const size_t top = std::min<size_t>(batch_size, srt.size());
+  std::partial_sort(srt.begin(), srt.begin() + top, srt.end(), std::greater<int>());
+  long long Pmax = 0;
+  for (size_t k = 0; k < top; k++) Pmax += srt[k];
+  return Pmax;
+}
+
 extern "C" int g4r_bl_srgnn_begin(g4r_baselines* h, int32_t step, int32_t max_len, int32_t batch_size, const int64_t* session_offsets,
                                   int64_t n_sessions, const int32_t* items, int64_t n_entries, const float* params, int64_t n_params) {
   if (!h) return G4R_ERR_INVALID;
@@ -470,21 +490,11 @@ extern "C" int g4r_bl_srgnn_begin(g4r_baselines* h, int32_t step, int32_t max_le
   for (int64_t e = 0; e < n_entries; e++) if (items[e] < 0 || items[e] >= NI) FAIL(G4R_ERR_INDEX, "g4r_bl_srgnn_begin: item index out of range");
   if ((uint64_t)batch_size * (uint64_t)max_len * (uint64_t)(step + 1) * 3ull * (uint64_t)dd >= 0x80000000ull)
     FAIL(G4R_ERR_INVALID, "g4r_bl_srgnn_begin: batch_size * max_len * (step + 1) * 3 d must stay below 2^31 (flat indices of a batch)");
-  // the samples: per session every (prefix, next item) pair, the prefix cut to its last max_len inputs
   std::vector<int64_t> s0; std::vector<int> sn;
-  for (int64_t s = 0; s < n_sessions; s++)
-    for (int64_t j = 1; j < session_offsets[s + 1] - session_offsets[s]; j++) {
-      const int64_t a = std::max<int64_t>(0, j - max_len);
-      s0.push_back(session_offsets[s] + a); sn.push_back((int)(j - a));
-    }
+  sg_samples(session_offsets, n_sessions, max_len, s0, sn);
   if (s0.empty()) FAIL(G4R_ERR_INVALID, "g4r_bl_srgnn_begin: no session of at least 2 events");
   if (s0.size() > (size_t)INT32_MAX) FAIL(G4R_ERR_INVALID, "g4r_bl_srgnn_begin: more than 2^31 - 1 samples");
-  // the largest batch: the batch_size longest samples
-  std::vector<int> srt(sn);
-  const size_t top = std::min<size_t>(batch_size, srt.size());
-  std::partial_sort(srt.begin(), srt.begin() + top, srt.end(), std::greater<int>());
-  long long Pmax = 0;
-  for (size_t k = 0; k < top; k++) Pmax += srt[k];
+  const long long Pmax = sg_longest(sn, batch_size);
   const SgLayout L = sg_layout(NI, dd);
   const size_t act = (size_t)Pmax * sg_pos_floats(dd, step, true) * 4 + (size_t)batch_size * sg_smp_floats(dd, true) * 4;
   const size_t need = (size_t)batch_size * NI * 4 + act + (size_t)Pmax * ((SG_INTS_POS + 1) * 4 + 16) + NM_PART_CAP * 4 + 3 * L.n * 4 +

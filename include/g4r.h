@@ -575,6 +575,34 @@ int g4r_bl_srgnn_import(g4r_baselines* b, int32_t step, int32_t max_len, const f
 int g4r_bl_srgnn_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                         const int32_t* n_history, float* q, int64_t n_q);
 
+/* ---- STAMP short-term attention/memory baseline (DESIGN §3v) ----------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_STAMP, n_items, d (1 .. 1024), ...).  The model is one flat float32 vector: E [n_items x d] (the input
+ * embedding and the scored item side), W1, W2, W3 [d x d], b_a, w0 [d], Ws [d x d], bs [d], Wt [d x d], bt [d]; n_params =
+ * n_items d + 5 d^2 + 4 d.  For the last max_len inputs x_1 .. x_n of a prefix (rows of E): m_s = (1/n) sum_i x_i, m_t = x_n,
+ * a_i = w0 . sig(x_i W1 + m_t W2 + m_s W3 + b_a) (not normalised over i), m_a = sum_i a_i x_i, h_s = tanh(m_a Ws + bs),
+ * h_t = tanh(m_t Wt + bt), q = h_s * h_t (elementwise) and score(i) = E[i] . q. */
+#define G4R_BL_STAMP 17
+/* Begins a fit: max_len 1 .. 512, batch_size >= 1 with batch_size max_len 2 d < 2^31, the training sessions as CSR (events in
+ * time order) and the initial parameters.  The samples are every (prefix, next item) pair in session order, the prefix cut to its
+ * last max_len inputs (SR-GNN's): sample k of g4r_bl_stamp_epoch / _grads counts them from 0.  Adam's moments start at 0.  Every
+ * argument is checked before any device write; G4R_ERR_CUDA with a message naming the sizes if the device cannot hold the
+ * largest batch's logits and activations. */
+int g4r_bl_stamp_begin(g4r_baselines* b, int32_t max_len, int32_t batch_size, const int64_t* session_offsets, int64_t n_sessions,
+                       const int32_t* items, int64_t n_entries, const float* params, int64_t n_params);
+/* One epoch: mini-batches of batch_size consecutive samples of order, the mean full-catalogue cross-entropy over the batch's
+ * samples and one Adam step each (NARM's constants, no L2).  A batch past the positions of the batch_size longest samples is
+ * refused before any device write. */
+int g4r_bl_stamp_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, float learning_rate, float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size samples at the current parameters, without an update: the mean loss and its gradient. */
+int g4r_bl_stamp_grads(g4r_baselines* b, const int32_t* samples, int32_t n, float* loss, float* grads);
+int g4r_bl_stamp_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (finite); ends any fit in progress. */
+int g4r_bl_stamp_import(g4r_baselines* b, int32_t max_len, const float* params, int64_t n_params);
+/* Every counted event's q (the last max_len inputs of items[start .. p]) in g4r_bl_evaluate's order.
+ * g4r_bl_evaluate of a STAMP handle ranks these q as NARM's, with I = double(E) and bI = 0. */
+int g4r_bl_stamp_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                        const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif
