@@ -57,7 +57,8 @@ EXPORTS = [
     'g4r_bl_sasrec_begin', 'g4r_bl_sasrec_epoch', 'g4r_bl_sasrec_grads', 'g4r_bl_sasrec_export', 'g4r_bl_sasrec_import',
     'g4r_bl_sasrec_encode', 'g4r_bl_srgnn_begin', 'g4r_bl_srgnn_epoch', 'g4r_bl_srgnn_grads', 'g4r_bl_srgnn_export',
     'g4r_bl_srgnn_import', 'g4r_bl_srgnn_encode', 'g4r_bl_stamp_begin', 'g4r_bl_stamp_epoch', 'g4r_bl_stamp_grads', 'g4r_bl_stamp_export',
-    'g4r_bl_stamp_import', 'g4r_bl_stamp_encode',
+    'g4r_bl_stamp_import', 'g4r_bl_stamp_encode', 'g4r_bl_nextitnet_begin', 'g4r_bl_nextitnet_epoch', 'g4r_bl_nextitnet_grads',
+    'g4r_bl_nextitnet_export', 'g4r_bl_nextitnet_import', 'g4r_bl_nextitnet_encode',
 ]
 
 _lib = None
@@ -189,6 +190,12 @@ def load():
     lib.g4r_bl_stamp_export.argtypes = [vp, vp, i64]
     lib.g4r_bl_stamp_import.argtypes = [vp, i32, vp, i64]
     lib.g4r_bl_stamp_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
+    lib.g4r_bl_nextitnet_begin.argtypes = [vp, vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_nextitnet_epoch.argtypes = [vp, vp, i64, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_nextitnet_grads.argtypes = [vp, vp, i32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_nextitnet_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_nextitnet_import.argtypes = [vp, vp, i32, i32, i32, vp, i64]
+    lib.g4r_bl_nextitnet_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -813,7 +820,8 @@ class Engine(object):
         self._check(self.lib.g4r_sessions_import(self.h, _ptr(keys), _ptr(states), _ptr(off), _ptr(it), keys.size))
 
 
-BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15, 'stamp': 17}
+BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15, 'stamp': 17,
+                  'nextitnet': 19}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -848,9 +856,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec, SR-GNN and STAMP fits and parameters (DESIGN §3s, §3t,
-    §3u, §3v).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec', 'srgnn' or
-    'stamp'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec, SR-GNN, STAMP and NextItNet fits and parameters (DESIGN
+    §3s, §3t, §3u, §3v, §3w).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec',
+    'srgnn', 'stamp' or 'nextitnet'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1266,4 +1274,61 @@ class Baselines(object):
         n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
         q = np.empty((n, self.n_keep), np.float32)
         self._check(self.lib.g4r_bl_stamp_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q
+
+    # ---- NextItNet (DESIGN §3w) ----
+    def nextitnet_n_params(self, n_dilations, kernel_size):
+        d = self.n_keep
+        return 2 * self.n_items * d + self.n_items + int(n_dilations) * (2 * int(kernel_size) * d * d + 6 * d)
+
+    def _nextitnet_params(self, dilations, kernel_size, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        n = self.nextitnet_n_params(len(dilations), kernel_size)
+        if th.size != n:
+            raise ValueError('nextitnet: need %d parameters (2 n_items d + n_items + n_dilations (2 kernel_size d^2 + 6 d)), not %d' % (n, th.size))
+        return th
+
+    def nextitnet_begin(self, dilations, kernel_size, max_len, batch_size, piece_offsets, items, params):
+        """starts a NextItNet fit: the training pieces (CSR of item indices, 2 .. max_len + 1 events each) and the initial flat
+        parameters"""
+        dl = np.ascontiguousarray(dilations, dtype=np.int32)
+        off = np.ascontiguousarray(piece_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._nextitnet_params(dl, kernel_size, params)
+        self._check(self.lib.g4r_bl_nextitnet_begin(self.h, _ptr(dl), dl.size, int(kernel_size), int(max_len), int(batch_size), _ptr(off),
+                                                    off.size - 1, _ptr(it), it.size, _ptr(th), th.size))
+        self.nextitnet_shape, self.nextitnet_batch = (dl.size, int(kernel_size)), int(batch_size)
+
+    def nextitnet_epoch(self, order, learning_rate):
+        """one epoch over the pieces in `order`; returns (per-step losses float32, device ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32)
+        losses = np.zeros(-(-od.size // self.nextitnet_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_nextitnet_epoch(self.h, _ptr(od), od.size, float(learning_rate), _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def nextitnet_grads(self, pieces):
+        """(loss, flat gradient float32) of one mini-batch of pieces at the current parameters, without an update"""
+        pc = np.ascontiguousarray(pieces, dtype=np.int32)
+        g = np.empty(self.nextitnet_n_params(*self.nextitnet_shape), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_nextitnet_grads(self.h, _ptr(pc), pc.size, C.byref(loss), _ptr(g)))
+        return loss.value, g
+
+    def nextitnet_export(self):
+        th = np.empty(self.nextitnet_n_params(*self.nextitnet_shape), np.float32)
+        self._check(self.lib.g4r_bl_nextitnet_export(self.h, _ptr(th), th.size))
+        return th
+
+    def nextitnet_import(self, dilations, kernel_size, max_len, params):
+        dl = np.ascontiguousarray(dilations, dtype=np.int32)
+        th = self._nextitnet_params(dl, kernel_size, params)
+        self._check(self.lib.g4r_bl_nextitnet_import(self.h, _ptr(dl), dl.size, int(kernel_size), int(max_len), _ptr(th), th.size))
+        self.nextitnet_shape = (dl.size, int(kernel_size))
+
+    def nextitnet_encode(self, items, session_offsets, n_history=None):
+        """every counted event's q [n, d] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_nextitnet_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
         return q

@@ -1,8 +1,8 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
 §3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s), SASRec
-(§3t), SR-GNN (§3u) and STAMP (§3v), trained on the device, with the same surface.  ItemKNN's fit runs on the device (the
-co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
+(§3t), SR-GNN (§3u), STAMP (§3v) and NextItNet (§3w), trained on the device, with the same surface.  ItemKNN's fit runs on the
+device (the co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
 provided: it has nothing to fit, and its scores are unseeded noise."""
@@ -1266,6 +1266,164 @@ class STAMP(Baseline):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
         p = self.params64()
         return p['E'] @ stamp_encode(p, list(prefix)[-self.max_len:])
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+NEXTITNET_BLOCK = ('C1', 'c1', 'g1', 'n1', 'C2', 'c2', 'g2', 'n2')
+
+
+def nextitnet_shapes(n_items, d, dilations, kernel_size):
+    """the parameters in the order of the flat vector (DESIGN §3w): E, per block b the NEXTITNET_BLOCK names with suffix _b (C*:
+    [kernel_size d x d], row k d + i tap k and input channel i; the rest [d]), W, bW"""
+    out = dict(E=(n_items, d))
+    for b in range(len(dilations)):
+        for name in NEXTITNET_BLOCK:
+            out['%s_%d' % (name, b)] = (kernel_size * d, d) if name[0] == 'C' else (d,)
+    out['W'], out['bW'] = (n_items, d), (n_items,)
+    return out
+
+
+def nextitnet_unpack(flat, n_items, d, dilations, kernel_size):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in nextitnet_shapes(n_items, d, dilations, kernel_size).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def nextitnet_init(n_items, d, dilations, kernel_size, rs):
+    """the initial parameters, float32 flat: in the order of the vector each matrix [r x c] (E and W included) drawn from
+    rs.uniform(-s, s) with s = sqrt(6 / (r + c)); biases 0 and gains 1, without draws"""
+    parts = []
+    for name, shp in nextitnet_shapes(n_items, d, dilations, kernel_size).items():
+        if len(shp) == 2:
+            s = np.sqrt(6.0 / (shp[0] + shp[1]))
+            parts.append(rs.uniform(-s, s, size=shp))
+        else:
+            parts.append(np.full(shp, 1.0 if name[0] == 'g' else 0.0))
+    return np.concatenate([p.ravel() for p in parts]).astype(np.float32)
+
+
+def _causal_taps(x, K, l):
+    """[n, K d]: row t holds x[t - (K - 1 - k) l] for k = 0 .. K - 1, zeros before the start"""
+    n, d = x.shape
+    out = np.zeros((n, K * d))
+    for k in range(K):
+        back = (K - 1 - k) * l
+        if back < n:
+            out[back:, k * d:(k + 1) * d] = x[:n - back]
+    return out
+
+
+def nextitnet_encode(p, x, dilations, kernel_size):
+    """q (float64) of the inputs x (item indices, oldest first, at most max_len): the encoder's last position; p maps the parameter
+    names to float64 arrays"""
+    h = p['E'][list(x)]
+    for b, l in enumerate(dilations):
+        w = {name: p['%s_%d' % (name, b)] for name in NEXTITNET_BLOCK}
+        a = np.maximum(_layer_norm(_causal_taps(h, kernel_size, l) @ w['C1'] + w['c1'], w['g1'], w['n1']), 0.0)
+        h = h + np.maximum(_layer_norm(_causal_taps(a, kernel_size, 2 * l) @ w['C2'] + w['c2'], w['g2'], w['n2']), 0.0)
+    return h[-1]
+
+
+class NextItNet(Baseline):
+    '''
+    NextItNet(embedding=100, dilations=(1, 2, 1, 2, 1, 2), kernel_size=3, n_epochs=10, batch_size=128, learning_rate=0.001, max_len=50,
+              seed=42, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Convolutional sequence model in the style of NextItNet (Yuan et al., WSDM 2019), trained on the device with full-catalogue
+    cross-entropy and Adam.  This is this project's definition (DESIGN §3w); no parity with another framework is claimed.  The
+    defaults follow the style of the published code's configuration and were not checked against the paper's experiments.
+
+    The input embedding E [n_items x embedding] and the output side W [n_items x embedding], bW [n_items] are separate tables.  For
+    the last max_len inputs x_0 .. x_(n-1) of a session prefix, positions before 0 reading zeros: h_t = E[x_t]; one residual block
+    per dilation l, u_t = c1 + sum_k h_(t - (K-1-k) l) C1[k], a = relu(LN1(u)), v_t = c2 + sum_k a_(t - (K-1-k) 2l) C2[k] and
+    h'_t = h_t + relu(LN2(v)), with K = kernel_size; q is the last position's h and item i scores W[i] . q + bW[i].  Training cuts
+    each session (events by time_key, ties by row order) into pieces of at most max_len + 1 events overlapping by one, encodes each
+    piece causally, and per mini-batch of batch_size pieces takes one Adam step on the mean cross-entropy over its positions.
+    There is no dropout.  The parameters are float32 and drawn, like the epochs' piece orders, from np.random.RandomState(seed).
+    fit prints the epoch's mean loss; `fit_stats` holds per epoch (mean loss, device ms, per-step losses).  predict_next computes
+    the scores on the host in float64 from the float32 parameters.
+    '''
+    _kind = 'nextitnet'
+
+    def __init__(self, embedding=100, dilations=(1, 2, 1, 2, 1, 2), kernel_size=3, n_epochs=10, batch_size=128, learning_rate=0.001,
+                 max_len=50, seed=42, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.dilations = dilations
+        self.kernel_size = kernel_size
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        self._integer('embedding', 1, 1024)
+        self._integer('kernel_size', 1, 8)
+        dl = self.dilations
+        if (isinstance(dl, (str, bytes)) or not hasattr(dl, '__len__') or not 1 <= len(dl) <= 16 or
+                any(isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= 256 for v in dl)):
+            raise ValueError('dilations must be 1 .. 16 integers, each in 1 .. 256, not %r' % (dl,))
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 1, 512)
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+
+    def pieces(self, data):
+        """(piece offsets, piece items) of the training data, after the item index (_index): pieces of at most max_len inputs"""
+        idx, _, offsets, o = self._sessions(data, 'time')
+        return narm_pieces(offsets, idx[o], self.max_len + 1)
+
+    def fit(self, data):
+        self._check()
+        poff, pitems = self.pieces(data)
+        if len(poff) < 2:
+            raise ValueError('NextItNet needs a training session of at least 2 events')
+        rs = np.random.RandomState(self.seed)
+        params = nextitnet_init(self.n_items, self.embedding, self.dilations, self.kernel_size, rs)
+        self._drop_caches()
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.nextitnet_begin(self.dilations, self.kernel_size, self.max_len, self.batch_size, poff, pitems, params)
+        self.fit_stats = []
+        for epoch in range(self.n_epochs):
+            losses, ms = dev.nextitnet_epoch(rs.permutation(len(poff) - 1), self.learning_rate)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.nextitnet_export()
+        self._upload(dev)                        # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.nextitnet_import(self.dilations, self.kernel_size, self.max_len, self.params)
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            p = self._p64 = {k: v.astype(np.float64) for k, v in
+                             nextitnet_unpack(self.params, self.n_items, self.embedding, self.dilations, self.kernel_size).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['W'] @ nextitnet_encode(p, list(prefix)[-self.max_len:], self.dilations, self.kernel_size) + p['bW']
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
         score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))

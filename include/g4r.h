@@ -603,6 +603,36 @@ int g4r_bl_stamp_import(g4r_baselines* b, int32_t max_len, const float* params, 
 int g4r_bl_stamp_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                         const int32_t* n_history, float* q, int64_t n_q);
 
+/* ---- NextItNet convolutional baseline (DESIGN §3w) -----------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_NEXTITNET, n_items, d (1 .. 1024), ...); kind 18 is not used.  The model is one flat float32 vector:
+ * E [n_items x d] (the input embedding), per block b (one per dilation l_b) C1 [K d x d], c1, g1, n1 [d], C2 [K d x d], c2, g2,
+ * n2 [d] (row k d + i of a kernel: tap k, input channel i), then W [n_items x d] and bW [n_items] (the scored item side);
+ * n_params = 2 n_items d + n_items + n_dilations (2 K d^2 + 6 d).  For the inputs x_0 .. x_(n-1) of a piece or window, positions before 0 reading zeros: h_t = E[x_t];
+ * per block u_t = c1 + sum_k h_(t - (K-1-k) l) C1[k], a = relu(LN1(u)), v_t = c2 + sum_k a_(t - (K-1-k) 2l) C2[k],
+ * h'_t = h_t + relu(LN2(v)); q_t = h_t after the last block and score(i) = W[i] . q_t + bW[i].  LN is SASRec's (eps 1e-8). */
+#define G4R_BL_NEXTITNET 19
+/* Begins a fit: 1 .. 16 dilations each in 1 .. 256, kernel_size 1 .. 8, max_len 1 .. 512, batch_size >= 1, the training pieces as
+ * CSR (2 .. max_len + 1 events each, inputs then the last target) and the initial parameters.  Adam's moments start at 0.  Every
+ * argument is checked before any device write; G4R_ERR_CUDA with a message naming the sizes if the device cannot hold the largest
+ * batch's logits and activations. */
+int g4r_bl_nextitnet_begin(g4r_baselines* b, const int32_t* dilations, int32_t n_dilations, int32_t kernel_size, int32_t max_len,
+                           int32_t batch_size, const int64_t* piece_offsets, int64_t n_pieces, const int32_t* items, int64_t n_entries,
+                           const float* params, int64_t n_params);
+/* One epoch: mini-batches of batch_size consecutive pieces of order, the mean full-catalogue cross-entropy over the batch's
+ * positions and one Adam step each (NARM's constants).  A batch past the positions of the batch_size longest pieces is refused
+ * before any device write. */
+int g4r_bl_nextitnet_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, float learning_rate, float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size pieces at the current parameters, without an update: the mean loss and its gradient. */
+int g4r_bl_nextitnet_grads(g4r_baselines* b, const int32_t* pieces, int32_t n, float* loss, float* grads);
+int g4r_bl_nextitnet_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (finite); ends any fit in progress. */
+int g4r_bl_nextitnet_import(g4r_baselines* b, const int32_t* dilations, int32_t n_dilations, int32_t kernel_size, int32_t max_len,
+                            const float* params, int64_t n_params);
+/* Every counted event's q (the last max_len inputs of items[start .. p]) in g4r_bl_evaluate's order.
+ * g4r_bl_evaluate of a NextItNet handle ranks these q as NARM's, with I = double(W) and bI = double(bW). */
+int g4r_bl_nextitnet_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                            const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif
