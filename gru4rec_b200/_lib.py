@@ -58,7 +58,8 @@ EXPORTS = [
     'g4r_bl_sasrec_encode', 'g4r_bl_srgnn_begin', 'g4r_bl_srgnn_epoch', 'g4r_bl_srgnn_grads', 'g4r_bl_srgnn_export',
     'g4r_bl_srgnn_import', 'g4r_bl_srgnn_encode', 'g4r_bl_stamp_begin', 'g4r_bl_stamp_epoch', 'g4r_bl_stamp_grads', 'g4r_bl_stamp_export',
     'g4r_bl_stamp_import', 'g4r_bl_stamp_encode', 'g4r_bl_nextitnet_begin', 'g4r_bl_nextitnet_epoch', 'g4r_bl_nextitnet_grads',
-    'g4r_bl_nextitnet_export', 'g4r_bl_nextitnet_import', 'g4r_bl_nextitnet_encode',
+    'g4r_bl_nextitnet_export', 'g4r_bl_nextitnet_import', 'g4r_bl_nextitnet_encode', 'g4r_bl_bert4rec_begin', 'g4r_bl_bert4rec_epoch',
+    'g4r_bl_bert4rec_grads', 'g4r_bl_bert4rec_export', 'g4r_bl_bert4rec_import', 'g4r_bl_bert4rec_encode',
 ]
 
 _lib = None
@@ -196,6 +197,12 @@ def load():
     lib.g4r_bl_nextitnet_export.argtypes = [vp, vp, i64]
     lib.g4r_bl_nextitnet_import.argtypes = [vp, vp, i32, i32, i32, vp, i64]
     lib.g4r_bl_nextitnet_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
+    lib.g4r_bl_bert4rec_begin.argtypes = [vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i64]
+    lib.g4r_bl_bert4rec_epoch.argtypes = [vp, vp, i64, vp, i64, u32, f32, f32, vp, C.POINTER(C.c_float)]
+    lib.g4r_bl_bert4rec_grads.argtypes = [vp, vp, i32, vp, i64, u32, i64, f32, C.POINTER(C.c_float), vp]
+    lib.g4r_bl_bert4rec_export.argtypes = [vp, vp, i64]
+    lib.g4r_bl_bert4rec_import.argtypes = [vp, i32, i32, i32, vp, i64]
+    lib.g4r_bl_bert4rec_encode.argtypes = [vp, vp, i64, vp, i64, vp, vp, i64]
     _lib = lib
     return lib
 
@@ -821,7 +828,7 @@ class Engine(object):
 
 
 BASELINE_KINDS = {'pop': 0, 'sessionpop': 1, 'itemknn': 2, 'bpr': 3, 'sknn': 5, 'stan': 6, 'sr': 8, 'ar': 9, 'vstan': 11, 'narm': 12, 'sasrec': 13, 'srgnn': 15, 'stamp': 17,
-                  'nextitnet': 19}
+                  'nextitnet': 19, 'bert4rec': 21}
 SKNN_SIMILARITY = {'cosine': 0, 'vector': 1}
 RULES_WEIGHTING = {'div': 0, 'same': 1}
 RULES_STEPS_MAX = 20
@@ -856,9 +863,9 @@ def rules_bound(session_offsets, items, n_items, steps, weighting):
 class Baselines(object):
     """Owns one g4r_baselines handle (DESIGN §3j): the fitted ItemKNN rows or Pop scores on the device, and the evaluation of
     a baseline, the BPR-MF fit and factors (DESIGN §3k), the SessionKNN, STAN and VSTAN indexes (DESIGN §3o, §3p, §3r), and the
-    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec, SR-GNN, STAMP and NextItNet fits and parameters (DESIGN
-    §3s, §3t, §3u, §3v, §3w).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm', 'sasrec',
-    'srgnn', 'stamp' or 'nextitnet'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
+    SR / AR fit into ItemKNN's rows (DESIGN §3q), and the NARM, SASRec, SR-GNN, STAMP, NextItNet and BERT4Rec fits and parameters
+    (DESIGN §3s, §3t, §3u, §3v, §3w, §3x).  kind: 'pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'sr', 'ar', 'vstan', 'narm',
+    'sasrec', 'srgnn', 'stamp', 'nextitnet' or 'bert4rec'; n_keep: top_n, n_sims, n_factors, k, pruning or embedding."""
 
     def __init__(self, kind, n_items, n_keep, device=0):
         lib = load()
@@ -1331,4 +1338,63 @@ class Baselines(object):
         n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
         q = np.empty((n, self.n_keep), np.float32)
         self._check(self.lib.g4r_bl_nextitnet_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
+        return q
+
+    # ---- BERT4Rec (DESIGN §3x) ----
+    def bert4rec_n_params(self, n_blocks, max_len):
+        d = self.n_keep
+        return (self.n_items + 1) * d + int(max_len) * d + 2 * d + int(n_blocks) * (12 * d * d + 13 * d) + d * d + 3 * d + self.n_items
+
+    def _bert4rec_params(self, n_blocks, max_len, params):
+        th = np.ascontiguousarray(params, dtype=np.float32).ravel()
+        n = self.bert4rec_n_params(n_blocks, max_len)
+        if th.size != n:
+            raise ValueError('bert4rec: need %d parameters ((n_items + 1) d + max_len d + 2 d + n_blocks (12 d^2 + 13 d) + d^2 + 3 d + n_items), '
+                             'not %d' % (n, th.size))
+        return th
+
+    def bert4rec_begin(self, n_blocks, n_heads, max_len, batch_size, piece_offsets, items, params):
+        """starts a BERT4Rec fit: the training pieces (CSR of item indices, 2 .. max_len events each, all inputs) and the initial
+        flat parameters"""
+        off = np.ascontiguousarray(piece_offsets, dtype=np.int64); it = np.ascontiguousarray(items, dtype=np.int32)
+        th = self._bert4rec_params(n_blocks, max_len, params)
+        self._check(self.lib.g4r_bl_bert4rec_begin(self.h, int(n_blocks), int(n_heads), int(max_len), int(batch_size), _ptr(off), off.size - 1,
+                                                   _ptr(it), it.size, _ptr(th), th.size))
+        self.bert4rec_shape, self.bert4rec_batch = (int(n_blocks), int(max_len)), int(batch_size)
+
+    def bert4rec_epoch(self, order, masks, seed, learning_rate, dropout):
+        """one epoch over the pieces in `order`, masks one byte (0 / 1) per stored entry; returns (per-step losses float32, device
+        ms)"""
+        od = np.ascontiguousarray(order, dtype=np.int32); mk = np.ascontiguousarray(masks, dtype=np.uint8)
+        losses = np.zeros(-(-od.size // self.bert4rec_batch), np.float32); ms = C.c_float()
+        self._check(self.lib.g4r_bl_bert4rec_epoch(self.h, _ptr(od), od.size, _ptr(mk), mk.size, int(seed) & 0xffffffff, float(learning_rate),
+                                                   float(dropout), _ptr(losses), C.byref(ms)))
+        return losses, ms.value
+
+    def bert4rec_grads(self, pieces, masks, seed, step, dropout):
+        """(loss, flat gradient float32) of one mini-batch of pieces at the current parameters, without an update"""
+        pc = np.ascontiguousarray(pieces, dtype=np.int32); mk = np.ascontiguousarray(masks, dtype=np.uint8)
+        g = np.empty(self.bert4rec_n_params(*self.bert4rec_shape), np.float32); loss = C.c_float()
+        self._check(self.lib.g4r_bl_bert4rec_grads(self.h, _ptr(pc), pc.size, _ptr(mk), mk.size, int(seed) & 0xffffffff, int(step),
+                                                   float(dropout), C.byref(loss), _ptr(g)))
+        return loss.value, g
+
+    def bert4rec_export(self):
+        th = np.empty(self.bert4rec_n_params(*self.bert4rec_shape), np.float32)
+        self._check(self.lib.g4r_bl_bert4rec_export(self.h, _ptr(th), th.size))
+        return th
+
+    def bert4rec_import(self, n_blocks, n_heads, max_len, params):
+        th = self._bert4rec_params(n_blocks, max_len, params)
+        self._check(self.lib.g4r_bl_bert4rec_import(self.h, int(n_blocks), int(n_heads), int(max_len), _ptr(th), th.size))
+        self.bert4rec_shape = (int(n_blocks), int(max_len))
+
+    def bert4rec_encode(self, items, session_offsets, n_history=None):
+        """every counted event's q [n, d] float32, in evaluate's order"""
+        it = np.ascontiguousarray(items, dtype=np.int32); off = np.ascontiguousarray(session_offsets, dtype=np.int64)
+        nh = None if n_history is None else np.ascontiguousarray(n_history, dtype=np.int32)
+        lens = np.diff(off)
+        n = int(np.maximum(0, lens - np.maximum(nh if nh is not None else 0, 1)).sum()) if lens.size else 0
+        q = np.empty((n, self.n_keep), np.float32)
+        self._check(self.lib.g4r_bl_bert4rec_encode(self.h, _ptr(it), it.size, _ptr(off), off.size - 1, _ptr(nh), _ptr(q), n))
         return q

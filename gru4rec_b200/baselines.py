@@ -1,11 +1,13 @@
 """Session baselines of the reference (baselines.py:52-418): Pop, SessionPop, ItemKNN and BPR (BPR-MF), with its constructor
 signatures, fit(data) and predict_next(session_id, input_item_id, predict_for_item_ids), session-based kNN (SessionKNN, DESIGN
 §3o; STAN, §3p; VSTAN, §3r), the rule-based baselines (SR and AR, §3q, fitted on the device) and the neural NARM (§3s), SASRec
-(§3t), SR-GNN (§3u), STAMP (§3v) and NextItNet (§3w), trained on the device, with the same surface.  ItemKNN's fit runs on the
+(§3t), SR-GNN (§3u), STAMP (§3v), NextItNet (§3w) and BERT4Rec (§3x), trained on the device, with the same surface.  ItemKNN's fit runs on the
 device (the co-occurrence counts, the normalisation and the top n_sims per row, DESIGN §3j), and so does BPR's SGD, equal to the reference's
 sequential run for the same np.random state (DESIGN §3k); evaluate_gpu / evaluate_events rank every test event of a baseline on the
 device under the same protocol as a GRU4Rec model.  predict_next is computed on the host from the fitted model.  RandomPred is not
 provided: it has nothing to fit, and its scores are unseeded noise."""
+import math
+
 import numpy as np
 import pandas as pd
 
@@ -1424,6 +1426,200 @@ class NextItNet(Baseline):
         """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
         p = self.params64()
         return p['W'] @ nextitnet_encode(p, list(prefix)[-self.max_len:], self.dilations, self.kernel_size) + p['bW']
+
+    def predict_next(self, session_id, input_item_id, predict_for_item_ids):
+        score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))
+        return pd.Series(data=score[self.itemidmap[predict_for_item_ids].values], index=predict_for_item_ids)
+
+
+BERT4REC_BLOCK = ('Wq', 'bq', 'Wk', 'bk', 'Wv', 'bv', 'Wo', 'bo', 'g1', 'c1', 'W1', 'b1', 'W2', 'b2', 'g2', 'c2')
+
+
+def bert4rec_shapes(n_items, d, n_blocks, max_len):
+    """the parameters in the order of the flat vector (DESIGN §3x): E (n_items + 1 rows, the last the mask token), Pe, g0, c0, per
+    block b the BERT4REC_BLOCK names with suffix _b (Wq .. Wo: [d x d], W1: [d x 4d], b1: [4d], W2: [4d x d], the rest [d]), Wp,
+    bp, gp, cp, bO [n_items]"""
+    out = dict(E=(n_items + 1, d), Pe=(max_len, d), g0=(d,), c0=(d,))
+    for b in range(n_blocks):
+        for name in BERT4REC_BLOCK:
+            out['%s_%d' % (name, b)] = {'W1': (d, 4 * d), 'b1': (4 * d,), 'W2': (4 * d, d)}.get(name, (d, d) if name[0] == 'W' else (d,))
+    out['Wp'], out['bp'], out['gp'], out['cp'], out['bO'] = (d, d), (d,), (d,), (d,), (n_items,)
+    return out
+
+
+def bert4rec_unpack(flat, n_items, d, n_blocks, max_len):
+    """name -> view of the flat parameter vector"""
+    out, o = {}, 0
+    for name, shp in bert4rec_shapes(n_items, d, n_blocks, max_len).items():
+        n = int(np.prod(shp))
+        out[name] = flat[o:o + n].reshape(shp)
+        o += n
+    return out
+
+
+def bert4rec_init(n_items, d, n_blocks, max_len, rs):
+    """the initial parameters, float32 flat, by sasrec_init's rule: in the order of the vector each matrix [r x c] (E and Pe
+    included) drawn from rs.uniform(-s, s) with s = sqrt(6 / (r + c)); biases 0 and gains 1, without draws"""
+    parts = []
+    for name, shp in bert4rec_shapes(n_items, d, n_blocks, max_len).items():
+        if len(shp) == 2:
+            s = np.sqrt(6.0 / (shp[0] + shp[1]))
+            parts.append(rs.uniform(-s, s, size=shp))
+        else:
+            parts.append(np.full(shp, 1.0 if name[0] == 'g' else 0.0))
+    return np.concatenate([p.ravel() for p in parts]).astype(np.float32)
+
+
+def bert4rec_masks(piece_offsets, mask_prob, rs):
+    """the cloze masks of one epoch, uint8 per stored entry: one rs.random_sample over the entries in storage order, an entry masked
+    when its draw is below mask_prob, and a piece with no masked entry gets its last entry masked"""
+    off = np.asarray(piece_offsets, dtype=np.int64)
+    mk = (rs.random_sample(int(off[-1])) < mask_prob).astype(np.uint8)
+    none = np.add.reduceat(mk.astype(np.int64), off[:-1]) == 0 if len(off) > 1 else np.zeros(0, bool)
+    mk[off[1:][none] - 1] = 1
+    return mk
+
+
+_erf = np.frompyfunc(math.erf, 1, 1)
+
+
+def _gelu(x):
+    """exact-erf GELU, x Phi(x)"""
+    return 0.5 * x * (1.0 + _erf(x / np.sqrt(2.0)).astype(np.float64))
+
+
+def bert4rec_encode(p, x, n_heads):
+    """q (float64) of the inputs x (item indices, oldest first, at most max_len - 1) followed by the mask token: the head's output at
+    the mask; p maps the parameter names to float64 arrays"""
+    d = p['E'].shape[1]
+    dh = d // n_heads
+    sh = sasrec_scales(d, n_heads)[1]
+    x = list(x) + [p['E'].shape[0] - 1]
+    n = len(x)
+    h = _layer_norm(p['E'][x] + p['Pe'][:n], p['g0'], p['c0'])
+    b = 0
+    while 'g1_%d' % b in p:
+        w = {name: p['%s_%d' % (name, b)] for name in BERT4REC_BLOCK}
+        Q, K, V = h @ w['Wq'] + w['bq'], h @ w['Wk'] + w['bk'], h @ w['Wv'] + w['bv']
+        A = np.empty_like(h)
+        for k in range(n_heads):
+            cs = slice(k * dh, (k + 1) * dh)
+            S = (Q[:, cs] @ K[:, cs].T) * sh
+            P = np.exp(S - S.max(axis=1, keepdims=True))
+            A[:, cs] = (P / P.sum(axis=1, keepdims=True)) @ V[:, cs]
+        a = _layer_norm(h + A @ w['Wo'] + w['bo'], w['g1'], w['c1'])
+        h = _layer_norm(a + _gelu(a @ w['W1'] + w['b1']) @ w['W2'] + w['b2'], w['g2'], w['c2'])
+        b += 1
+    return _layer_norm(_gelu(h[-1] @ p['Wp'] + p['bp']), p['gp'], p['cp'])
+
+
+class BERT4Rec(Baseline):
+    '''
+    BERT4Rec(embedding=64, n_blocks=2, n_heads=2, n_epochs=10, batch_size=256, learning_rate=0.001, dropout=0.1, mask_prob=0.2,
+             max_len=50, seed=42, session_key='SessionId', item_key='ItemId', time_key='Time')
+
+    Bidirectional self-attentive sequential recommender in the style of BERT4Rec (Sun et al., CIKM 2019), trained on the device by
+    the cloze objective with full-catalogue cross-entropy and Adam.  This is this project's definition (DESIGN §3x); no parity with
+    another framework is claimed.  The defaults follow the paper's architecture (embedding 64, 2 blocks of 2 heads, dropout 0.1,
+    max_len 50); the paper's training budget (about 400k steps at learning rate 1e-4), its weight decay and its learning-rate
+    schedule are not reproduced, and the defaults were not checked against the paper's experiments.
+
+    One item table E [(n_items + 1) x embedding], whose last row is the mask token, is the input embedding and the output item
+    side.  For inputs x_0 .. x_(n-1), some of them the mask token: h = drop(LN0(E[x_t] + Pe[t])); n_blocks post-LN Transformer
+    blocks, a = LN1(h + drop(A Wo + bo)) with A multi-head softmax attention over all n positions, h = LN2(a + drop(gelu(a W1 +
+    b1) W2 + b2)); the head q_t = LNp(gelu(h_t Wp + bp)), and item i scores E[i] . q_t + bO[i].  Training cuts each session (events
+    by time_key, ties by row order) into pieces of at most max_len events overlapping by one; each epoch masks every entry with
+    probability mask_prob (a piece with none gets its last entry masked, see bert4rec_masks), replaces the masked entries by the
+    mask token and, per mini-batch of batch_size pieces, takes one Adam step on the mean cross-entropy over the masked positions,
+    with dropout on h0 and on both residual branches of every block.  A prefix is scored from its last max_len - 1 inputs followed
+    by the mask token, q the head's output at the mask.  The parameters are float32 and drawn, like the epochs' piece orders and
+    masks, from np.random.RandomState(seed).  fit prints the epoch's mean loss; `fit_stats` holds per epoch (mean loss, device ms,
+    per-step losses).  predict_next computes the scores on the host in float64 from the float32 parameters.
+    '''
+    _kind = 'bert4rec'
+
+    def __init__(self, embedding=64, n_blocks=2, n_heads=2, n_epochs=10, batch_size=256, learning_rate=0.001, dropout=0.1, mask_prob=0.2,
+                 max_len=50, seed=42, session_key='SessionId', item_key='ItemId', time_key='Time'):
+        self.embedding = embedding
+        self.n_blocks = n_blocks
+        self.n_heads = n_heads
+        self.n_epochs = n_epochs
+        self.batch_size = batch_size
+        self.learning_rate = learning_rate
+        self.dropout = dropout
+        self.mask_prob = mask_prob
+        self.max_len = max_len
+        self.seed = seed
+        self.session_key = session_key
+        self.item_key = item_key
+        self.time_key = time_key
+        self.current_session = None
+
+    def _n_keep(self):
+        return self.embedding
+
+    def _check(self):
+        self._integer('embedding', 1, 1024)
+        self._integer('n_heads', 1, self.embedding)
+        if self.embedding % self.n_heads:
+            raise ValueError('n_heads must divide embedding, not %r into %r' % (self.n_heads, self.embedding))
+        self._integer('n_blocks', 1, 8)
+        self._integer('n_epochs', 0, 1 << 30)
+        self._integer('batch_size', 1, 1 << 20)
+        self._integer('max_len', 2, 512)
+        if (self.n_blocks + 1) * self.batch_size * self.max_len * self.embedding >= 1 << 32:
+            raise ValueError('(n_blocks + 1) * batch_size * max_len * embedding must stay below 2^32 (dropout indices)')
+        if not 0.0 < float(self.learning_rate) < np.inf:
+            raise ValueError('learning_rate must be finite and > 0, not %r' % (self.learning_rate,))
+        if not 0.0 <= float(self.dropout) < 1.0:
+            raise ValueError('dropout must be in [0, 1), not %r' % (self.dropout,))
+        if not 0.0 <= float(self.mask_prob) <= 1.0:
+            raise ValueError('mask_prob must be in [0, 1], not %r' % (self.mask_prob,))
+
+    def pieces(self, data):
+        """(piece offsets, piece items) of the training data, after the item index (_index): pieces of at most max_len events, all
+        of them inputs"""
+        idx, _, offsets, o = self._sessions(data, 'time')
+        return narm_pieces(offsets, idx[o], self.max_len)
+
+    def fit(self, data):
+        self._check()
+        poff, pitems = self.pieces(data)
+        if len(poff) < 2:
+            raise ValueError('BERT4Rec needs a training session of at least 2 events')
+        rs = np.random.RandomState(self.seed)
+        params = bert4rec_init(self.n_items, self.embedding, self.n_blocks, self.max_len, rs)
+        self._drop_caches()
+        dev = _lib.Baselines(self._kind, self.n_items, self.embedding)
+        dev.bert4rec_begin(self.n_blocks, self.n_heads, self.max_len, self.batch_size, poff, pitems, params)
+        self.fit_stats = []
+        for epoch in range(self.n_epochs):
+            order = rs.permutation(len(poff) - 1)
+            masks = bert4rec_masks(poff, self.mask_prob, rs)
+            losses, ms = dev.bert4rec_epoch(order, masks, self.seed, self.learning_rate, self.dropout)
+            mean = float(np.mean(losses.astype(np.float64)))
+            self.fit_stats.append((mean, ms, losses))
+            print(epoch, mean)
+        self.params = dev.bert4rec_export()
+        self._upload(dev)                        # ends the fit: the scratch leaves the device
+        self.current_session = None
+        self._dev = dev
+
+    def _upload(self, dev):
+        dev.bert4rec_import(self.n_blocks, self.n_heads, self.max_len, self.params)
+
+    def params64(self):
+        """name -> float64 copy of each parameter"""
+        p = self.__dict__.get('_p64')
+        if p is None:
+            p = self._p64 = {k: v.astype(np.float64) for k, v in
+                             bert4rec_unpack(self.params, self.n_items, self.embedding, self.n_blocks, self.max_len).items()}
+        return p
+
+    def score_prefix(self, prefix):
+        """float64 scores [n_items] after the session's input item indices so far `prefix` (the current input last)"""
+        p = self.params64()
+        return p['E'][:self.n_items] @ bert4rec_encode(p, list(prefix)[-(self.max_len - 1):], self.n_heads) + p['bO']
 
     def predict_next(self, session_id, input_item_id, predict_for_item_ids):
         score = self.score_prefix(self._prefix(session_id, self.itemidmap[input_item_id]))

@@ -6,7 +6,7 @@
 
 constexpr int BL_POP = 0, BL_SESSIONPOP = 1, BL_ITEMKNN = 2, BL_BPR = 3, BL_SKNN = 5, BL_STAN = 6, BL_SR = 8, BL_AR = 9,
               BL_VSTAN = 11, BL_NARM = 12, BL_SASREC = 13, BL_SRGNN = 15, BL_STAMP = 17,
-              BL_NEXTITNET = 19;                         // 4, 7, 10, 14, 16 and 18 stay unused
+              BL_NEXTITNET = 19, BL_BERT4REC = 21;       // 4, 7, 10, 14, 16, 18 and 20 stay unused
 constexpr int BPR_F_MAX = 1024;                        // n_factors bound of a BPR handle (g4r_bpr.cuh)
 constexpr int KF_THREADS = 256;
 constexpr int KF_KEEP_MAX = 1024;                       // n_sims bound: the kept entries of a row are sorted in shared memory
@@ -95,6 +95,12 @@ struct g4r_baselines {
   std::vector<int> ni_dil;
   int ni_K = 0;
   float* ni_f = nullptr;
+  // BERT4Rec (g4r_bert4rec.cuh) keeps its parameters, fit, plan and scratch in the NARM fields above (nm_len its max_len, nm_off
+  // the device's padded piece offsets) and its n_blocks / n_heads in SASRec's, plus its per-position activations, the masked rows'
+  // targets and the device copy of the mask bytes (b4_f, b4_my, b4_mk, in nm_mem)
+  float* b4_f = nullptr;
+  int* b4_my = nullptr;
+  unsigned char* b4_mk = nullptr;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -121,6 +127,7 @@ static int sasrec_rank(g4r_baselines* h, BlCall& c);   // g4r_sasrec.cuh
 static int srgnn_rank(g4r_baselines* h, BlCall& c);    // g4r_srgnn.cuh
 static int stamp_rank(g4r_baselines* h, BlCall& c);    // g4r_stamp.cuh
 static int nextitnet_rank(g4r_baselines* h, BlCall& c);   // g4r_nextitnet.cuh
+static int bert4rec_rank(g4r_baselines* h, BlCall& c);    // g4r_bert4rec.cuh
 enum BlStore { BL_STORE_NONE, BL_STORE_ROWS, BL_STORE_POP, BL_STORE_BPR };
 struct BlKind { int keep_max; BlStore store; int (*rank)(g4r_baselines*, BlCall&); };
 constexpr BlKind BL_KINDS[] = {
@@ -144,6 +151,8 @@ constexpr BlKind BL_KINDS[] = {
     {BPR_F_MAX, BL_STORE_NONE, stamp_rank},             // 17 STAMP
     {0, BL_STORE_NONE, nullptr},
     {BPR_F_MAX, BL_STORE_NONE, nextitnet_rank},         // 19 NextItNet
+    {0, BL_STORE_NONE, nullptr},
+    {BPR_F_MAX, BL_STORE_NONE, bert4rec_rank},          // 21 BERT4Rec
 };
 static bool bl_kind_ok(int kind) { return kind >= 0 && kind < (int)(sizeof(BL_KINDS) / sizeof(BL_KINDS[0])) && BL_KINDS[kind].rank; }
 // the kinds whose model is ItemKNN's rows
@@ -697,13 +706,13 @@ extern "C" int g4r_bl_destroy(g4r_baselines* h) {
 extern "C" int g4r_bl_create(int32_t kind, int32_t n_items, int32_t n_keep, int32_t device, g4r_baselines** out) {
   if (!out) { g_bl_create_error = "null argument"; return G4R_ERR_INVALID; }
   if (!bl_kind_ok(kind)) {
-    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR), 11 (VSTAN), 12 (NARM), 13 (SASRec), 15 (SR-GNN), 17 (STAMP) or 19 (NextItNet)";
+    g_bl_create_error = "kind must be 0 (Pop), 1 (SessionPop), 2 (ItemKNN), 3 (BPR), 5 (SessionKNN), 6 (STAN), 8 (SR), 9 (AR), 11 (VSTAN), 12 (NARM), 13 (SASRec), 15 (SR-GNN), 17 (STAMP), 19 (NextItNet) or 21 (BERT4Rec)";
     return G4R_ERR_INVALID;
   }
   const BlStore store = BL_KINDS[kind].store;
   if (n_items < 1 || n_keep < 1 || n_keep > BL_KINDS[kind].keep_max) {
     g_bl_create_error = "need n_items >= 1 and 1 <= n_keep (<= " + std::to_string(KF_KEEP_MAX) + " for ItemKNN, SessionKNN, STAN, SR, AR and VSTAN, <= " +
-                        std::to_string(BPR_F_MAX) + " n_factors for BPR and embedding for NARM, SASRec, SR-GNN, STAMP and NextItNet)";
+                        std::to_string(BPR_F_MAX) + " n_factors for BPR and embedding for NARM, SASRec, SR-GNN, STAMP, NextItNet and BERT4Rec)";
     return G4R_ERR_INVALID;
   }
   int dev_count = 0;

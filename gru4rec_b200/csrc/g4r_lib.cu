@@ -1758,3 +1758,4 @@ extern "C" int g4r_copy_item_tables(g4r_handle* h, g4r_handle* src, const float*
 #include "g4r_srgnn.cuh"
 #include "g4r_stamp.cuh"
 #include "g4r_nextitnet.cuh"
+#include "g4r_bert4rec.cuh"

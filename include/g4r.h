@@ -633,6 +633,42 @@ int g4r_bl_nextitnet_import(g4r_baselines* b, const int32_t* dilations, int32_t 
 int g4r_bl_nextitnet_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
                             const int32_t* n_history, float* q, int64_t n_q);
 
+/* ---- BERT4Rec bidirectional baseline (DESIGN §3x) ------------------------------------------------------------------------------
+ * g4r_bl_create(G4R_BL_BERT4REC, n_items, d (1 .. 1024), ...); kind 20 is not used.  The model is one flat float32 vector:
+ * E [(n_items + 1) x d] (row n_items the mask token; rows 0 .. n_items - 1 the input embedding and the scored item side),
+ * Pe [max_len x d], g0, c0 [d], per block Wq, bq, Wk, bk, Wv, bv, Wo, bo ([d x d], [d]), g1, c1 [d], W1 [d x 4d], b1 [4d],
+ * W2 [4d x d], b2, g2, c2 [d], then Wp [d x d], bp, gp, cp [d] and bO [n_items];
+ * n_params = (n_items + 1) d + max_len d + 2 d + n_blocks (12 d^2 + 13 d) + d^2 + 3 d + n_items.
+ * For inputs x_0 .. x_(n-1) (some of them the mask token): h = drop(LN0(E[x_t] + Pe[t])); per block a = LN1(h + drop(A Wo + bo)),
+ * A multi-head softmax attention over all n positions (scale 1 / sqrt(d / n_heads)), h = LN2(a + drop(gelu(a W1 + b1) W2 + b2))
+ * (exact-erf GELU); q_t = LNp(gelu(h_t Wp + bp)) and score(i) = E[i] . q_t + bO[i] over the n_items real items.  LN is SASRec's
+ * (eps 1e-8). */
+#define G4R_BL_BERT4REC 21
+/* Begins a fit: n_blocks 1 .. 8, n_heads dividing d, max_len 2 .. 512, batch_size >= 1, the training pieces as CSR (2 .. max_len
+ * events each, all of them inputs) and the initial parameters.  Adam's moments start at 0.  Every argument is checked before any
+ * device write; G4R_ERR_CUDA with a message naming the sizes if the device cannot hold the largest batch's logits and activations. */
+int g4r_bl_bert4rec_begin(g4r_baselines* b, int32_t n_blocks, int32_t n_heads, int32_t max_len, int32_t batch_size, const int64_t* piece_offsets,
+                          int64_t n_pieces, const int32_t* items, int64_t n_entries, const float* params, int64_t n_params);
+/* One epoch: mini-batches of batch_size consecutive pieces of order, masks one byte (0 or 1) per stored entry (n_masks = n_entries,
+ * at least one masked entry in every piece used): each masked entry is replaced by the mask token, and the mean full-catalogue
+ * cross-entropy over the batch's masked positions takes one Adam step (NARM's constants).  dropout in [0, 1) on h0 and both
+ * residual branches of every block, keyed by (seed, global step).  A batch past the positions of the batch_size longest pieces is
+ * refused before any device write. */
+int g4r_bl_bert4rec_epoch(g4r_baselines* b, const int32_t* order, int64_t n_order, const uint8_t* masks, int64_t n_masks, uint32_t seed,
+                          float learning_rate, float dropout, float* losses, float* device_ms);
+/* One mini-batch of n <= batch_size pieces at the current parameters and the given step's dropout, without an update: the mean
+ * loss and its gradient. */
+int g4r_bl_bert4rec_grads(g4r_baselines* b, const int32_t* pieces, int32_t n, const uint8_t* masks, int64_t n_masks, uint32_t seed, int64_t step,
+                          float dropout, float* loss, float* grads);
+int g4r_bl_bert4rec_export(g4r_baselines* b, float* params, int64_t n_params);
+/* The parameters of a fitted model (finite); ends any fit in progress. */
+int g4r_bl_bert4rec_import(g4r_baselines* b, int32_t n_blocks, int32_t n_heads, int32_t max_len, const float* params, int64_t n_params);
+/* Every counted event's q in g4r_bl_evaluate's order: the head's output at the mask token of the window of the last
+ * min(p, max_len - 1) inputs of items[start .. p] followed by the mask token.  g4r_bl_evaluate of a BERT4Rec handle ranks these q
+ * as NARM's, with I = double(E[0 .. n_items)) and bI = double(bO). */
+int g4r_bl_bert4rec_encode(g4r_baselines* b, const int32_t* items, int64_t n_events, const int64_t* session_offsets, int64_t n_sessions,
+                           const int32_t* n_history, float* q, int64_t n_q);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,7 +24,7 @@ _OPTIONS = [
     (('--load_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Load the model, with its optimizer and training state, from a checkpoint written by --save_checkpoint. Exclusive with -ps, -pf and -l.')),
     (('--save_checkpoint',), dict(metavar='CKPT_PATH', type=str, help='Save the model with its optimizer and training state to CKPT_PATH (.npz), so that a later run can train it further.')),
     (('--fit_more',), dict(action='store_true', help='With --load_checkpoint: continue training the loaded model on the training data PATH (new items are added to the catalogue) instead of building a new model.')),
-    (('--baseline',), dict(metavar='NAME', choices=['pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'vstan', 'sr', 'ar', 'narm', 'sasrec', 'srgnn', 'stamp', 'nextitnet'], help='Fit a session baseline (Pop, SessionPop, ItemKNN or BPR of the reference, sknn: session-based kNN, S-KNN / V-SKNN, stan: session kNN with STAN-style time and position decays, vstan: STAN with VSTAN-style vector similarity, neighbour weights and IDF, sr: sequential rules, ar: association rules, narm: the NARM neural session model, sasrec: the SASRec self-attentive model, srgnn: the SR-GNN session-graph model, stamp: the STAMP short-term attention/memory model, nextitnet: the NextItNet dilated convolutional model) instead of GRU4Rec; -ps gives its constructor parameters (e.g. n_sims=200,lmbd=20,alpha=0.5, k=100,sample_size=500,similarity=vector, k=100,lambda_spw=1.02,lambda_snh=inf,lambda_inh=2.05, k=100,similarity=vector,lambda_ipw=inf,lambda_idf=0, steps=10,weighting=div,pruning=20 embedding=50,hidden=100,n_epochs=10, embedding=50,n_blocks=2,n_heads=1,n_epochs=10, embedding=100,step=1,n_epochs=10, embedding=100,n_epochs=10 or embedding=100,dilations=1/2/1/2/1/2,n_epochs=10), each converted to the type of its default (a bool default takes True or False, a tuple default a /-separated list of integers). Exclusive with -pf, -l, -s and the checkpoint options.')),
+    (('--baseline',), dict(metavar='NAME', choices=['pop', 'sessionpop', 'itemknn', 'bpr', 'sknn', 'stan', 'vstan', 'sr', 'ar', 'narm', 'sasrec', 'srgnn', 'stamp', 'nextitnet', 'bert4rec'], help='Fit a session baseline (Pop, SessionPop, ItemKNN or BPR of the reference, sknn: session-based kNN, S-KNN / V-SKNN, stan: session kNN with STAN-style time and position decays, vstan: STAN with VSTAN-style vector similarity, neighbour weights and IDF, sr: sequential rules, ar: association rules, narm: the NARM neural session model, sasrec: the SASRec self-attentive model, srgnn: the SR-GNN session-graph model, stamp: the STAMP short-term attention/memory model, nextitnet: the NextItNet dilated convolutional model, bert4rec: the BERT4Rec bidirectional masked-item model) instead of GRU4Rec; -ps gives its constructor parameters (e.g. n_sims=200,lmbd=20,alpha=0.5, k=100,sample_size=500,similarity=vector, k=100,lambda_spw=1.02,lambda_snh=inf,lambda_inh=2.05, k=100,similarity=vector,lambda_ipw=inf,lambda_idf=0, steps=10,weighting=div,pruning=20 embedding=50,hidden=100,n_epochs=10, embedding=50,n_blocks=2,n_heads=1,n_epochs=10, embedding=100,step=1,n_epochs=10, embedding=100,n_epochs=10, embedding=100,dilations=1/2/1/2/1/2,n_epochs=10 or embedding=64,n_blocks=2,n_heads=2,mask_prob=0.2), each converted to the type of its default (a bool default takes True or False, a tuple default a /-separated list of integers). Exclusive with -pf, -l, -s and the checkpoint options.')),
     (('-t', '--test'), dict(metavar='TEST_PATH', type=str, nargs='+', help='Test data set(s).')),
     (('-m', '--measure'), dict(metavar='AT', type=int, nargs='+', default=[20], help='Recommendation list length(s) for recall & MRR (default: 20).')),
     (('-e', '--eval_type'), dict(metavar='EVAL_TYPE', choices=_TIE_MODES, default='standard', help='Tie handling of the ranking (see evaluate_gpu).')),
@@ -134,14 +134,14 @@ def _train_more(gru, args):
 
 
 def _train_baseline(args):
-    """a baselines.Pop / SessionPop / ItemKNN / BPR / SessionKNN / STAN / VSTAN / SR / AR / NARM / SASRec / SRGNN / STAMP / NextItNet from -ps (values converted to the type of the constructor's default; a bool
+    """a baselines.Pop / SessionPop / ItemKNN / BPR / SessionKNN / STAN / VSTAN / SR / AR / NARM / SASRec / SRGNN / STAMP / NextItNet / BERT4Rec from -ps (values converted to the type of the constructor's default; a bool
     takes True or False, a tuple a /-separated list of integers), fitted on PATH"""
     import inspect
     import baselines
     model_class = {'pop': baselines.Pop, 'sessionpop': baselines.SessionPop, 'itemknn': baselines.ItemKNN, 'bpr': baselines.BPR,
                    'sknn': baselines.SessionKNN, 'stan': baselines.STAN, 'vstan': baselines.VSTAN, 'sr': baselines.SR, 'ar': baselines.AR,
                    'narm': baselines.NARM, 'sasrec': baselines.SASRec, 'srgnn': baselines.SRGNN, 'stamp': baselines.STAMP,
-                   'nextitnet': baselines.NextItNet}[args.baseline]
+                   'nextitnet': baselines.NextItNet, 'bert4rec': baselines.BERT4Rec}[args.baseline]
     defaults = {n: p.default for n, p in inspect.signature(model_class.__init__).parameters.items() if n != 'self'}
     params = {}
     for name, value in (_training_parameters(args).items() if args.parameter_string else []):
